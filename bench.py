@@ -2,7 +2,7 @@
 """bench.py — BASELINE.json metric: EKF-SLAM frames/sec @320x240, N = 100 features (config C4:
 n = 313, m = 200, 11x11 patch, +-20 px search ellipse), aggregate over independent camera streams.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--streams B] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--streams B] [--impl ours|reference] [--dump-outputs DIR]
 
 A "step" = one GoOneStep pass (predict -> select -> patch search -> EKF update -> normalise ->
 cull -> symmetrise) of every camera stream resident on the GPU over one new frame each.
@@ -12,6 +12,7 @@ cull -> symmetrise) of every camera stream resident on the GPU over one new fram
 Multi-GPU: replicas only (independent camera sequences, no collective on the data path); the
 barrier + max-over-ranks timing uses torch.distributed (NCCL).
 `--impl reference`: the CPU oracle (a port: the reference cannot be built here) on all host cores.
+`--dump-outputs DIR`: after the timed steps, what the last timed step computed, as DIR/<name>.npy (see dump_outputs).
 """
 import argparse
 import json
@@ -39,7 +40,7 @@ def parse():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=40)
     ap.add_argument("--warmup", type=int, default=5)
-    ap.add_argument("--streams", type=int, default=296, help="camera streams per GPU")
+    ap.add_argument("--streams", type=int, default=264, help="camera streams per GPU (264 = 2 per SM of an H100 SXM)")
     ap.add_argument("--config", default="C4")
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--ring", type=int, default=4, help="distinct frames per stream")
@@ -51,6 +52,7 @@ def parse():
     ap.add_argument("--only-main", action="store_true", help="skip the legs of the other configs / single stream")
     ap.add_argument("--step-groups", type=int, default=1, choices=[1, 2],
                     help="staggered stream groups of the fused step (1 = serial kernel order)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the outputs of the last timed step to DIR/*.npy")
     return ap.parse_args()
 
 
@@ -58,11 +60,11 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return json.load(open(p)), "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0}, "fallback"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "data sheet (H100 SXM)"
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -210,8 +212,6 @@ def run_reference(args, rank, world):
         last = cpu_run(scenes, budget, threads)
         if k >= args.warmup:
             vals.append(last["fps"])
-        if len(vals) >= 3 and time.time() - T0 > 240:
-            break
     v = float(np.mean(vals))
     sample = "%d streams (1 per pinned thread) x ~%.0f s of oracle steps per bench step" % (threads, budget)
     ref_src = reference_sources_rate(args.config)
@@ -240,20 +240,29 @@ def run_reference(args, rank, world):
     print(json.dumps(line))
 
 
-def _traffic(config, kernel, B):
-    """dram__bytes_read + write per launch of `kernel`, from the ncu capture of THIS config (per stream x B), or None
-    when no capture of that config is committed (profiles/r02_dram_bytes.json, written by tools/ncu_traffic.py)."""
-    fp = os.path.join(ROOT, "profiles", "r02_dram_bytes.json")
-    if not os.path.exists(fp):
-        return None
-    try:
-        v = json.load(open(fp)).get(config, {}).get(kernel)
-        return None if v is None else v["bytes_per_stream"] * B
-    except Exception:
-        return None
+def dump_outputs(ctx, B, outdir):
+    """What a caller of the timed path (sl2_step) receives after the last timed step: every stream's state vector and
+    per-feature results (match positions, flags, selection ranks, counters), and the full covariance of 8 streams
+    picked by a fixed seed (all B covariances would be B x 0.8 MB at C4)."""
+    os.makedirs(outdir, exist_ok=True)
+    xs, feats = [], {k: [] for k in ("z", "h", "S", "flags", "select_rank", "attempted", "successful")}
+    for s in range(B):
+        x, _ = ctx.get_state(s)
+        xs.append(x)
+        f = ctx.features(s)
+        for k in feats:
+            feats[k].append(f[k])
+    picks = np.sort(np.random.default_rng(0).choice(B, size=min(8, B), replace=False))
+    out = {"x": np.stack(xs), "P_streams": picks.astype(np.float64),
+           "P": np.stack([ctx.get_state(int(s))[1] for s in picks])}
+    for k, v in feats.items():
+        out[k] = np.stack(v).astype(np.float64)
+    for k, v in out.items():
+        np.save(os.path.join(outdir, k + ".npy"), v)
 
 
-def measure_config(args, config, B, steps, warmup, rank, local_rank, world, stream, dev, e2e=True, clocks=False):
+def measure_config(args, config, B, steps, warmup, rank, local_rank, world, stream, dev, e2e=True, clocks=False,
+                   dump=None):
     """One workload (BASELINE config) on this rank's GPU: device-resident throughput, end-to-end throughput through
     the C ABI with host frames, per-kernel times.  Returns a dict (times already MAX-reduced over ranks)."""
     import torch
@@ -320,6 +329,8 @@ def measure_config(args, config, B, steps, warmup, rank, local_rank, world, stre
         out["clocks"] = sampler.summary()
     out["ms_per_step"] = ms / steps
     out["value"] = world * B * steps / (ms * 1e-3)
+    if dump:
+        dump_outputs(ctx, B, dump)
 
     # ---- per-kernel durations (CUDA events on the launching stream, one sync per step) ----------
     ctx.enable_timing(True)
@@ -365,23 +376,19 @@ def measure_config(args, config, B, steps, warmup, rank, local_rank, world, stre
     ach = search_bytes / (kt[1] * 1e-3) / 1e9
     m = 2 * nsel
     flops = synth.ekf_structured_flops(n, m) * B
-    fp64_peak, fp64_kind = 37.0, "nominal"
-    fp = os.path.join(ROOT, "profiles", "fp64_peak_measured.json")
-    if os.path.exists(fp):
-        fp64_peak, fp64_kind = json.load(open(fp))["fp64_tflops"], "measured (tools/fp64_pipes.cu)"
-    upd_tr = [_traffic(config, k, B) for k in ("upd_hp", "upd_chol", "upd_solve", "upd_syrk", "upd_finish")]
+    fp64_peak, fp64_kind = 67.0, "data sheet (H100 SXM, FP64 tensor core, 700 W)"
     out["roofline"] = {
         "kernel": "EKF update = upd_hp + upd_chol + upd_solve + upd_syrk + upd_finish (%.0f %% of the step)"
                   % (100 * kt[2] / kt.sum()),
         "bound": "tensor", "achieved": flops / (kt[2] * 1e-3) / 1e12, "peak": fp64_peak, "unit": "TFLOP/s",
         "frac": flops / (kt[2] * 1e-3) / 1e12 / fp64_peak,
-        "traffic": None if any(v is None for v in upd_tr) else float(sum(upd_tr)), "peak_kind": fp64_kind,
+        "traffic": None, "peak_kind": fp64_kind,
         "algorithmic_flops_per_launch": flops, "kernel_ms": float(kt[2]),
-        "note": "FP64 DMMA m8n8k4 (tcgen05 has no FP64 kind); structured-minimum FLOPs of SURVEY 8(d) over the "
+        "note": "FP64 DMMA m8n8k4 (the FP64 tensor-core MMA); structured-minimum FLOPs of SURVEY 8(d) over the "
                 "summed duration of the five update kernels"}
     out["roofline_patch_search"] = {
         "kernel": "search_kernel (patch search)", "bound": "hbm", "achieved": ach, "peak": pk["hbm_gbs"],
-        "unit": "GB/s", "frac": ach / pk["hbm_gbs"], "traffic": _traffic(config, "search", B), "peak_kind": pk_kind,
+        "unit": "GB/s", "frac": ach / pk["hbm_gbs"], "traffic": None, "peak_kind": pk_kind,
         "algorithmic_bytes_per_launch": search_bytes, "kernel_ms": float(kt[1]),
         "note": "integer / FP64 issue bound, not HBM bound: see DESIGN.md 3.1"}
     ctx.close()
@@ -542,7 +549,7 @@ def run_ours(args, rank, local_rank, world):
 
     B = args.streams
     main, scenes = measure_config(args, args.config, B, args.steps, args.warmup, rank, local_rank, world, stream, dev,
-                                  clocks=True)
+                                  clocks=True, dump=args.dump_outputs if rank == 0 else None)
     # the other BASELINE configs (north star: N in {20, 50, 100}; C3 on 8 GPUs = C5) and the single-stream latency
     extra = {}
     if not args.only_main:
@@ -575,7 +582,7 @@ def run_ours(args, rank, local_rank, world):
             "config": {"workload": main["workload"], "streams_per_gpu": B, "frames_per_step": B * world,
                        "state_dim": main["state_dim"], "measurements": 2 * min(sc0.n_select, sc0.n_features),
                        "parallelism": "replicas x%d (no collective)" % world,
-                       "l2": "per-step working set %.0f MB (P + scratch + frames of %d streams) exceeds the 126 MB L2"
+                       "l2": "per-step working set %.0f MB (P + scratch + frames of %d streams) exceeds the 50 MB L2"
                              % ((B * (sc0.n_features * 3 + 13) ** 2 * 8 * 2.1) / 1e6, B),
                        "matched_fraction": main["matched_fraction"], "features_left_stream0": main["features_left_stream0"],
                        "step_groups": args.step_groups,
@@ -583,8 +590,8 @@ def run_ours(args, rank, local_rank, world):
                                         "launch, CUDA events between launches); the timed `value` and `e2e` regions "
                                         "launch back to back"},
             "e2e": main["e2e"], "gpu_launches": main["gpu_launches"], "clocks": main.get("clocks"),
-            # the step's dominant stage = the EKF update (five kernels on the FP64 tensor path); MEASURED_PEAKS.json
-            # has no FP64 entry, so the peak is the DMMA rate measured on this pool by tools/fp64_pipes.cu
+            # the step's dominant stage = the EKF update (five kernels on the FP64 tensor path); the peak is the
+            # H100 SXM data-sheet FP64 tensor-core rate
             "roofline": main["roofline"],
             # the metric also asks for the patch search against the HBM roofline
             "roofline_patch_search": main["roofline_patch_search"],
@@ -597,8 +604,6 @@ def run_ours(args, rank, local_rank, world):
     if world > 1:
         dist.destroy_process_group()
 
-
-T0 = time.time()
 
 if __name__ == "__main__":
     a = parse()

@@ -1,9 +1,9 @@
-/* sl2b200.h — C ABI of libsl2b200.so: the B200-native (sm_100a) implementation of the
+/* sl2b200.h — C ABI of libsl2b200.so: the H100-native (sm_90a) implementation of the
  * SceneLib2 per-frame EKF-MonoSLAM hot path.
  *
  * The reference (hanmekim/SceneLib2) has no plugin / FFI seam; the boundary is the set of C++
  * member functions on the hot path.  Each entry point below names the reference interface it
- * replaces (paths relative to /root/reference/scenelib2/).  The C++ host shim under
+ * replaces (paths relative to scenelib2/ of the original repository).  The C++ host shim under
  * scenelib2_b200/host/ keeps the MonoSLAM / Kalman / Feature class surface on top of this ABI
  * (INTEGRATION.md shows the binding a maintainer would add).
  *
@@ -15,7 +15,7 @@
  *     on the context's CUDA stream and functions that return data synchronise that stream.
  *   - a context holds `num_streams` independent camera streams (one EKF + one frame each);
  *     stream_id selects one of them.  Batched entry points (sl2_step*) advance all of them.
- *   - NO CPU fallback: every function fails with SL2_ERR_CUDA when no sm_100 device is usable.
+ *   - NO CPU fallback: every function fails with SL2_ERR_CUDA when no sm_90 device is usable.
  */
 #ifndef SL2B200_H
 #define SL2B200_H
@@ -60,7 +60,7 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out);
 void sl2_destroy(sl2_ctx *ctx);
 const char *sl2_last_error(const sl2_ctx *ctx); /* ctx may be NULL: error of the last failed create */
 int sl2_sync(sl2_ctx *ctx);
-/* library self-description: "sl2b200 <version> sm_100a" */
+/* library self-description: "sl2b200 <version> sm_90a" */
 const char *sl2_version(void);
 
 /* ---- frames (replaces the cv::Mat `frame` argument of MonoSLAM::GoOneStep, monoslam.cpp:108) */
@@ -220,7 +220,7 @@ int sl2_step_host_async(sl2_ctx *ctx, int32_t slot, const uint8_t *gray, double 
 int sl2_wait_slot(sl2_ctx *ctx, int32_t slot);
 /* The fused step can run the camera streams of a context as `groups` (1 or 2, default 1) staggered groups
  * on internal CUDA streams: with 2, the patch search of one group is scheduled under the EKF update of
- * the other (measured neutral at 296 streams on B200; useful when the update does not fill the GPU).  The groups share no state, so results do not depend on the setting; the reference's GoOneStep
+ * the other (useful when the update does not fill the GPU).  The groups share no state, so results do not depend on the setting; the reference's GoOneStep
  * order (monoslam.cpp:108-180) holds within every camera stream.  Every other entry point first makes
  * the context's stream wait for both groups; sl2_join does only that (no host synchronisation) -- call
  * it before recording your own events on the context's stream after a run of sl2_step calls. */

@@ -4,7 +4,7 @@
 //
 // Minimal column-major FP64 dense algebra standing in for the Eigen3 calls on the
 // SceneLib2 hot path (Eigen3 is an un-vendored dependency of the reference, version
-// unpinned: /root/reference/CMakeModules/FindEigen3.cmake:17-30, README:71-72).
+// unpinned: CMakeModules/FindEigen3.cmake:17-30, README:71-72).
 //
 // Rules (SURVEY.md §8(c)): plain C++17, column-major, FP64, products evaluated in the
 // association order the reference writes them, inner-product accumulation in ascending k,

@@ -1,10 +1,10 @@
 // ORACLE — TEST INFRASTRUCTURE ONLY (see dense.hpp header).
 //
 // CPU restatement of the SceneLib2 patch-correlation search:
-//   A1  correlate2_warning                  /root/reference/scenelib2/improc/improc.cpp:55-134
-//   A2  MonoSLAM::elliptical_search         /root/reference/scenelib2/monoslam.cpp:401-477
-//   A3  MonoSLAM::measure_feature (S->PuInv) /root/reference/scenelib2/monoslam.cpp:368-386
-//   A11 SearchMultipleOverlappingEllipses   /root/reference/scenelib2/improc/
+//   A1  correlate2_warning                  scenelib2/improc/improc.cpp:55-134
+//   A2  MonoSLAM::elliptical_search         scenelib2/monoslam.cpp:401-477
+//   A3  MonoSLAM::measure_feature (S->PuInv) scenelib2/monoslam.cpp:368-386
+//   A11 SearchMultipleOverlappingEllipses   scenelib2/improc/
 //                                            search_multiple_overlapping_ellipses.cpp:41-196
 // Images are raw row-major u8 with an explicit width (the reference reads cv::Mat::data
 // with stride = size().width, improc.cpp:66-67,81-82).

@@ -1,11 +1,11 @@
 // ORACLE — TEST INFRASTRUCTURE ONLY (see dense.hpp header).
 //
 // CPU restatement of the closed-form models that feed the SceneLib2 hot path:
-//   camera            /root/reference/scenelib2/camera.cpp:49-300
-//   motion model      /root/reference/scenelib2/motion_model.cpp:84-380
-//   quaternion utils  /root/reference/scenelib2/support/math_util.cpp:61-114
-//   measurement model /root/reference/scenelib2/full_feature_model.cpp:67-200,
-//                     /root/reference/scenelib2/feature_model.cpp:99-238
+//   camera            scenelib2/camera.cpp:49-300
+//   motion model      scenelib2/motion_model.cpp:84-380
+//   quaternion utils  scenelib2/support/math_util.cpp:61-114
+//   measurement model scenelib2/full_feature_model.cpp:67-200,
+//                     scenelib2/feature_model.cpp:99-238
 // Every function cites the lines it follows.  Scalar expressions keep the reference's
 // left-to-right evaluation order; Eigen quaternion helpers follow Eigen3's generic
 // (non-vectorised) formulas.

@@ -35,8 +35,9 @@ class OrcConfig(C.Structure):
 
 
 def build(force=False):
-    """Compile liboracle.so (and _ref when /root/reference exists).  Building is not using."""
-    have_ref = os.path.isdir("/root/reference/scenelib2/improc")
+    """Compile liboracle.so, and _ref when SL2_REFERENCE_SRC names a checkout of the original SceneLib2 (only
+    tests/golden's generators use it).  Building is not using."""
+    have_ref = os.path.isdir(os.path.join(os.environ.get("SL2_REFERENCE_SRC", "/nonexistent"), "scenelib2", "improc"))
     refm = os.path.join(_HERE, "_ref", "libsl2refmodels.so")
     libs = [_LIB] + ([_REF, refm] if have_ref else [])
     stale = force or any(not os.path.exists(p) for p in libs)
@@ -52,7 +53,8 @@ def build(force=False):
     if stale:
         if not force and os.path.exists(_LIB):
             os.utime(os.path.join(_HERE, "capi.cpp"))  # make only tracks liboracle.so's own sources
-        subprocess.check_call(["make", "-C", _HERE, "-s"])
+        subprocess.check_call(["make", "-C", _HERE, "-s"] +
+                              (["REF=" + os.environ["SL2_REFERENCE_SRC"]] if have_ref else []))
     return _LIB
 
 

@@ -1,5 +1,5 @@
 // ORACLE — TEST INFRASTRUCTURE ONLY.  C entry points into the REFERENCE'S OWN model classes
-// (MotionModel, Camera, FullFeatureModel), compiled unmodified from /root/reference/scenelib2 against the
+// (MotionModel, Camera, FullFeatureModel), compiled unmodified from the original scenelib2/ against the
 // arithmetic stand-in of oracle/stubs_arith (see its header for what is and is not pinned).  Signatures
 // mirror the oracle's orc_* functions so tests can compare the two directly.
 #include <cstring>

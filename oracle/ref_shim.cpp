@@ -1,6 +1,6 @@
 // ORACLE — TEST INFRASTRUCTURE ONLY.
 // extern "C" doorway into the REFERENCE's own improc sources, which oracle/Makefile compiles
-// unmodified from /root/reference/scenelib2/improc/{improc,search_multiple_overlapping_ellipses}.cpp
+// unmodified from the original scenelib2/improc/{improc,search_multiple_overlapping_ellipses}.cpp
 // into oracle/_ref/libsl2ref.so against the storage-only stubs in oracle/stubs/.
 // Used to pin the oracle's A1 / A11 restatements bit-for-bit (tests/test_oracle_ref.py).
 #include <cstdint>

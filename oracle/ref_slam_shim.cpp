@@ -1,6 +1,6 @@
 // ORACLE — TEST INFRASTRUCTURE ONLY.  C entry points into the REFERENCE'S OWN MonoSLAM tracking step:
 // monoslam.cpp, kalman.cpp, feature.cpp, part_feature_model.cpp, the model files, support/*.cpp and improc/*.cpp
-// are compiled UNMODIFIED where they lie under /root/reference against the stand-ins of oracle/stubs_arith
+// are compiled UNMODIFIED where they lie in a SceneLib2 checkout against the stand-ins of oracle/stubs_arith
 // (matrix class with plain-loop arithmetic instead of Eigen, pixel container instead of OpenCV, "key = value;"
 // parser instead of Pangolin; GUI and frame grabber reduced to the empty definitions below).
 // So GoOneStep, KalmanFilterPredict/Update, auto_select_n_features, make_measurements, measure_feature,

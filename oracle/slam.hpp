@@ -2,14 +2,14 @@
 //
 // CPU restatement of the per-frame EKF-MonoSLAM step of SceneLib2, tracking only
 // (enable_mapping = false, no partially-initialised features):
-//   step order            /root/reference/scenelib2/monoslam.cpp:108-180
-//   selection             /root/reference/scenelib2/monoslam.cpp:187-323
-//   measurement           /root/reference/scenelib2/monoslam.cpp:336-496
-//   gather / scatter      /root/reference/scenelib2/monoslam.cpp:501-614
-//   normalise, symmetrise /root/reference/scenelib2/monoslam.cpp:616-637, 143-150
-//   feature culling       /root/reference/scenelib2/monoslam.cpp:644-703, 770-812
-//   EKF predict / update  /root/reference/scenelib2/kalman.cpp:50-119
-//   feature state layout  /root/reference/scenelib2/feature.h:56-143, feature.cpp:108-149
+//   step order            scenelib2/monoslam.cpp:108-180
+//   selection             scenelib2/monoslam.cpp:187-323
+//   measurement           scenelib2/monoslam.cpp:336-496
+//   gather / scatter      scenelib2/monoslam.cpp:501-614
+//   normalise, symmetrise scenelib2/monoslam.cpp:616-637, 143-150
+//   feature culling       scenelib2/monoslam.cpp:644-703, 770-812
+//   EKF predict / update  scenelib2/kalman.cpp:50-119
+//   feature state layout  scenelib2/feature.h:56-143, feature.cpp:108-149
 // "Faithful" storage: per-feature Pxy_ / Pyy_ / matrix_block_list_ blocks exactly like the
 // reference, dense P assembled and scattered around the update (4 gather/scatter passes per
 // frame).

@@ -3,7 +3,7 @@
 // (improc.cpp:66-67,81-82; search_multiple_overlapping_ellipses.cpp:114,160-177): a pixel
 // pointer, a size, a (size,type,fill) constructor and at<T>(row,col).  It contains NO
 // arithmetic: every FP/integer operation executed by oracle/_ref/libsl2ref.so is the
-// reference's own source, compiled unmodified from /root/reference.
+// reference's own source, compiled unmodified from the original SceneLib2 checkout.
 #pragma once
 #include <cmath>
 #include <cstdlib>

@@ -1,4 +1,4 @@
-"""scenelib2_b200 — B200-native (sm_100a) implementation of the SceneLib2 EKF-MonoSLAM hot path.
+"""scenelib2_b200 — H100-native (sm_90a) implementation of the SceneLib2 EKF-MonoSLAM hot path.
 
 Layout (hot path only, see DESIGN.md):
   csrc/      CUDA kernels + the C ABI (libsl2b200.so, declared in include/sl2b200.h)

@@ -1,4 +1,4 @@
-"""In-tree build of libsl2b200.so (sm_100a only).  nvcc cross-compiles without a GPU."""
+"""In-tree build of libsl2b200.so (sm_90a only).  nvcc cross-compiles without a GPU."""
 import os
 import subprocess
 
@@ -17,11 +17,11 @@ def _stale():
 
 
 def build(force=False, verbose=False):
-    """Compile every CUDA source for sm_100a into scenelib2_b200/libsl2b200.so."""
+    """Compile every CUDA source for sm_90a into scenelib2_b200/libsl2b200.so."""
     if not force and not _stale():
         return LIB
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    cmd = [nvcc, "-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+    cmd = [nvcc, "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
            "-Xcompiler", "-fPIC", "-shared", "-cudart", "static", "-o", LIB] + SOURCES
     if verbose:
         cmd.insert(1, "-Xptxas")

@@ -1,5 +1,5 @@
 // api.cu — context management and the extern "C" surface declared in include/sl2b200.h.
-// Host side only orchestrates: every arithmetic step of the hot path runs in the sm_100a
+// Host side only orchestrates: every arithmetic step of the hot path runs in the sm_90a
 // kernels of search.cu / ekf.cu.  There is deliberately no CPU fallback.
 #include <cstdio>
 #include <cstdlib>
@@ -45,19 +45,18 @@ struct sl2_ctx {
   // B's search, so the integer-bound search of one group runs under the FP64-bound update of the other
   // and the two update kernels are half a step out of phase.  Results are identical to the serial order
   // (the groups share nothing); every other entry point joins the two streams first (enter()).
-  int step_groups = 1;  // measured neutral on B200 at 296 streams (update loses its second CTA/SM): off by default
+  int step_groups = 1;  // off by default: with two streams per SM the update would lose its second CTA per SM
   cudaStream_t stream_b = nullptr;
   cudaEvent_t ev_main = nullptr, ev_a_search = nullptr, ev_b_search = nullptr, ev_b_done = nullptr;
   bool b_pending = false, b_search_valid = false;
   std::vector<cudaEvent_t> ev_cmp_b;  // per frame slot: group B is done with the slot
 };
 
-// Defaults of the scheduling knobs (measured on B200: profiles/r02_tuning_sweep.txt, r02_pdl_vs_batch.txt); the
-// environment variable SL2_TUNE="key=value,key=value" overrides them at context creation (experiments, and the
-// parity tests run once with everything switched on).
+// Defaults of the scheduling knobs; the environment variable SL2_TUNE="key=value,key=value" overrides them at context
+// creation (experiments, and the parity tests run once with everything switched on).
 static void tune_defaults(Sl2Dev &d) {
   d.tune[SL2_TUNE_PDL] = 2;           // automatic: on for a single camera stream (launch-latency bound), else off
-  d.tune[SL2_TUNE_HP_PIPELINED] = 1;  // 0.107 -> 0.105 ms at C4 x 296 streams
+  d.tune[SL2_TUNE_HP_PIPELINED] = 1;
   const char *e = getenv("SL2_TUNE");
   while (e && *e) {
     char *end = nullptr;
@@ -172,7 +171,7 @@ int device_nfeat(sl2_ctx *c, int s, int *out) {
 
 extern "C" {
 
-const char *sl2_version(void) { return "sl2b200 0.1.0 sm_100a"; }
+const char *sl2_version(void) { return "sl2b200 0.1.0 sm_90a"; }
 
 void sl2_default_config(sl2_config *cfg) {
   memset(cfg, 0, sizeof *cfg);
@@ -221,8 +220,8 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   cudaDeviceProp prop;
   e = cudaGetDeviceProperties(&prop, cfg->device);
   if (e != cudaSuccess) return fail(nullptr, SL2_ERR_CUDA, cudaGetErrorString(e));
-  if (prop.major != 10)
-    return fail(nullptr, SL2_ERR_CUDA, "libsl2b200 is built for sm_100a (B200) only");
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(nullptr, SL2_ERR_CUDA, "libsl2b200 is built for sm_90a (H100) only");
   e = cudaSetDevice(cfg->device);
   if (e != cudaSuccess) return fail(nullptr, SL2_ERR_CUDA, cudaGetErrorString(e));
 

@@ -1,4 +1,4 @@
-// detect.cu — Shi-Tomasi "best patch" detector on sm_100a (SURVEY.md §8(f) row N3).
+// detect.cu — Shi-Tomasi "best patch" detector on sm_90a (SURVEY.md §8(f) row N3).
 //
 // Replaces MonoSLAM::find_best_patch_inside_region + find_eigenvalues (monoslam.cpp:1070-1205):
 // the smaller eigenvalue of the BOXSIZE x BOXSIZE gradient structure tensor, maximised over a

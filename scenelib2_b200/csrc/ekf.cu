@@ -1,4 +1,4 @@
-// ekf.cu — EKF predict / measurement prediction + selection / cull on sm_100a (the update is update.cu).
+// ekf.cu — EKF predict / measurement prediction + selection / cull on sm_90a (the update is update.cu).
 //
 // Replaces, per camera stream (one CTA per stream, all streams of a context in one launch):
 //   Kalman::KalmanFilterPredict            kalman.cpp:50-69   (+ motion_model.cpp:84-217)

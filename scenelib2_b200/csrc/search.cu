@@ -1,4 +1,4 @@
-// search.cu — patch-correlation feature search on sm_100a.
+// search.cu — patch-correlation feature search on sm_90a.
 //
 // Replaces MonoSLAM::elliptical_search (monoslam.cpp:401-477) calling correlate2_warning
 // (improc/improc.cpp:55-134).  (SearchMultipleOverlappingEllipses::search lives in smoe.cu.)
@@ -8,7 +8,7 @@
 //     from the frame in HBM into shared memory by ONE TMA box load (cp.async.bulk.tensor.3d,
 //     tensor = [slot*stream][H][W] u8) that completes on a per-warp mbarrier; windows larger
 //     than the tile are walked tile by tile.  The TMA unit needs a 16-byte aligned box start
-//     (measured: tools/tma_probe3.cu), so the box is loaded from x & ~15 and is 15 B wider.
+//     so the box is loaded from x & ~15 and is 15 B wider.
 //   * while the TMA is in flight the warp evaluates the exact FP64 ellipse predicate for every
 //     candidate of the tile and compacts the non-empty vertical strips (SL2_STRIP candidates of
 //     one column) into a task list with ballots, so later rounds run with full lanes.

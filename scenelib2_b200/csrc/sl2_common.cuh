@@ -1,4 +1,4 @@
-// sl2_common.cuh — shared device/host declarations of libsl2b200.so (sm_100a only).
+// sl2_common.cuh — shared device/host declarations of libsl2b200.so (sm_90a only).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -97,15 +97,13 @@ __device__ __forceinline__ rd rsqrt_(rd a) { return rd(__dsqrt_rn(a.v)); }
 // executes the pair FIRST, so completion is transitive along the chain of launches.
 __device__ __forceinline__ void pdl_prologue() {
   // wait, THEN release the dependents: at most two kernels of the chain are resident at a time (triggering first
-  // lets the whole chain of a step pile up on the SMs: measured slower at every batch size, tools/run_pdl_order.sh)
+  // lets the whole chain of a step pile up on the SMs: measured slower at every batch size)
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 }
 // SL2_TUNE_PDL: 0 never, 1 always, 2 (default) when the launch covers fewer camera streams than
-// SL2_PDL_AUTO_STREAMS.  Measured (profiles/r02_pdl_vs_batch.txt, C4): ONE stream 0.184 -> 0.178 ms per frame (the step
-// is a chain of 8 kernels of 7-70 us, bound by launch-to-launch latency: a step on an empty map goes 0.047 -> 0.032 ms),
-// 16 streams neutral, 296 streams 1.049 -> 1.074 ms (with the trigger BEFORE the wait the whole chain of the step became
-// resident and waited on the SMs: 1.107 ms, and slower from 4 streams on).
+// SL2_PDL_AUTO_STREAMS: a single camera stream is a chain of 8 short kernels bound by launch-to-launch latency, which
+// PDL shortens; a full batch fills the GPU and PDL only adds resident waiting CTAs.
 #define SL2_PDL_AUTO_STREAMS 2
 inline bool sl2_use_pdl(const Sl2Dev &d, int stream_cnt) {
   const int mode = d.tune[SL2_TUNE_PDL];

@@ -14,7 +14,7 @@ struct PatchConst {
 // improc.cpp:99-133 op for op (never-fused, IEEE div/sqrt).  Deliberately NOT inlined: the
 // filtered kernel reaches it for a handful of candidates per warp, and eight inlined copies of the
 // div/sqrt sequences blew the kernel up to ~66 KB of SASS (instruction-cache misses were the top
-// stall reason, profiles/r01b).
+// stall reason).
 __device__ __noinline__ double exact_score_fn(const PatchConst pc, double Sg1d, double Sg1sqd,
                                               double Sg0g1d, double *sigma1_out) {
   const double g1bar = div_(Sg1d, pc.n);

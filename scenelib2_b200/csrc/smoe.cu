@@ -1,4 +1,4 @@
-// smoe.cu — SearchMultipleOverlappingEllipses::search on sm_100a (SURVEY.md §8 rows A11 / N2).
+// smoe.cu — SearchMultipleOverlappingEllipses::search on sm_90a (SURVEY.md §8 rows A11 / N2).
 //
 // Replaces improc/search_multiple_overlapping_ellipses.cpp:106-196 for the K ellipses (one per depth particle)
 // of each of F partially-initialised features of one frame: the reference evaluates correlate2_warning once per

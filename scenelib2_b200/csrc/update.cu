@@ -1,4 +1,4 @@
-// update.cu — EKF update on sm_100a as a pipeline of five kernels (all streams of a context per launch).
+// update.cu — EKF update on sm_90a as a pipeline of five kernels (all streams of a context per launch).
 //
 // Replaces, per camera stream:
 //   Kalman::KalmanFilterUpdate             kalman.cpp:72-119  (+ gather/scatter monoslam.cpp:501-614)
@@ -133,9 +133,9 @@ __device__ __forceinline__ double pivot_rsqrt(double dv) {
 // identity with the same multipliers (row_i -= U(r,i) * row_r), so it costs no shuffles and no serial tail.
 // All 32 lanes must call.  (Measured alternative, same bits: every lane factoring its own copy of the whole block
 // row by row with no shuffle at all -- 156 FP64 instructions per block instead of 136 + 36 shuffles -- left the
-// batched kernel at 0.116 ms and made the single-stream factor slower, 0.072 -> 0.076 ms; so did dropping the second
-// Newton step of the pivot's rsqrt: at 296 streams the panel's trailing update, fed from L2, is what the barrier
-// waits for, not the factor.)
+// batched kernel unchanged and made the single-stream factor slower; so did dropping the second Newton step of the
+// pivot's rsqrt: with a full batch the panel's trailing update, fed from L2, is what the barrier waits for, not the
+// factor.)
 __device__ __forceinline__ void chol8_inv(double *dg, double *Wm, int o, int lane) {
   const int j = lane & 7;
   double a[8], w[8];
@@ -178,8 +178,8 @@ __device__ __forceinline__ void chol8_inv(double *dg, double *Wm, int o, int lan
 // over P (0.75 MB in, 0.5 MB H P + S out per 100-feature stream) with ~16 FMAs per element, so it is laid out for
 // the memory system: thread = column (8 B x 32 lanes = whole lines), all 24 row loads of an 8-feature block in
 // flight before the first FMA, H rows broadcast from shared memory.  (The round-2 first version ran the 13 dense
-// columns on DMMA tiles and gathered P into fragments: 34 % of HBM peak, L1 request bound.  Measured on this
-// version: prefetch.global.L2 of the next block's rows before the S phase made it 4 % slower.)
+// columns on DMMA tiles and gathered P into fragments: L1 request bound.  Measured on this version:
+// prefetch.global.L2 of the next block's rows before the S phase made it slower.)
 // The CTA's 16 rows of H P also stay in shared memory for S = (H P) H^T + R: thread = measurement column i',
 // H(i', :) in registers, dense part from broadcast reads, structural part gathered from the rows.
 constexpr int HP_THREADS = 320;
@@ -552,8 +552,8 @@ __global__ void __launch_bounds__(HP_THREADS, 2) upd_hp2_kernel(
 // This kernel is a serial chain: 13 diagonal blocks per stream (m = 200), each factored by ONE warp (~7 k cycles:
 // two 8x8 register/shuffle factorizations joined by 8x8 DMMA products), and nothing in the update can start
 // before it ends.  What hides it is other streams on the same SM, so it is kept small enough for two CTAs per SM
-// (all 296 streams of the benchmark resident at once).  Measured alternative: S / U resident in shared memory
-// (193 KB, one CTA per SM, two waves) made every panel 1.7x faster and the kernel 17 % slower (0.159 vs 0.136 ms).
+// (all streams of the benchmark resident at once).  Measured alternative: S / U resident in shared memory
+// (193 KB, one CTA per SM, two waves) made every panel faster and the kernel slower.
 //
 // Left-looking by 16-row panels with a look-ahead, so that the only things between two block factorizations are
 // four DMMA k-steps from shared memory and the W * C product of the finished panel:
@@ -959,7 +959,7 @@ __device__ __forceinline__ double c_to_b(const double (&c)[2][2], int ks, int la
 // panel's, nobody computes a staging address, and there is NO CTA-wide barrier in the panel loop: a warp waits
 // on the mbarrier of the panel it needs and otherwise runs at its own pace.  (Measured before: a 2-deep cp.async
 // ring left the late, small panels bound by the L2 round trip of their own staging, and staging everything with
-// per-thread cp.async cost 22 % of the kernel in index arithmetic.)  NP = 16 does not fit one SM that way: its
+// per-thread cp.async cost a large share of the kernel in index arithmetic.)  NP = 16 does not fit one SM that way: its
 // panels >= SPLIT are requested at panel REUSE into the space of panels 0..REUSE-1 (one CTA barrier).
 template <int NP> struct SolveLayout {
   static constexpr int SPLIT = NP > 13 ? 6 : NP;   // panels >= SPLIT are staged late (second generation)
@@ -980,11 +980,11 @@ template <int NP> struct SolveLayout {
 
 // Two warps share a group of 8 columns: warp (g, rho) owns the row tiles j = 2t + rho, so a thread keeps NP
 // tiles (not 2 NP) and 16 warps fit one SM -- 4 per scheduler instead of 2, which is what hides the shared-memory
-// latency in front of every DMMA (measured: 8 warps x 228 registers ran the FP64 pipe at 40 %).  Per panel the
+// latency in front of every DMMA (8 warps x 228 registers left the FP64 pipe mostly idle).  Per panel the
 // two warps swap their C tile through shared memory (one named barrier of 64 threads), each forms ITS M tile of
 // Y_p = W_pp C_p (4 DMMAs), stores it, and the pair swaps the two tiles of Y_p through shared memory as well (a second
 // 64-thread barrier; the B fragments of Y_p are then plain shared loads).  (Until the middle of round 2 both warps
-// formed all of Y_p -- 8 DMMAs, 4 of them redundant, fragments moved by 8 shuffles: 0.213 ms against 0.195 ms.)
+// formed all of Y_p -- 8 DMMAs, 4 of them redundant, fragments moved by 8 shuffles: measured slower.)
 //
 // FULL: when the measurement rows reach into the last panel the instantiation covers (m > 16 NP - 16: the benchmark
 // shapes), every row tile of every panel exists except possibly the very last one, whose staged columns are zero-filled
@@ -1065,7 +1065,7 @@ __global__ void __launch_bounds__(64 * SOLVE_MAX_WARPS, 1) upd_solve_kernel(cons
     const int cval = wact ? min(2, ncols - cc) : 0;  // how many of them exist (<= 0: none)
     double *gcol = G + m + cc;
     double acc[NP][2];  // tile j = 2 t + rho: rows 8 j + lr, columns cc, cc + 1
-    {  // the next group's tiles: towards L2 now (H P is larger than L2 at 296 streams; the registers are all taken)
+    {  // the next group's tiles: towards L2 now (H P is larger than L2 at the benchmark's stream count; the registers are all taken)
       const int ccn = cc + 8 * (int)(gridDim.x * ngrp);
       if (L::SPLIT >= NP && ccn < ncols) {
 #pragma unroll
@@ -1172,10 +1172,10 @@ __global__ void __launch_bounds__(64 * SOLVE_MAX_WARPS, 1) upd_solve_kernel(cons
 // the slabs are staged by cp.async (LDGSTS) in chunks of KC rows into a ring of ST conflict-free (stride UPD_YS)
 // stages, one __syncthreads per chunk: the stage refilled after the barrier of chunk c is the one chunk c-1 was
 // read from.
-// Columns >= n + 1 and rows >= m are zero-filled.  Measured alternatives: skipping the 8x8 blocks below the
-// diagonal inside a diagonal tile as well (12 of 64 blocks fewer, a predicate per DMMA) was 4 % slower; the same ring filled by bulk copies
-// (cp.async.bulk, one 512-byte row per instruction, full/empty mbarriers, no CTA barrier) was 8 % slower (0.285 vs
-// 0.264 ms) with 2 x 32-row and with 4 x 16-row stages alike; 4 x 16 and 3 x 16 LDGSTS stages: 0.268-0.270 ms.
+// Columns >= n + 1 and rows >= m are zero-filled.  Alternatives that measured slower: skipping the 8x8 blocks below
+// the diagonal inside a diagonal tile as well (12 of 64 blocks fewer, a predicate per DMMA); the same ring filled by
+// bulk copies (cp.async.bulk, one 512-byte row per instruction, full/empty mbarriers, no CTA barrier) with 2 x 32-row
+// and with 4 x 16-row stages alike; 4 x 16 and 3 x 16 LDGSTS stages.
 // Warp w owns rows 16*(w%4).. and columns 32*(w/4).. of the tile:
 //   acc[i][j][e] = T(16*(w%4) + 8*i + lane/4, 32*(w/4) + 8*j + 2*(lane%4) + e).
 template <int KC, int ST>
@@ -1204,7 +1204,7 @@ __global__ void __launch_bounds__(UPD_THREADS, 3) upd_syrk_kernel(const Sl2Dev d
   // 8x8 blocks of the warp's 16 x 32 sub-tile (bit 4 i + j = block (i, j)): an off-diagonal tile computes all of them
   // and mirrors every one; a diagonal tile computes the blocks on / above the diagonal (36 of 64, not the 48 of the
   // sub-tile granularity) and mirrors the ones strictly above.  The three shapes that occur are compiled as separate
-  // loop bodies chosen per warp (no predicate per DMMA: that variant measured 4 % slower).
+  // loop bodies chosen per warp (no predicate per DMMA: that variant measured slower).
   const int bi0 = wa >> 3, bj0 = wb >> 3;
   unsigned cmask = 0xFFu, mmask = 0xFFu;
   if (diag) {
@@ -1236,7 +1236,7 @@ __global__ void __launch_bounds__(UPD_THREADS, 3) upd_syrk_kernel(const Sl2Dev d
   // stage loader: 2 slabs x KC rows x 64 columns; thread = (row warp + 8*j, 16-byte segment `lane`).  Chunks are
   // staged in increasing order, so the source pointers just advance; a full chunk costs the copies, two pointer
   // bumps and nothing else (the first version recomputed row / validity / offsets per copy: ~125 instructions per
-  // chunk and thread, as many as the DMMA loop of the chunk itself; ncu: 10 % of the kernel's warp samples).
+  // chunk and thread, as many as the DMMA loop of the chunk itself).
   const double *pa = srcA + (size_t)warp * ldg, *pb = srcB + (size_t)warp * ldg;  // row `warp` of the next chunk
   const uint32_t sdst = smem_u32(stage_buf + 2 * lane + warp * UPD_YS);
   const size_t rstep = (size_t)8 * ldg;
@@ -1510,10 +1510,10 @@ cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, in
   int nl = 0;
   auto mark = [&](int i) { return ev6 ? cudaEventRecord(ev6[i], st) : cudaSuccess; };
   if ((e = mark(0)) != cudaSuccess) return e;
-  // row blocks of H P / S per stream: spread over CTAs unless the batch already fills the GPU (measured at 296
-  // streams: 1 CTA per stream 0.156 ms, 2: 0.167, 7: 0.200 -- every CTA rebuilds the measurement list and H tables)
+  // row blocks of H P / S per stream: spread over CTAs unless the batch already fills the GPU with two streams per SM
+  // (then one CTA per stream is fastest: every CTA rebuilds the measurement list and H tables)
   const int hp_all = (2 * upd_keven(d.Nmax) + HP_ROWS - 1) / HP_ROWS;
-  const int hp_blocks = stream_cnt >= 2 * 148 ? 1 : hp_all;
+  const int hp_blocks = stream_cnt >= 2 * d.nsm ? 1 : hp_all;
   const bool pdl = sl2_use_pdl(d, stream_cnt);
   if (!only_normalise) {
     const dim3 grid(hp_blocks, stream_cnt);
@@ -1542,7 +1542,7 @@ cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, in
     const size_t smem = solve_smem(np);
     // two warps per 8-column group; a batch that fills the GPU runs one CTA per stream (U staged once per
     // stream, groups walked inside), a small one spreads a stream over nslab CTAs (latency)
-    const bool walk = np <= 13 && stream_cnt >= 148;  // measured at 296 streams: 0.219 ms against 0.270 ms
+    const bool walk = np <= 13 && stream_cnt >= d.nsm;
     if (walk) warps = SOLVE_MAX_WARPS;
     const dim3 grid(walk ? 1 : nslab, stream_cnt), block(64 * warps);
     switch (np) {
@@ -1557,8 +1557,8 @@ cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, in
   }
   if ((e = mark(3)) != cudaSuccess) return e;
   if (!only_normalise) {
-    // one 64x64 tile per CTA (measured: CTAs that walk several tiles with cross-tile prefetch were slower, 0.29-0.31
-    // against 0.264 ms, because they cost the third resident CTA per SM)
+    // one 64x64 tile per CTA (CTAs that walk several tiles with cross-tile prefetch measured slower: they cost the
+    // third resident CTA per SM)
     const int nt = (SL2_NXV + 3 * d.Nmax + 1 + 63) / 64;
     e = sl2_launch_kernel(upd_syrk_kernel<32, 2>, dim3(nt * (nt + 1) / 2, stream_cnt), dim3(UPD_THREADS), SYRK_SMEM,
                           st, pdl, d, stream_lo);

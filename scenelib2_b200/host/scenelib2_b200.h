@@ -3,7 +3,7 @@
 // feature.h:56-143, camera.h:42-78) on top of the C ABI of libsl2b200.so (include/sl2b200.h).
 //
 // Same names, same argument meaning, same `bool`/`int` returns as the reference; the arithmetic
-// runs in the sm_100a kernels.  Host mirrors (xv_, Pxx_, per-feature y_/Pxy_/Pyy_/
+// runs in the sm_90a kernels.  Host mirrors (xv_, Pxx_, per-feature y_/Pxy_/Pyy_/
 // matrix_block_list_, h_/z_/S_/flags/counters) are refreshed before GoOneStep / the Kalman calls
 // return, because the reference's GUI reads them on every redraw (graphic/graphictool.cpp:130-168).
 // Also here: the file-based FrameGrabber / FileGrabber (framegrabber/*.h).

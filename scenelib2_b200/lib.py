@@ -2,7 +2,7 @@
 
 This module is the Python mirror of the reference-facing boundary: the names and argument
 meaning follow MonoSLAM / Kalman (see the header for file:line of each replaced interface).
-There is NO fallback: if the CUDA library is missing or no sm_100 device is usable, calls raise.
+There is NO fallback: if the CUDA library is missing or no sm_90 device is usable, calls raise.
 """
 import ctypes as C
 import os

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 @pytest.fixture(scope="session")
@@ -19,17 +19,10 @@ def oracle():
     return pyoracle
 
 
-@pytest.fixture(scope="session")
-def refimpl(oracle):
-    r = oracle.ref()
-    if r is None:
-        pytest.skip("oracle/_ref/libsl2ref.so not built (reference tree absent)")
-    return r
-
-
-@pytest.fixture(scope="session")
-def refmodels(oracle):
-    r = oracle.ref_models()
-    if r is None:
-        pytest.skip("oracle/_ref/libsl2refmodels.so not built (reference tree absent)")
-    return r
+@pytest.fixture
+def reference(oracle, request):
+    """The reference's own code, replayed from tests/golden (see tests/ref_golden.py)."""
+    from ref_golden import Reference
+    r = Reference(request.node.name, oracle)
+    yield r
+    r.close()

@@ -2,7 +2,7 @@
 selected per frame, ellipses from the EKF's own S_i, known patches).  Frames: 32 synthetic frames walked forwards
 and backwards, so consecutive frames always differ by one step of the bounded random walk.
 
-    python tests/golden/make_c1_trajectory.py            # needs /root/reference (oracle/_ref is built from it)
+    SL2_REFERENCE_SRC=<checkout> python tests/golden/make_c1_trajectory.py   # oracle/_ref is built from it
 
 The fixture is an output of THE REFERENCE'S OWN CODE: monoslam.cpp / kalman.cpp / feature.cpp / models / improc
 compiled unmodified against the stand-ins of oracle/stubs_arith (oracle/_ref/libsl2refmodels.so, driven through
@@ -67,7 +67,7 @@ if __name__ == "__main__":
     from oracle import pyoracle as po
     po.build()
     use_ref = "--oracle" not in sys.argv
-    assert not use_ref or po.ref_models() is not None, "oracle/_ref/libsl2refmodels.so missing (make -C oracle)"
+    assert not use_ref or po.ref_models() is not None, "oracle/_ref/libsl2refmodels.so missing: set SL2_REFERENCE_SRC"
     out = run(po, use_ref=use_ref)
     out["source"] = np.array("reference sources + oracle/stubs_arith" if use_ref else "oracle")
     np.savez_compressed(os.path.join(HERE, "c1_trajectory_1000.npz"), **out)

@@ -1,6 +1,7 @@
-"""Generates tests/golden/*.npz.  Run in the build container (needs /root/reference):
+"""Generates tests/golden/*.npz from the original SceneLib2 sources:
 
-    python tests/golden/make_golden.py
+    SL2_REFERENCE_SRC=<checkout> python tests/golden/make_golden.py
+    SL2_REFERENCE_SRC=<checkout> SL2_RECORD_REFERENCE=1 python -m pytest tests -k reference   # ref_*.npz
 
 * known_patches.npy  : the four 11x11 templates shipped as data/known_patch{0..3}.pgm
                        (input fixtures of BASELINE config C1).
@@ -41,8 +42,10 @@ def read_pgm(path):
 
 
 def main():
-    assert po.ref() is not None, "build oracle/_ref first (make -C oracle)"
-    kp = np.stack([read_pgm("/root/reference/data/known_patch%d.pgm" % i) for i in range(4)])
+    po.build(force=True)
+    assert po.ref() is not None, "oracle/_ref not built: set SL2_REFERENCE_SRC"
+    kp = np.stack([read_pgm(os.path.join(os.environ["SL2_REFERENCE_SRC"], "data", "known_patch%d.pgm" % i))
+                   for i in range(4)])
     np.save(os.path.join(HERE, "known_patches.npy"), kp)
 
     rng = np.random.default_rng(20260923)

@@ -322,17 +322,17 @@ def test_c1_trajectory_1000_steps_matches_oracle_fixture():
     ctx.close()
 
 
-def test_cuda_path_against_the_reference_source(oracle, refmodels, tmp_path):
+def test_cuda_path_against_the_reference_source(oracle, reference, tmp_path):
     """The CUDA path vs the REFERENCE'S OWN MonoSLAM code (monoslam.cpp / kalman.cpp / feature.cpp / models /
-    improc compiled unmodified against oracle/stubs_arith, prebuilt oracle/_ref/libsl2refmodels.so; see
-    oracle/ref_slam_shim.cpp): selection ranks, flags, match positions and counters identical on every frame,
+    improc compiled unmodified against oracle/stubs_arith, oracle/_ref/libsl2refmodels.so; see
+    oracle/ref_slam_shim.cpp), replayed from tests/golden: selection ranks, flags, match positions and counters identical on every frame,
     state and covariance within the test tolerance (C1, and a 24-feature scene where every feature is measured)."""
     kp = np.load(os.path.join(G, "known_patches.npy"))
     cases = [(synth.make_scene("C1", n_frames=10, known_patches=kp), 10),
              (synth.make_scene("C2", n_frames=4, n_features=24, override=False), 4)]
     for ci, (sc, steps) in enumerate(cases):
         ctx = ctx_from_scenes([sc], frame_slots=1)
-        ref = oracle.RefSlam(sc, str(tmp_path / ("case%d" % ci)))
+        ref = reference.slam(sc, str(tmp_path / ("case%d" % ci)))
         for t in range(steps):
             ctx.set_frames(0, sc.frames[t:t + 1])
             ctx.step(0)
@@ -348,7 +348,8 @@ def test_cuda_path_against_the_reference_source(oracle, refmodels, tmp_path):
             assert (fg["attempted"] == fr["attempted"]).all() and (fg["successful"] == fr["successful"]).all()
             xg, Pg = ctx.get_state(0)
             xr, Pr = ref.get_state()
-            assert_state_close(xg, Pg, xr, Pr)
+            stored = np.isfinite(Pr)                          # the stored entries of the reference's P
+            assert_state_close(xg, np.where(stored, Pg, 0.0), xr, np.where(stored, Pr, 0.0))
         ctx.close()
 
 
@@ -367,15 +368,15 @@ def _check_streams_against_oracle(ctx, oracles, picks, scenes_of, frame):
         assert np.abs(Pg - Pg.T).max() == 0.0
 
 
-def test_c4_bench_shape_296_streams_against_oracle(oracle):
-    """The shape bench.py runs (BASELINE C4, 296 camera streams in one context: 2 per SM), 3 frames, with the first,
+def test_c4_bench_shape_264_streams_against_oracle(oracle):
+    """The shape bench.py runs (BASELINE C4, 264 camera streams in one context: 2 per SM of an H100), 3 frames, with the first,
     the two middle and the last stream compared with the oracle -- a stream-indexing bug above the sizes of the other
     tests (<= 37 streams) cannot hide.  The remaining streams are checked against the ground truth of the scene."""
-    B, T, U = 296, 3, 8
+    B, T, U = 264, 3, 8
     uniq = [synth.make_scene("C4", stream_id=u, n_frames=T) for u in range(U)]
     scene_of = lambda s: uniq[(s * 5) % U]          # neighbours get different scenes
     cfg_ctx = ctx_from_scenes([scene_of(s) for s in range(B)], frame_slots=2)
-    picks = (0, 147, 148, 295)
+    picks = (0, 131, 132, 263)
     assert len({(s * 5) % U for s in picks}) == 4
     oracles = {s: oracle_slam_from_scene(oracle, scene_of(s)) for s in picks}
     for t in range(T):
@@ -401,18 +402,18 @@ def test_c4_bench_shape_296_streams_against_oracle(oracle):
 
 def test_scheduling_knobs_leave_results_bit_identical():
     """sl2_set_tuning (programmatic dependent launch between the kernels of the step, the software-pipelined upd_hp
-    against the plain one) only changes how work is launched / pipelined: at the bench shape (C4, 296 streams, where
+    against the plain one) only changes how work is launched / pipelined: at the bench shape (C4, 264 streams, where
     the batched launch shapes are the ones in use) the non-default setting gives the same bits as the default --
     state, covariance, matches, counters -- for device-resident steps and for the asynchronous host ring."""
     import torch
     from scenelib2_b200 import lib
-    B, T, U = 296, 3, 6
+    B, T, U = 264, 3, 6
     uniq = [synth.make_scene("C4", stream_id=u, n_frames=2) for u in range(U)]
     scenes = [uniq[(s * 5) % U] for s in range(B)]
     host = torch.empty((2, B, 240, 320), dtype=torch.uint8, pin_memory=True)
     host.numpy()[:] = np.stack([np.stack([sc.frames[t] for sc in scenes]) for t in range(2)])
     settings = [{}, {lib.TUNE_PDL: 1, lib.TUNE_HP_PIPELINED: 0}]
-    picks = sorted(set(range(0, B, 37)) | {147, 148, B - 1})
+    picks = sorted(set(range(0, B, 37)) | {131, 132, B - 1})
     results = []
     for st in settings:
         c = ctx_from_scenes(scenes, frame_slots=2)
