@@ -60,6 +60,49 @@ def assert_state_close(xg, Pg, xo, Po, rtol=RTOL_TEST):
     return ex, eP
 
 
+def check_streams_against_oracle(ctx, oracles, picks, scenes_of, frame):
+    """Step the oracle of every stream in `picks` on `frame` of its scene and compare it with the stream's state after
+    the fused step: map size, selection, flags, match positions and counters exactly, x and P at RTOL_TEST, P exactly
+    symmetric.  Returns the worst (state, covariance) errors."""
+    worst = (0.0, 0.0)
+    for s in picks:
+        o = oracles[s]
+        o.step(scenes_of(s).frames[frame])
+        fg, fo = ctx.features(s), o.features()
+        assert ctx.num_features(s) == o.num_features, s
+        assert (fg["select_rank"] == fo["select_rank"]).all() and (fg["flags"] == fo["flags"]).all(), s
+        ok = (fo["flags"] & 2) > 0
+        assert (fg["z"][ok] == fo["z"][ok]).all(), s
+        assert (fg["attempted"] == fo["attempted"]).all() and (fg["successful"] == fo["successful"]).all(), s
+        xg, Pg = ctx.get_state(s)
+        e = assert_state_close(xg, Pg, *o.get_state())
+        worst = (max(worst[0], e[0]), max(worst[1], e[1]))
+        assert np.abs(Pg - Pg.T).max() == 0.0, s
+    return worst
+
+
+def update_variant(cap, nf, bad=0, out_of_view=False, stream_id=0, n_frames=12):
+    """C4-sized scene of `nf` features for a context of capacity `cap` that selects up to `cap` features, so that
+    every visible feature is selected.  The templates of `bad` features (spread over the map) are replaced by random
+    bytes: they are selected but never found, so K = nf - bad measurements per step, and the default
+    min_attempts = 10 culls them at step 10.  `out_of_view` moves every feature to the side of the view: nothing is
+    selected (K = 0 with nf > 0)."""
+    sc = synth.make_scene("C4", stream_id=stream_id, n_frames=n_frames, n_features=nf)
+    sc.n_select = cap
+    if bad:
+        idx = np.linspace(0, nf - 1, bad).round().astype(int)
+        assert len(set(idx)) == bad
+        patches = sc.patches.copy()
+        rng = np.random.default_rng(1000 + stream_id)
+        patches[idx] = rng.integers(0, 256, patches[idx].shape, dtype=np.uint8)
+        sc.patches = patches
+    if out_of_view:
+        sc.x0 = sc.x0.copy()
+        sc.x0[13:] += np.tile([3.0, 0.0, 0.0], nf)
+    sc.meta["variant"] = (nf, bad, out_of_view)
+    return sc
+
+
 def random_puinv(rng, n, lo, hi, iso_fraction=0.5):
     out = np.zeros((n, 3))
     for i in range(n):
