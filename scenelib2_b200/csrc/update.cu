@@ -66,6 +66,30 @@ __device__ __forceinline__ void dmma884(double &c0, double &c1, double a, double
       : "+d"(c0), "+d"(c1)
       : "d"(a), "d"(b));
 }
+// D(16x8) = A(16x4) * B(4x8) + C: lane (g, t) = (lane/4, lane%4) holds A(g + 8 i, t) in a[i], B(t, g) in b and
+// C(g + 8 (e/2), 2 t + e%2) in c[e].
+__device__ __forceinline__ void dmma1684(double (&c)[4], const double (&a)[2], double b) {
+  asm("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+      : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+      : "d"(a[0]), "d"(a[1]), "d"(b));
+}
+// D(16x8) = A(16x8) * B(8x8) + C: lane (g, t) = (lane/4, lane%4) holds A(g + 8 (i%2), t + 4 (i/2)) in a[i],
+// B(t + 4 i, g) in b[i] and C(g + 8 (e/2), 2 t + e%2) in c[e].
+__device__ __forceinline__ void dmma1688(double (&c)[4], const double (&a)[4], const double (&b)[2]) {
+  asm("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+      : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+      : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(b[0]), "d"(b[1]));
+}
+// D(16x8) = A(16x16) * B(16x8) + C, the same layout with i < 8 in a and i < 4 in b.  The two 8-row halves of C
+// are separate references: they need not be neighbours in memory or in an array.
+__device__ __forceinline__ void dmma16816(double &c0, double &c1, double &c2, double &c3, const double (&a)[8],
+                                          const double (&b)[4]) {
+  asm("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, "
+      "{%12,%13,%14,%15}, {%0,%1,%2,%3};"
+      : "+d"(c0), "+d"(c1), "+d"(c2), "+d"(c3)
+      : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]), "d"(b[0]),
+        "d"(b[1]), "d"(b[2]), "d"(b[3]));
+}
 __device__ __forceinline__ void cp_async16(void *smem_dst, const void *gsrc, int src_bytes) {
   const uint32_t d = (uint32_t)__cvta_generic_to_shared(smem_dst);
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(d), "l"(gsrc), "r"(src_bytes)
@@ -571,7 +595,8 @@ constexpr int CH_DPS = 18; // row stride of the pre-updated diagonal block
 // One batch item of the panel update: GB 8-column groups from group g0 on, C(16 x 8 GB) = S entries - A * B over the
 // nk finished k-steps (nk is a multiple of 4); A(r,k) = U(k,i0+r) (negated multipliers, shared memory), B = finished
 // rows of U (global / L2), D (4 or 8) k-steps of B fragments in flight.  The result goes to the panel buffer.
-// The k loop is kept to a pointer bump, GB loads, 2 shared loads and 2 GB DMMAs per step: columns past the width are
+// The k loop is kept to a pointer bump, GB loads, 2 shared loads and GB m16n8k4 DMMAs (both 8-row halves of the
+// panel in one product) per step: columns past the width are
 // loaded like any other (they are columns of H P in the same row: valid memory, finite, and they only reach entries
 // of C that are never used), so there is no per-element predicate or index arithmetic in it.
 template <int GB, int D>
@@ -579,7 +604,7 @@ __device__ __forceinline__ void chol_batch(const double *__restrict__ G, int ldg
                                            double *__restrict__ pan, int PW, int i0, int nbp, int nk, int ngroups,
                                            int width, int g0, int lr, int lc) {
   static_assert(D == 4 || D == 8, "nk is a multiple of 4");
-  double c[GB][2][2];
+  double c[GB][4];  // m16n8 C fragments: c[q][2 mt + e] = C(8 mt + lr, 8 (g0 + q) + 2 lc + e)
 #pragma unroll
   for (int q = 0; q < GB; ++q) {
     const int cc = i0 + (g0 + q) * 8 + 2 * lc;  // C fragment: rows lr / lr+8, columns cc, cc+1
@@ -587,8 +612,8 @@ __device__ __forceinline__ void chol_batch(const double *__restrict__ G, int ldg
     for (int mt = 0; mt < 2; ++mt) {
       const int r = mt * 8 + lr;
       const bool rv = r < nbp && (g0 + q) < ngroups;
-      c[q][mt][0] = (rv && cc < width) ? G[(size_t)(i0 + r) * ldg + cc] : 0.0;
-      c[q][mt][1] = (rv && cc + 1 < width) ? G[(size_t)(i0 + r) * ldg + cc + 1] : 0.0;
+      c[q][2 * mt] = (rv && cc < width) ? G[(size_t)(i0 + r) * ldg + cc] : 0.0;
+      c[q][2 * mt + 1] = (rv && cc + 1 < width) ? G[(size_t)(i0 + r) * ldg + cc + 1] : 0.0;
     }
   }
   // B fragment of k-step st, group q: G[(4 st + lc) * ldg + i0 + 8 (g0 + q) + lr]
@@ -602,13 +627,10 @@ __device__ __forceinline__ void chol_batch(const double *__restrict__ G, int ldg
     gpre += kstride;
   };
   auto step = [&](const double *bu) {
-    const double a0 = ap[0], a1 = ap[8];
+    const double a[2] = {ap[0], ap[8]};  // rows lr and 8 + lr of the panel: one m16n8k4 A fragment
     ap += 4 * UPD_MS;
 #pragma unroll
-    for (int q = 0; q < GB; ++q) {
-      dmma884(c[q][0][0], c[q][0][1], a0, bu[q]);
-      dmma884(c[q][1][0], c[q][1][1], a1, bu[q]);
-    }
+    for (int q = 0; q < GB; ++q) dmma1684(c[q], a, bu[q]);
   };
 #pragma unroll
   for (int u = 0; u < D - 1; ++u)
@@ -631,7 +653,7 @@ __device__ __forceinline__ void chol_batch(const double *__restrict__ G, int ldg
       const int pc = (g0 + q) * 8 + 2 * lc;
 #pragma unroll
       for (int mt = 0; mt < 2; ++mt)
-        *reinterpret_cast<double2 *>(pan + (size_t)(mt * 8 + lr) * PW + pc) = make_double2(c[q][mt][0], c[q][mt][1]);
+        *reinterpret_cast<double2 *>(pan + (size_t)(mt * 8 + lr) * PW + pc) = make_double2(c[q][2 * mt], c[q][2 * mt + 1]);
     }
   }
 }
@@ -711,15 +733,15 @@ __global__ void __launch_bounds__(UPD_THREADS, 2) upd_chol_kernel(const Sl2Dev d
       if (it == 0) {
         // ---- diagonal block of this panel: pre-updated block minus panel p-1's rows, then factor ----------
         first = false;
-        double c[2][2][2];  // [column group q][M tile mt][element]
+        double c[2][4];  // [column group q][2 M tile mt + element]
         if (pidx == 0) {
 #pragma unroll
           for (int q = 0; q < 2; ++q)
 #pragma unroll
             for (int mt = 0; mt < 2; ++mt) {
               const int r = mt * 8 + lr, cc = 8 * q + 2 * lc;
-              c[q][mt][0] = (r < nbp && cc < width) ? G[(size_t)r * ldg + cc] : 0.0;
-              c[q][mt][1] = (r < nbp && cc + 1 < width) ? G[(size_t)r * ldg + cc + 1] : 0.0;
+              c[q][2 * mt] = (r < nbp && cc < width) ? G[(size_t)r * ldg + cc] : 0.0;
+              c[q][2 * mt + 1] = (r < nbp && cc + 1 < width) ? G[(size_t)r * ldg + cc + 1] : 0.0;
             }
         } else {
 #pragma unroll
@@ -727,17 +749,15 @@ __global__ void __launch_bounds__(UPD_THREADS, 2) upd_chol_kernel(const Sl2Dev d
 #pragma unroll
             for (int mt = 0; mt < 2; ++mt) {
               const double2 v = *reinterpret_cast<const double2 *>(dcur + (mt * 8 + lr) * CH_DPS + 8 * q + 2 * lc);
-              c[q][mt][0] = v.x;
-              c[q][mt][1] = v.y;
+              c[q][2 * mt] = v.x;
+              c[q][2 * mt + 1] = v.y;
             }
 #pragma unroll
           for (int u = 0; u < 4; ++u) {
             const int st = nk - 4 + u;
-            const double a0 = mcur[(4 * st + lc) * UPD_MS + lr], a1 = mcur[(4 * st + lc) * UPD_MS + 8 + lr];
-            dmma884(c[0][0][0], c[0][0][1], a0, -a0);
-            dmma884(c[0][1][0], c[0][1][1], a1, -a0);
-            dmma884(c[1][0][0], c[1][0][1], a0, -a1);
-            dmma884(c[1][1][0], c[1][1][1], a1, -a1);
+            const double a[2] = {mcur[(4 * st + lc) * UPD_MS + lr], mcur[(4 * st + lc) * UPD_MS + 8 + lr]};
+            dmma1684(c[0], a, -a[0]);
+            dmma1684(c[1], a, -a[1]);
           }
         }
         // Factor the 16x16 diagonal block and form W = U_pp^-T (the panel is then finished with one
@@ -754,8 +774,8 @@ __global__ void __launch_bounds__(UPD_THREADS, 2) upd_chol_kernel(const Sl2Dev d
               const int r = mt * 8 + lr, cc = 8 * q + 2 * lc;
               const bool rv = r < nbp;
               *reinterpret_cast<double2 *>(dg + r * UPD_DS + cc) =
-                  make_double2((rv && cc < nbp) ? c[q][mt][0] : (r == cc ? 1.0 : 0.0),
-                               (rv && cc + 1 < nbp) ? c[q][mt][1] : (r == cc + 1 ? 1.0 : 0.0));
+                  make_double2((rv && cc < nbp) ? c[q][2 * mt] : (r == cc ? 1.0 : 0.0),
+                               (rv && cc + 1 < nbp) ? c[q][2 * mt + 1] : (r == cc + 1 ? 1.0 : 0.0));
             }
           // W12 = 0 (the two diagonal blocks of W are written whole by chol8_inv, W21 by the glue below)
           sm.Wm[(lane >> 3) * UPD_WS + 8 + (lane & 7)] = 0.0;
@@ -807,14 +827,14 @@ __global__ void __launch_bounds__(UPD_THREADS, 2) upd_chol_kernel(const Sl2Dev d
       } else if (it == 1) {
         // ---- look-ahead: diagonal block of panel p+1 minus the contributions of rows < i0 -----------------
         if (nbn == 0) continue;
-        double c[2][2][2];  // starts from the S entries of the block (their load overlaps the first B loads)
+        double c[2][4];  // starts from the S entries of the block (their load overlaps the first B loads)
 #pragma unroll
         for (int q = 0; q < 2; ++q)
 #pragma unroll
           for (int mt = 0; mt < 2; ++mt) {
             const int r = mt * 8 + lr, cc = 8 * q + 2 * lc;
-            c[q][mt][0] = (r < nbn && n0 + cc < width) ? G[(size_t)(n0 + r) * ldg + n0 + cc] : 0.0;
-            c[q][mt][1] = (r < nbn && n0 + cc + 1 < width) ? G[(size_t)(n0 + r) * ldg + n0 + cc + 1] : 0.0;
+            c[q][2 * mt] = (r < nbn && n0 + cc < width) ? G[(size_t)(n0 + r) * ldg + n0 + cc] : 0.0;
+            c[q][2 * mt + 1] = (r < nbn && n0 + cc + 1 < width) ? G[(size_t)(n0 + r) * ldg + n0 + cc + 1] : 0.0;
           }
         double v[CH_D][2];
         const size_t kstride = (size_t)4 * ldg;
@@ -828,14 +848,12 @@ __global__ void __launch_bounds__(UPD_THREADS, 2) upd_chol_kernel(const Sl2Dev d
           gpre += kstride;
         };
         auto step = [&](const double *vu) {
-          const double a0 = vu[0], a1 = vu[1];
-          mp[0] = a0;
-          mp[8] = a1;
+          const double a[2] = {vu[0], vu[1]};
+          mp[0] = a[0];
+          mp[8] = a[1];
           mp += 4 * UPD_MS;
-          dmma884(c[0][0][0], c[0][0][1], a0, -a0);
-          dmma884(c[0][1][0], c[0][1][1], a1, -a0);
-          dmma884(c[1][0][0], c[1][0][1], a0, -a1);
-          dmma884(c[1][1][0], c[1][1][1], a1, -a1);
+          dmma1684(c[0], a, -a[0]);
+          dmma1684(c[1], a, -a[1]);
         };
 #pragma unroll
         for (int u = 0; u < CH_D - 1; ++u)
@@ -857,7 +875,7 @@ __global__ void __launch_bounds__(UPD_THREADS, 2) upd_chol_kernel(const Sl2Dev d
 #pragma unroll
           for (int mt = 0; mt < 2; ++mt)
             *reinterpret_cast<double2 *>(dnext + (mt * 8 + lr) * CH_DPS + 8 * q + 2 * lc) =
-                make_double2(c[q][mt][0], c[q][mt][1]);
+                make_double2(c[q][2 * mt], c[q][2 * mt + 1]);
       } else {
         // ---- trailing columns of this panel: C(16 x cols) - A(16 x i0) * B(i0 x cols) ---------------------
         // few column groups left (late panels): narrow items with a deep B pipeline, so that every warp has an
@@ -882,18 +900,18 @@ __global__ void __launch_bounds__(UPD_THREADS, 2) upd_chol_kernel(const Sl2Dev d
     }
     if (tid == 0) s_next = 1;
     {
-      double aw[2][4];
+      double aw[4][2];  // m16n8k4 A fragments of W, k-step ks
 #pragma unroll
       for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
-        for (int ks = 0; ks < 4; ++ks) aw[mt][ks] = sm.Wm[(mt * 8 + lr) * UPD_WS + 4 * ks + lc];
+        for (int ks = 0; ks < 4; ++ks) aw[ks][mt] = sm.Wm[(mt * 8 + lr) * UPD_WS + 4 * ks + lc];
       // FG column groups per iteration: independent DMMA chains.  Only full panels reach this loop
       // with columns to do (a ragged last panel has ncol == nbp: nothing right of the diagonal block).
       constexpr int FG = 4;
       for (int gb = 2 + warp; gb * 8 < ncol; gb += FG * (UPD_THREADS / 32)) {
-        double c[FG][2][2];
+        double c[FG][4];  // c[f][2 mt + e]: row 8 mt + lr
 #pragma unroll
-        for (int f = 0; f < FG; ++f) c[f][0][0] = c[f][0][1] = c[f][1][0] = c[f][1][1] = 0.0;
+        for (int f = 0; f < FG; ++f) c[f][0] = c[f][1] = c[f][2] = c[f][3] = 0.0;
 #pragma unroll
         for (int ks = 0; ks < 4; ++ks) {
           double bv[FG];
@@ -903,10 +921,7 @@ __global__ void __launch_bounds__(UPD_THREADS, 2) upd_chol_kernel(const Sl2Dev d
             bv[f] = cb < ncol ? sm.pan[(size_t)(4 * ks + lc) * PW + cb] : 0.0;
           }
 #pragma unroll
-          for (int f = 0; f < FG; ++f) {
-            dmma884(c[f][0][0], c[f][0][1], aw[0][ks], bv[f]);
-            dmma884(c[f][1][0], c[f][1][1], aw[1][ks], bv[f]);
-          }
+          for (int f = 0; f < FG; ++f) dmma1684(c[f], aw[ks], bv[f]);
         }
 #pragma unroll
         for (int f = 0; f < FG; ++f) {
@@ -917,11 +932,11 @@ __global__ void __launch_bounds__(UPD_THREADS, 2) upd_chol_kernel(const Sl2Dev d
             const int r = mt * 8 + lr;
             if (r < nbp && cc < ncol) {
               double *dst = G + (size_t)(i0 + r) * ldg + i0 + cc;
-              if (cc + 1 < ncol) *reinterpret_cast<double2 *>(dst) = make_double2(c[f][mt][0], c[f][mt][1]);
-              else *dst = c[f][mt][0];
+              if (cc + 1 < ncol) *reinterpret_cast<double2 *>(dst) = make_double2(c[f][2 * mt], c[f][2 * mt + 1]);
+              else *dst = c[f][2 * mt];
               if (gq < 4) {  // columns of the next panel's diagonal block: its multipliers for these rows
-                mnext[(i0 + r) * UPD_MS + cc - UPD_NB] = -c[f][mt][0];
-                if (cc + 1 < ncol) mnext[(i0 + r) * UPD_MS + cc + 1 - UPD_NB] = -c[f][mt][1];
+                mnext[(i0 + r) * UPD_MS + cc - UPD_NB] = -c[f][2 * mt];
+                if (cc + 1 < ncol) mnext[(i0 + r) * UPD_MS + cc + 1 - UPD_NB] = -c[f][2 * mt + 1];
               }
             }
           }
@@ -951,8 +966,9 @@ __device__ __forceinline__ double c_to_b(const double (&c)[2][2], int ks, int la
 // Right-looking, everything in registers: the warp holds all rows of its 8 columns as DMMA ACCUMULATORS
 // (C layout: tile j = rows 8j..8j+7).  Per panel p: Y_p = W_pp C_p (8 DMMAs, C_p moved to the B layout by
 // shuffles), the finished rows go straight to G as 16-byte stores, and every later row tile j gets
-// acc_j -= U(panel, tile j)^T Y_p: 4 DMMAs per tile (k-step outer, tile inner: consecutive DMMAs never share an
-// accumulator), A from the panel's rows of U in shared memory, B = Y_p from registers.
+// acc_j -= U(panel, tile j)^T Y_p: 4 m16n8k4 DMMAs per pair of the warp's tiles (k-step outer, pair inner:
+// consecutive DMMAs never share an accumulator), A from the panel's rows of U in shared memory, B = Y_p from
+// registers.  On an H100 the 16-row FP64 MMA shapes run at about 1.5x the rate of m8n8k4 (tools/dmma_rate.cu).
 // Staging: ALL panels of U (the part right of the diagonal blocks, <= 166 KB at m = 208) and all W_pp are
 // requested up front by warp 0 as bulk copies (one instruction per 16-row x row-segment / per W row, completion
 // counted in bytes on one mbarrier per panel), so the only latency the kernel ever waits for is the first
@@ -1064,7 +1080,7 @@ __global__ void __launch_bounds__(64 * SOLVE_MAX_WARPS, 1) upd_solve_kernel(cons
     const int cc = c0 + 2 * lc;    // this lane's two columns (C layout)
     const int cval = wact ? min(2, ncols - cc) : 0;  // how many of them exist (<= 0: none)
     double *gcol = G + m + cc;
-    double acc[NP][2];  // tile j = 2 t + rho: rows 8 j + lr, columns cc, cc + 1
+    double acc[(NP + 1) & ~1][2];  // tile j = 2 t + rho: rows 8 j + lr, columns cc, cc + 1 (acc[NP]: zero pad)
     {  // the next group's tiles: towards L2 now (H P is larger than L2 at the benchmark's stream count; the registers are all taken)
       const int ccn = cc + 8 * (int)(gridDim.x * ngrp);
       if (L::SPLIT >= NP && ccn < ncols) {
@@ -1076,7 +1092,7 @@ __global__ void __launch_bounds__(64 * SOLVE_MAX_WARPS, 1) upd_solve_kernel(cons
       }
     }
 #pragma unroll
-    for (int t = 0; t < NP; ++t) {
+    for (int t = 0; t < ((NP + 1) & ~1); ++t) {
       const int row = 8 * (2 * t + rho) + lr;
       acc[t][0] = acc[t][1] = 0.0;
       if (row < m) {
@@ -1139,15 +1155,29 @@ __global__ void __launch_bounds__(64 * SOLVE_MAX_WARPS, 1) upd_solve_kernel(cons
           double yb[4];
 #pragma unroll
           for (int ks = 0; ks < 4; ++ks) yb[ks] = -yg[(4 * ks + lc) * 8 + lr];
-          // this warp's later row tiles: acc_j -= U(panel, tile j)^T Y_p
+          // this warp's later row tiles: acc_j -= U(panel, tile j)^T Y_p as m16n8k4 products over the fixed pairs
+          // of its tiles (2u, 2u + 1): the pair's rows are the two halves of M, so the accumulators of a pair stay
+          // in one register quad for every panel (k-step outer, pair inner: consecutive DMMAs never share an
+          // accumulator).  A tile that is finished (<= p), past the last one or, without FULL, past m8 (its columns
+          // are not staged) gets zero rows of A.
           const double *pbr = pb + 8 * rho + lr;
 #pragma unroll
           for (int ks = 0; ks < 4; ++ks) {
 #pragma unroll
-            for (int t = p + 1; t < NP; ++t) {
-              // warp-uniform; without FULL a tile past m8 is never touched (its columns are not staged)
-              if (FULL || 8 * (2 * t + rho) < m)
-                dmma884(acc[t][0], acc[t][1], pbr[(4 * ks + lc) * PW + 16 * (t - p - 1)], yb[ks]);
+            for (int t = (p + 1) & ~1; t < NP; t += 2) {
+              const bool has[2] = {t > p && (FULL || 8 * (2 * t + rho) < m),
+                                   t + 1 < NP && (FULL || 8 * (2 * t + 2 + rho) < m)};  // warp-uniform
+              if (has[0] || has[1]) {
+                double a[2];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) a[h] = has[h] ? pbr[(4 * ks + lc) * PW + 16 * (t + h - p - 1)] : 0.0;
+                double c[4] = {acc[t][0], acc[t][1], acc[t + 1][0], acc[t + 1][1]};
+                dmma1684(c, a, yb[ks]);
+                acc[t][0] = c[0];
+                acc[t][1] = c[1];
+                acc[t + 1][0] = c[2];
+                acc[t + 1][1] = c[3];
+              }
             }
           }
         }
@@ -1172,15 +1202,18 @@ __global__ void __launch_bounds__(64 * SOLVE_MAX_WARPS, 1) upd_solve_kernel(cons
 // the slabs are staged by cp.async (LDGSTS) in chunks of KC rows into a ring of ST conflict-free (stride UPD_YS)
 // stages, one __syncthreads per chunk: the stage refilled after the barrier of chunk c is the one chunk c-1 was
 // read from.
-// Columns >= n + 1 and rows >= m are zero-filled.  Alternatives that measured slower: skipping the 8x8 blocks below
-// the diagonal inside a diagonal tile as well (12 of 64 blocks fewer, a predicate per DMMA); the same ring filled by
-// bulk copies (cp.async.bulk, one 512-byte row per instruction, full/empty mbarriers, no CTA barrier) with 2 x 32-row
-// and with 4 x 16-row stages alike; 4 x 16 and 3 x 16 LDGSTS stages.
-// Warp w owns rows 16*(w%4).. and columns 32*(w/4).. of the tile:
-//   acc[i][j][e] = T(16*(w%4) + 8*i + lane/4, 32*(w/4) + 8*j + 2*(lane%4) + e).
+// Columns >= n + 1 and rows >= m are zero-filled.
+// Four warps, each a 32x32 quarter of the tile as 2 x 4 m16n8k8 products per 8-row k-step: per k-row a warp reads
+// 64 doubles of the slabs for 1024 FMAs (0.5 B of shared memory per FMA) and the fill writes 0.25 B per FMA more.
+// The 16x32 warp tiles of 8 warps this replaced read 0.75 B per FMA, which with the fill is the 1 B per FMA an
+// H100 SM's shared memory delivers at its FP64 tensor rate (128 B and 128 FMA per clock).
+// Warp w owns rows 32*(w%2).. and columns 32*(w/2).. of the tile:
+//   acc[i][j][e] = T(32*(w%2) + 16*i + 8*(e/2) + lane/4, 32*(w/2) + 8*j + 2*(lane%4) + e%2).
+constexpr int SYRK_THREADS = 128;
 template <int KC, int ST>
-__global__ void __launch_bounds__(UPD_THREADS, 3) upd_syrk_kernel(const Sl2Dev d, int stream_lo) {
+__global__ void __launch_bounds__(SYRK_THREADS, 3) upd_syrk_kernel(const Sl2Dev d, int stream_lo) {
   constexpr int STAGE = 2 * KC * UPD_YS;  // doubles per stage (A slab, B slab)
+  constexpr int NW = SYRK_THREADS / 32;
   extern __shared__ __align__(16) uint8_t smem_raw[];
   double *stage_buf = reinterpret_cast<double *>(smem_raw);
   pdl_prologue();
@@ -1195,33 +1228,34 @@ __global__ void __launch_bounds__(UPD_THREADS, 3) upd_syrk_kernel(const Sl2Dev d
   const int ta = t - tb * (tb + 1) / 2;
   if (tb * 64 >= n + 1) return;  // this stream's map is smaller than the capacity the grid was sized for
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, lr = lane >> 2, lc = lane & 3;
-  const int wa = (warp & 3) * 16, wb = (warp >> 2) * 32;
+  const int wa = (warp & 1) * 32, wb = (warp >> 1) * 32;
   const int ld = d.ld, ldg = d.ldg;
   double *__restrict__ P = d.P + (size_t)s * ld * ld;
   double *__restrict__ x = d.x + (size_t)s * ld;
   const double *__restrict__ G = d.G + (size_t)s * d.mmax * ldg;
   const bool diag = ta == tb;
-  // 8x8 blocks of the warp's 16 x 32 sub-tile (bit 4 i + j = block (i, j)): an off-diagonal tile computes all of them
-  // and mirrors every one; a diagonal tile computes the blocks on / above the diagonal (36 of 64, not the 48 of the
-  // sub-tile granularity) and mirrors the ones strictly above.  The three shapes that occur are compiled as separate
-  // loop bodies chosen per warp (no predicate per DMMA: that variant measured slower).
+  // 8x8 blocks of the warp's 32 x 32 sub-tile (bit 4 bi + bj = block (bi, bj)): an off-diagonal tile computes all of
+  // them and mirrors every one; a diagonal tile writes the blocks on / above the diagonal and mirrors the ones strictly
+  // above.  A diagonal warp issues the 6 of its 8 products that hold such a block (product (i, j) holds blocks
+  // (2i, j) and (2i+1, j)); the warp below the diagonal issues none.  The shapes are compiled as separate loop
+  // bodies chosen per warp, with no predicate per DMMA.
   const int bi0 = wa >> 3, bj0 = wb >> 3;
-  unsigned cmask = 0xFFu, mmask = 0xFFu;
+  unsigned cmask = 0xFFFFu, mmask = 0xFFFFu;
   if (diag) {
     cmask = mmask = 0u;
 #pragma unroll
-    for (int i = 0; i < 2; ++i)
+    for (int bi = 0; bi < 4; ++bi)
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        if (bi0 + i <= bj0 + j) cmask |= 1u << (4 * i + j);
-        if (bi0 + i < bj0 + j) mmask |= 1u << (4 * i + j);
+      for (int bj = 0; bj < 4; ++bj) {
+        if (bi0 + bi <= bj0 + bj) cmask |= 1u << (4 * bi + bj);
+        if (bi0 + bi < bj0 + bj) mmask |= 1u << (4 * bi + bj);
       }
   }
   const bool skip = cmask == 0u;  // sub-tile strictly below the diagonal: mirrored instead
   // the tile of P this warp updates: into L2 while the products run (the epilogue reads it once)
   if (!skip) {
 #pragma unroll
-    for (int i = 0; i < 2; ++i) {
+    for (int i = 0; i < 4; ++i) {
       const int a = ta * 64 + wa + i * 8, bq = tb * 64 + wb + lane;
       if (a < n && bq < n) asm volatile("prefetch.global.L2 [%0];" ::"l"(P + a + (size_t)ld * bq));
     }
@@ -1233,35 +1267,34 @@ __global__ void __launch_bounds__(UPD_THREADS, 3) upd_syrk_kernel(const Sl2Dev d
   const int bytesB = cB + 1 < lim ? 16 : (cB < lim ? 8 : 0);
   const double *srcA = G + (bytesA ? cA : 0);
   const double *srcB = G + (bytesB ? cB : 0);
-  // stage loader: 2 slabs x KC rows x 64 columns; thread = (row warp + 8*j, 16-byte segment `lane`).  Chunks are
+  // stage loader: 2 slabs x KC rows x 64 columns; thread = (row warp + NW*j, 16-byte segment `lane`).  Chunks are
   // staged in increasing order, so the source pointers just advance; a full chunk costs the copies, two pointer
-  // bumps and nothing else (the first version recomputed row / validity / offsets per copy: ~125 instructions per
-  // chunk and thread, as many as the DMMA loop of the chunk itself).
+  // bumps and nothing else.
   const double *pa = srcA + (size_t)warp * ldg, *pb = srcB + (size_t)warp * ldg;  // row `warp` of the next chunk
   const uint32_t sdst = smem_u32(stage_buf + 2 * lane + warp * UPD_YS);
-  const size_t rstep = (size_t)8 * ldg;
+  const size_t rstep = (size_t)NW * ldg;
   auto stage = [&](int chunk) {
     const uint32_t dd = sdst + (uint32_t)(chunk % ST) * (STAGE * 8);
     if ((chunk + 1) * KC <= kr) {  // every row of the chunk exists (CTA-uniform)
 #pragma unroll
-      for (int j = 0; j < KC / 8; ++j) {
-        asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dd + j * 8 * UPD_YS * 8),
+      for (int j = 0; j < KC / NW; ++j) {
+        asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dd + j * NW * UPD_YS * 8),
                      "l"(pa + j * rstep), "r"(bytesA)
                      : "memory");
         if (!diag)
-          asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dd + (KC + j * 8) * UPD_YS * 8),
+          asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dd + (KC + j * NW) * UPD_YS * 8),
                        "l"(pb + j * rstep), "r"(bytesB)
                        : "memory");
       }
     } else {  // the ragged last chunk: rows past kr are zero-filled
 #pragma unroll
-      for (int j = 0; j < KC / 8; ++j) {
-        const bool kv = chunk * KC + warp + 8 * j < kr;
-        asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dd + j * 8 * UPD_YS * 8),
+      for (int j = 0; j < KC / NW; ++j) {
+        const bool kv = chunk * KC + warp + NW * j < kr;
+        asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dd + j * NW * UPD_YS * 8),
                      "l"(kv ? pa + j * rstep : srcA), "r"(kv ? bytesA : 0)
                      : "memory");
         if (!diag)
-          asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dd + (KC + j * 8) * UPD_YS * 8),
+          asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dd + (KC + j * NW) * UPD_YS * 8),
                        "l"(kv ? pb + j * rstep : srcB), "r"(kv ? bytesB : 0)
                        : "memory");
       }
@@ -1269,11 +1302,13 @@ __global__ void __launch_bounds__(UPD_THREADS, 3) upd_syrk_kernel(const Sl2Dev d
     pa += (size_t)KC * ldg;
     pb += (size_t)KC * ldg;
   };
-  double acc[2][4][2];
+  double acc[2][4][4];
 #pragma unroll
   for (int i = 0; i < 2; ++i)
 #pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j][0] = acc[i][j][1] = 0.0;
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) acc[i][j][e] = 0.0;
 #pragma unroll
   for (int c = 0; c < ST - 1; ++c) {
     if (c < nchunk) stage(c);
@@ -1287,58 +1322,62 @@ __global__ void __launch_bounds__(UPD_THREADS, 3) upd_syrk_kernel(const Sl2Dev d
     if (!skip) {
       const double *Ya = stage_buf + (size_t)(ch % ST) * STAGE;
       const double *Yb = diag ? Ya : Ya + KC * UPD_YS;
-      const int krem = kr - ch * KC;  // rows of this chunk that exist (the rest is zero fill)
-      auto chunk = [&](auto mask_c) {
-        constexpr unsigned MASK = decltype(mask_c)::value;
+      const int krem = kr - ch * KC;  // rows of this chunk that exist (the rest, to the chunk's end, is zero fill)
+      auto chunk = [&](auto diag_c) {
+        constexpr bool DIAG = decltype(diag_c)::value;  // products (1, 0) and (1, 1) lie below the diagonal
         auto kstep = [&](int kk) {
-          double a[2], b[4];
+          double a[2][4], b[4][2];
 #pragma unroll
           for (int i = 0; i < 2; ++i)
-            if ((MASK >> (4 * i)) & 0xFu) a[i] = Ya[(kk + lc) * UPD_YS + wa + i * 8 + lr];
+#pragma unroll
+            for (int e = 0; e < 4; ++e)
+              a[i][e] = Ya[(kk + lc + 4 * (e >> 1)) * UPD_YS + wa + 16 * i + 8 * (e & 1) + lr];
 #pragma unroll
           for (int j = 0; j < 4; ++j)
-            if ((MASK >> j) & 0x11u) b[j] = Yb[(kk + lc) * UPD_YS + wb + j * 8 + lr];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) b[j][e] = Yb[(kk + lc + 4 * e) * UPD_YS + wb + j * 8 + lr];
 #pragma unroll
           for (int i = 0; i < 2; ++i)
 #pragma unroll
             for (int j = 0; j < 4; ++j)
-              if ((MASK >> (4 * i + j)) & 1u) dmma884(acc[i][j][0], acc[i][j][1], a[i], b[j]);
+              if (!DIAG || 2 * i <= j) dmma1688(acc[i][j], a[i], b[j]);
         };
         if (krem >= KC) {
 #pragma unroll
-          for (int kk = 0; kk < KC; kk += 4) kstep(kk);
+          for (int kk = 0; kk < KC; kk += 8) kstep(kk);
         } else {
-#pragma unroll 2
-          for (int kk = 0; kk < krem; kk += 4) kstep(kk);
+#pragma unroll 1
+          for (int kk = 0; kk < krem; kk += 8) kstep(kk);
         }
       };
-      if (cmask == 0xFFu) chunk(std::integral_constant<unsigned, 0xFFu>{});
-      else if (cmask == 0xEFu) chunk(std::integral_constant<unsigned, 0xEFu>{});   // all but block (1, 0)
-      else chunk(std::integral_constant<unsigned, 0x8Cu>{});                       // blocks (0, 2), (0, 3), (1, 3)
+      if (cmask == 0xFFFFu) chunk(std::false_type{});
+      else chunk(std::true_type{});
     }
   }
   if (skip) return;
   // the warp's computed blocks of P: the loads of a row group first (independent), then the subtraction and the stores
 #pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    const int a = ta * 64 + wa + i * 8 + lr;
+  for (int bi = 0; bi < 4; ++bi) {
+    const int i = bi >> 1, h = bi & 1;  // product row i, C half h
+    const int a = ta * 64 + wa + bi * 8 + lr;
     double pold[4][2];
 #pragma unroll
     for (int j = 0; j < 4; ++j)
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         const int bq = tb * 64 + wb + j * 8 + 2 * lc + e;
-        pold[j][e] = (((cmask >> (4 * i + j)) & 1u) && a < n && bq < n) ? P[a + (size_t)ld * bq] : 0.0;
+        pold[j][e] = (((cmask >> (4 * bi + j)) & 1u) && a < n && bq < n) ? P[a + (size_t)ld * bq] : 0.0;
       }
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      if (!((cmask >> (4 * i + j)) & 1u)) continue;  // a block below the diagonal: written by the mirror of its twin
+      if (!((cmask >> (4 * bi + j)) & 1u)) continue;  // a block below the diagonal: written by the mirror of its twin
       const int bq = tb * 64 + wb + j * 8 + 2 * lc;
-      const double v0 = pold[j][0] - acc[i][j][0], v1 = pold[j][1] - acc[i][j][1];
+      const double c0 = acc[i][j][2 * h], c1 = acc[i][j][2 * h + 1];
+      const double v0 = pold[j][0] - c0, v1 = pold[j][1] - c1;
       if (a < n && bq < n) {
         P[a + (size_t)ld * bq] = v0;
         if (bq + 1 < n) P[a + (size_t)ld * (bq + 1)] = v1;
-        if ((mmask >> (4 * i + j)) & 1u) {  // lower counterpart: rows = b range (contiguous in P), column a
+        if ((mmask >> (4 * bi + j)) & 1u) {  // lower counterpart: rows = b range (contiguous in P), column a
           double *dst = P + bq + (size_t)ld * a;
           if (bq + 1 < n) *reinterpret_cast<double2 *>(dst) = make_double2(v0, v1);
           else *dst = v0;
@@ -1346,8 +1385,8 @@ __global__ void __launch_bounds__(UPD_THREADS, 3) upd_syrk_kernel(const Sl2Dev d
       }
       // column n of Y is w = U^-T nu: (Y^T Y)(a, n) = (Y^T w)(a)  =>  x += Y^T w   (kalman.cpp:112)
       if (a < n) {
-        if (bq == n) x[a] += acc[i][j][0];
-        if (bq + 1 == n) x[a] += acc[i][j][1];
+        if (bq == n) x[a] += c0;
+        if (bq + 1 == n) x[a] += c1;
       }
     }
   }
@@ -1459,7 +1498,7 @@ inline void solve_shape(int Nmax, int &nslab, int &warps) {
   nslab = (ngroups + SOLVE_MAX_WARPS - 1) / SOLVE_MAX_WARPS;
   warps = (ngroups + nslab - 1) / nslab;
 }
-constexpr size_t SYRK_SMEM = (size_t)4 * 2 * 16 * UPD_YS * sizeof(double);
+constexpr size_t SYRK_SMEM = (size_t)2 * 2 * 32 * UPD_YS * sizeof(double);  // upd_syrk_kernel<32, 2>
 
 }  // namespace
 
@@ -1560,7 +1599,7 @@ cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, in
     // one 64x64 tile per CTA (CTAs that walk several tiles with cross-tile prefetch measured slower: they cost the
     // third resident CTA per SM)
     const int nt = (SL2_NXV + 3 * d.Nmax + 1 + 63) / 64;
-    e = sl2_launch_kernel(upd_syrk_kernel<32, 2>, dim3(nt * (nt + 1) / 2, stream_cnt), dim3(UPD_THREADS), SYRK_SMEM,
+    e = sl2_launch_kernel(upd_syrk_kernel<32, 2>, dim3(nt * (nt + 1) / 2, stream_cnt), dim3(SYRK_THREADS), SYRK_SMEM,
                           st, pdl, d, stream_lo);
     if (e != cudaSuccess) return e;
     ++nl;
