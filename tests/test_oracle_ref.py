@@ -7,6 +7,8 @@ import os
 import numpy as np
 import pytest
 
+from model_cases import measurement_cases, motion_cases, random_xv
+
 G = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
@@ -89,27 +91,9 @@ def test_a2_equals_a11_where_they_coincide(oracle):
 # matrix class with plain-loop arithmetic, NOT Eigen), vs the oracle's restatement.  Pins every formula
 # (Jacobians, Q, projection + distortion, R_i, S_i, visibility); Eigen's summation order stays unpinned.
 
-def _random_xv(rng, normalise=True):
-    xv = np.zeros(13)
-    xv[:3] = rng.normal(0, 0.3, 3)
-    q = rng.normal(0, 1, 4)
-    if normalise:
-        q /= np.linalg.norm(q)
-    xv[3:7] = q
-    xv[7:10] = rng.normal(0, 0.2, 3)
-    xv[10:13] = rng.normal(0, 0.3, 3)
-    return xv
-
-
 def test_motion_model_matches_reference_source(oracle, reference):
-    rng = np.random.default_rng(31)
     worst = 0.0
-    for k in range(200):
-        xv = _random_xv(rng, normalise=(k % 3 != 0))        # the reference never renormalises q (Q1)
-        if k % 10 == 0:
-            xv[10:13] = [0.0, 0.0, 0.01]                    # the cfg's starting omega (data/SceneLib2.cfg:81-83)
-        dt = [1 / 30.0, 0.05, 0.01][k % 3]
-        u = rng.normal(0, 1, 3) if k % 4 == 0 else np.zeros(3)
+    for xv, dt, u in motion_cases():
         a = oracle.motion(xv, dt, u)
         b = reference.call("motion", xv, dt, u)
         for x, y in zip(a, b):
@@ -123,21 +107,9 @@ def test_motion_model_matches_reference_source(oracle, reference):
 
 
 def test_measurement_model_matches_reference_source(oracle, reference):
-    rng = np.random.default_rng(32)
-    cams = [np.array([320, 240, 195.0, 195.0, 162.0, 125.0, 9e-6, 1.0]),
-            np.array([640, 480, 390.0, 392.0, 322.0, 247.0, 2e-6, 2.0])]
     worst = 0.0
     flags_seen = set()
-    for k in range(300):
-        cam8 = cams[k % 2]
-        xv = _random_xv(rng)
-        xv[:3] *= 0.2
-        xv[3:7] = [1, 0, 0, 0] + rng.normal(0, 0.15 if k % 5 else 1.0, 4)
-        y = np.array([rng.uniform(-0.6, 0.6), rng.uniform(-0.4, 0.4), rng.uniform(0.3, 3.0)])
-        if k % 17 == 0:
-            y[2] = -abs(y[2])                                # behind the camera
-        A = rng.normal(0, 1, (16, 16))
-        P = A @ A.T * 1e-4 + 1e-6 * np.eye(16)
+    for k, (cam8, xv, y, P, xp_org) in enumerate(measurement_cases()):
         Pxx, Pxy, Pyy = P[:13, :13], P[:13, 13:], P[13:, 13:]
         a = oracle.predict_feature(cam8, xv, y, Pxx, Pxy, Pyy)
         b = reference.call("predict_feature", cam8, xv, y, Pxx, Pxy, Pyy)
@@ -146,9 +118,6 @@ def test_measurement_model_matches_reference_source(oracle, reference):
                 worst = max(worst, np.abs(x - r).max() / max(1.0, np.abs(r).max()))
             else:
                 assert not np.isfinite(x).all()
-        xp_org = _random_xv(rng)[:7]
-        xp_org[:3] *= 0.2
-        xp_org[3:7] = [1, 0, 0, 0] + rng.normal(0, 0.3, 4)
         h = a[0] if np.isfinite(a[0]).all() else np.array([100.0, 100.0])
         va = oracle.visibility_test(cam8, xv[:7], y, xp_org, h)
         vb = reference.call("visibility_test", cam8, xv[:7], y, xp_org, h)
@@ -168,7 +137,7 @@ def test_particle_prediction_matches_reference_source(oracle, reference):
     worst = 0.0
     for k in range(120):
         cam8 = cams[k % 2]
-        xv = _random_xv(rng)
+        xv = random_xv(rng)
         xv[:3] *= 0.2
         xv[3:7] = [1, 0, 0, 0] + rng.normal(0, 0.15, 4)
         hh = np.array([rng.uniform(-0.5, 0.5), rng.uniform(-0.4, 0.4), 1.0])
