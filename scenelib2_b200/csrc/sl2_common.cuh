@@ -164,7 +164,7 @@ cudaError_t sl2_launch_append(const Sl2Dev &d, int s, const double *y3_dev, cons
 size_t sl2_update_smem_bytes(const Sl2Dev &d);
 cudaError_t sl2_configure_search(const Sl2Dev &d);  // per context: dynamic smem opt-in
 cudaError_t sl2_configure_update(const Sl2Dev &d);
-// partially-initialised features (particles.cu, smoe.cu): F features x Kmax particle slots (K_dev[f] used)
+// partially-initialised features (ekf.cu, smoe.cu, particles.cu): F features x Kmax particle slots (K_dev[f] used)
 cudaError_t sl2_launch_particle_predict(const Sl2Dev &d, int s, int F, int Kmax, const int *K_dev,
                                         const double *ypi, const double *Pxy, const double *Pyy,
                                         const double *lambda, double *h, double *sinv3, double *detS,

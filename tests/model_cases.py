@@ -58,6 +58,23 @@ def measurement_cases():
         yield cam8, xv, y, P, xp_org
 
 
+def particle_cases():
+    """(cam8, xv, ypi, P (19 x 19), lambda (9)) of the particle-prediction comparison: 120 cases over the two cameras,
+    camera poses with a non-unit q, a ray from near the camera centre, 9 sorted depths per ray."""
+    rng = np.random.default_rng(57)
+    for k in range(120):
+        cam8 = CAMS[k % 2]
+        xv = random_xv(rng)
+        xv[:3] *= 0.2
+        xv[3:7] = [1, 0, 0, 0] + rng.normal(0, 0.15, 4)
+        hh = np.array([rng.uniform(-0.5, 0.5), rng.uniform(-0.4, 0.4), 1.0])
+        ypi = np.concatenate([xv[:3] + rng.normal(0, 0.05, 3), hh / np.linalg.norm(hh)])
+        A = rng.normal(0, 1, (19, 19))
+        P = A @ A.T * 1e-4 + 1e-6 * np.eye(19)
+        lam = np.sort(rng.uniform(0.3, 6.0, 9))
+        yield cam8, xv, ypi, P, lam
+
+
 # ---- float64 mirror of the geometry of predict_feature / visibility_test (ekf.cu) -----------------------------------
 def quat_inverse(q):
     return np.array([q[0], -q[1], -q[2], -q[3]]) / (q @ q)

@@ -1,7 +1,8 @@
-"""The device's closed-form models (predict_kernel, ekf.cu) at general camera poses and viewpoints: the motion model's
-fv, F and Q and the normalisation Jacobian read out exactly and compared with the reference's stored outputs, the
-measurement model (h, dh/dxv, dh/dy, R, S) and the visibility gates against the oracle bit for bit, per-feature
-xp_org through deletions, appends and culls, and a fused run in a rigidly moved world.
+"""The device's closed-form models (predict_kernel and particle_predict_kernel, ekf.cu) at general camera poses and
+viewpoints: the motion model's fv, F and Q and the normalisation Jacobian read out exactly and compared with the
+reference's stored outputs, the measurement model (h, dh/dxv, dh/dy, R, S), the depth-particle prediction (h, S^-1,
+det S) and the visibility gates against the oracle bit for bit, per-feature xp_org through deletions, appends and
+culls, and a fused run in a rigidly moved world.
 
 The CPU tests at the top check that the inputs reach what the GPU tests claim to cover."""
 import collections
@@ -295,6 +296,57 @@ def test_measurement_model_matches_reference_outputs(oracle):
     print("\nmeasurement model vs reference: scaled worst %.2e; visibility codes %s" % (worst, sorted(codes.items())))
     assert worst <= 1e-13
     assert codes[0] > 0 and len(codes) >= 5
+
+
+# ---- GPU: particle prediction against the reference's stored outputs -----------------------------------------------
+def _device_particles(ctx, xv, ypi, P, lam):
+    """h, S^-1 (00, 01, 11) and det S of the depth particles lam of the ray ypi, predicted on the device by
+    sl2_measure_partial_features from the camera state xv, P[:13, :13] of stream 0 and the ray's blocks of P."""
+    _load(ctx, 0, np.concatenate([xv, ypi[:3]]), P[:16, :16], xv[None, :7])
+    B = ctx.cfg.boxsize
+    out = ctx.measure_partial_features(0, 0, np.zeros((1, B, B), np.uint8), ypi[None], P[None, :13, 13:],
+                                       P[None, 13:, 13:], lam[None], 0.05, np.full((1, lam.size), 1.0 / lam.size))
+    return out["h"][0], out["Sinv3"][0], out["detS"][0]
+
+
+PARTICLE_OUTPUTS = (("h", 0), ("Sinv3", 2), ("detS", 3))    # positions in the result of predict_particles
+
+
+@pytest.mark.gpu
+def test_particle_prediction_matches_reference_outputs(oracle):
+    """The 120 rays of test_particle_prediction_matches_reference_source (both cameras, camera poses with a non-unit
+    q, 9 depths each): every particle's h, S^-1 and det S bit-identical to oracle.predict_particles and within 1e-13
+    of the reference."""
+    ctxs = [sl2.Context(_cfg(cam8, 1)) for cam8 in mc.CAMS]
+    ref = Reference("test_particle_prediction_matches_reference_source", oracle)
+    worst = 0.0
+    for k, (cam8, xv, ypi, P, lam) in enumerate(mc.particle_cases()):
+        dev = _device_particles(ctxs[k % 2], xv, ypi, P, lam)
+        args = (cam8, xv, ypi, lam, P[:13, :13], P[:13, 13:], P[13:, 13:])
+        a, r = oracle.predict_particles(*args), ref.call("predict_particles", *args)
+        for d, (name, i) in zip(dev, PARTICLE_OUTPUTS):
+            assert d.tobytes() == a[i].tobytes(), (k, name, d, a[i])
+            worst = max(worst, np.abs(d - r[i]).max() / max(1.0, np.abs(r[i]).max()))
+    ref.close()
+    for c in ctxs:
+        c.close()
+    print("\nparticle prediction vs reference: scaled worst %.2e" % worst)
+    assert worst <= 1e-13
+
+
+@pytest.mark.gpu
+def test_particle_prediction_at_zero_norm_q(oracle):
+    """A camera quaternion of zero norm: Eigen's inverse() returns the zero quaternion (its squaredNorm > 0 guard),
+    so the rotation matrix is the identity and the prediction is finite; the device must give the oracle's bits."""
+    cam8, xv, ypi, P, lam = next(mc.particle_cases())
+    xv = xv.copy()
+    xv[3:7] = 0.0
+    ctx = sl2.Context(_cfg(cam8, 1))
+    dev = _device_particles(ctx, xv, ypi, P, lam)
+    ctx.close()
+    a = oracle.predict_particles(cam8, xv, ypi, lam, P[:13, :13], P[:13, 13:], P[13:, 13:])
+    for d, (name, i) in zip(dev, PARTICLE_OUTPUTS):
+        assert np.isfinite(a[i]).all() and d.tobytes() == a[i].tobytes(), (name, d, a[i])
 
 
 # ---- GPU: viewpoint gates, selection and xp_org bookkeeping --------------------------------------------------------

@@ -7,7 +7,7 @@ import os
 import numpy as np
 import pytest
 
-from model_cases import measurement_cases, motion_cases, random_xv
+from model_cases import measurement_cases, motion_cases, particle_cases
 
 G = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
@@ -131,20 +131,8 @@ def test_particle_prediction_matches_reference_source(oracle, reference):
     """N2 prediction (monoslam.cpp:1347-1400): the oracle's PartFeatureModel::predict_particle against the
     reference's own part_feature_model.cpp / feature_model.cpp / feature_init_info.cpp (compiled unmodified
     against oracle/stubs_arith): h, S, S^-1, det S per depth particle."""
-    rng = np.random.default_rng(57)
-    cams = [np.array([320, 240, 195.0, 195.0, 162.0, 125.0, 9e-6, 1.0]),
-            np.array([640, 480, 390.0, 392.0, 322.0, 247.0, 2e-6, 2.0])]
     worst = 0.0
-    for k in range(120):
-        cam8 = cams[k % 2]
-        xv = random_xv(rng)
-        xv[:3] *= 0.2
-        xv[3:7] = [1, 0, 0, 0] + rng.normal(0, 0.15, 4)
-        hh = np.array([rng.uniform(-0.5, 0.5), rng.uniform(-0.4, 0.4), 1.0])
-        ypi = np.concatenate([xv[:3] + rng.normal(0, 0.05, 3), hh / np.linalg.norm(hh)])
-        A = rng.normal(0, 1, (19, 19))
-        P = A @ A.T * 1e-4 + 1e-6 * np.eye(19)
-        lam = np.sort(rng.uniform(0.3, 6.0, 9))
+    for cam8, xv, ypi, P, lam in particle_cases():
         a = oracle.predict_particles(cam8, xv, ypi, lam, P[:13, :13], P[:13, 13:], P[13:, 13:])
         b = reference.call("predict_particles", cam8, xv, ypi, lam, P[:13, :13], P[:13, 13:], P[13:, 13:])
         for x, r in zip(a, b):
