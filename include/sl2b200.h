@@ -31,7 +31,13 @@ extern "C" {
 #define SL2_ERR_CUDA (-2)
 #define SL2_ERR_STATE (-3)
 
-#define SL2_MAX_FEATURES 128 /* per stream; state dimension n = 13 + 3 * features <= 397 */
+/* Map capacity per stream: state dimension n = 13 + 3 * features <= 781.  x, P and the per-feature records live in
+ * device memory and every kernel that scales with n loops over it. */
+#define SL2_MAX_FEATURES 256
+/* Features one step can measure: the rows of S = H P H^T + R are m = 2 * measured <= 256, because the Cholesky
+ * factor and solve of the update keep all of S's factor in shared memory.  A context measures at most
+ * min(max_features, SL2_MAX_MEASURED) features per step. */
+#define SL2_MAX_MEASURED 128
 
 typedef struct sl2_ctx sl2_ctx;
 
@@ -41,8 +47,10 @@ typedef struct sl2_config {
   int32_t frame_slots; /* frames kept in HBM per stream (ring, >= 1) */
   int32_t width, height;
   int32_t boxsize;      /* BOXSIZE: 11 (MonoSLAM::kBoxSize_, monoslam.cpp:48) or 15 */
-  int32_t max_features; /* capacity per stream, <= SL2_MAX_FEATURES */
-  int32_t number_of_features_to_select; /* params.number_of_features_to_select (cfg:60) */
+  int32_t max_features; /* capacity per stream, 1 .. SL2_MAX_FEATURES */
+  int32_t number_of_features_to_select; /* params.number_of_features_to_select (cfg:60); with max_features >
+                                           SL2_MAX_MEASURED it must be <= SL2_MAX_MEASURED (a step never selects
+                                           more than the map holds, so any value is valid below that) */
   int32_t search_tile_radius; /* search half-extent served by ONE TMA window tile (default 20);
                                  larger ellipses are searched in several tiles */
   double fku, fkv, u0, v0, kd1, sd; /* Camera::SetCameraParameters (camera.cpp:58-82) */
@@ -91,7 +99,8 @@ int sl2_delete_feature(sl2_ctx *ctx, int32_t stream_id, int32_t index);
  * (n + 3) x 3 with n the state size before the call (rows 0..n-1: P_{x,y_new} / P_{y_j,y_new}, rows n..n+2: Pyy_,
  * whose upper triangle is taken) -- what the conversion of a partially-initialised feature produces
  * (monoslam.cpp:1262, feature.cpp:45-95).  Nothing else of the map moves (the mirror of sl2_delete_feature).
- * Returns the index of the new feature (>= 0), SL2_ERR_STATE when the map already holds max_features. */
+ * Returns the index of the new feature (>= 0), SL2_ERR_STATE when the map already holds max_features
+ * (<= SL2_MAX_FEATURES). */
 int sl2_append_feature(sl2_ctx *ctx, int32_t stream_id, const double *y, const double *xp_org,
                        const uint8_t *patch, const double *Pcol);
 
@@ -195,7 +204,7 @@ int sl2_make_measurements(sl2_ctx *ctx, int32_t stream_id, int32_t slot);
  * order of construct_total_measurement_stuff (monoslam.cpp:548-572): row pair k belongs to
  * feature feat_index[k]; H_xv is (2k_meas) x 13 row-major, H_y (2k_meas) x 3 row-major,
  * R k_meas x (2x2 col-major, symmetric: SL2_ERR_ARG otherwise; the full block enters S), nu 2k_meas.
- * m = 2 * k_meas. */
+ * m = 2 * k_meas <= 2 * min(max_features, SL2_MAX_MEASURED); SL2_ERR_ARG above that. */
 int sl2_ekf_update(sl2_ctx *ctx, int32_t stream_id, int32_t m, const int32_t *feat_index,
                    const double *H_xv, const double *H_y, const double *R, const double *nu);
 /* same, using the device-resident predictions/measurements of the two calls above */

@@ -206,6 +206,11 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   if (cfg->num_streams < 1 || cfg->frame_slots < 1 || cfg->width < 16 || cfg->height < 16 ||
       cfg->max_features < 1 || cfg->max_features > SL2_MAX_FEATURES)
     return fail(nullptr, SL2_ERR_ARG, "bad sizes in sl2_config");
+  // a step measures at most min(max_features, SL2_MAX_MEASURED) features; below that capacity the selection is
+  // bounded by the map itself, so only a larger map needs the bound on the selection
+  if (cfg->max_features > SL2_MAX_MEASURED && cfg->number_of_features_to_select > SL2_MAX_MEASURED)
+    return fail(nullptr, SL2_ERR_ARG,
+                "number_of_features_to_select must be <= SL2_MAX_MEASURED (128) when max_features > 128");
   if (cfg->boxsize != 11 && cfg->boxsize != 15)
     return fail(nullptr, SL2_ERR_ARG, "boxsize must be 11 or 15");
   if (cfg->width < cfg->boxsize || cfg->height < cfg->boxsize)
@@ -249,7 +254,8 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   d.slots = cfg->frame_slots;
   d.box = cfg->boxsize;
   d.ld = ((SL2_NXV + 3 * d.Nmax) + 7) & ~7;
-  d.mmax = 2 * d.Nmax;
+  d.kmax = d.Nmax < SL2_MAX_MEASURED ? d.Nmax : SL2_MAX_MEASURED;  // the measurement capacity of every step
+  d.mmax = 2 * d.kmax;
   d.ldg = ((d.mmax + SL2_NXV + 3 * d.Nmax + 1) + 7) & ~7;
   d.n_select = cfg->number_of_features_to_select;
   const int radius = cfg->search_tile_radius > 0 ? cfg->search_tile_radius : 20;
@@ -945,7 +951,7 @@ int sl2_make_measurements(sl2_ctx *c, int32_t s, int32_t slot) {
 
 int sl2_ekf_update(sl2_ctx *c, int32_t s, int32_t m, const int32_t *feat_index, const double *H_xv,
                    const double *H_y, const double *R, const double *nu) {
-  if (bad_stream(c, s) || m < 0 || (m & 1) || m > 2 * c->cfg.max_features)
+  if (bad_stream(c, s) || m < 0 || (m & 1) || m > c->d.mmax)
     return fail(c, SL2_ERR_ARG, "sl2_ekf_update: bad m");
   if (m == 0) return SL2_OK;
   if (!feat_index || !H_xv || !H_y || !R || !nu) return fail(c, SL2_ERR_ARG, "sl2_ekf_update: null argument");

@@ -770,8 +770,8 @@ cudaError_t sl2_launch_append(const Sl2Dev &d, int s, const double *y3_dev, cons
 cudaError_t sl2_launch_predict(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *u3_dev,
                                int do_predict, int do_measure, cudaStream_t st) {
   if (stream_cnt <= 0) return cudaSuccess;
-  // 128 threads = one per feature (SL2_MAX_FEATURES); the kernel needs ~255 registers per thread,
-  // so 128-thread CTAs are what lets two streams share an SM
+  // 128 threads, one feature each per pass over the map (two passes at SL2_MAX_FEATURES); the kernel needs ~255
+  // registers per thread, so 128-thread CTAs are what lets two streams share an SM
   return sl2_launch_kernel(predict_kernel, dim3(stream_cnt), dim3(128), 0, st, sl2_use_pdl(d, stream_cnt), d,
                            stream_lo, u3_dev, do_predict, do_measure);
 }

@@ -4,11 +4,13 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "../../include/sl2b200.h"  // SL2_MAX_FEATURES, SL2_MAX_MEASURED
+
 #define SL2_NXV 13          // vehicle state size (motion_model.cpp:44)
 #define SL2_NB 8            // Cholesky row-panel height
 #define SL2_SEARCH_WARPS 4  // features (warps) per search CTA
 #define SL2_STRIP 8         // candidates per vertical strip task
-#define SL2_MAX_FEAT_SMEM 128  // == SL2_MAX_FEATURES (include/sl2b200.h)
+#define SL2_MAX_FEAT_SMEM SL2_MAX_FEATURES  // per-feature shared arrays of the predict and cull kernels
 
 // keys of sl2_set_tuning (include/sl2b200.h: SL2_TUNE_*)
 #define SL2_TUNE_PDL 0           // programmatic dependent launch between the kernels of the fused step (0 / 1 / 2 = auto)
@@ -24,7 +26,8 @@ struct Sl2Dev {
   int box;     // BOXSIZE
   int ld;      // leading dimension of P (>= 13 + 3*Nmax, multiple of 8)
   int ldg;     // leading dimension of the update scratch G
-  int mmax;    // 2 * Nmax
+  int kmax;    // features one step can measure: min(Nmax, SL2_MAX_MEASURED); sizes every measurement table
+  int mmax;    // 2 * kmax: rows of S and of the update scratch G
   int n_select;
   int tile_w, tile_h;  // TMA window tile (bytes x rows)
   int min_attempts;
@@ -68,7 +71,8 @@ struct Sl2Dev {
   int nsm;             // SMs of the device
 };
 
-#define SL2_MAX_PANELS 16  // 16-row panels of S: m <= 2 * SL2_MAX_FEATURES = 256
+#define SL2_MAX_PANELS 16  // 16-row panels of S: m <= 2 * SL2_MAX_MEASURED = 256
+static_assert(2 * SL2_MAX_MEASURED <= 16 * SL2_MAX_PANELS, "every panel of S must fit the panel tables");
 
 // ---- correctly-rounded, never-fused FP64 helpers: the oracle is built with
 // -ffp-contract=off, so every bit-critical expression must avoid FMA contraction.

@@ -51,13 +51,15 @@ constexpr int UPD_MS = 20;   // row stride of the multiplier table: 32 B (mod 12
 constexpr int UPD_YS = 68;   // padded row stride of a staged Y slab (doubles): conflict-free DMMA reads
 constexpr int SOLVE_MAX_WARPS = 8;   // warps (8-column groups) per upd_solve CTA: 2 per SM sub-partition, <= 255 registers
 
-__host__ __device__ inline int upd_keven(int Nmax) { return (Nmax + 1) & ~1; }
-__host__ __device__ inline int upd_panw(int Nmax) {
+// Every measurement-sized table below is sized from kmax = Sl2Dev::kmax (features one step can measure), never from
+// the map capacity: S and its factor live in shared memory, H P rows and P in HBM.
+__host__ __device__ inline int upd_keven(int kmax) { return (kmax + 1) & ~1; }
+__host__ __device__ inline int upd_panw(int kmax) {
   // panel buffer of the factor kernel: S columns only; row stride = 2 (mod 16) doubles: the 8 rows of a DMMA
   // C fragment hit distinct banks
-  return ((2 * upd_keven(Nmax) + 15) & ~15) + 2;
+  return ((2 * upd_keven(kmax) + 15) & ~15) + 2;
 }
-__host__ __device__ inline size_t upd_pan_doubles(int Nmax) { return (size_t)UPD_NB * upd_panw(Nmax); }
+__host__ __device__ inline size_t upd_pan_doubles(int kmax) { return (size_t)UPD_NB * upd_panw(kmax); }
 
 // D(8x8) = A(8x4) * B(4x8) + C on the FP64 tensor path: lane holds A(lane/4, lane%4),
 // B(lane%4, lane/4) and C(lane/4, 2*(lane%4) + {0,1}).
@@ -217,13 +219,13 @@ struct HpSmem {
   int *mfeat;    // [K]
   int *wcount;   // [16]
 };
-__host__ __device__ inline size_t hp_smem_doubles(int Nmax, int ld) {
-  const size_t K = upd_keven(Nmax);
+__host__ __device__ inline size_t hp_smem_doubles(int kmax, int ld) {
+  const size_t K = upd_keven(kmax);
   return (size_t)2 * K * HP_HRS + K * 3 + (K & 1) + 2 * K + (size_t)HP_ROWS * ld;
 }
-__device__ __forceinline__ HpSmem hp_carve(uint8_t *base, int Nmax, int ld) {
+__device__ __forceinline__ HpSmem hp_carve(uint8_t *base, int kmax, int ld) {
   HpSmem u;
-  const int K = upd_keven(Nmax);
+  const int K = upd_keven(kmax);
   double *p = reinterpret_cast<double *>(base);
   u.Hrow = p;  p += (size_t)2 * K * HP_HRS;
   u.Rv = p;  p += (size_t)K * 3 + (K & 1);
@@ -258,7 +260,7 @@ __device__ __forceinline__ int hp_tables(const Sl2Dev &d, const HpSmem &sm, int 
     if (lane == 0) sm.wcount[warp] = __popc(bal);
     __syncthreads();
     int base = 0, total = 0;
-    for (int w = 0; w < (SL2_MAX_FEAT_SMEM + 31) / 32; ++w) {
+    for (int w = 0; w < (SL2_MAX_MEASURED + 31) / 32; ++w) {  // nsel <= kmax: later warps select nothing
       if (w < warp) base += sm.wcount[w];
       total += sm.wcount[w];
     }
@@ -324,7 +326,7 @@ __global__ void __launch_bounds__(HP_THREADS, 2) upd_hp_kernel(
   extern __shared__ __align__(16) uint8_t smem_raw[];
   pdl_prologue();
   const int ld = d.ld, ldg = d.ldg;
-  const HpSmem sm = hp_carve(smem_raw, d.Nmax, ld);
+  const HpSmem sm = hp_carve(smem_raw, d.kmax, ld);
   const int s = stream_lo + blockIdx.y;
   const int tid = threadIdx.x;
   const int nf = d.nfeat[s];
@@ -441,7 +443,7 @@ __global__ void __launch_bounds__(HP_THREADS, 2) upd_hp2_kernel(
   pdl_prologue();
   constexpr int R2 = 8, F2 = 4;  // rows / features per block
   const int ld = d.ld, ldg = d.ldg;
-  const HpSmem sm = hp_carve(smem_raw, d.Nmax, ld);
+  const HpSmem sm = hp_carve(smem_raw, d.kmax, ld);
   const int s = stream_lo + blockIdx.y;
   const int tid = threadIdx.x;
   const int n = SL2_NXV + 3 * d.nfeat[s];
@@ -667,13 +669,13 @@ struct CholSmem {
   double *pan;      // panel buffer [NB][panw]
   int panw;
 };
-__host__ __device__ inline size_t chol_smem_doubles(int Nmax) {
-  const size_t mmax = 2 * upd_keven(Nmax);
-  return 2 * mmax * UPD_MS + 2 * UPD_NB * CH_DPS + UPD_NB * UPD_DS + UPD_NB * UPD_WS + upd_pan_doubles(Nmax);
+__host__ __device__ inline size_t chol_smem_doubles(int kmax) {
+  const size_t mmax = 2 * upd_keven(kmax);
+  return 2 * mmax * UPD_MS + 2 * UPD_NB * CH_DPS + UPD_NB * UPD_DS + UPD_NB * UPD_WS + upd_pan_doubles(kmax);
 }
-__device__ __forceinline__ CholSmem chol_carve(uint8_t *base, int Nmax) {
+__device__ __forceinline__ CholSmem chol_carve(uint8_t *base, int kmax) {
   CholSmem u;
-  const int mmax = 2 * upd_keven(Nmax);
+  const int mmax = 2 * upd_keven(kmax);
   double *p = reinterpret_cast<double *>(base);
   u.msz = mmax * UPD_MS;
   u.mult = p;  p += (size_t)2 * u.msz;
@@ -681,14 +683,14 @@ __device__ __forceinline__ CholSmem chol_carve(uint8_t *base, int Nmax) {
   u.dg = p;  p += UPD_NB * UPD_DS;
   u.Wm = p;  p += UPD_NB * UPD_WS;
   u.pan = p;
-  u.panw = upd_panw(Nmax);
+  u.panw = upd_panw(kmax);
   return u;
 }
 
 __global__ void __launch_bounds__(UPD_THREADS, 2) upd_chol_kernel(const Sl2Dev d, int stream_lo) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   pdl_prologue();
-  const CholSmem sm = chol_carve(smem_raw, d.Nmax);
+  const CholSmem sm = chol_carve(smem_raw, d.kmax);
   const int s = stream_lo + blockIdx.x;
   const int tid = threadIdx.x;
   const int ldg = d.ldg;
@@ -1479,9 +1481,9 @@ __global__ void __launch_bounds__(UPD_THREADS) upd_finish_kernel(const Sl2Dev d,
 }
 
 // ---- host-side shapes ---------------------------------------------------------------------------
-inline int solve_panels(int Nmax) { return (2 * upd_keven(Nmax) + 15) / 16; }
-inline int solve_np(int Nmax) {  // instantiation that covers the capacity
-  const int p = solve_panels(Nmax);
+inline int solve_panels(int kmax) { return (2 * upd_keven(kmax) + 15) / 16; }
+inline int solve_np(int kmax) {  // instantiation that covers the measurement capacity
+  const int p = solve_panels(kmax);
   return p <= 4 ? 4 : (p <= 7 ? 7 : (p <= 10 ? 10 : (p <= 13 ? 13 : 16)));
 }
 inline size_t solve_smem(int np) {
@@ -1503,11 +1505,11 @@ constexpr size_t SYRK_SMEM = (size_t)2 * 2 * 32 * UPD_YS * sizeof(double);  // u
 }  // namespace
 
 size_t sl2_update_smem_bytes(const Sl2Dev &d) {  // upd_chol
-  return chol_smem_doubles(d.Nmax) * sizeof(double);
+  return chol_smem_doubles(d.kmax) * sizeof(double);
 }
 
 static size_t hp_smem_bytes(const Sl2Dev &d) {
-  return hp_smem_doubles(d.Nmax, d.ld) * sizeof(double) + (upd_keven(d.Nmax) + 16) * sizeof(int);
+  return hp_smem_doubles(d.kmax, d.ld) * sizeof(double) + (upd_keven(d.kmax) + 16) * sizeof(int);
 }
 static size_t hp2_smem_bytes(const Sl2Dev &d, int kd) {  // + the parked leading rows of P: [kd][HP_THREADS]
   return hp_smem_bytes(d) + (size_t)kd * HP_THREADS * sizeof(double);
@@ -1528,7 +1530,7 @@ cudaError_t sl2_configure_update(const Sl2Dev &d) {
   if (e != cudaSuccess) return e;
   e = cudaFuncSetAttribute(upd_syrk_kernel<32, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SYRK_SMEM);
   if (e != cudaSuccess) return e;
-  const int np = solve_np(d.Nmax);
+  const int np = solve_np(d.kmax);
   const int smem = (int)solve_smem(np);
   switch (np) {
     case 4: return cudaFuncSetAttribute(upd_solve_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
@@ -1551,7 +1553,7 @@ cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, in
   if ((e = mark(0)) != cudaSuccess) return e;
   // row blocks of H P / S per stream: spread over CTAs unless the batch already fills the GPU with two streams per SM
   // (then one CTA per stream is fastest: every CTA rebuilds the measurement list and H tables)
-  const int hp_all = (2 * upd_keven(d.Nmax) + HP_ROWS - 1) / HP_ROWS;
+  const int hp_all = (2 * upd_keven(d.kmax) + HP_ROWS - 1) / HP_ROWS;
   const int hp_blocks = stream_cnt >= 2 * d.nsm ? 1 : hp_all;
   const bool pdl = sl2_use_pdl(d, stream_cnt);
   if (!only_normalise) {
@@ -1577,7 +1579,7 @@ cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, in
   if (!only_normalise) {
     int nslab, warps;
     solve_shape(d.Nmax, nslab, warps);
-    const int np = solve_np(d.Nmax);
+    const int np = solve_np(d.kmax);
     const size_t smem = solve_smem(np);
     // two warps per 8-column group; a batch that fills the GPU runs one CTA per stream (U staged once per
     // stream, groups walked inside), a small one spreads a stream over nslab CTAs (latency)

@@ -196,7 +196,9 @@ class MonoSLAM {  // monoslam.h:73-218 (hot-path subset + the calls of examples/
 
   // ---- device side (not in the reference) ----------------------------------------------------
   // Creates the GPU context; called by Init(), or directly when the map is built in code.
-  // max_features bounds the map size; device = CUDA ordinal.  Throws std::runtime_error on failure.
+  // max_features bounds the map size (<= SL2_MAX_FEATURES; above SL2_MAX_MEASURED the configuration's
+  // number_of_features_to_select must be <= SL2_MAX_MEASURED); device = CUDA ordinal.  Init() reads the known
+  // features f1 .. fN, N <= SL2_MAX_FEATURES.  Throws std::runtime_error on failure.
   void CreateDevice(int max_features = 100, int device = 0);
   void UploadMap();    // host y_/xp_org_/patch_/xv_/P blocks -> device (whole map; first upload)
   void SyncFromDevice();  // device state + per-feature results -> host mirrors

@@ -17,7 +17,8 @@ i32p = C.POINTER(C.c_int32)
 f64p = C.POINTER(C.c_double)
 f32p = C.POINTER(C.c_float)
 
-SL2_MAX_FEATURES = 128
+SL2_MAX_FEATURES = 256   # map capacity per stream (n <= 781)
+SL2_MAX_MEASURED = 128   # features one step can measure (m <= 256)
 # keys of Context.set_tuning (SL2_TUNE_* of include/sl2b200.h)
 TUNE_PDL, TUNE_HP_PIPELINED = 0, 1
 
