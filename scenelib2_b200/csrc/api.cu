@@ -52,25 +52,6 @@ struct sl2_ctx {
   std::vector<cudaEvent_t> ev_cmp_b;  // per frame slot: group B is done with the slot
 };
 
-// Defaults of the scheduling knobs; the environment variable SL2_TUNE="key=value,key=value" overrides them at context
-// creation (experiments, and the parity tests run once with everything switched on).
-static void tune_defaults(Sl2Dev &d) {
-  d.tune[SL2_TUNE_PDL] = 2;           // automatic: on for a single camera stream (launch-latency bound), else off
-  d.tune[SL2_TUNE_HP_PIPELINED] = 1;
-  const char *e = getenv("SL2_TUNE");
-  while (e && *e) {
-    char *end = nullptr;
-    const long k = strtol(e, &end, 10);
-    if (end == e || *end != '=') break;
-    e = end + 1;
-    const long v = strtol(e, &end, 10);
-    if (end == e) break;
-    if (k >= 0 && k < SL2_TUNE_COUNT && v >= 0) d.tune[k] = (int)v;
-    e = (*end == ',') ? end + 1 : end;
-  }
-}
-
-
 namespace {
 
 int fail(sl2_ctx *c, int code, const std::string &msg) {
@@ -245,7 +226,6 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   Sl2Dev &d = c->d;
   memset(&d, 0, sizeof d);
   d.nsm = prop.multiProcessorCount;
-  tune_defaults(d);
   d.B = cfg->num_streams;
   d.Nmax = cfg->max_features;
   d.W = cfg->width;
@@ -1147,13 +1127,6 @@ int sl2_set_step_groups(sl2_ctx *c, int32_t groups) {
   if (!c || groups < 1 || groups > 2) return fail(c, SL2_ERR_ARG, "sl2_set_step_groups: 1 or 2");
   enter(c);
   c->step_groups = groups;
-  return SL2_OK;
-}
-
-int sl2_set_tuning(sl2_ctx *c, int32_t key, int32_t value) {
-  if (!c || key < 0 || key >= SL2_TUNE_COUNT || value < 0) return fail(c, SL2_ERR_ARG, "sl2_set_tuning: bad key / value");
-  enter(c);
-  c->d.tune[key] = value;  // Sl2Dev travels by value with every launch: the next launch sees it
   return SL2_OK;
 }
 

@@ -772,7 +772,7 @@ cudaError_t sl2_launch_predict(const Sl2Dev &d, int stream_lo, int stream_cnt, c
   if (stream_cnt <= 0) return cudaSuccess;
   // 128 threads, one feature each per pass over the map (two passes at SL2_MAX_FEATURES); the kernel needs ~255
   // registers per thread, so 128-thread CTAs are what lets two streams share an SM
-  return sl2_launch_kernel(predict_kernel, dim3(stream_cnt), dim3(128), 0, st, sl2_use_pdl(d, stream_cnt), d,
+  return sl2_launch_kernel(predict_kernel, dim3(stream_cnt), dim3(128), 0, st, sl2_use_pdl(stream_cnt), d,
                            stream_lo, u3_dev, do_predict, do_measure);
 }
 
@@ -789,6 +789,6 @@ cudaError_t sl2_launch_particle_predict(const Sl2Dev &d, int s, int F, int Kmax,
 cudaError_t sl2_launch_cull(const Sl2Dev &d, int stream_lo, int stream_cnt, int force_index,
                             cudaStream_t st) {
   if (stream_cnt <= 0) return cudaSuccess;
-  return sl2_launch_kernel(cull_kernel, dim3(stream_cnt), dim3(256), 0, st, sl2_use_pdl(d, stream_cnt), d,
+  return sl2_launch_kernel(cull_kernel, dim3(stream_cnt), dim3(256), 0, st, sl2_use_pdl(stream_cnt), d,
                            stream_lo, force_index);
 }

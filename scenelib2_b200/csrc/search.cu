@@ -22,26 +22,11 @@
 //     urel-major / vrel-minor scan order wins) carried as (score, scan index) through a
 //     warp-shuffle reduction.
 #include "sl2_common.cuh"
+#include "sl2_ptx.cuh"
 #include "sl2_score.cuh"
 
 namespace {
 
-__device__ __forceinline__ uint32_t smem_u32(const void *p) {
-  return (uint32_t)__cvta_generic_to_shared(p);
-}
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void fence_barrier_init() {
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void fence_proxy_async() {
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes)
-               : "memory");
-}
 __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap *map, uint32_t bar,
                                             int c0, int c1, int c2) {
   asm volatile(
@@ -49,19 +34,6 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap *map
       "[%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
       "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t phase) {
-  uint32_t ok;
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-      "selp.u32 %0, 1, 0, p;\n"
-      "}\n"
-      : "=r"(ok)
-      : "r"(bar), "r"(phase)
-      : "memory");
-  return ok != 0;
 }
 
 struct Best {
@@ -325,8 +297,7 @@ __global__ void __launch_bounds__(SL2_SEARCH_WARPS * 32, FILTER ? (BOX <= 11 ? 4
         }
         }
         __syncwarp();
-        while (!mbar_try_wait(bar, phase)) {
-        }
+        mbar_wait(bar, phase);
         phase ^= 1;
 
         // ---- strips ------------------------------------------------------------------------
@@ -517,7 +488,7 @@ cudaError_t launch_t(const Sl2Dev &d, const CUtensorMap &tmap, const SearchLaunc
   const int grid = groups * L.stream_cnt;
   if (grid <= 0) return cudaSuccess;
   return sl2_launch_kernel(search_kernel<BOX, FILTER>, dim3(grid), dim3(SL2_SEARCH_WARPS * 32), smem, st,
-                           sl2_use_pdl(d, L.stream_cnt), tmap, d, L, dump);
+                           sl2_use_pdl(L.stream_cnt), tmap, d, L, dump);
 }
 
 cudaError_t launch_any(const Sl2Dev &d, const CUtensorMap &tmap, const SearchLaunch &L,

@@ -7,15 +7,9 @@
 #include "../../include/sl2b200.h"  // SL2_MAX_FEATURES, SL2_MAX_MEASURED
 
 #define SL2_NXV 13          // vehicle state size (motion_model.cpp:44)
-#define SL2_NB 8            // Cholesky row-panel height
 #define SL2_SEARCH_WARPS 4  // features (warps) per search CTA
 #define SL2_STRIP 8         // candidates per vertical strip task
 #define SL2_MAX_FEAT_SMEM SL2_MAX_FEATURES  // per-feature shared arrays of the predict and cull kernels
-
-// keys of sl2_set_tuning (include/sl2b200.h: SL2_TUNE_*)
-#define SL2_TUNE_PDL 0           // programmatic dependent launch between the kernels of the fused step (0 / 1 / 2 = auto)
-#define SL2_TUNE_HP_PIPELINED 1  // upd_hp: 8-row blocks, S phase of block b under the loads of block b+1
-#define SL2_TUNE_COUNT 4
 
 // Device view of one context: everything the kernels need, passed by value.
 struct Sl2Dev {
@@ -66,8 +60,6 @@ struct Sl2Dev {
   // EKF update pipeline (update.cu): factor -> solve -> syrk -> finish
   int *upd_m;          // [B]  measurement rows m of the running update (0: nothing to do)
   double *Wp;          // [B][SL2_MAX_PANELS][16*16]  W_pp = U_pp^-T of every 16-row Cholesky panel
-  // scheduling knobs (sl2_set_tuning; they never change a result, only when / where the work runs)
-  int tune[SL2_TUNE_COUNT];
   int nsm;             // SMs of the device
 };
 
@@ -105,14 +97,11 @@ __device__ __forceinline__ void pdl_prologue() {
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 }
-// SL2_TUNE_PDL: 0 never, 1 always, 2 (default) when the launch covers fewer camera streams than
-// SL2_PDL_AUTO_STREAMS: a single camera stream is a chain of 8 short kernels bound by launch-to-launch latency, which
-// PDL shortens; a full batch fills the GPU and PDL only adds resident waiting CTAs.
+// PDL when the launch covers fewer camera streams than SL2_PDL_AUTO_STREAMS: a single camera stream is a chain of 8
+// short kernels bound by launch-to-launch latency, which PDL shortens; a full batch fills the GPU and PDL only adds
+// resident waiting CTAs.
 #define SL2_PDL_AUTO_STREAMS 2
-inline bool sl2_use_pdl(const Sl2Dev &d, int stream_cnt) {
-  const int mode = d.tune[SL2_TUNE_PDL];
-  return mode == 1 || (mode == 2 && stream_cnt < SL2_PDL_AUTO_STREAMS);
-}
+inline bool sl2_use_pdl(int stream_cnt) { return stream_cnt < SL2_PDL_AUTO_STREAMS; }
 
 #ifdef __CUDACC__
 // one launch path for every kernel of the step: plain launch, or with the PDL attribute
@@ -156,11 +145,11 @@ cudaError_t sl2_launch_score_map(const Sl2Dev &d, const CUtensorMap &tmap, int s
                                  cudaStream_t st);
 cudaError_t sl2_launch_predict(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *u3_dev,
                                int do_predict, int do_measure, cudaStream_t st);
-// EKF update = 4 kernels (factor, solve, syrk, finish); ev5 (optional) = 5 events recorded around them
+// EKF update = 5 kernels (hp, chol, solve, syrk, finish); ev6 (optional) = 6 events recorded around them
 cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, int staged_m,
                               const int *st_feat, const double *st_Hxv, const double *st_Hy,
                               const double *st_R, const double *st_nu, int only_normalise,
-                              cudaStream_t st, cudaEvent_t *ev5 = nullptr, int *launches = nullptr);
+                              cudaStream_t st, cudaEvent_t *ev6 = nullptr, int *launches = nullptr);
 cudaError_t sl2_launch_cull(const Sl2Dev &d, int stream_lo, int stream_cnt, int force_index,
                             cudaStream_t st);
 cudaError_t sl2_launch_append(const Sl2Dev &d, int s, const double *y3_dev, const double *xp7_dev,

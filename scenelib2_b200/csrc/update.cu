@@ -40,6 +40,7 @@
 #include <type_traits>
 
 #include "sl2_common.cuh"
+#include "sl2_ptx.cuh"
 
 namespace {
 
@@ -82,55 +83,13 @@ __device__ __forceinline__ void dmma1688(double (&c)[4], const double (&a)[4], c
       : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
       : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(b[0]), "d"(b[1]));
 }
-// D(16x8) = A(16x16) * B(16x8) + C, the same layout with i < 8 in a and i < 4 in b.  The two 8-row halves of C
-// are separate references: they need not be neighbours in memory or in an array.
-__device__ __forceinline__ void dmma16816(double &c0, double &c1, double &c2, double &c3, const double (&a)[8],
-                                          const double (&b)[4]) {
-  asm("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, "
-      "{%12,%13,%14,%15}, {%0,%1,%2,%3};"
-      : "+d"(c0), "+d"(c1), "+d"(c2), "+d"(c3)
-      : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]), "d"(b[0]),
-        "d"(b[1]), "d"(b[2]), "d"(b[3]));
-}
-__device__ __forceinline__ void cp_async16(void *smem_dst, const void *gsrc, int src_bytes) {
-  const uint32_t d = (uint32_t)__cvta_generic_to_shared(smem_dst);
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(d), "l"(gsrc), "r"(src_bytes)
-               : "memory");
-}
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
-// ---- mbarrier + bulk copy (cp.async.bulk: the TMA engine moves a contiguous run of bytes global -> shared and
-//      reports completion as transaction bytes on an mbarrier; one instruction per row, no per-chunk index math,
-//      and the consumers wait on the mbarrier instead of a CTA-wide barrier) ------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t phase) {
-  uint32_t ok;
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-      "selp.u32 %0, 1, 0, p;\n"
-      "}\n"
-      : "=r"(ok)
-      : "r"(bar), "r"(phase)
-      : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t phase) {
-  while (!mbar_try_wait(bar, phase)) {
-  }
-}
+// bulk copy (cp.async.bulk): the TMA engine moves a contiguous run of bytes global -> shared and reports completion
+// as transaction bytes on an mbarrier; one instruction per row, no per-chunk index math.
 // bytes: multiple of 16; dst / src 16-byte aligned
 __device__ __forceinline__ void bulk_g2s(void *smem_dst, const void *gsrc, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
@@ -195,7 +154,7 @@ __device__ __forceinline__ void chol8_inv(double *dg, double *Wm, int o, int lan
 }
 
 // =============================================================================================
-// kernel 0: upd_hp — measurement list, G = [ S | H P | nu ]: streams P once, one thread per state column
+// kernel 0: upd_hp / upd_hp2 — measurement list, G = [ S | H P | nu ]: streams P once, one thread per state column
 // =============================================================================================
 // H has 7 (fused step: dh/dxv = [dh/dxp | 0]) or 13 (staged API) dense columns and 3 structural dh/dy columns per
 // row, so   (H P)(i, j) = sum_k Hx(i, k) P(k, j) + sum_c Hy(i, c) P(pos_i + c, j):
@@ -209,30 +168,46 @@ __device__ __forceinline__ void chol8_inv(double *dg, double *Wm, int o, int lan
 // The CTA's 16 rows of H P also stay in shared memory for S = (H P) H^T + R: thread = measurement column i',
 // H(i', :) in registers, dense part from broadcast reads, structural part gathered from the rows.
 constexpr int HP_THREADS = 320;
-constexpr int HP_ROWS = 16;   // measurement rows per block (8 features)
+constexpr int HP_ROWS = 16;   // measurement rows per block of upd_hp (8 features); upd_hp2: two buffers of 8 rows
 constexpr int HP_HRS = 18;    // row stride of the H table: [13 dense | 3 dh/dy | 2 pad] doubles (16 B aligned rows)
 struct HpSmem {
   double *Hrow;  // [mmax][HP_HRS]
   double *Rv;    // [K][3]  (R00, R01, R11)
   double *nu;    // [mmax]
-  double *hprow; // [HP_ROWS][ld]  H P rows of the running block
+  double *hprow; // [HP_ROWS][ld]  H P rows of the running block (upd_hp2: of the two blocks in flight)
   int *mfeat;    // [K]
   int *wcount;   // [16]
+  double *park;  // [KD][HP_THREADS]  upd_hp2 only: the KD leading rows of P, one column per thread
 };
-__host__ __device__ inline size_t hp_smem_doubles(int kmax, int ld) {
+// The one layout of that shared memory, for the launcher (bytes) and the kernels (hp_carve): byte offsets of the
+// tables in the order above.  K = upd_keven(kmax) is even, so hprow is 16-byte aligned and park 8-byte aligned.
+// kd_park = KD for upd_hp2, 0 for upd_hp.
+struct HpLayout {
+  size_t Hrow, Rv, nu, hprow, mfeat, wcount, park, bytes;
+};
+__host__ __device__ inline HpLayout hp_layout(int kmax, int ld, int kd_park) {
   const size_t K = upd_keven(kmax);
-  return (size_t)2 * K * HP_HRS + K * 3 + (K & 1) + 2 * K + (size_t)HP_ROWS * ld;
+  HpLayout l;
+  l.Hrow = 0;
+  l.Rv = l.Hrow + 2 * K * HP_HRS * sizeof(double);
+  l.nu = l.Rv + 3 * K * sizeof(double);
+  l.hprow = l.nu + 2 * K * sizeof(double);
+  l.mfeat = l.hprow + (size_t)HP_ROWS * ld * sizeof(double);
+  l.wcount = l.mfeat + K * sizeof(int);
+  l.park = l.wcount + 16 * sizeof(int);
+  l.bytes = l.park + (size_t)kd_park * HP_THREADS * sizeof(double);
+  return l;
 }
 __device__ __forceinline__ HpSmem hp_carve(uint8_t *base, int kmax, int ld) {
+  const HpLayout l = hp_layout(kmax, ld, 0);
   HpSmem u;
-  const int K = upd_keven(kmax);
-  double *p = reinterpret_cast<double *>(base);
-  u.Hrow = p;  p += (size_t)2 * K * HP_HRS;
-  u.Rv = p;  p += (size_t)K * 3 + (K & 1);
-  u.nu = p;  p += 2 * K;
-  u.hprow = p;  p += (size_t)HP_ROWS * ld;
-  u.mfeat = reinterpret_cast<int *>(p);
-  u.wcount = u.mfeat + K;
+  u.Hrow = reinterpret_cast<double *>(base + l.Hrow);
+  u.Rv = reinterpret_cast<double *>(base + l.Rv);
+  u.nu = reinterpret_cast<double *>(base + l.nu);
+  u.hprow = reinterpret_cast<double *>(base + l.hprow);
+  u.mfeat = reinterpret_cast<int *>(base + l.mfeat);
+  u.wcount = reinterpret_cast<int *>(base + l.wcount);
+  u.park = reinterpret_cast<double *>(base + l.park);
   return u;
 }
 
@@ -318,6 +293,133 @@ __device__ __forceinline__ int hp_tables(const Sl2Dev &d, const HpSmem &sm, int 
   return K;
 }
 
+// ---- the per-block steps of upd_hp and upd_hp2: the two kernels differ only in the loop around them -------------
+// The KD leading rows of P for state column j (zero past the last column n).
+template <int KD>
+__device__ __forceinline__ void hp_load_dense(double (&Pd)[KD], const double *__restrict__ P, int ld, int j, int n) {
+#pragma unroll
+  for (int k = 0; k < KD; ++k) Pd[k] = j < n ? P[(size_t)k * ld + j] : 0.0;
+}
+
+// The 3 structural rows of P of the F features from k0 on, column j: every load of the block in flight at once.
+template <int F>
+__device__ __forceinline__ void hp_load_struct(double (&pv)[F][3], const HpSmem &sm, const double *__restrict__ P,
+                                               int ld, int j, int n, int k0, int K) {
+#pragma unroll
+  for (int f = 0; f < F; ++f) {
+    const int kk = k0 + f;
+    const int pos = SL2_NXV + 3 * sm.mfeat[kk < K ? kk : 0];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) pv[f][c] = (kk < K && j < n) ? P[(size_t)(pos + c) * ld + j] : 0.0;
+  }
+}
+
+// (H P)(i, j) of one measurement row (hrow = its H row in shared memory): the KD dense terms in pairs of H entries,
+// then the 3 structural terms.
+template <int KD>
+__device__ __forceinline__ double hp_row_value(const double *hrow, const double (&Pd)[KD], const double (&pv)[3]) {
+  const double2 *hr = reinterpret_cast<const double2 *>(hrow);
+  double acc = 0.0;
+#pragma unroll
+  for (int k2 = 0; k2 < (KD + 1) / 2; ++k2) {
+    const double2 hv = hr[k2];
+    acc += hv.x * Pd[2 * k2];
+    if (2 * k2 + 1 < KD) acc += hv.y * Pd[2 * k2 + 1];
+  }
+  const double2 hy0 = hr[6], hy1 = hr[7];  // columns 12..15: (dense 12 | dh/dy 0..2)
+  acc += hy0.y * pv[0];
+  acc += hy1.x * pv[1];
+  acc += hy1.y * pv[2];
+  return acc;
+}
+
+// H P of the 2 F rows of the block from row0 on, column j: to G and to the block's rows in shared memory (buf,
+// row stride ld).
+template <int F, int KD>
+__device__ __forceinline__ void hp_block_rows(const HpSmem &sm, const double (&Pd)[KD], const double (&pv)[F][3],
+                                              double *__restrict__ G, int ldg, double *__restrict__ buf, int ld,
+                                              int row0, int K, int j, int n) {
+  const int m = 2 * K, k0 = row0 >> 1;
+#pragma unroll
+  for (int f = 0; f < F; ++f) {
+    if (k0 + f < K) {  // CTA-uniform
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const int i = row0 + 2 * f + r;
+        const double acc = hp_row_value(sm.Hrow + (size_t)i * HP_HRS, Pd, pv[f]);
+        if (j < n) {
+          G[(size_t)i * ldg + m + j] = acc;
+          buf[(size_t)(2 * f + r) * ld + j] = acc;
+        }
+      }
+    }
+  }
+}
+
+// The nu column of the block's rows: G(i, m + n) = nu_i.
+__device__ __forceinline__ void hp_store_nu(const HpSmem &sm, double *__restrict__ G, int ldg, int m, int n, int row0,
+                                            int rows) {
+  const int tid = threadIdx.x;
+  if (tid < rows) G[(size_t)(row0 + tid) * ldg + m + n] = sm.nu[row0 + tid];
+}
+
+// S = (H P) H^T + R for the rows row0 .. row0 + rows - 1 (rows <= R) of a block, columns from the row's own feature
+// on: thread = measurement column i', H(i', :) in registers, the block's H P rows from shared memory (buf, row stride
+// ld; dense columns read as 16-byte pairs), four rows at a time (independent accumulation chains: a single chain is
+// 10-16 dependent FMAs per entry).
+template <int R, int KD>
+__device__ __forceinline__ void hp_s_rows(const HpSmem &sm, const double *__restrict__ buf, int ld,
+                                          double *__restrict__ G, int ldg, int m, int row0, int rows) {
+  for (int ip = threadIdx.x; ip < m; ip += HP_THREADS) {
+    if (ip < row0) continue;
+    const int kp = ip >> 1, rp = ip & 1;
+    const double2 *hr = reinterpret_cast<const double2 *>(sm.Hrow + (size_t)ip * HP_HRS);
+    double hd[KD + 1];
+#pragma unroll
+    for (int k2 = 0; k2 < (KD + 1) / 2; ++k2) {
+      const double2 hv = hr[k2];
+      hd[2 * k2] = hv.x;
+      hd[2 * k2 + 1] = hv.y;
+    }
+    const double2 hy0 = hr[6], hy1 = hr[7];
+    const double hys[3] = {hy0.y, hy1.x, hy1.y};
+    const int pos = SL2_NXV + 3 * sm.mfeat[kp];
+    const double r_same = sm.Rv[kp * 3 + 2 * rp], r_cross = sm.Rv[kp * 3 + 1];
+#pragma unroll
+    for (int il0 = 0; il0 < R; il0 += 4) {
+      if (il0 < rows) {
+        double acc[4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) acc[q] = 0.0;
+#pragma unroll
+        for (int c2 = 0; c2 < KD / 2; ++c2)
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const double2 v = *reinterpret_cast<const double2 *>(buf + (size_t)(il0 + q) * ld + 2 * c2);
+            acc[q] += v.x * hd[2 * c2];
+            acc[q] += v.y * hd[2 * c2 + 1];
+          }
+        if (KD & 1) {
+#pragma unroll
+          for (int q = 0; q < 4; ++q) acc[q] += buf[(size_t)(il0 + q) * ld + KD - 1] * hd[KD - 1];
+        }
+#pragma unroll
+        for (int c = 0; c < 3; ++c)
+#pragma unroll
+          for (int q = 0; q < 4; ++q) acc[q] += buf[(size_t)(il0 + q) * ld + pos + c] * hys[c];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int i = row0 + il0 + q;
+          if (il0 + q < rows && ip >= (i & ~1)) {
+            if ((i >> 1) == kp) acc[q] += (i == ip) ? r_same : r_cross;
+            G[(size_t)i * ldg + ip] = acc[q];
+          }
+        }
+      }
+    }
+  }
+}
+
 // KD = dense columns of H that can be nonzero (7: fused step, 13: staged)
 template <int KD>
 __global__ void __launch_bounds__(HP_THREADS, 2) upd_hp_kernel(
@@ -329,8 +431,7 @@ __global__ void __launch_bounds__(HP_THREADS, 2) upd_hp_kernel(
   const HpSmem sm = hp_carve(smem_raw, d.kmax, ld);
   const int s = stream_lo + blockIdx.y;
   const int tid = threadIdx.x;
-  const int nf = d.nfeat[s];
-  const int n = SL2_NXV + 3 * nf;
+  const int n = SL2_NXV + 3 * d.nfeat[s];
   const double *__restrict__ P = d.P + (size_t)s * ld * ld;
   double *__restrict__ G = d.G + (size_t)s * d.mmax * ldg;
   const int K = hp_tables(d, sm, s, HP_ROWS, staged_m, st_feat, st_Hxv, st_Hy, st_R, st_nu);
@@ -340,108 +441,36 @@ __global__ void __launch_bounds__(HP_THREADS, 2) upd_hp_kernel(
   constexpr int FB = HP_ROWS / 2;            // features per block
   const int nch = (n + HP_THREADS - 1) / HP_THREADS;  // column chunks (1 up to 102 features)
   double Pd[KD];
-  auto load_dense = [&](int j) {
-#pragma unroll
-    for (int k = 0; k < KD; ++k) Pd[k] = j < n ? P[(size_t)k * ld + j] : 0.0;
-  };
-  if (nch == 1) load_dense(tid);
+  if (nch == 1) hp_load_dense(Pd, P, ld, tid, n);
   // row blocks blockIdx.x, blockIdx.x + gridDim.x, ...: the measurement list and the H tables are built once
   for (int rb = blockIdx.x; HP_ROWS * rb < m; rb += gridDim.x) {
-    const int row0 = HP_ROWS * rb, rows = min(HP_ROWS, m - row0), k0 = row0 >> 1;
-    // ---- H*P for the block's rows ---------------------------------------------------------------------
+    const int row0 = HP_ROWS * rb, rows = min(HP_ROWS, m - row0);
     for (int ch = 0; ch < nch; ++ch) {
       const int j = ch * HP_THREADS + tid;
-      if (nch > 1) load_dense(j);
+      if (nch > 1) hp_load_dense(Pd, P, ld, j, n);
       double pv[FB][3];
-#pragma unroll
-      for (int f = 0; f < FB; ++f) {  // every structural row load of the block first
-        const int kk = k0 + f;
-        const int pos = SL2_NXV + 3 * sm.mfeat[kk < K ? kk : 0];
-#pragma unroll
-        for (int c = 0; c < 3; ++c) pv[f][c] = (kk < K && j < n) ? P[(size_t)(pos + c) * ld + j] : 0.0;
-      }
-#pragma unroll
-      for (int f = 0; f < FB; ++f) {
-        if (k0 + f < K) {  // CTA-uniform
-#pragma unroll
-          for (int r = 0; r < 2; ++r) {
-            const int i = row0 + 2 * f + r;
-            const double2 *hr = reinterpret_cast<const double2 *>(sm.Hrow + (size_t)i * HP_HRS);
-            double acc = 0.0;
-#pragma unroll
-            for (int k2 = 0; k2 < (KD + 1) / 2; ++k2) {
-              const double2 hv = hr[k2];
-              acc += hv.x * Pd[2 * k2];
-              if (2 * k2 + 1 < KD) acc += hv.y * Pd[2 * k2 + 1];
-            }
-            const double2 hy0 = hr[6], hy1 = hr[7];  // columns 12..15: (dense 12 | dh/dy 0..2)
-            acc += hy0.y * pv[f][0];
-            acc += hy1.x * pv[f][1];
-            acc += hy1.y * pv[f][2];
-            if (j < n) {
-              G[(size_t)i * ldg + m + j] = acc;
-              sm.hprow[(size_t)(2 * f + r) * ld + j] = acc;
-            }
-          }
-        }
-      }
+      hp_load_struct(pv, sm, P, ld, j, n, row0 >> 1, K);
+      hp_block_rows(sm, Pd, pv, G, ldg, sm.hprow, ld, row0, K, j, n);
     }
-    if (tid < rows) G[(size_t)(row0 + tid) * ldg + m + n] = sm.nu[row0 + tid];
+    hp_store_nu(sm, G, ldg, m, n, row0, rows);
     __syncthreads();
-    // ---- S = (H P) H^T + R for the block's rows, columns from the row's own feature on ------------------
-    for (int ip = tid; ip < m; ip += HP_THREADS) {
-      if (ip < row0) continue;
-      const int kp = ip >> 1, rp = ip & 1;
-      const double2 *hr = reinterpret_cast<const double2 *>(sm.Hrow + (size_t)ip * HP_HRS);
-      double hreg[16];
-#pragma unroll
-      for (int k2 = 0; k2 < 8; ++k2) {
-        const double2 hv = hr[k2];
-        hreg[2 * k2] = hv.x;
-        hreg[2 * k2 + 1] = hv.y;
-      }
-      const int pos = SL2_NXV + 3 * sm.mfeat[kp];
-      const double r_same = sm.Rv[kp * 3 + 2 * rp], r_cross = sm.Rv[kp * 3 + 1];
-      // four rows at a time: independent accumulation chains (a single chain is 10-16 dependent FMAs per entry)
-      for (int il0 = 0; il0 < rows; il0 += 4) {
-        double acc[4];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) acc[q] = 0.0;
-#pragma unroll
-        for (int c = 0; c < KD; ++c)
-#pragma unroll
-          for (int q = 0; q < 4; ++q) acc[q] += sm.hprow[(size_t)(il0 + q) * ld + c] * hreg[c];
-#pragma unroll
-        for (int c = 0; c < 3; ++c)
-#pragma unroll
-          for (int q = 0; q < 4; ++q) acc[q] += sm.hprow[(size_t)(il0 + q) * ld + pos + c] * hreg[13 + c];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const int i = row0 + il0 + q;
-          if (il0 + q < rows && ip >= (i & ~1)) {
-            if ((i >> 1) == kp) acc[q] += (i == ip) ? r_same : r_cross;
-            G[(size_t)i * ldg + ip] = acc[q];
-          }
-        }
-      }
-    }
+    hp_s_rows<HP_ROWS, KD>(sm, sm.hprow, ld, G, ldg, m, row0, rows);
     __syncthreads();  // hprow of this block is rewritten by the next one
   }
 }
 
-// upd_hp, software-pipelined (SL2_TUNE_HP_PIPELINED; maps of up to (HP_THREADS - 13) / 3 features): the same
-// stream over P in 8-row blocks (4 features) with the shared-memory rows of H P double-buffered, so that
+// upd_hp, software-pipelined (maps of up to (HP_THREADS - 13) / 3 features): the same stream over P in 8-row blocks
+// (4 features) with the shared-memory rows of H P double-buffered, so that
 //   loads of block b+1 issued  ->  S = (H P) H^T + R of block b from shared memory  ->  FMAs / stores of block b+1
 // and the structural row loads (the HBM stream) are in flight WHILE the S phase runs instead of after it; one
-// __syncthreads per block.  Same arithmetic in the same order as upd_hp_kernel (identical results); the dense
-// columns of the S phase are read as 16-byte pairs.
+// __syncthreads per block.  The per-block steps are upd_hp's, so the results are identical.
 template <int KD>
 __global__ void __launch_bounds__(HP_THREADS, 2) upd_hp2_kernel(
     const Sl2Dev d, int stream_lo, int staged_m, const int *st_feat, const double *st_Hxv,
     const double *st_Hy, const double *st_R, const double *st_nu) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   pdl_prologue();
-  constexpr int R2 = 8, F2 = 4;  // rows / features per block
+  constexpr int R2 = HP_ROWS / 2, F2 = R2 / 2;  // rows / features per block
   const int ld = d.ld, ldg = d.ldg;
   const HpSmem sm = hp_carve(smem_raw, d.kmax, ld);
   const int s = stream_lo + blockIdx.y;
@@ -453,116 +482,36 @@ __global__ void __launch_bounds__(HP_THREADS, 2) upd_hp2_kernel(
   if (K < 0) return;
   const int m = 2 * K;
   const int j = tid;  // this thread's state column (n <= HP_THREADS: the launcher's condition)
-  const bool jv = j < n;
   // the KD leading rows of P for this thread's column: parked in shared memory (own slot per thread, no barrier
   // needed) so that they do not occupy registers during the S phase, when the 12 structural loads are in flight
-  double *const pdcol = reinterpret_cast<double *>(sm.wcount + 16) + tid;
+  double *const park = sm.park + tid;
+  {
+    double Pd[KD];
+    hp_load_dense(Pd, P, ld, j, n);
 #pragma unroll
-  for (int k = 0; k < KD; ++k) pdcol[k * HP_THREADS] = jv ? P[(size_t)k * ld + j] : 0.0;
+    for (int k = 0; k < KD; ++k) park[k * HP_THREADS] = Pd[k];
+  }
   double pv[F2][3];
-  auto issue = [&](int rb) {  // the structural rows of block rb: 12 loads in flight per thread
-    const int k0 = F2 * rb;
-#pragma unroll
-    for (int f = 0; f < F2; ++f) {
-      const int kk = k0 + f;
-      const int pos = SL2_NXV + 3 * sm.mfeat[kk < K ? kk : 0];
-#pragma unroll
-      for (int c = 0; c < 3; ++c) pv[f][c] = (kk < K && jv) ? P[(size_t)(pos + c) * ld + j] : 0.0;
-    }
-  };
   auto consume = [&](int rb, double *__restrict__ buf) {  // H P of block rb -> G and the shared rows
-    const int row0 = R2 * rb, k0 = F2 * rb;
+    const int row0 = R2 * rb;
     double Pd[KD];
 #pragma unroll
-    for (int k = 0; k < KD; ++k) Pd[k] = pdcol[k * HP_THREADS];
-#pragma unroll
-    for (int f = 0; f < F2; ++f) {
-      if (k0 + f < K) {  // CTA-uniform
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          const int i = row0 + 2 * f + r;
-          const double2 *hr = reinterpret_cast<const double2 *>(sm.Hrow + (size_t)i * HP_HRS);
-          double acc = 0.0;
-#pragma unroll
-          for (int k2 = 0; k2 < (KD + 1) / 2; ++k2) {
-            const double2 hv = hr[k2];
-            acc += hv.x * Pd[2 * k2];
-            if (2 * k2 + 1 < KD) acc += hv.y * Pd[2 * k2 + 1];
-          }
-          const double2 hy0 = hr[6], hy1 = hr[7];  // columns 12..15: (dense 12 | dh/dy 0..2)
-          acc += hy0.y * pv[f][0];
-          acc += hy1.x * pv[f][1];
-          acc += hy1.y * pv[f][2];
-          if (jv) {
-            G[(size_t)i * ldg + m + j] = acc;
-            buf[(size_t)(2 * f + r) * ld + j] = acc;
-          }
-        }
-      }
-    }
-    const int rows = min(R2, m - row0);
-    if (tid < rows) G[(size_t)(row0 + tid) * ldg + m + n] = sm.nu[row0 + tid];
+    for (int k = 0; k < KD; ++k) Pd[k] = park[k * HP_THREADS];
+    hp_block_rows(sm, Pd, pv, G, ldg, buf, ld, row0, K, j, n);
+    hp_store_nu(sm, G, ldg, m, n, row0, min(R2, m - row0));
   };
-  auto sphase = [&](int rb, const double *__restrict__ buf) {  // S rows of block rb, columns from the row's feature on
-    const int row0 = R2 * rb, rows = min(R2, m - row0);
-    for (int ip = tid; ip < m; ip += HP_THREADS) {
-      if (ip < row0) continue;
-      const int kp = ip >> 1, rp = ip & 1;
-      const double2 *hr = reinterpret_cast<const double2 *>(sm.Hrow + (size_t)ip * HP_HRS);
-      double hd[KD + 1];
-#pragma unroll
-      for (int k2 = 0; k2 < (KD + 1) / 2; ++k2) {
-        const double2 hv = hr[k2];
-        hd[2 * k2] = hv.x;
-        hd[2 * k2 + 1] = hv.y;
-      }
-      const double2 hy0 = hr[6], hy1 = hr[7];
-      const double hys[3] = {hy0.y, hy1.x, hy1.y};
-      const int pos = SL2_NXV + 3 * sm.mfeat[kp];
-      const double r_same = sm.Rv[kp * 3 + 2 * rp], r_cross = sm.Rv[kp * 3 + 1];
-#pragma unroll
-      for (int il0 = 0; il0 < R2; il0 += 4) {
-        if (il0 < rows) {
-          double acc[4];
-#pragma unroll
-          for (int q = 0; q < 4; ++q) acc[q] = 0.0;
-#pragma unroll
-          for (int c2 = 0; c2 < KD / 2; ++c2)
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const double2 v = *reinterpret_cast<const double2 *>(buf + (size_t)(il0 + q) * ld + 2 * c2);
-              acc[q] += v.x * hd[2 * c2];
-              acc[q] += v.y * hd[2 * c2 + 1];
-            }
-          if (KD & 1) {
-#pragma unroll
-            for (int q = 0; q < 4; ++q) acc[q] += buf[(size_t)(il0 + q) * ld + KD - 1] * hd[KD - 1];
-          }
-#pragma unroll
-          for (int c = 0; c < 3; ++c)
-#pragma unroll
-            for (int q = 0; q < 4; ++q) acc[q] += buf[(size_t)(il0 + q) * ld + pos + c] * hys[c];
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const int i = row0 + il0 + q;
-            if (il0 + q < rows && ip >= (i & ~1)) {
-              if ((i >> 1) == kp) acc[q] += (i == ip) ? r_same : r_cross;
-              G[(size_t)i * ldg + ip] = acc[q];
-            }
-          }
-        }
-      }
-    }
+  auto sphase = [&](int rb, const double *__restrict__ buf) {
+    hp_s_rows<R2, KD>(sm, buf, ld, G, ldg, m, R2 * rb, min(R2, m - R2 * rb));
   };
   int rb = blockIdx.x, par = 0;
   double *const buf0 = sm.hprow, *const buf1 = sm.hprow + (size_t)R2 * ld;
-  issue(rb);
+  hp_load_struct(pv, sm, P, ld, j, n, F2 * rb, K);
   consume(rb, buf0);
   __syncthreads();
   for (;;) {
     const int nb = rb + gridDim.x;
     const bool more = R2 * nb < m;  // CTA-uniform
-    if (more) issue(nb);
+    if (more) hp_load_struct(pv, sm, P, ld, j, n, F2 * nb, K);
     sphase(rb, par ? buf1 : buf0);
     if (!more) break;
     consume(nb, par ? buf0 : buf1);
@@ -592,6 +541,7 @@ __global__ void __launch_bounds__(HP_THREADS, 2) upd_hp2_kernel(
 //                       software pipelined 4 / 8 / 16 k-steps deep: the fewer groups are left, the narrower and deeper)
 //   finish (all warps)  U_panel = W * C_panel -> G; the 16 columns that are panel p+1's multipliers -> mult_next
 constexpr int CH_D = 4;    // k-steps in flight of the look-ahead item (2 loads per step)
+static_assert(4 % CH_D == 0, "nk is a multiple of 4: the look-ahead's pipelined loop runs every k-step");
 constexpr int CH_DPS = 18; // row stride of the pre-updated diagonal block
 
 // One batch item of the panel update: GB 8-column groups from group g0 on, C(16 x 8 GB) = S entries - A * B over the
@@ -867,10 +817,6 @@ __global__ void __launch_bounds__(UPD_THREADS, 2) upd_chol_kernel(const Sl2Dev d
             if (kb + u + CH_D - 1 < nk) loadv(v[(u + CH_D - 1) % CH_D]);  // warp-uniform
             step(v[u]);
           }
-        }
-        if (CH_D == 8 && kb < nk) {  // nk is a multiple of 4: four steps left
-#pragma unroll
-          for (int u = 0; u < 4; ++u) step(v[u]);
         }
 #pragma unroll
         for (int q = 0; q < 2; ++q)
@@ -1481,19 +1427,21 @@ __global__ void __launch_bounds__(UPD_THREADS) upd_finish_kernel(const Sl2Dev d,
 }
 
 // ---- host-side shapes ---------------------------------------------------------------------------
-inline int solve_panels(int kmax) { return (2 * upd_keven(kmax) + 15) / 16; }
-inline int solve_np(int kmax) {  // instantiation that covers the measurement capacity
-  const int p = solve_panels(kmax);
-  return p <= 4 ? 4 : (p <= 7 ? 7 : (p <= 10 ? 10 : (p <= 13 ? 13 : 16)));
+// The upd_solve instantiation that covers the measurement capacity (NP 16-row panels) and its shared memory.
+struct SolveKernel {
+  void (*kern)(Sl2Dev, int);
+  int np;
+  size_t smem;
+};
+template <int NP>
+SolveKernel solve_kernel_np() {
+  return {upd_solve_kernel<NP>, NP, SolveLayout<NP>::SMEM_DOUBLES * sizeof(double)};
 }
-inline size_t solve_smem(int np) {
-  switch (np) {
-    case 4: return SolveLayout<4>::SMEM_DOUBLES * sizeof(double);
-    case 7: return SolveLayout<7>::SMEM_DOUBLES * sizeof(double);
-    case 10: return SolveLayout<10>::SMEM_DOUBLES * sizeof(double);
-    case 13: return SolveLayout<13>::SMEM_DOUBLES * sizeof(double);
-    default: return SolveLayout<16>::SMEM_DOUBLES * sizeof(double);
-  }
+inline SolveKernel solve_kernel(int kmax) {
+  const int p = (2 * upd_keven(kmax) + 15) / 16;  // panels of S at capacity
+  return p <= 4 ? solve_kernel_np<4>()
+                : (p <= 7 ? solve_kernel_np<7>()
+                          : (p <= 10 ? solve_kernel_np<10>() : (p <= 13 ? solve_kernel_np<13>() : solve_kernel_np<16>())));
 }
 inline void solve_shape(int Nmax, int &nslab, int &warps) {
   const int ngroups = (SL2_NXV + 3 * Nmax + 1 + 7) / 8;
@@ -1508,37 +1456,25 @@ size_t sl2_update_smem_bytes(const Sl2Dev &d) {  // upd_chol
   return chol_smem_doubles(d.kmax) * sizeof(double);
 }
 
-static size_t hp_smem_bytes(const Sl2Dev &d) {
-  return hp_smem_doubles(d.kmax, d.ld) * sizeof(double) + (upd_keven(d.kmax) + 16) * sizeof(int);
-}
-static size_t hp2_smem_bytes(const Sl2Dev &d, int kd) {  // + the parked leading rows of P: [kd][HP_THREADS]
-  return hp_smem_bytes(d) + (size_t)kd * HP_THREADS * sizeof(double);
-}
-
 cudaError_t sl2_configure_update(const Sl2Dev &d) {
-  cudaError_t e = cudaFuncSetAttribute(upd_hp_kernel<7>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)hp_smem_bytes(d));
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(upd_hp_kernel<13>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hp_smem_bytes(d));
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(upd_hp2_kernel<7>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hp2_smem_bytes(d, 7));
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(upd_hp2_kernel<13>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hp2_smem_bytes(d, 13));
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(upd_chol_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                           (int)sl2_update_smem_bytes(d));
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(upd_syrk_kernel<32, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SYRK_SMEM);
-  if (e != cudaSuccess) return e;
-  const int np = solve_np(d.kmax);
-  const int smem = (int)solve_smem(np);
-  switch (np) {
-    case 4: return cudaFuncSetAttribute(upd_solve_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    case 7: return cudaFuncSetAttribute(upd_solve_kernel<7>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    case 10: return cudaFuncSetAttribute(upd_solve_kernel<10>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    case 13: return cudaFuncSetAttribute(upd_solve_kernel<13>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    default: return cudaFuncSetAttribute(upd_solve_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  const SolveKernel solve = solve_kernel(d.kmax);
+  const struct {
+    const void *kern;
+    size_t smem;
+  } opt_in[] = {
+      {(const void *)upd_hp_kernel<7>, hp_layout(d.kmax, d.ld, 0).bytes},
+      {(const void *)upd_hp_kernel<13>, hp_layout(d.kmax, d.ld, 0).bytes},
+      {(const void *)upd_hp2_kernel<7>, hp_layout(d.kmax, d.ld, 7).bytes},
+      {(const void *)upd_hp2_kernel<13>, hp_layout(d.kmax, d.ld, 13).bytes},
+      {(const void *)upd_chol_kernel, sl2_update_smem_bytes(d)},
+      {(const void *)solve.kern, solve.smem},
+      {(const void *)upd_syrk_kernel<32, 2>, SYRK_SMEM},
+  };
+  for (const auto &k : opt_in) {
+    const cudaError_t e = cudaFuncSetAttribute(k.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k.smem);
+    if (e != cudaSuccess) return e;
   }
+  return cudaSuccess;
 }
 
 // ev6 (optional): 6 events recorded around the 5 kernels (hp, chol, solve, syrk, finish)
@@ -1555,15 +1491,16 @@ cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, in
   // (then one CTA per stream is fastest: every CTA rebuilds the measurement list and H tables)
   const int hp_all = (2 * upd_keven(d.kmax) + HP_ROWS - 1) / HP_ROWS;
   const int hp_blocks = stream_cnt >= 2 * d.nsm ? 1 : hp_all;
-  const bool pdl = sl2_use_pdl(d, stream_cnt);
+  const bool pdl = sl2_use_pdl(stream_cnt);
   if (!only_normalise) {
     const dim3 grid(hp_blocks, stream_cnt);
     // the software-pipelined form: one CTA per stream, one state column per thread
-    const bool piped = d.tune[SL2_TUNE_HP_PIPELINED] != 0 && hp_blocks == 1 && SL2_NXV + 3 * d.Nmax <= HP_THREADS;
+    const bool piped = hp_blocks == 1 && SL2_NXV + 3 * d.Nmax <= HP_THREADS;
+    const int kd = staged_m >= 0 ? 13 : 7;
     auto *k13 = piped ? upd_hp2_kernel<13> : upd_hp_kernel<13>;
     auto *k7 = piped ? upd_hp2_kernel<7> : upd_hp_kernel<7>;
-    const size_t smem = piped ? hp2_smem_bytes(d, staged_m >= 0 ? 13 : 7) : hp_smem_bytes(d);
-    e = sl2_launch_kernel(staged_m >= 0 ? k13 : k7, grid, dim3(HP_THREADS), smem, st, pdl, d, stream_lo, staged_m,
+    const size_t smem = hp_layout(d.kmax, d.ld, piped ? kd : 0).bytes;
+    e = sl2_launch_kernel(kd == 13 ? k13 : k7, grid, dim3(HP_THREADS), smem, st, pdl, d, stream_lo, staged_m,
                           st_feat, st_Hxv, st_Hy, st_R, st_nu);
     if (e != cudaSuccess) return e;
     ++nl;
@@ -1579,20 +1516,13 @@ cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, in
   if (!only_normalise) {
     int nslab, warps;
     solve_shape(d.Nmax, nslab, warps);
-    const int np = solve_np(d.kmax);
-    const size_t smem = solve_smem(np);
+    const SolveKernel solve = solve_kernel(d.kmax);
     // two warps per 8-column group; a batch that fills the GPU runs one CTA per stream (U staged once per
     // stream, groups walked inside), a small one spreads a stream over nslab CTAs (latency)
-    const bool walk = np <= 13 && stream_cnt >= d.nsm;
+    const bool walk = solve.np <= 13 && stream_cnt >= d.nsm;
     if (walk) warps = SOLVE_MAX_WARPS;
-    const dim3 grid(walk ? 1 : nslab, stream_cnt), block(64 * warps);
-    switch (np) {
-      case 4: e = sl2_launch_kernel(upd_solve_kernel<4>, grid, block, smem, st, pdl, d, stream_lo); break;
-      case 7: e = sl2_launch_kernel(upd_solve_kernel<7>, grid, block, smem, st, pdl, d, stream_lo); break;
-      case 10: e = sl2_launch_kernel(upd_solve_kernel<10>, grid, block, smem, st, pdl, d, stream_lo); break;
-      case 13: e = sl2_launch_kernel(upd_solve_kernel<13>, grid, block, smem, st, pdl, d, stream_lo); break;
-      default: e = sl2_launch_kernel(upd_solve_kernel<16>, grid, block, smem, st, pdl, d, stream_lo); break;
-    }
+    e = sl2_launch_kernel(solve.kern, dim3(walk ? 1 : nslab, stream_cnt), dim3(64 * warps), solve.smem, st, pdl, d,
+                          stream_lo);
     if (e != cudaSuccess) return e;
     ++nl;
   }

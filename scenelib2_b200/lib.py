@@ -19,8 +19,6 @@ f32p = C.POINTER(C.c_float)
 
 SL2_MAX_FEATURES = 256   # map capacity per stream (n <= 781)
 SL2_MAX_MEASURED = 128   # features one step can measure (m <= 256)
-# keys of Context.set_tuning (SL2_TUNE_* of include/sl2b200.h)
-TUNE_PDL, TUNE_HP_PIPELINED = 0, 1
 
 
 class Sl2Config(C.Structure):
@@ -46,7 +44,7 @@ EXPORTS = [
     "sl2_patch_search", "sl2_score_map", "sl2_smoe_search", "sl2_find_best_patch", "sl2_ekf_predict",
     "sl2_predict_measurements", "sl2_make_measurements", "sl2_ekf_update",
     "sl2_ekf_update_measured", "sl2_normalise_state", "sl2_step", "sl2_step_host",
-    "sl2_step_host_async", "sl2_wait_slot", "sl2_set_step_groups", "sl2_join", "sl2_set_tuning", "sl2_measure_particles", "sl2_measure_particles_patch",
+    "sl2_step_host_async", "sl2_wait_slot", "sl2_set_step_groups", "sl2_join", "sl2_measure_particles", "sl2_measure_particles_patch",
     "sl2_smoe_search_patch", "sl2_measure_partial_features",
     "sl2_get_features", "sl2_get_feature_jacobians", "sl2_enable_timing", "sl2_last_step_times", "sl2_last_update_times", "sl2_launch_count",
 ]
@@ -83,7 +81,6 @@ def load():
         L.sl2_wait_slot.argtypes = [C.c_void_p, C.c_int32]
         L.sl2_set_step_groups.argtypes = [C.c_void_p, C.c_int32]
         L.sl2_join.argtypes = [C.c_void_p]
-        L.sl2_set_tuning.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
         L.sl2_measure_particles.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, f64p, f64p,
                                             f64p, f64p, C.c_double, f64p, i32p, u8p, u8p, f64p, f64p]
         L.sl2_measure_particles_patch.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, f64p,
@@ -362,10 +359,6 @@ class Context:
 
     def join(self):
         self._ck(self.L.sl2_join(self.h))
-
-    def set_tuning(self, key, value):
-        """scheduling knob of the fused step (TUNE_* below = SL2_TUNE_* of include/sl2b200.h)"""
-        self._ck(self.L.sl2_set_tuning(self.h, int(key), int(value)))
 
     def sync(self):
         self._ck(self.L.sl2_sync(self.h))

@@ -79,7 +79,7 @@ def variant_of(s, U):
 
 def regimes(nsm, U):
     """(name, B, step groups): the batched launch regimes of the update (upd_hp2 is never chosen above 102
-    features, so the pipelined-off regime of test_gpu_update_shapes is the same launch here)."""
+    features: the batch regimes here run upd_hp with one CTA per stream)."""
     return [("small", U, 1), ("walk", nsm, 1), ("batch", 2 * nsm, 1), ("groups", 2 * nsm, 2)]
 
 

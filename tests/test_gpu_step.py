@@ -385,54 +385,6 @@ def test_c4_bench_shape_264_streams_against_oracle(oracle):
     cfg_ctx.close()
 
 
-def test_scheduling_knobs_leave_results_bit_identical():
-    """sl2_set_tuning (programmatic dependent launch between the kernels of the step, the software-pipelined upd_hp
-    against the plain one) only changes how work is launched / pipelined: at the bench shape (C4, 264 streams, where
-    the batched launch shapes are the ones in use) the non-default setting gives the same bits as the default --
-    state, covariance, matches, counters -- for device-resident steps and for the asynchronous host ring."""
-    import torch
-    from scenelib2_b200 import lib
-    B, T, U = 264, 3, 6
-    uniq = [synth.make_scene("C4", stream_id=u, n_frames=2) for u in range(U)]
-    scenes = [uniq[(s * 5) % U] for s in range(B)]
-    host = torch.empty((2, B, 240, 320), dtype=torch.uint8, pin_memory=True)
-    host.numpy()[:] = np.stack([np.stack([sc.frames[t] for sc in scenes]) for t in range(2)])
-    settings = [{}, {lib.TUNE_PDL: 1, lib.TUNE_HP_PIPELINED: 0}]
-    picks = sorted(set(range(0, B, 37)) | {131, 132, B - 1})
-    results = []
-    for st in settings:
-        c = ctx_from_scenes(scenes, frame_slots=2)
-        for k, v in st.items():
-            c.set_tuning(k, v)
-        xo = torch.zeros((2, B, 13), dtype=torch.float64, pin_memory=True)
-        for t in range(2):
-            c.set_frames(t, host[t].numpy())
-        for t in range(T):
-            c.step(t % 2)
-        for t in range(T):
-            c.step_host_async(t % 2, host[t % 2].data_ptr(), xo[t % 2].data_ptr())
-        c.sync()
-        res = {"xv": xo.numpy().copy()}
-        for s in picks:
-            x, P = c.get_state(s)
-            f = c.features(s)
-            res[s] = (x, P, f["z"].copy(), f["flags"].copy(), f["attempted"].copy(), f["successful"].copy())
-        assert ((c.features(0)["flags"] & 3) == 3).all()
-        results.append(res)
-        c.close()
-    a, b = results
-    assert (a["xv"] == b["xv"]).all()
-    for s in picks:
-        for u, v in zip(a[s], b[s]):
-            assert (u == v).all(), s
-    with pytest.raises(sl2.Sl2Error):
-        c2 = ctx_from_scenes(scenes[:1])
-        try:
-            c2.set_tuning(99, 1)
-        finally:
-            c2.close()
-
-
 def test_c3_four_streams_four_frames_against_oracle(oracle):
     """BASELINE C3 (640x480, N = 100, 15x15 patch, +-40 px: the FP64-moment filter path of the search and the
     multi-tile window walk) through the FUSED step: 4 streams x 4 frames, all compared with the oracle."""
