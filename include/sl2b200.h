@@ -64,6 +64,16 @@ typedef struct sl2_config {
 /* fills *cfg with the reference's defaults (data/SceneLib2.cfg:24-31,59-61; monoslam.cpp:47-49) */
 void sl2_default_config(sl2_config *cfg);
 
+/* The per-instance cfg values of MonoSLAM::Init (monoslam.cpp:1583-1602, 1853) for ONE camera stream: each stream of
+ * a context may have its own camera, image size, frame period and selection count.  sl2_create gives every stream
+ * the values of its sl2_config. */
+typedef struct sl2_stream_config {
+  int32_t width, height;            /* cam.width / cam.height: this camera's image, <= the context's frame size */
+  double fku, fkv, u0, v0, kd1, sd; /* Camera::SetCameraParameters (camera.cpp:58-82) */
+  double delta_t;                   /* params.delta_t */
+  int32_t number_of_features_to_select;
+} sl2_stream_config;
+
 int sl2_create(const sl2_config *cfg, sl2_ctx **out);
 void sl2_destroy(sl2_ctx *ctx);
 const char *sl2_last_error(const sl2_ctx *ctx); /* ctx may be NULL: error of the last failed create */
@@ -71,11 +81,24 @@ int sl2_sync(sl2_ctx *ctx);
 /* library self-description: "sl2b200 <version> sm_90a" */
 const char *sl2_version(void);
 
+/* ---- per-stream camera ---------------------------------------------------------------------- */
+/* Sets the camera of stream_id.  Ordered like every other entry point: work queued before the call uses the old
+ * values, the next call that predicts, searches or detects (including the next fused step, also between two
+ * sl2_step_host_async calls) uses the new ones.  A stream's filter state is left as it is.
+ * SL2_ERR_ARG, with the stream's config unchanged, for: a bad stream_id or NULL sc; a non-finite value; fku, fkv or
+ * delta_t <= 0; width or height outside [max(16, boxsize), the context's width or height];
+ * number_of_features_to_select < 0, or > SL2_MAX_MEASURED when max_features > SL2_MAX_MEASURED. */
+int sl2_set_stream_config(sl2_ctx *ctx, int32_t stream_id, const sl2_stream_config *sc);
+int sl2_get_stream_config(sl2_ctx *ctx, int32_t stream_id, sl2_stream_config *sc);
+
 /* ---- frames (replaces the cv::Mat `frame` argument of MonoSLAM::GoOneStep, monoslam.cpp:108) */
-/* one stream, one slot; `stride` = bytes between image rows */
+/* The frame ring keeps the context's width x height per stream.  A stream whose image is smaller
+ * (sl2_set_stream_config) occupies the top-left width_s x height_s of its block; the rest of the block
+ * is never read into a result. */
+/* one stream, one slot: copies the stream's width_s x height_s image; `stride` = bytes between image rows */
 int sl2_set_frame(sl2_ctx *ctx, int32_t stream_id, int32_t slot, const uint8_t *gray, size_t stride);
-/* all streams of a slot at once: gray is [num_streams][height][width] contiguous (pinned memory
- * makes the copy asynchronous) */
+/* all streams of a slot at once: gray is [num_streams][height][width] contiguous, in the context's size (pinned
+ * memory makes the copy asynchronous) */
 int sl2_set_frames(sl2_ctx *ctx, int32_t slot, const uint8_t *gray);
 /* device-resident producer: copy device -> device, same layout as sl2_set_frames */
 int sl2_set_frames_dev(sl2_ctx *ctx, int32_t slot, const uint8_t *gray_dev);
@@ -217,7 +240,7 @@ int sl2_normalise_state(sl2_ctx *ctx, int32_t stream_id);
  *      the context: predict -> select -> measure -> update -> normalise -> cull -> symmetrise.
  *      Everything stays on the device; no host round trip inside the frame. */
 int sl2_step(sl2_ctx *ctx, int32_t slot);
-/* end-to-end form: host frames in ([num_streams][height][width]), camera states out
+/* end-to-end form: host frames in ([num_streams][height][width], the layout of sl2_set_frames), camera states out
  * (xv_out: [num_streams][13], may be NULL).  Copies run on the context's stream. */
 int sl2_step_host(sl2_ctx *ctx, int32_t slot, const uint8_t *gray, double *xv_out);
 /* asynchronous end-to-end form for a frame ring: enqueues the H2D copy of `gray` into `slot` on a

@@ -1,6 +1,7 @@
 // api.cu — context management and the extern "C" surface declared in include/sl2b200.h.
 // Host side only orchestrates: every arithmetic step of the hot path runs in the sm_90a
 // kernels of search.cu / ekf.cu.  There is deliberately no CPU fallback.
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -19,6 +20,7 @@ thread_local std::string g_create_error;
 struct sl2_ctx {
   sl2_config cfg;
   Sl2Dev d;
+  std::vector<sl2_stream_config> cams;  // host mirror of d.cams, updated with it
   cudaStream_t stream = nullptr;
   bool own_stream = false;
   CUtensorMap tmap;
@@ -148,6 +150,24 @@ int device_nfeat(sl2_ctx *c, int s, int *out) {
   return SL2_OK;
 }
 
+// A step measures at most min(max_features, SL2_MAX_MEASURED) features; below that capacity the selection is bounded
+// by the map itself, so only a larger map needs the bound on the selection.
+bool selection_fits(int max_features, int n_select) {
+  return !(max_features > SL2_MAX_MEASURED && n_select > SL2_MAX_MEASURED);
+}
+
+Sl2StreamCam cam_row(const sl2_stream_config &sc) {
+  Sl2StreamCam r = {};
+  const double cam[8] = {(double)sc.width, (double)sc.height, sc.fku, sc.fkv, sc.u0, sc.v0, sc.kd1, sc.sd};
+  for (int i = 0; i < 8; ++i) r.cam[i] = cam[i];
+  r.dt = sc.delta_t;
+  r.n_select = sc.number_of_features_to_select;
+  return r;
+}
+
+// the row travels as a kernel parameter, so the write is ordered on the stream like any other launch
+__global__ void write_cam_row_kernel(Sl2StreamCam *dst, const Sl2StreamCam row) { *dst = row; }
+
 }  // namespace
 
 extern "C" {
@@ -187,9 +207,7 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   if (cfg->num_streams < 1 || cfg->frame_slots < 1 || cfg->width < 16 || cfg->height < 16 ||
       cfg->max_features < 1 || cfg->max_features > SL2_MAX_FEATURES)
     return fail(nullptr, SL2_ERR_ARG, "bad sizes in sl2_config");
-  // a step measures at most min(max_features, SL2_MAX_MEASURED) features; below that capacity the selection is
-  // bounded by the map itself, so only a larger map needs the bound on the selection
-  if (cfg->max_features > SL2_MAX_MEASURED && cfg->number_of_features_to_select > SL2_MAX_MEASURED)
+  if (!selection_fits(cfg->max_features, cfg->number_of_features_to_select))
     return fail(nullptr, SL2_ERR_ARG,
                 "number_of_features_to_select must be <= SL2_MAX_MEASURED (128) when max_features > 128");
   if (cfg->boxsize != 11 && cfg->boxsize != 15)
@@ -237,7 +255,6 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   d.kmax = d.Nmax < SL2_MAX_MEASURED ? d.Nmax : SL2_MAX_MEASURED;  // the measurement capacity of every step
   d.mmax = 2 * d.kmax;
   d.ldg = ((d.mmax + SL2_NXV + 3 * d.Nmax + 1) + 7) & ~7;
-  d.n_select = cfg->number_of_features_to_select;
   const int radius = cfg->search_tile_radius > 0 ? cfg->search_tile_radius : 20;
   d.tile_h = 2 * radius + d.box;
   if (d.tile_h > 255) d.tile_h = 255;
@@ -245,20 +262,27 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   if (d.tile_w > 256) d.tile_w = 256;
   d.min_attempts = cfg->minimum_attempted_measurements_of_feature;
   d.match_fraction = cfg->successful_match_fraction;
-  d.cam[0] = cfg->width;
-  d.cam[1] = cfg->height;
-  d.cam[2] = cfg->fku;
-  d.cam[3] = cfg->fkv;
-  d.cam[4] = cfg->u0;
-  d.cam[5] = cfg->v0;
-  d.cam[6] = cfg->kd1;
-  d.cam[7] = cfg->sd;
-  d.dt = cfg->delta_t;
   for (int i = 0; i < 3; ++i) d.ovr[i] = cfg->search_override[i];
+  sl2_stream_config sc0 = {};
+  sc0.width = cfg->width;
+  sc0.height = cfg->height;
+  sc0.fku = cfg->fku;
+  sc0.fkv = cfg->fkv;
+  sc0.u0 = cfg->u0;
+  sc0.v0 = cfg->v0;
+  sc0.kd1 = cfg->kd1;
+  sc0.sd = cfg->sd;
+  sc0.delta_t = cfg->delta_t;
+  sc0.number_of_features_to_select = cfg->number_of_features_to_select;
+  c->cams.assign(d.B, sc0);
+  const std::vector<Sl2StreamCam> rows(d.B, cam_row(sc0));  // read by the copy below until the final synchronise
 
   const size_t B = d.B, N = d.Nmax;
   bool ok = true;
 #define ALLOC(ptr, count) ok = ok && (dev_alloc(c, &(ptr), (count)) == cudaSuccess)
+  ALLOC(d.cams, B);
+  ok = ok && cudaMemcpyAsync(d.cams, rows.data(), B * sizeof(Sl2StreamCam), cudaMemcpyHostToDevice, c->stream) ==
+                 cudaSuccess;
   ALLOC(d.frames, (size_t)d.slots * B * d.H * d.pitch);
   ALLOC(d.patches, (B * N + SL2_MAX_PARTIAL) * d.box * 16);  // + scratch templates (partially-initialised features)
   ALLOC(d.x, B * d.ld);
@@ -375,12 +399,42 @@ int sl2_sync(sl2_ctx *c) {
 
 int64_t sl2_launch_count(const sl2_ctx *c) { return c ? c->launches : 0; }
 
+// ---- per-stream camera --------------------------------------------------------------------------
+int sl2_set_stream_config(sl2_ctx *c, int32_t s, const sl2_stream_config *sc) {
+  if (bad_stream(c, s) || !sc) return fail(c, SL2_ERR_ARG, "sl2_set_stream_config: bad argument");
+  const double v[7] = {sc->fku, sc->fkv, sc->u0, sc->v0, sc->kd1, sc->sd, sc->delta_t};
+  for (double x : v)
+    if (!std::isfinite(x)) return fail(c, SL2_ERR_ARG, "sl2_set_stream_config: non-finite value");
+  if (!(sc->fku > 0.0) || !(sc->fkv > 0.0) || !(sc->delta_t > 0.0))
+    return fail(c, SL2_ERR_ARG, "sl2_set_stream_config: fku, fkv and delta_t must be > 0");
+  const int lo = c->cfg.boxsize > 16 ? c->cfg.boxsize : 16;
+  if (sc->width < lo || sc->height < lo || sc->width > c->cfg.width || sc->height > c->cfg.height)
+    return fail(c, SL2_ERR_ARG, "sl2_set_stream_config: image size outside [max(16, boxsize), the context's size]");
+  if (sc->number_of_features_to_select < 0 ||
+      !selection_fits(c->cfg.max_features, sc->number_of_features_to_select))
+    return fail(c, SL2_ERR_ARG,
+                "sl2_set_stream_config: number_of_features_to_select must be >= 0, and <= SL2_MAX_MEASURED (128) "
+                "when max_features > 128");
+  write_cam_row_kernel<<<1, 1, 0, c->stream>>>(c->d.cams + s, cam_row(*sc));
+  CU_TRY(c, cudaGetLastError());
+  ++c->launches;
+  c->cams[s] = *sc;
+  return SL2_OK;
+}
+
+int sl2_get_stream_config(sl2_ctx *c, int32_t s, sl2_stream_config *sc) {
+  if (bad_stream(c, s) || !sc) return fail(c, SL2_ERR_ARG, "sl2_get_stream_config: bad argument");
+  *sc = c->cams[s];
+  return SL2_OK;
+}
+
 // ---- frames -----------------------------------------------------------------------------------
 int sl2_set_frame(sl2_ctx *c, int32_t s, int32_t slot, const uint8_t *gray, size_t stride) {
   if (bad_stream(c, s) || bad_slot(c, slot) || !gray) return fail(c, SL2_ERR_ARG, "sl2_set_frame: bad argument");
   const Sl2Dev &d = c->d;
   uint8_t *dst = d.frames + ((size_t)slot * d.B + s) * d.H * d.pitch;
-  CU_TRY(c, cudaMemcpy2DAsync(dst, d.pitch, gray, stride, d.W, d.H, cudaMemcpyHostToDevice, c->stream));
+  const sl2_stream_config &sc = c->cams[s];  // the stream's image, top-left of its block
+  CU_TRY(c, cudaMemcpy2DAsync(dst, d.pitch, gray, stride, sc.width, sc.height, cudaMemcpyHostToDevice, c->stream));
   CU_TRY(c, cudaEventRecord(c->ev_cmp[slot], c->stream));  // slot busy until the copy has landed
   return SL2_OK;
 }

@@ -395,19 +395,22 @@ __global__ void __launch_bounds__(128) predict_kernel(const Sl2Dev d, int stream
   __shared__ double score[SL2_MAX_FEAT_SMEM];
   __shared__ int vis[SL2_MAX_FEAT_SMEM];
   __shared__ int s_nvis, s_r0;
+  __shared__ Sl2StreamCam sc;  // this stream's camera row, loaded once per CTA
 
+  if (tid < (int)(sizeof(Sl2StreamCam) / sizeof(double)))
+    reinterpret_cast<double *>(&sc)[tid] = reinterpret_cast<const double *>(d.cams + s)[tid];
   if (tid < 13) xv[tid] = x[tid];
   for (int e = tid; e < 169; e += blockDim.x) Pxx[e] = P[(e % 13) + (size_t)ld * (e / 13)];
   __syncthreads();
 
   if (do_predict) {
-    if (tid == 0) motion_model(xv, u3, d.dt, fv, F, Gn);
+    if (tid == 0) motion_model(xv, u3, sc.dt, fv, F, Gn);
     __syncthreads();
     // Q = (G * Pnn) * G^T, Pnn = diag(lin x3, ang x3)   (motion_model.cpp:157-216)
     // TT = F * Pxx
     for (int e = tid; e < 169; e += blockDim.x) {
       const int i = e % 13, j = e / 13;
-      const rd dt(d.dt);
+      const rd dt(sc.dt);
       const rd lin = rd(4.0) * rd(4.0) * dt * dt, ang = rd(6.0) * rd(6.0) * dt * dt;
       rd q(0.0), t(0.0);
       for (int k = 0; k < 6; ++k) {
@@ -466,7 +469,7 @@ __global__ void __launch_bounds__(128) predict_kernel(const Sl2Dev d, int stream
       const int pos = SL2_NXV + 3 * i;
       const rd yi[3] = {rd(x[pos]), rd(x[pos + 1]), rd(x[pos + 2])};
       FeatPred fp;
-      predict_feature(d.cam, xv, yi, Pxx, P + (size_t)ld * pos, ld, pos, fp);
+      predict_feature(sc.cam, xv, yi, Pxx, P + (size_t)ld * pos, ld, pos, fp);
       d.h[(fb + i) * 2 + 0] = fp.h[0].v;
       d.h[(fb + i) * 2 + 1] = fp.h[1].v;
       for (int r = 0; r < 2; ++r) {
@@ -478,7 +481,7 @@ __global__ void __launch_bounds__(128) predict_kernel(const Sl2Dev d, int stream
       d.S[(fb + i) * 4 + 1] = fp.S[1][0].v;
       d.S[(fb + i) * 4 + 2] = fp.S[0][1].v;
       d.S[(fb + i) * 4 + 3] = fp.S[1][1].v;
-      const int cant = visibility_test(d.cam, xv, yi, d.xp_org + (fb + i) * 7, fp.h);
+      const int cant = visibility_test(sc.cam, xv, yi, d.xp_org + (fb + i) * 7, fp.h);
       vis[i] = (cant == 0);
       score[i] = (fp.S[0][0] + fp.S[1][1]).v;  // trace, full_feature_model.cpp:172-176
     }
@@ -503,7 +506,7 @@ __global__ void __launch_bounds__(128) predict_kernel(const Sl2Dev d, int stream
     }
   }
   __syncthreads();
-  const int nsel = min(min(d.n_select, s_r0), s_nvis);
+  const int nsel = min(min(sc.n_select, s_r0), s_nvis);
   for (int i = tid; i < nf; i += blockDim.x) {
     int rank = d.sel_rank[fb + i];
     if (rank >= nsel) rank = -1;
@@ -543,6 +546,10 @@ __global__ void __launch_bounds__(128) particle_predict_kernel(const Sl2Dev d, i
   const double *ypi = ypi_all + 6 * f, *Pxy = Pxy_all + 78 * f, *Pyy = Pyy_all + 36 * f;
   const double *xv = d.x + (size_t)s * d.ld;
   const double *P = d.P + (size_t)s * d.ld * d.ld;  // Pxx = P(0:13, 0:13), column-major with stride ld
+  __shared__ Sl2StreamCam sc;  // this stream's camera row, loaded once per CTA
+  if (threadIdx.x < sizeof(Sl2StreamCam) / sizeof(double))
+    reinterpret_cast<double *>(&sc)[threadIdx.x] = reinterpret_cast<const double *>(d.cams + s)[threadIdx.x];
+  __syncthreads();
   // qRW and RRW: one camera pose for every particle
   const Quat qi = quat_inverse(Quat{rd(xv[3]), rd(xv[4]), rd(xv[5]), rd(xv[6])});
   rd R[3][3];
@@ -560,7 +567,7 @@ __global__ void __launch_bounds__(128) particle_predict_kernel(const Sl2Dev d, i
     dRq_times_a_by_dq(qi, hh, Dh);
     const rd hLR[3] = {zr[0] + lam * zh[0], zr[1] + lam * zh[1], zr[2] + lam * zh[2]};
     rd h[2], J[2][3];
-    project(d.cam, hLR, h, J);
+    project(sc.cam, hLR, h, J);
     // dhpi_by_dxp (2x7) and dhpi_by_dyi (2x6) = J [I | lambda I] dzeroedyi (part_feature_model.cpp:262-264): the
     // lambda columns of dh/dy, and one accumulator for the r and hhat terms of each quaternion column of dh/dxp
     rd dxp[2][7], dy[2][6];
@@ -586,7 +593,7 @@ __global__ void __launch_bounds__(128) particle_predict_kernel(const Sl2Dev d, i
       }
     }
     rd S[2][2], Sinv[3];
-    func_Si<6>(dxp, dy, measurement_noise(d.cam, h), P, d.ld, Pxy, 13, Pyy, 6, S);
+    func_Si<6>(dxp, dy, measurement_noise(sc.cam, h), P, d.ld, Pxy, 13, Pyy, 6, S);
     sinv_from_S(S[0][0], S[1][0], S[1][1], Sinv);
     h_out[2 * o] = h[0].v;
     h_out[2 * o + 1] = h[1].v;

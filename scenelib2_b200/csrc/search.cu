@@ -146,11 +146,13 @@ __global__ void __launch_bounds__(SL2_SEARCH_WARPS * 32, FILTER ? (BOX <= 11 ? 4
       __double2int_rz(div_(3.0, sqrt_(sub_(P11, div_(mul_(P01, P01), P00)))));
   const int uc = __double2int_rz(add_(cx, 0.5));
   const int vc = __double2int_rz(add_(cy, 0.5));
+  // clamped to the stream's own image, so no window reads past it (the tile loads may: those bytes feed nothing)
+  const int Ws = stream_width(d.cams[s]), Hs = stream_height(d.cams[s]);
   int us = -halfwidth, uf = halfwidth, vs = -halfheight, vf = halfheight;
   if (uc + us - HALF < 0) us = HALF - uc;
-  if (uc + uf - HALF > d.W - BOX) uf = d.W - BOX - uc + HALF;
+  if (uc + uf - HALF > Ws - BOX) uf = Ws - BOX - uc + HALF;
   if (vc + vs - HALF < 0) vs = HALF - vc;
-  if (vc + vf - HALF > d.H - BOX) vf = d.H - BOX - vc + HALF;
+  if (vc + vf - HALF > Hs - BOX) vf = Hs - BOX - vc + HALF;
   const int CW = uf - us + 1, CH = vf - vs + 1;
   const int x0 = uc + us - HALF, y0 = vc + vs - HALF;
   const double twoP01 = mul_(2.0, P01);

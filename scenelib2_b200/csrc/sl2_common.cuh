@@ -11,26 +11,37 @@
 #define SL2_STRIP 8         // candidates per vertical strip task
 #define SL2_MAX_FEAT_SMEM SL2_MAX_FEATURES  // per-feature shared arrays of the predict and cull kernels
 
+// One camera stream's camera, frame period and selection count (the per-instance cfg values of MonoSLAM::Init,
+// monoslam.cpp:1583-1602, 1853): one row per stream in Sl2Dev::cams, written by sl2_create and
+// sl2_set_stream_config.  Kernels that predict, search or detect read the row of their stream.
+struct Sl2StreamCam {
+  double cam[8];  // width, height, fku, fkv, u0, v0, kd1, sd (the stream's image: width x height <= W x H)
+  double dt;      // delta_t of the motion model
+  int n_select;   // number_of_features_to_select
+  int pad_;
+};
+static_assert(sizeof(Sl2StreamCam) % sizeof(double) == 0, "rows are copied as doubles");
+__device__ __forceinline__ int stream_width(const Sl2StreamCam &c) { return (int)c.cam[0]; }
+__device__ __forceinline__ int stream_height(const Sl2StreamCam &c) { return (int)c.cam[1]; }
+
 // Device view of one context: everything the kernels need, passed by value.
 struct Sl2Dev {
   // geometry / constants
   int B;       // camera streams in this context
   int Nmax;    // feature capacity per stream
-  int W, H, pitch, slots;
+  int W, H, pitch, slots;  // layout of the frame ring and of the SMOE score map; a stream's image may be smaller
   int box;     // BOXSIZE
   int ld;      // leading dimension of P (>= 13 + 3*Nmax, multiple of 8)
   int ldg;     // leading dimension of the update scratch G
   int kmax;    // features one step can measure: min(Nmax, SL2_MAX_MEASURED); sizes every measurement table
   int mmax;    // 2 * kmax: rows of S and of the update scratch G
-  int n_select;
   int tile_w, tile_h;  // TMA window tile (bytes x rows)
   int min_attempts;
   double match_fraction;
-  double cam[8];  // width,height,fku,fkv,u0,v0,kd1,sd
-  double dt;
   double ovr[3];
   // resident state
-  uint8_t *frames;   // [slots][B][H][pitch]
+  Sl2StreamCam *cams;  // [B]
+  uint8_t *frames;   // [slots][B][H][pitch]  stream s's image in the top-left width_s x height_s of its block
   uint8_t *patches;  // [B][Nmax][box][16]   rows zero-padded to 16 bytes
   double *x;         // [B][ld]
   double *P;         // [B][ld][ld] col-major, both triangles kept consistent

@@ -36,10 +36,20 @@ class Sl2Config(C.Structure):
     ]
 
 
+class Sl2StreamConfig(C.Structure):
+    """sl2_stream_config: one camera stream's camera, image size, frame period and selection count."""
+    _fields_ = [
+        ("width", C.c_int32), ("height", C.c_int32),
+        ("fku", C.c_double), ("fkv", C.c_double), ("u0", C.c_double), ("v0", C.c_double),
+        ("kd1", C.c_double), ("sd", C.c_double), ("delta_t", C.c_double),
+        ("number_of_features_to_select", C.c_int32),
+    ]
+
+
 # every symbol include/sl2b200.h declares (checked by tests/test_abi.py)
 EXPORTS = [
     "sl2_default_config", "sl2_create", "sl2_destroy", "sl2_last_error", "sl2_sync", "sl2_version",
-    "sl2_set_frame", "sl2_set_frames", "sl2_set_frames_dev", "sl2_set_features",
+    "sl2_set_stream_config", "sl2_get_stream_config", "sl2_set_frame", "sl2_set_frames", "sl2_set_frames_dev", "sl2_set_features",
     "sl2_num_features", "sl2_state_size", "sl2_set_state", "sl2_get_state", "sl2_delete_feature", "sl2_append_feature",
     "sl2_patch_search", "sl2_score_map", "sl2_smoe_search", "sl2_find_best_patch", "sl2_ekf_predict",
     "sl2_predict_measurements", "sl2_make_measurements", "sl2_ekf_update",
@@ -72,6 +82,8 @@ def load():
         L.sl2_destroy.restype = None
         L.sl2_destroy.argtypes = [C.c_void_p]
         L.sl2_default_config.restype = None
+        L.sl2_set_stream_config.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamConfig)]
+        L.sl2_get_stream_config.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamConfig)]
         L.sl2_set_frame.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_size_t]
         L.sl2_set_frames.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
         L.sl2_set_frames_dev.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
@@ -138,6 +150,25 @@ class Context:
         if rc < 0:
             raise Sl2Error("libsl2b200 error %d: %s" % (rc, self.L.sl2_last_error(self.h).decode()))
         return rc
+
+    # ---- per-stream camera ----------------------------------------------------------------------
+    def set_stream_config(self, stream_id, sc=None, **fields):
+        """sl2_set_stream_config: `sc` (an Sl2StreamConfig, default the stream's current one) with `fields`
+        (width, height, fku, fkv, u0, v0, kd1, sd, delta_t, number_of_features_to_select) replaced."""
+        if sc is None:
+            sc = self.stream_config(stream_id)
+        else:
+            sc = Sl2StreamConfig.from_buffer_copy(sc)
+        for k, v in fields.items():
+            if k not in dict(Sl2StreamConfig._fields_):
+                raise TypeError("unknown sl2_stream_config field %r" % k)
+            setattr(sc, k, v)
+        self._ck(self.L.sl2_set_stream_config(self.h, stream_id, C.byref(sc)))
+
+    def stream_config(self, stream_id):
+        sc = Sl2StreamConfig()
+        self._ck(self.L.sl2_get_stream_config(self.h, stream_id, C.byref(sc)))
+        return sc
 
     # ---- frames -------------------------------------------------------------------------------
     def set_frame(self, stream_id, slot, gray):
@@ -422,6 +453,16 @@ def config_for_scene(sc, num_streams=1, frame_slots=1, device=0, max_features=No
     if cuda_stream is not None:
         cfg.cuda_stream = cuda_stream
     return cfg
+
+
+def stream_config_for_scene(sc):
+    """sl2_stream_config matching a synth.Scene's camera, frame period and selection count."""
+    out = Sl2StreamConfig()
+    out.width, out.height = sc.width, sc.height
+    out.fku, out.fkv, out.u0, out.v0, out.kd1, out.sd = [float(v) for v in sc.cam8[2:8]]
+    out.delta_t = sc.delta_t
+    out.number_of_features_to_select = sc.n_select
+    return out
 
 
 def load_scene(ctx, stream_id, sc):

@@ -146,19 +146,34 @@ def make_prior_covariance(rng, n, sig_r=0.010, sig_q=0.005, sig_v=0.05, sig_w=0.
 
 
 def make_scene(name="C2", stream_id=0, n_frames=8, known_patches=None, override=True,
-               n_features=None, seed_extra=0):
-    """Build the synthetic scene of one camera stream for BASELINE config `name`."""
+               n_features=None, seed_extra=0, camera=None, delta_t=None):
+    """Build the synthetic scene of one camera stream for BASELINE config `name`.  `camera` (width, height, fku, fkv,
+    u0, v0, kd1, sd) renders it for that camera and image instead of the config's; `delta_t` sets its frame period
+    (default 0.033333333).  With both left at None the scene is the config's own, draw for draw."""
     cfg = dict(CONFIGS[name])
     if n_features is not None:
         cfg["n_features"] = n_features
         cfg["n_select"] = min(cfg["n_select"], n_features) if name != "C1" else cfg["n_select"]
     rng = np.random.default_rng((SEED0 ^ (cfg["config_id"] << 16) ^ stream_id) + (seed_extra << 40))
+    if camera is None:
+        cam8 = camera_params(cfg["width"], cfg["height"])
+    else:
+        cam8 = np.array(camera, dtype=np.float64).reshape(8)
+        cfg["width"], cfg["height"] = int(cam8[0]), int(cam8[1])
     W, H, N, B = cfg["width"], cfg["height"], cfg["n_features"], cfg["boxsize"]
-    cam8 = camera_params(W, H)
     half = (B - 1) // 2
 
     frame0 = make_texture(rng, H, W)
     pix = _feature_pixels(rng, W, H, N, cfg["margin"])
+    if camera is not None:
+        # the camera model reaches only the pixels with 2 kd1 r^2 < 1 (r: distance to the principal point; the
+        # undistortion of camera.cpp:132-157): with strong distortion, pull features towards the principal point
+        pp = cam8[4:6]
+        r2 = ((pix - pp) ** 2).sum(axis=1)
+        far = 2.0 * cam8[6] * r2 > 0.8
+        if far.any():
+            scale = np.sqrt(0.8 / (2.0 * cam8[6] * r2[far]))
+            pix[far] = np.floor(pp + (pix[far] - pp) * scale[:, None]).astype(np.int64)
 
     # C1: the first four features are the reference's known target corners
     # (data/SceneLib2.cfg:267-305) drawn with the shipped 11x11 templates.
@@ -203,7 +218,7 @@ def make_scene(name="C2", stream_id=0, n_frames=8, known_patches=None, override=
         search_override = (9.0 / (r * r), 0.0, 9.0 / (r * r))
     else:
         search_override = (0.0, 0.0, 0.0)
-    return Scene(name=name, cam8=cam8, delta_t=0.033333333, boxsize=B, n_select=cfg["n_select"],
+    return Scene(name=name, cam8=cam8, delta_t=0.033333333 if delta_t is None else float(delta_t), boxsize=B, n_select=cfg["n_select"],
                  search_override=search_override, x0=x0, P0=P0, xp_org=xp_org, patches=patches,
                  pix=pix, frames=frames, shifts=shifts,
                  meta=dict(config=cfg, stream_id=stream_id, depth=depth))
