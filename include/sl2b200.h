@@ -279,6 +279,101 @@ int sl2_last_update_times(sl2_ctx *ctx, float *ms5);
 /* kernels launched by this context since creation */
 int64_t sl2_launch_count(const sl2_ctx *ctx);
 
+/* ---- stream snapshots: save, restore and move camera streams (no reference counterpart) ----------------------
+ * A snapshot is ONE stream's blob: everything a later entry point reads of that stream, so that a stream loaded
+ * into any stream id of any context (same boxsize, capacity >= its map, frame at least its image; another device
+ * through the host form) continues bit for bit like the stream it was saved from.  Uses: checkpoint / resume,
+ * moving a camera to another GPU or to a context of another capacity, rollback after a bad frame, cloning a stream.
+ *
+ * Format (version 1).  Host byte order; a blob of the other byte order fails the magic.  No checksum, no
+ * compression.  The header below, then these sections, in this order, each starting 8-byte aligned (zero bytes pad
+ * a section to the next multiple of 8), each sized from nfeat and boxsize only (never from the context's capacity):
+ *    x          double[n]                  n = 13 + 3 nfeat
+ *    P          double[n * n]              column-major, dense: what sl2_get_state returns
+ *    xp_org     double[nfeat][7]           camera position state each feature was first seen from
+ *    attempted  int32[nfeat]               measurement attempts (the cull of delete_bad_features reads them)
+ *    successful int32[nfeat]               successful measurements
+ *    h          double[nfeat][2]           last prediction
+ *    S          double[nfeat][4]           column-major 2x2
+ *    Rvar       double[nfeat]              measurement noise variance
+ *    dh_dxp     double[nfeat][2][7]        row-major
+ *    dh_dy      double[nfeat][2][3]        row-major
+ *    sel_rank   int32[nfeat]               rank in the selected list, -1 = not selected
+ *    z_uv       int32[nfeat][2]            last match
+ *    found      uint8[nfeat]               1 = the last measurement of the feature succeeded
+ *    best       double[nfeat]              last correlation score
+ *    job_feat   int32[nfeat]               feature of measurement job r (-1 = none): only jobs r < nsel hold one
+ *    job_centre double[nfeat][2]           search centre of job r
+ *    job_puinv  double[nfeat][3]           search ellipse (P00, P01, P11) of job r
+ *    templates  uint8[nfeat][box][box]     row-major, without the device's row padding
+ * The rule for what goes in: every per-stream array of the device state that an entry point reads before a later
+ * kernel overwrites it.  Out: scratch of one update, the frame ring, and the context-wide settings (boxsize, search
+ * tile radius, minimum_attempted_measurements_of_feature, successful_match_fraction, search_override), which belong
+ * to the receiving context.  The format is canonical: a blob saved, loaded anywhere and saved again is
+ * byte-identical. */
+#define SL2_SNAPSHOT_MAGIC 0x53324C53u /* the bytes "SL2S" on a little-endian host */
+#define SL2_SNAPSHOT_VERSION 1
+
+typedef struct sl2_snapshot_header {
+  uint32_t magic;         /* SL2_SNAPSHOT_MAGIC */
+  uint32_t version;       /* SL2_SNAPSHOT_VERSION */
+  uint32_t header_bytes;  /* sizeof(sl2_snapshot_header) = 128 */
+  uint32_t reserved0;     /* 0 (a load refuses anything else) */
+  uint64_t total_bytes;   /* the whole blob, header included */
+  int32_t boxsize;        /* template size; must equal the receiving context's */
+  int32_t nfeat;          /* map features */
+  int32_t n;              /* state size 13 + 3 nfeat */
+  int32_t reserved1;      /* 0 (a load refuses anything else) */
+  sl2_stream_config cam;  /* the stream's camera (sl2_set_stream_config), padding bytes zero */
+  int32_t nsel;           /* job slots of the last prediction (<= SL2_MAX_MEASURED) */
+  int32_t nvisible;       /* visible features of the last prediction (<= SL2_MAX_FEATURES) */
+  int32_t nmeas;          /* successful measurements of the last update (<= SL2_MAX_MEASURED) */
+  int32_t ncull;          /* features the cull of the last update found (<= SL2_MAX_FEATURES) */
+} sl2_snapshot_header;
+/* The four counts describe the last prediction / update and are not renewed by every call that changes the map: a
+ * cull, sl2_delete_feature and sl2_set_features leave nvisible, ncull and (sl2_set_features) nsel as they were, so a
+ * saved stream may hold nvisible, ncull or nsel above nfeat, and job slots below nsel that hold -1.  Loads accept
+ * these states, which the library produces itself: no kernel indexes with nvisible, nmeas or ncull, and nsel only
+ * bounds a walk over the job slots, which a load fills with -1 beyond nfeat. */
+
+/* Byte offsets of the sections of a blob of nfeat features with boxsize x boxsize templates, in the order above
+ * (field[0] = xp_org ... field[14] = job_puinv), and the blob's total size.  SL2_ERR_ARG unless
+ * 0 <= nfeat <= SL2_MAX_FEATURES and boxsize > 0. */
+#define SL2_SNAPSHOT_FIELDS 15
+typedef struct sl2_snapshot_sections {
+  uint64_t x, P, field[SL2_SNAPSHOT_FIELDS], templates, total;
+} sl2_snapshot_sections;
+int sl2_snapshot_layout(int32_t nfeat, int32_t boxsize, sl2_snapshot_sections *out);
+
+/* Upper bound of one stream's blob in this context: the size of a map of max_features features. */
+size_t sl2_snapshot_bytes(const sl2_ctx *ctx);
+/* Blob i belongs to stream lo + i and lies at buf + i * stride.
+ * Ordering: like every other entry point, these join both step groups first.  A save captures the state after
+ * everything queued before it (an sl2_step_host_async that has not been waited for included); a load is seen by
+ * the next call (the next fused step and an sl2_step_host_async queued after it included).
+ * sl2_save_streams synchronises and writes each blob's size to sizes[i] (sizes may be NULL);
+ * sl2_save_streams_dev is asynchronous on the context's stream, like sl2_set_frames_dev.  The host forms stage the
+ * batch through the context's pinned staging buffer in groups of streams of at most 64 MB (at least one stream), so
+ * the buffer stays bounded whatever the batch.  Saves need
+ * stride >= the context's snapshot size; the device forms need buf_dev and stride to be multiples of 8.
+ * Loads are all or nothing: every header of the batch (for the device form: copied down first) and the index
+ * fields later kernels index with (job_feat, sel_rank; the device form checks them with a kernel) are validated
+ * before anything is written, and the kernels use the validated sizes.  Both loads synchronise.  SL2_ERR_ARG for a
+ * bad range, NULL pointer or short stride; a wrong magic, version or header size, non-zero reserved fields, a total
+ * size above the stride or different from the one nfeat and boxsize give; n != 13 + 3 nfeat; a negative count;
+ * nsel or nmeas above SL2_MAX_MEASURED, nvisible or ncull above SL2_MAX_FEATURES; a boxsize other than the
+ * context's; a job_feat that is neither -1 nor in [0, nfeat) for r < nsel, or not -1 for r >= nsel; a sel_rank that
+ * is neither -1 nor in [0, min(nsel, nfeat)) (the cull writes job slot sel_rank); a camera sl2_set_stream_config
+ * would refuse in this context.  SL2_ERR_STATE when nfeat exceeds the context's max_features.  On an error no
+ * stream of the batch changes.
+ * A load resets what the blob does not cover to the values sl2_create / sl2_set_features leave: x and P outside
+ * n x n, the per-feature records, job slots and templates beyond nfeat are zero, sel_rank and job_feat -1.  A
+ * stream's results therefore never depend on what it held before the load. */
+int sl2_save_streams(sl2_ctx *ctx, int32_t lo, int32_t cnt, void *buf, size_t stride, size_t *sizes);
+int sl2_load_streams(sl2_ctx *ctx, int32_t lo, int32_t cnt, const void *buf, size_t stride);
+int sl2_save_streams_dev(sl2_ctx *ctx, int32_t lo, int32_t cnt, void *buf_dev, size_t stride);
+int sl2_load_streams_dev(sl2_ctx *ctx, int32_t lo, int32_t cnt, const void *buf_dev, size_t stride);
+
 #ifdef __cplusplus
 }
 #endif

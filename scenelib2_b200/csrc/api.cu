@@ -1,6 +1,7 @@
 // api.cu — context management and the extern "C" surface declared in include/sl2b200.h.
 // Host side only orchestrates: every arithmetic step of the hot path runs in the sm_90a
 // kernels of search.cu / ekf.cu.  There is deliberately no CPU fallback.
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -400,21 +401,28 @@ int sl2_sync(sl2_ctx *c) {
 int64_t sl2_launch_count(const sl2_ctx *c) { return c ? c->launches : 0; }
 
 // ---- per-stream camera --------------------------------------------------------------------------
-int sl2_set_stream_config(sl2_ctx *c, int32_t s, const sl2_stream_config *sc) {
-  if (bad_stream(c, s) || !sc) return fail(c, SL2_ERR_ARG, "sl2_set_stream_config: bad argument");
+// the camera values a stream of this context accepts (sl2_set_stream_config and the snapshot loads)
+static int check_stream_config(sl2_ctx *c, const sl2_stream_config *sc, const std::string &who) {
   const double v[7] = {sc->fku, sc->fkv, sc->u0, sc->v0, sc->kd1, sc->sd, sc->delta_t};
   for (double x : v)
-    if (!std::isfinite(x)) return fail(c, SL2_ERR_ARG, "sl2_set_stream_config: non-finite value");
+    if (!std::isfinite(x)) return fail(c, SL2_ERR_ARG, who + ": non-finite value");
   if (!(sc->fku > 0.0) || !(sc->fkv > 0.0) || !(sc->delta_t > 0.0))
-    return fail(c, SL2_ERR_ARG, "sl2_set_stream_config: fku, fkv and delta_t must be > 0");
+    return fail(c, SL2_ERR_ARG, who + ": fku, fkv and delta_t must be > 0");
   const int lo = c->cfg.boxsize > 16 ? c->cfg.boxsize : 16;
   if (sc->width < lo || sc->height < lo || sc->width > c->cfg.width || sc->height > c->cfg.height)
-    return fail(c, SL2_ERR_ARG, "sl2_set_stream_config: image size outside [max(16, boxsize), the context's size]");
+    return fail(c, SL2_ERR_ARG, who + ": image size outside [max(16, boxsize), the context's size]");
   if (sc->number_of_features_to_select < 0 ||
       !selection_fits(c->cfg.max_features, sc->number_of_features_to_select))
     return fail(c, SL2_ERR_ARG,
-                "sl2_set_stream_config: number_of_features_to_select must be >= 0, and <= SL2_MAX_MEASURED (128) "
-                "when max_features > 128");
+                who + ": number_of_features_to_select must be >= 0, and <= SL2_MAX_MEASURED (128) "
+                      "when max_features > 128");
+  return SL2_OK;
+}
+
+int sl2_set_stream_config(sl2_ctx *c, int32_t s, const sl2_stream_config *sc) {
+  if (bad_stream(c, s) || !sc) return fail(c, SL2_ERR_ARG, "sl2_set_stream_config: bad argument");
+  const int rc = check_stream_config(c, sc, "sl2_set_stream_config");
+  if (rc) return rc;
   write_cam_row_kernel<<<1, 1, 0, c->stream>>>(c->d.cams + s, cam_row(*sc));
   CU_TRY(c, cudaGetLastError());
   ++c->launches;
@@ -1275,6 +1283,190 @@ int sl2_get_features(sl2_ctx *c, int32_t s, double *h, double *z, double *S, uin
     if (select_rank) select_rank[i] = rk[i];
   }
   return nf;
+}
+
+// ---- stream snapshots ---------------------------------------------------------------------------
+static bool bad_range(sl2_ctx *c, int32_t lo, int32_t cnt) {
+  enter(c);
+  return !c || lo < 0 || cnt < 0 || lo > c->cfg.num_streams - cnt;
+}
+
+// Checks the header of one blob (and, with `index`, its job_feat / sel_rank) against this context; fills `q` with
+// the validated counts for stream s.  `blob` is host memory of at least `avail` bytes, any alignment.
+static int snap_validate(sl2_ctx *c, const uint8_t *blob, size_t stride, bool index, int s, Sl2SnapLoad *q,
+                         const std::string &who) {
+  sl2_snapshot_header h;
+  memcpy(&h, blob, sizeof h);
+  if (h.magic != SL2_SNAPSHOT_MAGIC || h.version != SL2_SNAPSHOT_VERSION || h.header_bytes != sizeof h)
+    return fail(c, SL2_ERR_ARG, who + ": not a snapshot of this version and byte order");
+  if (h.reserved0 != 0 || h.reserved1 != 0) return fail(c, SL2_ERR_ARG, who + ": reserved header fields are not 0");
+  if (h.total_bytes > stride) return fail(c, SL2_ERR_ARG, who + ": blob larger than the stride");
+  if (h.nfeat < 0 || h.nsel < 0 || h.nvisible < 0 || h.nmeas < 0 || h.ncull < 0)
+    return fail(c, SL2_ERR_ARG, who + ": negative count");
+  if ((int64_t)h.n != SL2_NXV + 3 * (int64_t)h.nfeat) return fail(c, SL2_ERR_ARG, who + ": n != 13 + 3 nfeat");
+  if (h.boxsize != c->cfg.boxsize) return fail(c, SL2_ERR_ARG, who + ": boxsize differs from the context's");
+  if (h.nfeat > c->cfg.max_features) return fail(c, SL2_ERR_STATE, who + ": map larger than max_features");
+  const Sl2SnapLayout L = sl2_snap_layout(h.nfeat, h.boxsize);
+  if (h.total_bytes != L.total) return fail(c, SL2_ERR_ARG, who + ": total size does not match nfeat and boxsize");
+  // the counts are not renewed by a cull, sl2_delete_feature or sl2_set_features, so they are bounded by what any
+  // prediction / update can produce, not by nfeat (include/sl2b200.h)
+  if (h.nsel > SL2_MAX_MEASURED || h.nmeas > SL2_MAX_MEASURED || h.nvisible > SL2_MAX_FEATURES ||
+      h.ncull > SL2_MAX_FEATURES)
+    return fail(c, SL2_ERR_ARG, who + ": count above what a step can produce");
+  const int rc = check_stream_config(c, &h.cam, who);
+  if (rc) return rc;
+  if (index) {
+    for (int f = 0; f < h.nfeat; ++f) {
+      int32_t r, j;
+      memcpy(&r, blob + L.field[SL2_SNAP_SEL_RANK] + 4 * (size_t)f, 4);
+      memcpy(&j, blob + L.field[SL2_SNAP_JOB_FEAT] + 4 * (size_t)f, 4);
+      // the same rules as snap_check_kernel: a job below nsel may be empty, the cull writes job slot sel_rank
+      if (!(r == -1 || (r >= 0 && r < h.nsel && r < h.nfeat)) || !(f < h.nsel ? (j >= -1 && j < h.nfeat) : j == -1))
+        return fail(c, SL2_ERR_ARG, who + ": sel_rank or job_feat out of range");
+    }
+  }
+  memset(q, 0, sizeof *q);
+  q->cam = cam_row(h.cam);
+  q->stream = s;
+  q->nfeat = h.nfeat;
+  q->nsel = h.nsel;
+  q->nvisible = h.nvisible;
+  q->nmeas = h.nmeas;
+  q->ncull = h.ncull;
+  return SL2_OK;
+}
+
+size_t sl2_snapshot_bytes(const sl2_ctx *c) { return c ? sl2_snap_layout(c->cfg.max_features, c->cfg.boxsize).total : 0; }
+
+int sl2_snapshot_layout(int32_t nfeat, int32_t boxsize, sl2_snapshot_sections *out) {
+  if (nfeat < 0 || nfeat > SL2_MAX_FEATURES || boxsize <= 0 || !out) return SL2_ERR_ARG;
+  const Sl2SnapLayout L = sl2_snap_layout(nfeat, boxsize);
+  out->x = L.x;
+  out->P = L.P;
+  for (int k = 0; k < SL2_SNAPSHOT_FIELDS; ++k) out->field[k] = L.field[k];
+  out->templates = L.templates;
+  out->total = L.total;
+  return SL2_OK;
+}
+
+// The host forms stage groups of streams of at most this many bytes (at least one stream), so a save or load of a
+// whole large context does not grow the staging buffers to the size of all its blobs.
+static const size_t SL2_SNAP_STAGE_BYTES = (size_t)64 << 20;
+static int snap_group(size_t sb) { return (int)std::max<size_t>(1, SL2_SNAP_STAGE_BYTES / sb); }
+
+int sl2_save_streams(sl2_ctx *c, int32_t lo, int32_t cnt, void *buf, size_t stride, size_t *sizes) {
+  if (bad_range(c, lo, cnt) || (cnt && !buf)) return fail(c, SL2_ERR_ARG, "sl2_save_streams: bad argument");
+  const size_t sb = sl2_snapshot_bytes(c);
+  if (stride < sb) return fail(c, SL2_ERR_ARG, "sl2_save_streams: stride below sl2_snapshot_bytes");
+  if (cnt == 0) return SL2_OK;
+  const int g = std::min(cnt, snap_group(sb));
+  int rc = stage_reserve(c, (size_t)g * sb);
+  if (rc) return rc;
+  CU_TRY(c, cudaStreamSynchronize(c->stream));  // staging buffer reuse
+  for (int i0 = 0; i0 < cnt; i0 += g) {
+    const int k = std::min(g, cnt - i0);
+    CU_TRY(c, sl2_launch_pack(c->d, lo + i0, k, c->stg_dev, sb, c->stream));
+    ++c->launches;
+    CU_TRY(c, cudaMemcpyAsync(c->stg_host, c->stg_dev, (size_t)k * sb, cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    for (int i = 0; i < k; ++i) {
+      sl2_snapshot_header h;
+      memcpy(&h, c->stg_host + (size_t)i * sb, sizeof h);
+      memcpy(static_cast<uint8_t *>(buf) + (size_t)(i0 + i) * stride, c->stg_host + (size_t)i * sb, h.total_bytes);
+      if (sizes) sizes[i0 + i] = h.total_bytes;
+    }
+  }
+  return SL2_OK;
+}
+
+int sl2_save_streams_dev(sl2_ctx *c, int32_t lo, int32_t cnt, void *buf_dev, size_t stride) {
+  if (bad_range(c, lo, cnt) || (cnt && !buf_dev) || ((uintptr_t)buf_dev & 7) || (stride & 7))
+    return fail(c, SL2_ERR_ARG, "sl2_save_streams_dev: bad argument");
+  if (stride < sl2_snapshot_bytes(c)) return fail(c, SL2_ERR_ARG, "sl2_save_streams_dev: stride below sl2_snapshot_bytes");
+  if (cnt == 0) return SL2_OK;
+  CU_TRY(c, sl2_launch_pack(c->d, lo, cnt, static_cast<uint8_t *>(buf_dev), stride, c->stream));
+  ++c->launches;
+  return SL2_OK;
+}
+
+
+int sl2_load_streams(sl2_ctx *c, int32_t lo, int32_t cnt, const void *buf, size_t stride) {
+  if (bad_range(c, lo, cnt) || (cnt && !buf) || stride < sizeof(sl2_snapshot_header))
+    return fail(c, SL2_ERR_ARG, "sl2_load_streams: bad argument");
+  if (cnt == 0) return SL2_OK;
+  const uint8_t *in = static_cast<const uint8_t *>(buf);
+  std::vector<Sl2SnapLoad> q(cnt);
+  std::vector<sl2_stream_config> cams(cnt);
+  for (int i = 0; i < cnt; ++i) {
+    const int rc = snap_validate(c, in + (size_t)i * stride, stride, true, lo + i, &q[i], "sl2_load_streams");
+    if (rc) return rc;
+    memcpy(&cams[i], in + (size_t)i * stride + offsetof(sl2_snapshot_header, cam), sizeof(sl2_stream_config));
+  }
+  // staging, one group of streams at a time: its load records, then its blobs at the context's snapshot size
+  const size_t sb = sl2_snapshot_bytes(c);
+  const int g = std::min(cnt, snap_group(sb));
+  const size_t pb = ((size_t)g * sizeof(Sl2SnapLoad) + 255) & ~(size_t)255;
+  int rc = stage_reserve(c, pb + (size_t)g * sb);
+  if (rc) return rc;
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  for (int i0 = 0; i0 < cnt; i0 += g) {
+    const int k = std::min(g, cnt - i0);
+    CU_TRY(c, cudaStreamSynchronize(c->stream));  // the previous group's unpack has read the staging buffer
+    memcpy(c->stg_host, q.data() + i0, (size_t)k * sizeof(Sl2SnapLoad));
+    size_t end = 0;
+    for (int i = 0; i < k; ++i) {
+      const size_t tb = sl2_snap_layout(q[i0 + i].nfeat, c->cfg.boxsize).total;
+      memcpy(c->stg_host + pb + (size_t)i * sb, in + (size_t)(i0 + i) * stride, tb);
+      end = pb + (size_t)i * sb + tb;
+    }
+    CU_TRY(c, cudaMemcpyAsync(c->stg_dev, c->stg_host, end, cudaMemcpyHostToDevice, c->stream));
+    CU_TRY(c, sl2_launch_unpack(c->d, k, reinterpret_cast<const Sl2SnapLoad *>(c->stg_dev), c->stg_dev + pb, sb,
+                                c->stream));
+    ++c->launches;
+  }
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  for (int i = 0; i < cnt; ++i) c->cams[lo + i] = cams[i];
+  return SL2_OK;
+}
+
+int sl2_load_streams_dev(sl2_ctx *c, int32_t lo, int32_t cnt, const void *buf_dev, size_t stride) {
+  if (bad_range(c, lo, cnt) || (cnt && !buf_dev) || ((uintptr_t)buf_dev & 7) || (stride & 7) ||
+      stride < sizeof(sl2_snapshot_header))
+    return fail(c, SL2_ERR_ARG, "sl2_load_streams_dev: bad argument");
+  if (cnt == 0) return SL2_OK;
+  const uint8_t *in = static_cast<const uint8_t *>(buf_dev);
+  const size_t hb = sizeof(sl2_snapshot_header);
+  // staging: load records | verdict (int) | headers copied down
+  const size_t pb = ((size_t)cnt * sizeof(Sl2SnapLoad) + 255) & ~(size_t)255, o_bad = pb, o_h = pb + 256;
+  int rc = stage_reserve(c, o_h + (size_t)cnt * hb);
+  if (rc) return rc;
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  CU_TRY(c, cudaMemcpy2DAsync(c->stg_host + o_h, hb, in, stride, hb, cnt, cudaMemcpyDeviceToHost, c->stream));
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  std::vector<Sl2SnapLoad> q(cnt);
+  std::vector<sl2_stream_config> cams(cnt);
+  for (int i = 0; i < cnt; ++i) {
+    const uint8_t *h = c->stg_host + o_h + (size_t)i * hb;
+    rc = snap_validate(c, h, stride, false, lo + i, &q[i], "sl2_load_streams_dev");
+    if (rc) return rc;
+    memcpy(&cams[i], h + offsetof(sl2_snapshot_header, cam), sizeof(sl2_stream_config));
+  }
+  memcpy(c->stg_host, q.data(), (size_t)cnt * sizeof(Sl2SnapLoad));
+  memset(c->stg_host + o_bad, 0, sizeof(int));
+  CU_TRY(c, cudaMemcpyAsync(c->stg_dev, c->stg_host, o_bad + sizeof(int), cudaMemcpyHostToDevice, c->stream));
+  const Sl2SnapLoad *q_dev = reinterpret_cast<const Sl2SnapLoad *>(c->stg_dev);
+  int *bad_dev = reinterpret_cast<int *>(c->stg_dev + o_bad);
+  CU_TRY(c, sl2_launch_snap_check(c->d, cnt, q_dev, in, stride, bad_dev, c->stream));
+  ++c->launches;
+  int bad = 0;
+  CU_TRY(c, cudaMemcpyAsync(&bad, bad_dev, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  if (bad) return fail(c, SL2_ERR_ARG, "sl2_load_streams_dev: sel_rank or job_feat out of range");
+  CU_TRY(c, sl2_launch_unpack(c->d, cnt, q_dev, in, stride, c->stream));
+  ++c->launches;
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  for (int i = 0; i < cnt; ++i) c->cams[lo + i] = cams[i];
+  return SL2_OK;
 }
 
 }  // extern "C"

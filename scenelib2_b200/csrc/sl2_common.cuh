@@ -184,3 +184,53 @@ cudaError_t sl2_launch_particles(int F, int Kmax, const int *K_dev, const double
 size_t sl2_detect_scratch_bytes(const Sl2Dev &d, int n);
 cudaError_t sl2_launch_detect(const Sl2Dev &d, int stream, int slot, int n, const int *regions_dev,
                               int *out_uv_dev, double *out_ev_dev, void *scratch_dev, cudaStream_t st);
+
+// ---- stream snapshots (snapshot.cu): the blob format of include/sl2b200.h --------------------------------------
+// The per-feature sections of a blob, in blob order: each is the stream's first nfeat records of one Sl2Dev array
+// of `per` elements of `esz` bytes per feature (x, P and the templates are laid out separately).
+struct Sl2SnapLayout {
+  size_t x, P, field[SL2_SNAPSHOT_FIELDS], templates, total;  // byte offsets in the blob, total size
+};
+__host__ __device__ inline size_t sl2_snap_align8(size_t b) { return (b + 7) & ~(size_t)7; }
+__host__ __device__ inline void sl2_snap_field(int k, int *per, int *esz) {
+  // xp_org attempted successful h S Rvar dh_dxp dh_dy sel_rank z_uv found best job_feat job_centre job_puinv
+  const int P_[SL2_SNAPSHOT_FIELDS] = {7, 1, 1, 2, 4, 1, 14, 6, 1, 2, 1, 1, 1, 2, 3};
+  const int E_[SL2_SNAPSHOT_FIELDS] = {8, 4, 4, 8, 8, 8, 8, 8, 4, 4, 1, 8, 4, 8, 8};
+  *per = P_[k];
+  *esz = E_[k];
+}
+__host__ __device__ inline Sl2SnapLayout sl2_snap_layout(int nfeat, int box) {
+  Sl2SnapLayout L;
+  const size_t n = SL2_NXV + 3 * (size_t)nfeat;
+  size_t o = sizeof(sl2_snapshot_header);
+  L.x = o;
+  o += sl2_snap_align8(8 * n);
+  L.P = o;
+  o += 8 * n * n;
+  for (int k = 0; k < SL2_SNAPSHOT_FIELDS; ++k) {
+    int per, esz;
+    sl2_snap_field(k, &per, &esz);
+    L.field[k] = o;
+    o += sl2_snap_align8((size_t)nfeat * per * esz);
+  }
+  L.templates = o;
+  o += sl2_snap_align8((size_t)nfeat * box * box);
+  L.total = o;
+  return L;
+}
+enum { SL2_SNAP_SEL_RANK = 8, SL2_SNAP_JOB_FEAT = 12 };  // the index fields, set to -1 beyond the map by a load
+
+// what the host validated for one blob of a load: the kernels take sizes and counts from here, never from the blob
+struct Sl2SnapLoad {
+  Sl2StreamCam cam;
+  int stream, nfeat, nsel, nvisible, nmeas, ncull;
+  int pad_[2];
+};
+// pack the streams [lo, lo + cnt) into blobs at buf + i * stride (nfeat read on the device, header written)
+cudaError_t sl2_launch_pack(const Sl2Dev &d, int lo, int cnt, uint8_t *buf, size_t stride, cudaStream_t st);
+// adds the number of blobs whose job_feat / sel_rank fail the index rules (with the validated counts) to *bad
+cudaError_t sl2_launch_snap_check(const Sl2Dev &d, int cnt, const Sl2SnapLoad *ld_dev, const uint8_t *buf,
+                                  size_t stride, int *bad, cudaStream_t st);
+// unpack blob i into stream ld_dev[i].stream and reset what the blob does not cover
+cudaError_t sl2_launch_unpack(const Sl2Dev &d, int cnt, const Sl2SnapLoad *ld_dev, const uint8_t *buf, size_t stride,
+                              cudaStream_t st);

@@ -456,6 +456,73 @@ void MonoSLAM::SyncFromDevice() {  // fill_states / fill_covariances, monoslam.c
   selected_feature_list_.resize(nsel);
 }
 
+void MonoSLAM::SaveState(const std::string &path) {
+  if (!ctx_) throw std::runtime_error("SaveState: Init()/CreateDevice() has not been called");
+  if (map_dirty_) UploadMap();
+  std::vector<uint8_t> blob(sl2_snapshot_bytes(ctx_));
+  size_t size = 0;
+  check(ctx_, sl2_save_streams(ctx_, 0, 1, blob.data(), blob.size(), &size), "sl2_save_streams");
+  std::ofstream o(path, std::ios::binary);
+  if (!o.write(reinterpret_cast<const char *>(blob.data()), (std::streamsize)size))
+    throw std::runtime_error("SaveState: cannot write " + path);
+}
+
+void MonoSLAM::LoadState(const std::string &path) {
+  if (!ctx_) throw std::runtime_error("LoadState: Init()/CreateDevice() has not been called");
+  std::ifstream f(path, std::ios::binary);
+  const std::vector<uint8_t> blob((std::istreambuf_iterator<char>(f)), std::istreambuf_iterator<char>());
+  if (!f.eof() && f.fail()) throw std::runtime_error("LoadState: cannot read " + path);
+  if (blob.size() < sizeof(sl2_snapshot_header)) throw std::runtime_error("LoadState: " + path + " is not a snapshot");
+  check(ctx_, sl2_load_streams(ctx_, 0, 1, blob.data(), blob.size()), "sl2_load_streams");
+  sl2_snapshot_header h;
+  std::memcpy(&h, blob.data(), sizeof h);
+  const size_t nf = (size_t)h.nfeat, box = (size_t)h.boxsize;
+  sl2_snapshot_sections L;
+  check(ctx_, sl2_snapshot_layout(h.nfeat, h.boxsize, &L), "sl2_snapshot_layout");
+  const size_t o_xp = L.field[0], o_tp = L.templates;  // xp_org, the templates
+  for (Feature *g : feature_list_) delete g;
+  feature_list_.clear();
+  selected_feature_list_.clear();
+  total_state_size_ = 13;
+  next_free_label_ = 0;
+  marked_feature_label_ = -1;
+  for (size_t i = 0; i < nf; ++i) {
+    Feature *g = new Feature();
+    g->y_.resize(3);
+    g->xp_org_.resize(7);
+    std::memcpy(g->xp_org_.data(), blob.data() + o_xp + 56 * i, 56);
+    g->patch_ = cv::Mat((int)box, (int)box, CV_8UC1);
+    for (size_t r = 0; r < box; ++r) std::memcpy(g->patch_.data + r * g->patch_.step, blob.data() + o_tp + (i * box + r) * box, box);
+    g->label_ = next_free_label_++;
+    g->Pxy_.resize(13, 3);
+    g->Pyy_.resize(3, 3);
+    g->h_.resize(2);
+    g->z_.resize(2);
+    g->nu_.resize(2);
+    g->dh_by_dxv_.resize(2, 13);
+    g->dh_by_dy_.resize(2, 3);
+    g->R_.resize(2, 2);
+    g->S_.resize(2, 2);
+    feature_list_.push_back(g);
+    total_state_size_ += 3;
+  }
+  // the stream's camera travels with the blob
+  camera_->width_ = h.cam.width;
+  camera_->height_ = h.cam.height;
+  camera_->fku_ = h.cam.fku;
+  camera_->fkv_ = h.cam.fkv;
+  camera_->centre_(0) = h.cam.u0;
+  camera_->centre_(1) = h.cam.v0;
+  camera_->kd1_ = h.cam.kd1;
+  camera_->measurement_sd_ = h.cam.sd;
+  kDeltaT_ = h.cam.delta_t;
+  kNumberOfFeaturesToSelect_ = h.cam.number_of_features_to_select;
+  map_dirty_ = false;
+  SyncFromDevice();  // y_, P blocks, counters, flags and the last step's results
+  number_of_visible_features_ = h.nvisible;
+  successful_measurement_vector_size_ = 2 * h.nmeas;
+}
+
 void Kalman::KalmanFilterPredict(MonoSLAM *m, Eigen::Vector3d &u) {  // kalman.cpp:50-69
   if (!m->ctx_) throw std::runtime_error("KalmanFilterPredict: no device context");
   check(m->ctx_, sl2_ekf_predict(m->ctx_, 0, u.data()), "sl2_ekf_predict");

@@ -202,6 +202,16 @@ class MonoSLAM {  // monoslam.h:73-218 (hot-path subset + the calls of examples/
   void CreateDevice(int max_features = 100, int device = 0);
   void UploadMap();    // host y_/xp_org_/patch_/xv_/P blocks -> device (whole map; first upload)
   void SyncFromDevice();  // device state + per-feature results -> host mirrors
+  // Checkpoint / resume of the tracker (no counterpart in the reference, which cannot save its state): the stream
+  // snapshot of include/sl2b200.h for stream 0 -- filter, map with its counters and templates, the last step's
+  // results and the camera -- written to / read from one file with sl2_save_streams / sl2_load_streams.  LoadState
+  // rebuilds feature_list_ from the blob (y_, xp_org_, patch_, counters), numbers the labels in map order and
+  // refreshes every host mirror (SyncFromDevice).  The file holds the device state only: the trajectory store and
+  // the pending features (templates the caller asked to initialise, pending_features_) are not in it, and
+  // LoadState leaves them as they are.  A run that has none continues from the file bit-identically to the run that
+  // saved it.  Both throw std::runtime_error.
+  void SaveState(const std::string &path);
+  void LoadState(const std::string &path);
   sl2_ctx *ctx_ = nullptr;
 
  private:

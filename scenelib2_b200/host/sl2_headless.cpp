@@ -6,6 +6,9 @@
 // FrameGrabber / FileGrabber pair like the reference's file mode (sorted file names, reader thread,
 // bounded queue).  Prints the camera state per frame and optionally writes the final total state and
 // covariance for comparison.
+// SL2_HEADLESS_LOAD_STATE=file resumes from a MonoSLAM::SaveState file (loaded after Init, before the first frame);
+// SL2_HEADLESS_SAVE_STATE=file writes one after the last frame.  A run split at frame k into two runs chained by the
+// file tracks exactly like the unsplit run.
 #include <algorithm>
 #include <chrono>
 #include <cstdio>
@@ -34,6 +37,7 @@ int main(int argc, char **argv) {
   try {
     SceneLib2::MonoSLAM *g_monoslam = new SceneLib2::MonoSLAM();
     g_monoslam->Init(argv[1]);
+    if (const char *load = std::getenv("SL2_HEADLESS_LOAD_STATE")) g_monoslam->LoadState(load);
     if (dir_mode) {
       // examples/MonoSlamSceneLib1.cpp:132-142: poll GetFrame, step on every frame that arrives
       SceneLib2::FrameGrabber grabber;
@@ -80,6 +84,7 @@ int main(int argc, char **argv) {
       }
     }
     g_monoslam->print_robot_state();
+    if (const char *save = std::getenv("SL2_HEADLESS_SAVE_STATE")) g_monoslam->SaveState(save);
     if (out_path) {
       Eigen::VectorXd V;
       Eigen::MatrixXd M;

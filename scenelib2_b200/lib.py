@@ -57,7 +57,86 @@ EXPORTS = [
     "sl2_step_host_async", "sl2_wait_slot", "sl2_set_step_groups", "sl2_join", "sl2_measure_particles", "sl2_measure_particles_patch",
     "sl2_smoe_search_patch", "sl2_measure_partial_features",
     "sl2_get_features", "sl2_get_feature_jacobians", "sl2_enable_timing", "sl2_last_step_times", "sl2_last_update_times", "sl2_launch_count",
+    "sl2_snapshot_layout", "sl2_snapshot_bytes", "sl2_save_streams", "sl2_load_streams", "sl2_save_streams_dev", "sl2_load_streams_dev",
 ]
+
+SL2_SNAPSHOT_MAGIC = 0x53324C53
+SL2_SNAPSHOT_VERSION = 1
+
+
+class Sl2SnapshotHeader(C.Structure):
+    """sl2_snapshot_header: the fixed header of one stream's snapshot blob."""
+    _fields_ = [
+        ("magic", C.c_uint32), ("version", C.c_uint32), ("header_bytes", C.c_uint32), ("reserved0", C.c_uint32),
+        ("total_bytes", C.c_uint64),
+        ("boxsize", C.c_int32), ("nfeat", C.c_int32), ("n", C.c_int32), ("reserved1", C.c_int32),
+        ("cam", Sl2StreamConfig),
+        ("nsel", C.c_int32), ("nvisible", C.c_int32), ("nmeas", C.c_int32), ("ncull", C.c_int32),
+    ]
+
+
+class Sl2SnapshotSections(C.Structure):
+    """sl2_snapshot_sections: byte offsets of a blob's sections (what sl2_snapshot_layout returns)."""
+    _fields_ = [("x", C.c_uint64), ("P", C.c_uint64), ("field", C.c_uint64 * 15), ("templates", C.c_uint64),
+                ("total", C.c_uint64)]
+
+
+# the per-feature sections of a snapshot in blob order: (name, per-feature shape, dtype)
+SNAPSHOT_FIELDS = (
+    ("xp_org", (7,), np.float64), ("attempted", (), np.int32), ("successful", (), np.int32),
+    ("h", (2,), np.float64), ("S", (4,), np.float64), ("Rvar", (), np.float64), ("dh_dxp", (2, 7), np.float64),
+    ("dh_dy", (2, 3), np.float64), ("sel_rank", (), np.int32), ("z_uv", (2,), np.int32), ("found", (), np.uint8),
+    ("best", (), np.float64), ("job_feat", (), np.int32), ("job_centre", (2,), np.float64),
+    ("job_puinv", (3,), np.float64),
+)
+
+
+def _align8(b):
+    return (b + 7) & ~7
+
+
+def snapshot_layout(nfeat, boxsize):
+    """Byte offset of every section of a snapshot of `nfeat` features and the blob's total size (the format of
+    include/sl2b200.h): dict name -> (offset, shape, dtype), and total."""
+    n = 13 + 3 * nfeat
+    out = {}
+    o = C.sizeof(Sl2SnapshotHeader)
+    for name, shape, dt in (("x", (n,), np.float64), ("P", (n, n), np.float64)) + tuple(
+            (nm, (nfeat,) + sh, dt) for nm, sh, dt in SNAPSHOT_FIELDS) + (
+            ("templates", (nfeat, boxsize, boxsize), np.uint8),):
+        out[name] = (o, shape, dt)
+        o += _align8(int(np.prod(shape, dtype=np.int64)) * np.dtype(dt).itemsize)
+    return out, o
+
+
+def read_snapshot(blob):
+    """Parse one stream's snapshot blob: a dict with the header fields, the stream config as `cam` (a dict) and every
+    section as a NumPy array (P as an n x n array, column-major like sl2_get_state).  Raises ValueError for a blob
+    that is not a snapshot of this version, or is shorter than its header says."""
+    blob = bytes(blob)
+    hsz = C.sizeof(Sl2SnapshotHeader)
+    if len(blob) < hsz:
+        raise ValueError("snapshot shorter than its header")
+    h = Sl2SnapshotHeader.from_buffer_copy(blob[:hsz])
+    if h.magic != SL2_SNAPSHOT_MAGIC or h.version != SL2_SNAPSHOT_VERSION or h.header_bytes != hsz:
+        raise ValueError("not a version-%d snapshot in this byte order" % SL2_SNAPSHOT_VERSION)
+    if h.reserved0 or h.reserved1:
+        raise ValueError("reserved snapshot header fields are not 0")
+    if h.nfeat < 0 or h.n != 13 + 3 * h.nfeat:
+        raise ValueError("bad map size in the snapshot header")
+    layout, total = snapshot_layout(h.nfeat, h.boxsize)
+    if h.total_bytes != total:
+        raise ValueError("snapshot total size %d does not match nfeat and boxsize (%d)" % (h.total_bytes, total))
+    if len(blob) < total:
+        raise ValueError("truncated snapshot: %d of %d bytes" % (len(blob), total))
+    out = {k: getattr(h, k) for k, _ in Sl2SnapshotHeader._fields_ if k not in ("cam", "reserved0", "reserved1")}
+    out["cam"] = {k: getattr(h.cam, k) for k, _ in Sl2StreamConfig._fields_}
+    for name, (o, shape, dt) in layout.items():
+        cnt = int(np.prod(shape, dtype=np.int64))
+        a = np.frombuffer(blob, dtype=dt, count=cnt, offset=o)
+        out[name] = a.reshape(shape[::-1]).T.copy() if name == "P" else a.reshape(shape).copy()
+    return out
+
 
 _lib = None
 
@@ -102,6 +181,14 @@ def load():
         L.sl2_sync.argtypes = [C.c_void_p]
         L.sl2_score_map.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, f64p, f64p, i32p,
                                     f64p, f64p, u8p, C.c_size_t]
+        L.sl2_snapshot_layout.argtypes = [C.c_int32, C.c_int32, C.POINTER(Sl2SnapshotSections)]
+        L.sl2_snapshot_bytes.restype = C.c_size_t
+        L.sl2_snapshot_bytes.argtypes = [C.c_void_p]
+        L.sl2_save_streams.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_size_t,
+                                       C.POINTER(C.c_size_t)]
+        L.sl2_load_streams.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_size_t]
+        L.sl2_save_streams_dev.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_size_t]
+        L.sl2_load_streams_dev.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_size_t]
         _lib = L
     return _lib
 
@@ -429,6 +516,44 @@ class Context:
             _p(out["flags"], u8p), _p(out["attempted"], i32p), _p(out["successful"], i32p),
             _p(out["select_rank"], i32p)))
         return {k: v[:nf] for k, v in out.items()}
+
+    # ---- stream snapshots -----------------------------------------------------------------------
+    def snapshot_bytes(self):
+        """Upper bound of one stream's snapshot in this context (a map of max_features features)."""
+        return int(self.L.sl2_snapshot_bytes(self.h))
+
+    def save_streams(self, lo=0, cnt=None):
+        """Snapshots of the streams [lo, lo + cnt) (default: to the last stream) as a list of bytes."""
+        if cnt is None:
+            cnt = self.cfg.num_streams - lo
+        stride = self.snapshot_bytes()
+        buf = np.empty(max(cnt, 0) * stride, np.uint8)
+        sizes = (C.c_size_t * max(cnt, 1))()
+        self._ck(self.L.sl2_save_streams(self.h, lo, cnt, buf.ctypes.data, stride, sizes))
+        return [buf[i * stride:i * stride + sizes[i]].tobytes() for i in range(cnt)]
+
+    def save_stream(self, stream_id):
+        return self.save_streams(stream_id, 1)[0]
+
+    def load_streams(self, blobs, lo=0):
+        """Load blobs[i] into stream lo + i (all or nothing: on an error no stream changes)."""
+        blobs = [bytes(b) for b in blobs]
+        stride = _align8(max([len(b) for b in blobs] + [C.sizeof(Sl2SnapshotHeader)]))
+        buf = np.zeros(len(blobs) * stride, np.uint8)
+        for i, b in enumerate(blobs):
+            buf[i * stride:i * stride + len(b)] = np.frombuffer(b, np.uint8)
+        self._ck(self.L.sl2_load_streams(self.h, lo, len(blobs), buf.ctypes.data, stride))
+
+    def load_stream(self, stream_id, blob):
+        self.load_streams([blob], stream_id)
+
+    def save_streams_dev(self, lo, cnt, dev_ptr, stride):
+        """Snapshots of [lo, lo + cnt) into device memory at dev_ptr + i * stride, asynchronous on the context's
+        stream (stride >= snapshot_bytes(), both multiples of 8)."""
+        self._ck(self.L.sl2_save_streams_dev(self.h, lo, cnt, dev_ptr, stride))
+
+    def load_streams_dev(self, lo, cnt, dev_ptr, stride):
+        self._ck(self.L.sl2_load_streams_dev(self.h, lo, cnt, dev_ptr, stride))
 
 
 def config_for_scene(sc, num_streams=1, frame_slots=1, device=0, max_features=None,
