@@ -374,6 +374,46 @@ int sl2_load_streams(sl2_ctx *ctx, int32_t lo, int32_t cnt, const void *buf, siz
 int sl2_save_streams_dev(sl2_ctx *ctx, int32_t lo, int32_t cnt, void *buf_dev, size_t stride);
 int sl2_load_streams_dev(sl2_ctx *ctx, int32_t lo, int32_t cnt, const void *buf_dev, size_t stride);
 
+/* ---- step records: every camera stream's trajectory and filter health, kept on the device --------------------
+ * MonoSLAM::GoOneStep(frame, save_trajectory, ...) appends the camera position to trajectory_store_ (capped at 1000
+ * entries, monoslam.cpp:172-177).  With records on, the fused step (sl2_step, sl2_step_host, sl2_step_host_async)
+ * writes one record per camera stream per step into a ring of `depth` records per stream, so the trajectory and the
+ * health of hundreds of streams come back in one call instead of one synchronising call per stream and quantity.
+ * The staged entry points, snapshots, sl2_set_*, sl2_append_feature and sl2_delete_feature write no record and alter
+ * none; a snapshot load does not rewrite a stream's past records (the snapshot format is unchanged).
+ *
+ * nis and logdet_s are the two standard consistency checks of the step's EKF update, S = H P H^T + R of the m
+ * measured rows: nis = nu^T S^-1 nu (chi-square with m degrees of freedom when the filter is consistent) and
+ * log det S.  Both are reduced on the device in a fixed order, so a stream's record does not depend on its position in
+ * the batch or on the step groups. */
+#define SL2_MAX_RECORDS 4096
+typedef struct sl2_step_record { /* 256 bytes, no padding */
+  int64_t step;         /* index of the fused step since records were (re-)enabled: 0, 1, 2, ... */
+  int32_t nfeat;        /* map features after the step's cull */
+  int32_t nvisible;     /* visible features of the step's prediction */
+  int32_t nsel;         /* features of the step's selection still in the map after the cull (the reference's
+                           selected_feature_list_ after GoOneStep) */
+  int32_t nmeas;        /* successful measurements (= rows m / 2 of the update) */
+  int32_t nculled;      /* features the step's cull deleted */
+  int32_t m;            /* rows of S; 0 when nothing was measured */
+  double nis;           /* nu^T S^-1 nu of the step's update; 0 when m == 0 */
+  double logdet_s;      /* log det S; 0 when m == 0 */
+  double xv[13];        /* camera state after the step (xv[0..2] = the trajectory point of trajectory_store_) */
+  double pxx_diag[13];  /* diagonal of Pxx after the step */
+} sl2_step_record;
+
+/* depth 0 = off (the default; frees the ring), 1 .. SL2_MAX_RECORDS = records per stream kept.  Joins both step groups
+ * like every entry point, (re)allocates the ring (num_streams x depth x 256 bytes) and restarts `step` at 0; calling
+ * it with the current depth also clears the ring.  SL2_ERR_ARG for a depth outside [0, SL2_MAX_RECORDS]. */
+int sl2_enable_records(sl2_ctx *ctx, int32_t depth);
+/* The most recent k = min(max, steps recorded, depth) records of each stream lo + i, oldest first, at
+ * out[i * max + j], j < k.  All streams step together, so k is the same for every stream; returns k.
+ * sl2_get_records synchronises; sl2_get_records_dev is asynchronous on the context's stream and needs out_dev to be
+ * 8-byte aligned.  SL2_ERR_ARG for a bad range, a NULL pointer or max < 1; SL2_ERR_STATE while records are off.
+ * On an error nothing changes. */
+int sl2_get_records(sl2_ctx *ctx, int32_t lo, int32_t cnt, int32_t max, sl2_step_record *out);
+int sl2_get_records_dev(sl2_ctx *ctx, int32_t lo, int32_t cnt, int32_t max, void *out_dev);
+
 #ifdef __cplusplus
 }
 #endif

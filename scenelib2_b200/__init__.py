@@ -7,8 +7,10 @@ Layout (hot path only, see DESIGN.md):
   synth.py   deterministic synthetic inputs for BASELINE configs C1..C5
 """
 from . import synth  # noqa: F401
-from .lib import (Context, Sl2Config, Sl2Error, Sl2SnapshotHeader, Sl2StreamConfig, config_for_scene,  # noqa: F401
-                  default_config, load, load_scene, read_snapshot, stream_config_for_scene)
+from .lib import (STEP_RECORD_DTYPE, Context, Sl2Config, Sl2Error, Sl2SnapshotHeader, Sl2StepRecord,  # noqa: F401
+                  Sl2StreamConfig, config_for_scene, default_config, load, load_scene, read_snapshot,
+                  stream_config_for_scene)
 
-__all__ = ["synth", "Context", "Sl2Config", "Sl2Error", "Sl2SnapshotHeader", "Sl2StreamConfig", "config_for_scene",
-           "default_config", "load", "load_scene", "read_snapshot", "stream_config_for_scene"]
+__all__ = ["synth", "STEP_RECORD_DTYPE", "Context", "Sl2Config", "Sl2Error", "Sl2SnapshotHeader", "Sl2StepRecord",
+           "Sl2StreamConfig", "config_for_scene", "default_config", "load", "load_scene", "read_snapshot",
+           "stream_config_for_scene"]

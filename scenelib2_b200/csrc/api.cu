@@ -53,6 +53,7 @@ struct sl2_ctx {
   cudaEvent_t ev_main = nullptr, ev_a_search = nullptr, ev_b_search = nullptr, ev_b_done = nullptr;
   bool b_pending = false, b_search_valid = false;
   std::vector<cudaEvent_t> ev_cmp_b;  // per frame slot: group B is done with the slot
+  int64_t rec_steps = 0;  // fused steps recorded since sl2_enable_records (the ring itself is d.rec)
 };
 
 namespace {
@@ -378,6 +379,7 @@ void sl2_destroy(sl2_ctx *c) {
   for (cudaEvent_t e : {c->ev_main, c->ev_a_search, c->ev_b_search, c->ev_b_done})
     if (e) cudaEventDestroy(e);
   for (void *p : c->allocs) cudaFree(p);
+  if (c->d.rec) cudaFree(c->d.rec);
   if (c->stg_dev) cudaFree(c->stg_dev);
   if (c->smoe_map) cudaFree(c->smoe_map);
   if (c->stg_host) cudaFreeHost(c->stg_host);
@@ -1074,6 +1076,10 @@ static int step_group(sl2_ctx *c, int32_t slot, int lo, int cnt, cudaStream_t st
   if (t) CU_TRY(c, cudaEventRecord(c->ev[3], st));
   CU_TRY(c, sl2_launch_cull(d, lo, cnt, -1, st));
   if (t) CU_TRY(c, cudaEventRecord(c->ev[4], st));
+  if (d.rec_depth) {  // after ev[4]: the step times keep their meaning
+    CU_TRY(c, sl2_launch_records(d, lo, cnt, c->rec_steps, st));
+    ++nl;
+  }
   c->launches += nl;
   return SL2_OK;
 }
@@ -1083,7 +1089,7 @@ static int split_point(const sl2_ctx *c) {
   return (c->step_groups >= 2 && !c->timing && c->d.B >= 2) ? (c->d.B + 1) / 2 : 0;
 }
 
-static int step_enqueue(sl2_ctx *c, int32_t slot, bool serial = false) {
+static int step_enqueue_groups(sl2_ctx *c, int32_t slot, bool serial) {
   const Sl2Dev &d = c->d;
   const int BA = serial ? 0 : split_point(c);
   if (BA == 0) {
@@ -1103,6 +1109,12 @@ static int step_enqueue(sl2_ctx *c, int32_t slot, bool serial = false) {
   CU_TRY(c, cudaEventRecord(c->ev_b_done, c->stream_b));
   c->b_pending = true;
   return SL2_OK;
+}
+
+static int step_enqueue(sl2_ctx *c, int32_t slot, bool serial = false) {
+  const int rc = step_enqueue_groups(c, slot, serial);
+  if (rc == SL2_OK && c->d.rec_depth) ++c->rec_steps;  // both groups recorded this step under the same index
+  return rc;
 }
 
 // the slot's frames are busy until everything queued so far on the step stream(s) has run
@@ -1467,6 +1479,68 @@ int sl2_load_streams_dev(sl2_ctx *c, int32_t lo, int32_t cnt, const void *buf_de
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   for (int i = 0; i < cnt; ++i) c->cams[lo + i] = cams[i];
   return SL2_OK;
+}
+
+// ---- step records -------------------------------------------------------------------------------
+int sl2_enable_records(sl2_ctx *c, int32_t depth) {
+  if (!c) return SL2_ERR_ARG;
+  enter(c);
+  if (depth < 0 || depth > SL2_MAX_RECORDS)
+    return fail(c, SL2_ERR_ARG, "sl2_enable_records: depth outside [0, SL2_MAX_RECORDS]");
+  // the new ring first, so that a failed allocation leaves the old one in place
+  sl2_step_record *ring = nullptr;
+  if (depth) {
+    const size_t bytes = (size_t)c->d.B * depth * sizeof(sl2_step_record);
+    CU_TRY(c, cudaMalloc((void **)&ring, bytes));
+    const cudaError_t e = cudaMemsetAsync(ring, 0, bytes, c->stream);
+    if (e != cudaSuccess) {
+      cudaFree(ring);
+      return fail(c, SL2_ERR_CUDA, std::string("sl2_enable_records: ") + cudaGetErrorString(e));
+    }
+  }
+  // steps queued before the call (either group: enter() joined them) have written the old ring
+  const cudaError_t e = cudaStreamSynchronize(c->stream);
+  if (e != cudaSuccess) {
+    if (ring) cudaFree(ring);
+    return fail(c, SL2_ERR_CUDA, std::string("sl2_enable_records: ") + cudaGetErrorString(e));
+  }
+  if (c->d.rec) cudaFree(c->d.rec);
+  c->d.rec = ring;
+  c->d.rec_depth = depth;
+  c->rec_steps = 0;
+  return SL2_OK;
+}
+
+// The most recent k records of streams [lo, lo + cnt), oldest first, as one or two 2-D copies (two when the k rows
+// wrap around the end of the ring): row pitch `depth` records in the ring, `mx` records in the output.
+static int get_records(sl2_ctx *c, int32_t lo, int32_t cnt, int32_t mx, void *out, cudaMemcpyKind kind,
+                       const char *who) {
+  if (bad_range(c, lo, cnt) || !out || mx < 1 ||
+      (kind == cudaMemcpyDeviceToDevice && ((uintptr_t)out & 7)))
+    return fail(c, SL2_ERR_ARG, std::string(who) + ": bad argument");
+  const int64_t depth = c->d.rec_depth;
+  if (!depth) return fail(c, SL2_ERR_STATE, std::string(who) + ": records are off (sl2_enable_records)");
+  const int k = (int)std::min<int64_t>(std::min<int64_t>(mx, c->rec_steps), depth);
+  if (k == 0 || cnt == 0) return k;
+  const size_t R = sizeof(sl2_step_record);
+  const int r0 = (int)((c->rec_steps - k) % depth);  // ring row of the oldest record returned
+  const int k1 = (int)std::min<int64_t>(k, depth - r0);
+  const sl2_step_record *src = c->d.rec + (size_t)lo * depth;
+  uint8_t *dst = static_cast<uint8_t *>(out);
+  CU_TRY(c, cudaMemcpy2DAsync(dst, (size_t)mx * R, src + r0, (size_t)depth * R, (size_t)k1 * R, cnt, kind, c->stream));
+  if (k1 < k)
+    CU_TRY(c, cudaMemcpy2DAsync(dst + (size_t)k1 * R, (size_t)mx * R, src, (size_t)depth * R, (size_t)(k - k1) * R,
+                                cnt, kind, c->stream));
+  if (kind == cudaMemcpyDeviceToHost) CU_TRY(c, cudaStreamSynchronize(c->stream));
+  return k;
+}
+
+int sl2_get_records(sl2_ctx *c, int32_t lo, int32_t cnt, int32_t max, sl2_step_record *out) {
+  return get_records(c, lo, cnt, max, out, cudaMemcpyDeviceToHost, "sl2_get_records");
+}
+
+int sl2_get_records_dev(sl2_ctx *c, int32_t lo, int32_t cnt, int32_t max, void *out_dev) {
+  return get_records(c, lo, cnt, max, out_dev, cudaMemcpyDeviceToDevice, "sl2_get_records_dev");
 }
 
 }  // extern "C"

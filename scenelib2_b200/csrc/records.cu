@@ -1,0 +1,69 @@
+// records.cu — step records: one sl2_step_record per camera stream per fused step, written into the ring Sl2Dev::rec
+// by one CTA per stream after the cull (include/sl2b200.h).  The kernel reads and writes nothing but the ring.
+//
+// Where the update leaves what the record needs (update.cu), for the step's m = upd_m rows:
+//   w = U^-T nu   upd_solve writes Y = U^-T [H P | nu] over the [H P | nu] part of G, so w_i = G(i, m + n) with
+//                 n = 13 + 3 nfeat the state size OF THE UPDATE.  The cull ran in between and deleted ncull features,
+//                 so n = 13 + 3 (nfeat + ncull).  NIS = nu^T S^-1 nu = w^T w.
+//   U_ii          upd_chol leaves U (true diagonal) in G's S block, but the cull uses row 0 of G as scratch when it
+//                 deletes features, which overwrites U_00.  upd_chol also keeps W_pp = U_pp^-T of every 16-row panel in
+//                 Sl2Dev::Wp for the solve, and nothing else writes Wp: its diagonal holds the reciprocal pivots
+//                 W_ii = 1 / U_ii the solve applied.  log det S = 2 sum log U_ii = -2 sum log W_ii.
+// When m == 0 the update wrote neither G nor Wp (they hold another update's values) and the kernel reads neither.
+#include "sl2_common.cuh"
+
+namespace {
+
+constexpr int REC_THREADS = 256;  // one thread per row of S: m <= 2 * SL2_MAX_MEASURED
+static_assert(2 * SL2_MAX_MEASURED <= REC_THREADS, "one thread per measurement row");
+static_assert(sizeof(sl2_step_record) == 256, "sl2_step_record is 256 bytes without padding");
+
+__global__ void __launch_bounds__(REC_THREADS) record_kernel(const Sl2Dev d, int stream_lo, long long step) {
+  pdl_prologue();
+  const int s = stream_lo + blockIdx.x, tid = threadIdx.x;
+  __shared__ double s_nis[REC_THREADS], s_ld[REC_THREADS];
+  const int m = d.upd_m[s], nf = d.nfeat[s], nc = d.ncull[s];
+  double q = 0.0, l = 0.0;
+  if (tid < m) {
+    const int n = SL2_NXV + 3 * (nf + nc);
+    const double w = d.G[((size_t)s * d.mmax + tid) * d.ldg + m + n];
+    q = mul_(w, w);
+    l = -log(d.Wp[((size_t)s * SL2_MAX_PANELS + (tid >> 4)) * 256 + (tid & 15) * 17]);
+  }
+  s_nis[tid] = q;
+  s_ld[tid] = l;
+  __syncthreads();
+  // pairwise tree over all REC_THREADS slots: the same order for every stream, every m and every launch shape
+#pragma unroll
+  for (int h = REC_THREADS / 2; h > 0; h >>= 1) {
+    if (tid < h) {
+      s_nis[tid] = add_(s_nis[tid], s_nis[tid + h]);
+      s_ld[tid] = add_(s_ld[tid], s_ld[tid + h]);
+    }
+    __syncthreads();
+  }
+  sl2_step_record *r = d.rec + (size_t)s * d.rec_depth + (size_t)(step % d.rec_depth);
+  if (tid < SL2_NXV) {
+    const size_t ld = d.ld;
+    r->xv[tid] = d.x[(size_t)s * ld + tid];
+    r->pxx_diag[tid] = d.P[(size_t)s * ld * ld + (size_t)tid * (ld + 1)];
+  } else if (tid == 32) {
+    r->step = step;
+    r->nfeat = nf;
+    r->nvisible = d.nvisible[s];
+    r->nsel = d.nsel[s];
+    r->nmeas = d.nmeas[s];
+    r->nculled = nc;
+    r->m = m;
+    r->nis = s_nis[0];
+    r->logdet_s = mul_(2.0, s_ld[0]);
+  }
+}
+
+}  // namespace
+
+cudaError_t sl2_launch_records(const Sl2Dev &d, int stream_lo, int stream_cnt, int64_t step, cudaStream_t st) {
+  if (stream_cnt <= 0) return cudaSuccess;
+  return sl2_launch_kernel(record_kernel, dim3(stream_cnt), dim3(REC_THREADS), 0, st, sl2_use_pdl(stream_cnt), d,
+                           stream_lo, (long long)step);
+}

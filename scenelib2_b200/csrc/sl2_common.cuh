@@ -72,6 +72,9 @@ struct Sl2Dev {
   int *upd_m;          // [B]  measurement rows m of the running update (0: nothing to do)
   double *Wp;          // [B][SL2_MAX_PANELS][16*16]  W_pp = U_pp^-T of every 16-row Cholesky panel
   int nsm;             // SMs of the device
+  // step records (records.cu): written by the fused step only, when rec_depth > 0
+  sl2_step_record *rec;  // [B][rec_depth]  ring: the record of step t of stream s is rec[s][t % rec_depth]
+  int rec_depth;         // 0 = records off
 };
 
 #define SL2_MAX_PANELS 16  // 16-row panels of S: m <= 2 * SL2_MAX_MEASURED = 256
@@ -165,6 +168,9 @@ cudaError_t sl2_launch_cull(const Sl2Dev &d, int stream_lo, int stream_cnt, int 
                             cudaStream_t st);
 cudaError_t sl2_launch_append(const Sl2Dev &d, int s, const double *y3_dev, const double *xp7_dev,
                               const uint8_t *patch_rows16_dev, const double *Pcol_dev, cudaStream_t st);
+// one step record per stream of [stream_lo, stream_lo + stream_cnt) into ring row step % d.rec_depth; launched after
+// the cull of the fused step (records.cu)
+cudaError_t sl2_launch_records(const Sl2Dev &d, int stream_lo, int stream_cnt, int64_t step, cudaStream_t st);
 size_t sl2_update_smem_bytes(const Sl2Dev &d);
 cudaError_t sl2_configure_search(const Sl2Dev &d);  // per context: dynamic smem opt-in
 cudaError_t sl2_configure_update(const Sl2Dev &d);

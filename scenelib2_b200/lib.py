@@ -58,6 +58,7 @@ EXPORTS = [
     "sl2_smoe_search_patch", "sl2_measure_partial_features",
     "sl2_get_features", "sl2_get_feature_jacobians", "sl2_enable_timing", "sl2_last_step_times", "sl2_last_update_times", "sl2_launch_count",
     "sl2_snapshot_layout", "sl2_snapshot_bytes", "sl2_save_streams", "sl2_load_streams", "sl2_save_streams_dev", "sl2_load_streams_dev",
+    "sl2_enable_records", "sl2_get_records", "sl2_get_records_dev",
 ]
 
 SL2_SNAPSHOT_MAGIC = 0x53324C53
@@ -138,6 +139,25 @@ def read_snapshot(blob):
     return out
 
 
+SL2_MAX_RECORDS = 4096   # records kept per stream at most (sl2_enable_records)
+
+
+class Sl2StepRecord(C.Structure):
+    """sl2_step_record: one camera stream's record of one fused step (256 bytes)."""
+    _fields_ = [
+        ("step", C.c_int64), ("nfeat", C.c_int32), ("nvisible", C.c_int32), ("nsel", C.c_int32), ("nmeas", C.c_int32),
+        ("nculled", C.c_int32), ("m", C.c_int32), ("nis", C.c_double), ("logdet_s", C.c_double),
+        ("xv", C.c_double * 13), ("pxx_diag", C.c_double * 13),
+    ]
+
+
+# the same record as a NumPy structured dtype: Context.records returns arrays of it
+STEP_RECORD_DTYPE = np.dtype([
+    ("step", np.int64), ("nfeat", np.int32), ("nvisible", np.int32), ("nsel", np.int32), ("nmeas", np.int32),
+    ("nculled", np.int32), ("m", np.int32), ("nis", np.float64), ("logdet_s", np.float64),
+    ("xv", np.float64, (13,)), ("pxx_diag", np.float64, (13,)),
+])
+
 _lib = None
 
 
@@ -189,6 +209,9 @@ def load():
         L.sl2_load_streams.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_size_t]
         L.sl2_save_streams_dev.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_size_t]
         L.sl2_load_streams_dev.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_size_t]
+        L.sl2_enable_records.argtypes = [C.c_void_p, C.c_int32]
+        L.sl2_get_records.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
+        L.sl2_get_records_dev.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
         _lib = L
     return _lib
 
@@ -554,6 +577,29 @@ class Context:
 
     def load_streams_dev(self, lo, cnt, dev_ptr, stride):
         self._ck(self.L.sl2_load_streams_dev(self.h, lo, cnt, dev_ptr, stride))
+
+    # ---- step records ---------------------------------------------------------------------------
+    def enable_records(self, depth):
+        """sl2_enable_records: keep the last `depth` step records of every stream (0 = off); restarts `step` at 0."""
+        self._ck(self.L.sl2_enable_records(self.h, depth))
+        self._rec_depth = depth
+
+    def records(self, lo=0, cnt=None, max=None):
+        """The most recent step records of the streams [lo, lo + cnt) (default: to the last stream), oldest first, as a
+        structured array of STEP_RECORD_DTYPE of shape [cnt, k], k = min(max, steps recorded, depth); max defaults to
+        the depth."""
+        if cnt is None:
+            cnt = self.cfg.num_streams - lo
+        if max is None:
+            max = getattr(self, "_rec_depth", 0) or 1
+        out = np.zeros((cnt if cnt > 0 else 0, max if max > 0 else 0), STEP_RECORD_DTYPE)  # bad sizes: refused by the C call
+        k = self._ck(self.L.sl2_get_records(self.h, lo, cnt, max, out.ctypes.data))
+        return out[:, :k]
+
+    def records_dev(self, lo, cnt, max, dev_ptr):
+        """sl2_get_records_dev: the same records into device memory at dev_ptr (record i * max + j, 8-byte aligned),
+        asynchronous on the context's stream.  Returns k."""
+        return self._ck(self.L.sl2_get_records_dev(self.h, lo, cnt, max, dev_ptr))
 
 
 def config_for_scene(sc, num_streams=1, frame_slots=1, device=0, max_features=None,
