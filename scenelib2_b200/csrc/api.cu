@@ -291,21 +291,9 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   ALLOC(d.P, B * d.ld * d.ld);
   ALLOC(d.G, B * d.mmax * d.ldg);
   ALLOC(d.nfeat, B);
-  ALLOC(d.xp_org, B * N * 7);
-  ALLOC(d.attempted, B * N);
-  ALLOC(d.successful, B * N);
-  ALLOC(d.h, B * N * 2);
-  ALLOC(d.S, B * N * 4);
-  ALLOC(d.Rvar, B * N);
-  ALLOC(d.dh_dxp, B * N * 14);
-  ALLOC(d.dh_dy, B * N * 6);
-  ALLOC(d.sel_rank, B * N);
-  ALLOC(d.z_uv, B * N * 2);
-  ALLOC(d.found, B * N);
-  ALLOC(d.best, B * N);
-  ALLOC(d.job_feat, B * N);
-  ALLOC(d.job_centre, B * N * 2);
-  ALLOC(d.job_puinv, B * N * 3);
+#define SL2_ALLOC(T, name, per, by, reset) ALLOC(d.name, B * N * per);
+  SL2_STREAM_ARRAYS(SL2_ALLOC)
+#undef SL2_ALLOC
   ALLOC(d.nsel, B);
   ALLOC(d.nvisible, B);
   ALLOC(d.nmeas, B);
@@ -1330,8 +1318,8 @@ static int snap_validate(sl2_ctx *c, const uint8_t *blob, size_t stride, bool in
   if (index) {
     for (int f = 0; f < h.nfeat; ++f) {
       int32_t r, j;
-      memcpy(&r, blob + L.field[SL2_SNAP_SEL_RANK] + 4 * (size_t)f, 4);
-      memcpy(&j, blob + L.field[SL2_SNAP_JOB_FEAT] + 4 * (size_t)f, 4);
+      memcpy(&r, blob + L.field[SL2_FIELD_sel_rank] + 4 * (size_t)f, 4);
+      memcpy(&j, blob + L.field[SL2_FIELD_job_feat] + 4 * (size_t)f, 4);
       // the same rules as snap_check_kernel: a job below nsel may be empty, the cull writes job slot sel_rank
       if (!(r == -1 || (r >= 0 && r < h.nsel && r < h.nfeat)) || !(f < h.nsel ? (j >= -1 && j < h.nfeat) : j == -1))
         return fail(c, SL2_ERR_ARG, who + ": sel_rank or job_feat out of range");

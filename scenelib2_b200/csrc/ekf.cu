@@ -685,23 +685,14 @@ __global__ void __launch_bounds__(256) cull_kernel(const Sl2Dev d, int stream_lo
     for (int i = 0; i < nf; ++i) {
       const int k = keep[i];
       if (k < 0 || k == i) continue;
-      for (int e = 0; e < 7; ++e) d.xp_org[(fb + k) * 7 + e] = d.xp_org[(fb + i) * 7 + e];
-      d.attempted[fb + k] = d.attempted[fb + i];
-      d.successful[fb + k] = d.successful[fb + i];
       for (int e = 0; e < box16; ++e)
         d.patches[(fb + k) * box16 + e] = d.patches[(fb + i) * box16 + e];
-      for (int e = 0; e < 2; ++e) {
-        d.h[(fb + k) * 2 + e] = d.h[(fb + i) * 2 + e];
-        d.z_uv[(fb + k) * 2 + e] = d.z_uv[(fb + i) * 2 + e];
-      }
-      for (int e = 0; e < 4; ++e) d.S[(fb + k) * 4 + e] = d.S[(fb + i) * 4 + e];
-      // Feature::dh_by_dxv_ / dh_by_dy_ / R_ move with the Feature object in the reference
-      for (int e = 0; e < 14; ++e) d.dh_dxp[(fb + k) * 14 + e] = d.dh_dxp[(fb + i) * 14 + e];
-      for (int e = 0; e < 6; ++e) d.dh_dy[(fb + k) * 6 + e] = d.dh_dy[(fb + i) * 6 + e];
-      d.Rvar[fb + k] = d.Rvar[fb + i];
-      d.best[fb + k] = d.best[fb + i];
-      d.sel_rank[fb + k] = d.sel_rank[fb + i];
-      d.found[fb + k] = d.found[fb + i];
+      // every per-feature record moves with the Feature object, as in the reference
+#define SL2_MOVE(T, name, per, by, reset) \
+  if (by == SL2_BY_FEATURE)               \
+    for (int e = 0; e < per; ++e) d.name[(fb + k) * per + e] = d.name[(fb + i) * per + e];
+      SL2_STREAM_ARRAYS(SL2_MOVE)
+#undef SL2_MOVE
     }
     // the job list of this step indexes the old feature numbering: rebuild it from the compacted ranks
     for (int r = 0; r < d.Nmax; ++r) d.job_feat[fb + r] = -1;
@@ -750,17 +741,12 @@ __global__ void __launch_bounds__(256) append_kernel(const Sl2Dev d, int s, cons
   const int box16 = d.box * 16;
   for (int e = tid; e < box16; e += blockDim.x) d.patches[f * box16 + e] = patch_rows16[e];
   if (tid == 0) {
-    d.attempted[f] = 0;
-    d.successful[f] = 0;
-    d.sel_rank[f] = -1;
-    d.found[f] = 0;
-    d.best[f] = 0.0;
-    d.h[f * 2] = d.h[f * 2 + 1] = 0.0;
-    d.z_uv[f * 2] = d.z_uv[f * 2 + 1] = 0;
-    for (int e = 0; e < 4; ++e) d.S[f * 4 + e] = 0.0;
-    for (int e = 0; e < 14; ++e) d.dh_dxp[f * 14 + e] = 0.0;
-    for (int e = 0; e < 6; ++e) d.dh_dy[f * 6 + e] = 0.0;
-    d.Rvar[f] = 0.0;
+    // every per-feature record but xp_org (written above) starts at its reset value
+#define SL2_RESET(T, name, per, by, reset)                          \
+  if (by == SL2_BY_FEATURE && SL2_FIELD_##name != SL2_FIELD_xp_org) \
+    for (int e = 0; e < per; ++e) d.name[f * per + e] = (T)(reset);
+    SL2_STREAM_ARRAYS(SL2_RESET)
+#undef SL2_RESET
   }
   __syncthreads();
   if (tid == 0) d.nfeat[s] = nf + 1;

@@ -24,6 +24,39 @@ static_assert(sizeof(Sl2StreamCam) % sizeof(double) == 0, "rows are copied as do
 __device__ __forceinline__ int stream_width(const Sl2StreamCam &c) { return (int)c.cam[0]; }
 __device__ __forceinline__ int stream_height(const Sl2StreamCam &c) { return (int)c.cam[1]; }
 
+// The per-stream arrays with one record of `per` elements of type T per map feature (SL2_BY_FEATURE) or per
+// measurement job (SL2_BY_JOB), each [B][Nmax][per], in snapshot section order (include/sl2b200.h).  Everything that
+// handles all of them expands this one table: the Sl2Dev members, their allocation, the snapshot sections, the cull
+// (which moves the SL2_BY_FEATURE records of a kept feature) and the append.  `reset` is what the append starts a new
+// feature with and what a load writes beyond the map; sl2_create zero-fills.
+enum { SL2_BY_FEATURE, SL2_BY_JOB };
+//      X(type,    name,       per, indexed by,     reset)
+#define SL2_STREAM_ARRAYS(X)                                                                                    \
+  X(double,  xp_org,      7, SL2_BY_FEATURE, 0)                                                                 \
+  X(int,     attempted,   1, SL2_BY_FEATURE, 0)                                                                 \
+  X(int,     successful,  1, SL2_BY_FEATURE, 0)                                                                 \
+  /* per step, per feature */                                                                                   \
+  X(double,  h,           2, SL2_BY_FEATURE, 0)                                                                 \
+  X(double,  S,           4, SL2_BY_FEATURE, 0)  /* col-major */                                                \
+  X(double,  Rvar,        1, SL2_BY_FEATURE, 0)                                                                 \
+  X(double,  dh_dxp,     14, SL2_BY_FEATURE, 0)  /* [2][7] row-major */                                         \
+  X(double,  dh_dy,       6, SL2_BY_FEATURE, 0)  /* [2][3] row-major */                                         \
+  X(int,     sel_rank,    1, SL2_BY_FEATURE, -1) /* rank in the selected list or -1 */                          \
+  X(int,     z_uv,        2, SL2_BY_FEATURE, 0)                                                                 \
+  X(uint8_t, found,       1, SL2_BY_FEATURE, 0)  /* 1 = successful measurement this step */                     \
+  X(double,  best,        1, SL2_BY_FEATURE, 0)                                                                 \
+  /* per step, per job (rank order = measurement order) */                                                      \
+  X(int,     job_feat,    1, SL2_BY_JOB,     -1) /* feature index of job r, -1 = none */                        \
+  X(double,  job_centre,  2, SL2_BY_JOB,     0)                                                                 \
+  X(double,  job_puinv,   3, SL2_BY_JOB,     0)
+
+// the snapshot section of each array: L.field[SL2_FIELD_sel_rank]
+#define SL2_FIELD_INDEX(T, name, per, by, reset) SL2_FIELD_##name,
+enum { SL2_STREAM_ARRAYS(SL2_FIELD_INDEX) SL2_NUM_FIELDS };
+#undef SL2_FIELD_INDEX
+// a new array changes the blob format: the header's format list, SL2_SNAPSHOT_VERSION and lib.SNAPSHOT_FIELDS
+static_assert(SL2_NUM_FIELDS == SL2_SNAPSHOT_FIELDS, "every per-stream array is a snapshot section");
+
 // Device view of one context: everything the kernels need, passed by value.
 struct Sl2Dev {
   // geometry / constants
@@ -47,23 +80,9 @@ struct Sl2Dev {
   double *P;         // [B][ld][ld] col-major, both triangles kept consistent
   double *G;         // [B][mmax][ldg]  row-major scratch: [ S | H*P | nu ]
   int *nfeat;        // [B]
-  double *xp_org;    // [B][Nmax][7]
-  int *attempted;    // [B][Nmax]
-  int *successful;   // [B][Nmax]
-  // per-step, per-feature (indexed by feature)
-  double *h;       // [B][Nmax][2]
-  double *S;       // [B][Nmax][4] col-major
-  double *Rvar;    // [B][Nmax]
-  double *dh_dxp;  // [B][Nmax][2][7] row-major
-  double *dh_dy;   // [B][Nmax][2][3] row-major
-  int *sel_rank;   // [B][Nmax]  rank in the selected list or -1
-  int *z_uv;       // [B][Nmax][2]
-  uint8_t *found;  // [B][Nmax]  1 = successful measurement this step
-  double *best;    // [B][Nmax]
-  // per-step, per job (rank order = measurement order)
-  int *job_feat;       // [B][Nmax]  feature index of job r, -1 = none
-  double *job_centre;  // [B][Nmax][2]
-  double *job_puinv;   // [B][Nmax][3]
+#define SL2_MEMBER(T, name, per, by, reset) T *name;
+  SL2_STREAM_ARRAYS(SL2_MEMBER)  // [B][Nmax][per] each
+#undef SL2_MEMBER
   int *nsel;           // [B]
   int *nvisible;       // [B]
   int *nmeas;          // [B]  successful measurements of the last step
@@ -76,6 +95,7 @@ struct Sl2Dev {
   sl2_step_record *rec;  // [B][rec_depth]  ring: the record of step t of stream s is rec[s][t % rec_depth]
   int rec_depth;         // 0 = records off
 };
+static_assert(sizeof(Sl2Dev) == 336, "Sl2Dev is every kernel's by-value parameter: a new member changes every launch");
 
 #define SL2_MAX_PANELS 16  // 16-row panels of S: m <= 2 * SL2_MAX_MEASURED = 256
 static_assert(2 * SL2_MAX_MEASURED <= 16 * SL2_MAX_PANELS, "every panel of S must fit the panel tables");
@@ -192,19 +212,12 @@ cudaError_t sl2_launch_detect(const Sl2Dev &d, int stream, int slot, int n, cons
                               int *out_uv_dev, double *out_ev_dev, void *scratch_dev, cudaStream_t st);
 
 // ---- stream snapshots (snapshot.cu): the blob format of include/sl2b200.h --------------------------------------
-// The per-feature sections of a blob, in blob order: each is the stream's first nfeat records of one Sl2Dev array
-// of `per` elements of `esz` bytes per feature (x, P and the templates are laid out separately).
+// Section field[k] of a blob is the stream's first nfeat records of array k of SL2_STREAM_ARRAYS (x, P and the
+// templates are laid out separately).
 struct Sl2SnapLayout {
   size_t x, P, field[SL2_SNAPSHOT_FIELDS], templates, total;  // byte offsets in the blob, total size
 };
 __host__ __device__ inline size_t sl2_snap_align8(size_t b) { return (b + 7) & ~(size_t)7; }
-__host__ __device__ inline void sl2_snap_field(int k, int *per, int *esz) {
-  // xp_org attempted successful h S Rvar dh_dxp dh_dy sel_rank z_uv found best job_feat job_centre job_puinv
-  const int P_[SL2_SNAPSHOT_FIELDS] = {7, 1, 1, 2, 4, 1, 14, 6, 1, 2, 1, 1, 1, 2, 3};
-  const int E_[SL2_SNAPSHOT_FIELDS] = {8, 4, 4, 8, 8, 8, 8, 8, 4, 4, 1, 8, 4, 8, 8};
-  *per = P_[k];
-  *esz = E_[k];
-}
 __host__ __device__ inline Sl2SnapLayout sl2_snap_layout(int nfeat, int box) {
   Sl2SnapLayout L;
   const size_t n = SL2_NXV + 3 * (size_t)nfeat;
@@ -213,18 +226,16 @@ __host__ __device__ inline Sl2SnapLayout sl2_snap_layout(int nfeat, int box) {
   o += sl2_snap_align8(8 * n);
   L.P = o;
   o += 8 * n * n;
-  for (int k = 0; k < SL2_SNAPSHOT_FIELDS; ++k) {
-    int per, esz;
-    sl2_snap_field(k, &per, &esz);
-    L.field[k] = o;
-    o += sl2_snap_align8((size_t)nfeat * per * esz);
-  }
+#define SL2_SECTION(T, name, per, by, reset) \
+  L.field[SL2_FIELD_##name] = o;             \
+  o += sl2_snap_align8((size_t)nfeat * per * sizeof(T));
+  SL2_STREAM_ARRAYS(SL2_SECTION)
+#undef SL2_SECTION
   L.templates = o;
   o += sl2_snap_align8((size_t)nfeat * box * box);
   L.total = o;
   return L;
 }
-enum { SL2_SNAP_SEL_RANK = 8, SL2_SNAP_JOB_FEAT = 12 };  // the index fields, set to -1 beyond the map by a load
 
 // what the host validated for one blob of a load: the kernels take sizes and counts from here, never from the blob
 struct Sl2SnapLoad {

@@ -12,27 +12,6 @@ constexpr int SNAP_WARPS = SNAP_THREADS / 32;
 static_assert(sizeof(sl2_snapshot_header) == 128, "the header is 16 words");
 static_assert(sizeof(Sl2SnapLoad) % 8 == 0, "load records are copied as one array");
 
-// the Sl2Dev array behind per-feature section k of sl2_snap_field
-__device__ __forceinline__ uint8_t *snap_field_base(const Sl2Dev &d, int k) {
-  switch (k) {
-    case 0: return reinterpret_cast<uint8_t *>(d.xp_org);
-    case 1: return reinterpret_cast<uint8_t *>(d.attempted);
-    case 2: return reinterpret_cast<uint8_t *>(d.successful);
-    case 3: return reinterpret_cast<uint8_t *>(d.h);
-    case 4: return reinterpret_cast<uint8_t *>(d.S);
-    case 5: return reinterpret_cast<uint8_t *>(d.Rvar);
-    case 6: return reinterpret_cast<uint8_t *>(d.dh_dxp);
-    case 7: return reinterpret_cast<uint8_t *>(d.dh_dy);
-    case 8: return reinterpret_cast<uint8_t *>(d.sel_rank);
-    case 9: return reinterpret_cast<uint8_t *>(d.z_uv);
-    case 10: return d.found;
-    case 11: return reinterpret_cast<uint8_t *>(d.best);
-    case 12: return reinterpret_cast<uint8_t *>(d.job_feat);
-    case 13: return reinterpret_cast<uint8_t *>(d.job_centre);
-    default: return reinterpret_cast<uint8_t *>(d.job_puinv);
-  }
-}
-
 // dst[r] = src[r] for r < cnt by one warp, four independent loads in flight per lane before their stores
 __device__ __forceinline__ void warp_copy(const double *__restrict__ src, double *__restrict__ dst, int cnt,
                                           int lane) {
@@ -54,17 +33,6 @@ __device__ __forceinline__ void copy_fill(const T *__restrict__ src, T *__restri
   for (size_t e = t; e < len; e += nt) dst[e] = e < cnt ? src[e] : fill;
 }
 
-// one per-feature section: `cnt` elements of esz bytes, `len` elements written (the rest of len is `fill`)
-__device__ __forceinline__ void copy_section(const uint8_t *src, uint8_t *dst, int esz, size_t cnt, size_t len,
-                                             int fill, size_t t, size_t nt) {
-  if (esz == 8)
-    copy_fill(reinterpret_cast<const double *>(src), reinterpret_cast<double *>(dst), cnt, len, 0.0, t, nt);
-  else if (esz == 4)
-    copy_fill(reinterpret_cast<const int *>(src), reinterpret_cast<int *>(dst), cnt, len, fill, t, nt);
-  else
-    copy_fill(src, dst, cnt, len, (uint8_t)0, t, nt);
-}
-
 __global__ void __launch_bounds__(SNAP_THREADS) pack_streams_kernel(const Sl2Dev d, int lo, uint8_t *buf,
                                                                     size_t stride) {
   const int i = blockIdx.x, s = lo + i, tid = threadIdx.x, lane = tid & 31;
@@ -80,13 +48,11 @@ __global__ void __launch_bounds__(SNAP_THREADS) pack_streams_kernel(const Sl2Dev
   const size_t t = (size_t)blockIdx.y * SNAP_THREADS + tid, nt = (size_t)gridDim.y * SNAP_THREADS;
   copy_fill(d.x + (size_t)s * ld, reinterpret_cast<double *>(blob + L.x), (size_t)n, (size_t)n, 0.0, t, nt);
   const size_t fb = (size_t)s * d.Nmax;
-  for (int k = 0; k < SL2_SNAPSHOT_FIELDS; ++k) {
-    int per, esz;
-    sl2_snap_field(k, &per, &esz);
-    const size_t cnt = (size_t)nf * per;
-    copy_section(snap_field_base(d, k) + fb * per * esz, blob + L.field[k], esz, cnt,
-                 sl2_snap_align8(cnt * esz) / esz, 0, t, nt);
-  }
+#define SL2_PACK(T, name, per, by, reset)                                                                       \
+  copy_fill(d.name + fb * per, reinterpret_cast<T *>(blob + L.field[SL2_FIELD_##name]), (size_t)nf * per,       \
+            sl2_snap_align8((size_t)nf * per * sizeof(T)) / sizeof(T), (T)0, t, nt);
+  SL2_STREAM_ARRAYS(SL2_PACK)
+#undef SL2_PACK
   // templates: rows of box bytes out of the device's 16-byte rows
   const int box = d.box, bb = box * box;
   const uint8_t *pt = d.patches + fb * box * 16;
@@ -138,8 +104,8 @@ __global__ void __launch_bounds__(SNAP_THREADS) snap_check_kernel(const Sl2Dev d
   const Sl2SnapLoad q = ld[blockIdx.x];
   const Sl2SnapLayout L = sl2_snap_layout(q.nfeat, d.box);
   const uint8_t *blob = buf + (size_t)blockIdx.x * stride;
-  const int *rank = reinterpret_cast<const int *>(blob + L.field[SL2_SNAP_SEL_RANK]);
-  const int *job = reinterpret_cast<const int *>(blob + L.field[SL2_SNAP_JOB_FEAT]);
+  const int *rank = reinterpret_cast<const int *>(blob + L.field[SL2_FIELD_sel_rank]);
+  const int *job = reinterpret_cast<const int *>(blob + L.field[SL2_FIELD_job_feat]);
   int ok = 1;
   for (int f = threadIdx.x; f < q.nfeat; f += blockDim.x) {
     const int r = rank[f], j = job[f];
@@ -168,13 +134,11 @@ __global__ void __launch_bounds__(SNAP_THREADS) unpack_streams_kernel(const Sl2D
   const size_t t = (size_t)blockIdx.y * SNAP_THREADS + tid, nt = (size_t)gridDim.y * SNAP_THREADS;
   copy_fill(reinterpret_cast<const double *>(blob + L.x), d.x + (size_t)s * ld, (size_t)n, (size_t)ld, 0.0, t, nt);
   const size_t fb = (size_t)s * d.Nmax;
-  for (int k = 0; k < SL2_SNAPSHOT_FIELDS; ++k) {
-    int per, esz;
-    sl2_snap_field(k, &per, &esz);
-    const int fill = (k == SL2_SNAP_SEL_RANK || k == SL2_SNAP_JOB_FEAT) ? -1 : 0;
-    copy_section(blob + L.field[k], snap_field_base(d, k) + fb * per * esz, esz, (size_t)nf * per,
-                 (size_t)d.Nmax * per, fill, t, nt);
-  }
+#define SL2_UNPACK(T, name, per, by, reset)                                                                     \
+  copy_fill(reinterpret_cast<const T *>(blob + L.field[SL2_FIELD_##name]), d.name + fb * per, (size_t)nf * per, \
+            (size_t)d.Nmax * per, (T)(reset), t, nt);
+  SL2_STREAM_ARRAYS(SL2_UNPACK)
+#undef SL2_UNPACK
   const int box = d.box, b16 = box * 16;
   uint8_t *pt = d.patches + fb * b16;
   const uint8_t *tp = blob + L.templates;

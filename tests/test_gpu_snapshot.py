@@ -171,8 +171,9 @@ def _c4_scenes(count, n_frames, first=0):
 @pytest.mark.gpu
 def test_round_trip_eight_c4_streams():
     """8 C4 streams, 3 steps, all saved and loaded into a fresh context of the same config: every getter is
-    bit-identical; the blob agrees with the getters field by field; 5 more steps on both stay bit-identical and the
-    blobs saved then are byte-identical."""
+    bit-identical; every section of the blob agrees with the getters or, for the job list and the search results,
+    with a staged search of the last frame; 5 more steps on both stay bit-identical and the blobs saved then are
+    byte-identical."""
     scenes = _c4_scenes(8, 8)
     a = ctx_from_scenes(scenes, frame_slots=2)
     for t in range(3):
@@ -189,6 +190,22 @@ def test_round_trip_eight_c4_streams():
         assert (snap["S"] == r["S"]).all() and (snap["z_uv"] == r["z"]).all()
         assert (snap["xp_org"] == sc.xp_org).all() and (snap["templates"] == sc.patches).all()
         assert snap["nsel"] == (r["select_rank"] >= 0).sum() > 0 and snap["nfeat"] == sc.n_features
+        nf, nsel = snap["nfeat"], snap["nsel"]
+        J = r["dh_dxv"].reshape(nf, 13, 2).transpose(0, 2, 1)  # each feature's column-major 2 x 13
+        assert (snap["dh_dxp"] == J[:, :, :7]).all() and (J[:, :, 7:] == 0).all()
+        assert (snap["dh_dy"] == r["dh_dy"].reshape(nf, 3, 2).transpose(0, 2, 1)).all()
+        assert (snap["Rvar"] == r["R"][:, 0]).all() and (snap["Rvar"] == r["R"][:, 3]).all()
+        assert (snap["found"] == ((r["flags"] & 2) >> 1)).all()
+        jobs = np.full(nf, -1, np.int32)
+        sel = np.flatnonzero(r["select_rank"] >= 0)
+        jobs[r["select_rank"][sel]] = sel
+        assert (snap["job_feat"] == jobs).all()
+        # no cull in these steps (nfeat is the scene's), so the job list is the one the last step searched: the staged
+        # search of its frame (slot 0) with that list reproduces the matches
+        feat = snap["job_feat"][:nsel]
+        u, v, found, best = a.patch_search(s, 0, feat, snap["job_centre"][:nsel], snap["job_puinv"][:nsel])
+        assert (found == snap["found"][feat]).all() and best.tobytes() == snap["best"][feat].tobytes()
+        assert (np.stack([u, v], 1) == snap["z_uv"][feat]).all()
     b = _blank_ctx(scenes[0], 8)
     b.load_streams(blobs)
     for s in range(8):
