@@ -195,22 +195,25 @@ size_t sl2_detect_scratch_bytes(const Sl2Dev &d, int n) {
 }
 
 cudaError_t sl2_launch_detect(const Sl2Dev &d, int stream, int slot, int n, const int *regions_dev,
-                              int *out_uv_dev, double *out_ev_dev, void *scratch_dev, cudaStream_t st) {
+                              int *out_uv_dev, double *out_ev_dev, void *scratch_dev, Sl2Queue q) {
   if (n <= 0) return cudaSuccess;
   const int max_tiles = ((d.W + DT - 1) / DT) * ((d.H + DT - 1) / DT);
   double *part_ev = reinterpret_cast<double *>(scratch_dev);
   int *part_idx = reinterpret_cast<int *>(part_ev + (size_t)n * max_tiles);
   const dim3 grid(max_tiles, n);
+  cudaError_t e;
   switch (d.box) {
     case 11:
-      detect_tiles_kernel<11><<<grid, DTHREADS, 0, st>>>(d, stream, slot, regions_dev, max_tiles, part_ev, part_idx);
+      e = sl2_launch_kernel(detect_tiles_kernel<11>, grid, dim3(DTHREADS), 0, q, false, d, stream, slot, regions_dev,
+                            max_tiles, part_ev, part_idx);
       break;
     case 15:
-      detect_tiles_kernel<15><<<grid, DTHREADS, 0, st>>>(d, stream, slot, regions_dev, max_tiles, part_ev, part_idx);
+      e = sl2_launch_kernel(detect_tiles_kernel<15>, grid, dim3(DTHREADS), 0, q, false, d, stream, slot, regions_dev,
+                            max_tiles, part_ev, part_idx);
       break;
     default: return cudaErrorInvalidValue;
   }
-  detect_reduce_kernel<<<n, 128, 0, st>>>(d, stream, regions_dev, (d.box - 1) / 2, max_tiles, part_ev, part_idx, out_uv_dev,
-                                          out_ev_dev);
-  return cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  return sl2_launch_kernel(detect_reduce_kernel, dim3(n), dim3(128), 0, q, false, d, stream, regions_dev,
+                           (d.box - 1) / 2, max_tiles, part_ev, part_idx, out_uv_dev, out_ev_dev);
 }

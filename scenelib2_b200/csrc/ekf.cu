@@ -755,17 +755,17 @@ __global__ void __launch_bounds__(256) append_kernel(const Sl2Dev d, int s, cons
 }  // namespace
 
 cudaError_t sl2_launch_append(const Sl2Dev &d, int s, const double *y3_dev, const double *xp7_dev,
-                              const uint8_t *patch_rows16_dev, const double *Pcol_dev, cudaStream_t st) {
-  append_kernel<<<1, 256, 0, st>>>(d, s, y3_dev, xp7_dev, patch_rows16_dev, Pcol_dev);
-  return cudaGetLastError();
+                              const uint8_t *patch_rows16_dev, const double *Pcol_dev, Sl2Queue q) {
+  return sl2_launch_kernel(append_kernel, dim3(1), dim3(256), 0, q, false, d, s, y3_dev, xp7_dev, patch_rows16_dev,
+                           Pcol_dev);
 }
 
 cudaError_t sl2_launch_predict(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *u3_dev,
-                               int do_predict, int do_measure, cudaStream_t st) {
+                               int do_predict, int do_measure, Sl2Queue q) {
   if (stream_cnt <= 0) return cudaSuccess;
   // 128 threads, one feature each per pass over the map (two passes at SL2_MAX_FEATURES); the kernel needs ~255
   // registers per thread, so 128-thread CTAs are what lets two streams share an SM
-  return sl2_launch_kernel(predict_kernel, dim3(stream_cnt), dim3(128), 0, st, sl2_use_pdl(stream_cnt), d,
+  return sl2_launch_kernel(predict_kernel, dim3(stream_cnt), dim3(128), 0, q, sl2_use_pdl(stream_cnt), d,
                            stream_lo, u3_dev, do_predict, do_measure);
 }
 
@@ -773,15 +773,14 @@ cudaError_t sl2_launch_predict(const Sl2Dev &d, int stream_lo, int stream_cnt, c
 cudaError_t sl2_launch_particle_predict(const Sl2Dev &d, int s, int F, int Kmax, const int *K_dev,
                                         const double *ypi, const double *Pxy, const double *Pyy,
                                         const double *lambda, double *h, double *sinv3, double *detS,
-                                        cudaStream_t st) {
+                                        Sl2Queue q) {
   if (F <= 0) return cudaSuccess;
-  particle_predict_kernel<<<F, 128, 0, st>>>(d, s, Kmax, K_dev, ypi, Pxy, Pyy, lambda, h, sinv3, detS);
-  return cudaGetLastError();
+  return sl2_launch_kernel(particle_predict_kernel, dim3(F), dim3(128), 0, q, false, d, s, Kmax, K_dev, ypi, Pxy, Pyy,
+                           lambda, h, sinv3, detS);
 }
 
-cudaError_t sl2_launch_cull(const Sl2Dev &d, int stream_lo, int stream_cnt, int force_index,
-                            cudaStream_t st) {
+cudaError_t sl2_launch_cull(const Sl2Dev &d, int stream_lo, int stream_cnt, int force_index, Sl2Queue q) {
   if (stream_cnt <= 0) return cudaSuccess;
-  return sl2_launch_kernel(cull_kernel, dim3(stream_cnt), dim3(256), 0, st, sl2_use_pdl(stream_cnt), d,
+  return sl2_launch_kernel(cull_kernel, dim3(stream_cnt), dim3(256), 0, q, sl2_use_pdl(stream_cnt), d,
                            stream_lo, force_index);
 }

@@ -91,9 +91,8 @@ __global__ void __launch_bounds__(128) particle_kernel(int Kmax, const int *__re
 cudaError_t sl2_launch_particles(int F, int Kmax, const int *K_dev, const double *h, const double *sinv3,
                                  const double *detS, const double *lambda, const int *z_uv, const uint8_t *found,
                                  double prune_threshold, double *prob, uint8_t *keep, double *cumulative,
-                                 double *mean_var, int *left_out, cudaStream_t st) {
+                                 double *mean_var, int *left_out, Sl2Queue q) {
   if (F <= 0) return cudaSuccess;
-  particle_kernel<<<F, 128, 0, st>>>(Kmax, K_dev, h, sinv3, detS, lambda, z_uv, found, prune_threshold, prob, keep,
-                                     cumulative, mean_var, left_out);
-  return cudaGetLastError();
+  return sl2_launch_kernel(particle_kernel, dim3(F), dim3(128), 0, q, false, Kmax, K_dev, h, sinv3, detS, lambda, z_uv,
+                           found, prune_threshold, prob, keep, cumulative, mean_var, left_out);
 }

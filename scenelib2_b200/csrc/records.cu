@@ -62,8 +62,8 @@ __global__ void __launch_bounds__(REC_THREADS) record_kernel(const Sl2Dev d, int
 
 }  // namespace
 
-cudaError_t sl2_launch_records(const Sl2Dev &d, int stream_lo, int stream_cnt, int64_t step, cudaStream_t st) {
+cudaError_t sl2_launch_records(const Sl2Dev &d, int stream_lo, int stream_cnt, int64_t step, Sl2Queue q) {
   if (stream_cnt <= 0) return cudaSuccess;
-  return sl2_launch_kernel(record_kernel, dim3(stream_cnt), dim3(REC_THREADS), 0, st, sl2_use_pdl(stream_cnt), d,
+  return sl2_launch_kernel(record_kernel, dim3(stream_cnt), dim3(REC_THREADS), 0, q, sl2_use_pdl(stream_cnt), d,
                            stream_lo, (long long)step);
 }

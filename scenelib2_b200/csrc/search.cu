@@ -484,23 +484,23 @@ size_t search_smem_bytes(const Sl2Dev &d) {
 
 template <int BOX, bool FILTER>
 cudaError_t launch_t(const Sl2Dev &d, const CUtensorMap &tmap, const SearchLaunch &L,
-                     const DumpPtrs &dump, cudaStream_t st) {
+                     const DumpPtrs &dump, Sl2Queue q) {
   const size_t smem = search_smem_bytes(d);
   const int groups = (L.jobs_per_stream + SL2_SEARCH_WARPS - 1) / SL2_SEARCH_WARPS;
   const int grid = groups * L.stream_cnt;
   if (grid <= 0) return cudaSuccess;
-  return sl2_launch_kernel(search_kernel<BOX, FILTER>, dim3(grid), dim3(SL2_SEARCH_WARPS * 32), smem, st,
+  return sl2_launch_kernel(search_kernel<BOX, FILTER>, dim3(grid), dim3(SL2_SEARCH_WARPS * 32), smem, q,
                            sl2_use_pdl(L.stream_cnt), tmap, d, L, dump);
 }
 
 cudaError_t launch_any(const Sl2Dev &d, const CUtensorMap &tmap, const SearchLaunch &L,
-                       const DumpPtrs &dump, cudaStream_t st) {
+                       const DumpPtrs &dump, Sl2Queue q) {
   const bool exact_all = dump.corr != nullptr;  // score dump: every candidate through the exact chain
   switch (d.box) {
     case 11:
-      return exact_all ? launch_t<11, false>(d, tmap, L, dump, st) : launch_t<11, true>(d, tmap, L, dump, st);
+      return exact_all ? launch_t<11, false>(d, tmap, L, dump, q) : launch_t<11, true>(d, tmap, L, dump, q);
     case 15:
-      return exact_all ? launch_t<15, false>(d, tmap, L, dump, st) : launch_t<15, true>(d, tmap, L, dump, st);
+      return exact_all ? launch_t<15, false>(d, tmap, L, dump, q) : launch_t<15, true>(d, tmap, L, dump, q);
     default: return cudaErrorInvalidValue;
   }
 }
@@ -526,25 +526,23 @@ cudaError_t sl2_configure_search(const Sl2Dev &d) {
   return e;
 }
 
-cudaError_t sl2_launch_search(const Sl2Dev &d, const CUtensorMap &tmap, const SearchLaunch &L,
-                              cudaStream_t st) {
+cudaError_t sl2_launch_search(const Sl2Dev &d, const CUtensorMap &tmap, const SearchLaunch &L, Sl2Queue q) {
   DumpPtrs none = {nullptr, nullptr, nullptr, nullptr, 0};
-  return launch_any(d, tmap, L, none, st);
+  return launch_any(d, tmap, L, none, q);
 }
 
+// one job (centre, puinv, feature index: device arrays of 2, 3 and 1) with every candidate's score dumped
 cudaError_t sl2_launch_score_map(const Sl2Dev &d, const CUtensorMap &tmap, int stream_id, int slot,
-                                 int feat, const double *cp, int *box_dev, double *corr_dev,
-                                 double *sd_dev, uint8_t *inside_dev, int cap, cudaStream_t st) {
-  // cp = device array: centre(2), puinv(3), then one int job_feat stored after them by the caller
+                                 const double *centre_dev, const double *puinv_dev, const int *feat_dev, int *box_dev,
+                                 double *corr_dev, double *sd_dev, uint8_t *inside_dev, int cap, Sl2Queue q) {
   SearchLaunch L = {};
-  L.job_centre = cp;
-  L.job_puinv = cp + 2;
-  L.job_feat = reinterpret_cast<const int *>(cp + 5);
+  L.job_centre = centre_dev;
+  L.job_puinv = puinv_dev;
+  L.job_feat = feat_dev;
   L.jobs_per_stream = 1;
   L.stream_lo = stream_id;
   L.stream_cnt = 1;
   L.slot = slot;
-  (void)feat;
   DumpPtrs dump = {corr_dev, sd_dev, inside_dev, box_dev, cap};
-  return launch_any(d, tmap, L, dump, st);
+  return launch_any(d, tmap, L, dump, q);
 }

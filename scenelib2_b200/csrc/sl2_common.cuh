@@ -137,22 +137,31 @@ __device__ __forceinline__ void pdl_prologue() {
 #define SL2_PDL_AUTO_STREAMS 2
 inline bool sl2_use_pdl(int stream_cnt) { return stream_cnt < SL2_PDL_AUTO_STREAMS; }
 
+// Where a launcher enqueues: the stream, and the context's launch counter (sl2_launch_count)
+struct Sl2Queue {
+  cudaStream_t stream;
+  int64_t *launches;
+};
+
 #ifdef __CUDACC__
-// one launch path for every kernel of the step: plain launch, or with the PDL attribute
+// one launch path for every kernel: plain launch, or with the PDL attribute (only for kernels that begin with
+// pdl_prologue()); a successful launch is counted
 template <typename... KArgs, typename... Args>
-inline cudaError_t sl2_launch_kernel(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+inline cudaError_t sl2_launch_kernel(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, Sl2Queue q,
                                      bool pdl, Args &&...args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
+  cfg.stream = q.stream;
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = at;
   cfg.numAttrs = pdl ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
+  if (e == cudaSuccess) ++*q.launches;
+  return e;
 }
 #endif
 
@@ -171,26 +180,23 @@ struct SearchLaunch {
   int scatter_to_features;   // 1: also write d.z_uv/found/best indexed by feature
 };
 
-cudaError_t sl2_launch_search(const Sl2Dev &d, const CUtensorMap &tmap, const SearchLaunch &L,
-                              cudaStream_t st);
+cudaError_t sl2_launch_search(const Sl2Dev &d, const CUtensorMap &tmap, const SearchLaunch &L, Sl2Queue q);
 cudaError_t sl2_launch_score_map(const Sl2Dev &d, const CUtensorMap &tmap, int stream_id, int slot,
-                                 int feat, const double *centre_puinv_dev /*5*/, int *box_dev,
-                                 double *corr_dev, double *sd_dev, uint8_t *inside_dev, int cap,
-                                 cudaStream_t st);
+                                 const double *centre_dev, const double *puinv_dev, const int *feat_dev, int *box_dev,
+                                 double *corr_dev, double *sd_dev, uint8_t *inside_dev, int cap, Sl2Queue q);
 cudaError_t sl2_launch_predict(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *u3_dev,
-                               int do_predict, int do_measure, cudaStream_t st);
+                               int do_predict, int do_measure, Sl2Queue q);
 // EKF update = 5 kernels (hp, chol, solve, syrk, finish); ev6 (optional) = 6 events recorded around them
 cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, int staged_m,
                               const int *st_feat, const double *st_Hxv, const double *st_Hy,
                               const double *st_R, const double *st_nu, int only_normalise,
-                              cudaStream_t st, cudaEvent_t *ev6 = nullptr, int *launches = nullptr);
-cudaError_t sl2_launch_cull(const Sl2Dev &d, int stream_lo, int stream_cnt, int force_index,
-                            cudaStream_t st);
+                              Sl2Queue q, cudaEvent_t *ev6 = nullptr);
+cudaError_t sl2_launch_cull(const Sl2Dev &d, int stream_lo, int stream_cnt, int force_index, Sl2Queue q);
 cudaError_t sl2_launch_append(const Sl2Dev &d, int s, const double *y3_dev, const double *xp7_dev,
-                              const uint8_t *patch_rows16_dev, const double *Pcol_dev, cudaStream_t st);
+                              const uint8_t *patch_rows16_dev, const double *Pcol_dev, Sl2Queue q);
 // one step record per stream of [stream_lo, stream_lo + stream_cnt) into ring row step % d.rec_depth; launched after
 // the cull of the fused step (records.cu)
-cudaError_t sl2_launch_records(const Sl2Dev &d, int stream_lo, int stream_cnt, int64_t step, cudaStream_t st);
+cudaError_t sl2_launch_records(const Sl2Dev &d, int stream_lo, int stream_cnt, int64_t step, Sl2Queue q);
 size_t sl2_update_smem_bytes(const Sl2Dev &d);
 cudaError_t sl2_configure_search(const Sl2Dev &d);  // per context: dynamic smem opt-in
 cudaError_t sl2_configure_update(const Sl2Dev &d);
@@ -198,18 +204,18 @@ cudaError_t sl2_configure_update(const Sl2Dev &d);
 cudaError_t sl2_launch_particle_predict(const Sl2Dev &d, int s, int F, int Kmax, const int *K_dev,
                                         const double *ypi, const double *Pxy, const double *Pyy,
                                         const double *lambda, double *h, double *sinv3, double *detS,
-                                        cudaStream_t st);
+                                        Sl2Queue q);
 size_t sl2_smoe_map_bytes(const Sl2Dev &d, int F);
 cudaError_t sl2_launch_smoe(const Sl2Dev &d, int s, int slot, int F, int Kmax, const int *K_dev, const int *feat_dev,
                             const double *centre_dev, const double *puinv_dev, double *map_dev, int *out_uv_dev,
-                            uint8_t *out_found_dev, double *out_best_dev, cudaStream_t st);
+                            uint8_t *out_found_dev, double *out_best_dev, Sl2Queue q);
 cudaError_t sl2_launch_particles(int F, int Kmax, const int *K_dev, const double *h, const double *sinv3,
                                  const double *detS, const double *lambda, const int *z_uv, const uint8_t *found,
                                  double prune_threshold, double *prob, uint8_t *keep, double *cumulative,
-                                 double *mean_var, int *left_out, cudaStream_t st);
+                                 double *mean_var, int *left_out, Sl2Queue q);
 size_t sl2_detect_scratch_bytes(const Sl2Dev &d, int n);
 cudaError_t sl2_launch_detect(const Sl2Dev &d, int stream, int slot, int n, const int *regions_dev,
-                              int *out_uv_dev, double *out_ev_dev, void *scratch_dev, cudaStream_t st);
+                              int *out_uv_dev, double *out_ev_dev, void *scratch_dev, Sl2Queue q);
 
 // ---- stream snapshots (snapshot.cu): the blob format of include/sl2b200.h --------------------------------------
 // Section field[k] of a blob is the stream's first nfeat records of array k of SL2_STREAM_ARRAYS (x, P and the
@@ -244,10 +250,10 @@ struct Sl2SnapLoad {
   int pad_[2];
 };
 // pack the streams [lo, lo + cnt) into blobs at buf + i * stride (nfeat read on the device, header written)
-cudaError_t sl2_launch_pack(const Sl2Dev &d, int lo, int cnt, uint8_t *buf, size_t stride, cudaStream_t st);
+cudaError_t sl2_launch_pack(const Sl2Dev &d, int lo, int cnt, uint8_t *buf, size_t stride, Sl2Queue q);
 // adds the number of blobs whose job_feat / sel_rank fail the index rules (with the validated counts) to *bad
 cudaError_t sl2_launch_snap_check(const Sl2Dev &d, int cnt, const Sl2SnapLoad *ld_dev, const uint8_t *buf,
-                                  size_t stride, int *bad, cudaStream_t st);
+                                  size_t stride, int *bad, Sl2Queue q);
 // unpack blob i into stream ld_dev[i].stream and reset what the blob does not cover
 cudaError_t sl2_launch_unpack(const Sl2Dev &d, int cnt, const Sl2SnapLoad *ld_dev, const uint8_t *buf, size_t stride,
-                              cudaStream_t st);
+                              Sl2Queue q);

@@ -199,17 +199,18 @@ size_t sl2_smoe_map_bytes(const Sl2Dev &d, int F) { return (size_t)F * d.W * d.H
 // stream's first template), all on one frame.  2 launches.
 cudaError_t sl2_launch_smoe(const Sl2Dev &d, int s, int slot, int F, int Kmax, const int *K_dev, const int *feat_dev,
                             const double *centre_dev, const double *puinv_dev, double *map_dev, int *out_uv_dev,
-                            uint8_t *out_found_dev, double *out_best_dev, cudaStream_t st) {
+                            uint8_t *out_found_dev, double *out_best_dev, Sl2Queue q) {
   if (F <= 0 || Kmax <= 0) return cudaSuccess;
   if (Kmax > SM_MAXK) return cudaErrorInvalidValue;
   SmoeArgs A = {s, slot, F, Kmax, K_dev, feat_dev, centre_dev, puinv_dev, map_dev, out_uv_dev, out_found_dev,
                 out_best_dev};
   const int tiles = ((d.W + SM_TW - 1) / SM_TW) * ((d.H + SM_TH - 1) / SM_TH);
+  cudaError_t e;
   switch (d.box) {
-    case 11: smoe_map_kernel<11><<<dim3(tiles, F), SM_TW * SM_TH, 0, st>>>(d, A); break;
-    case 15: smoe_map_kernel<15><<<dim3(tiles, F), SM_TW * SM_TH, 0, st>>>(d, A); break;
+    case 11: e = sl2_launch_kernel(smoe_map_kernel<11>, dim3(tiles, F), dim3(SM_TW * SM_TH), 0, q, false, d, A); break;
+    case 15: e = sl2_launch_kernel(smoe_map_kernel<15>, dim3(tiles, F), dim3(SM_TW * SM_TH), 0, q, false, d, A); break;
     default: return cudaErrorInvalidValue;
   }
-  smoe_argmin_kernel<<<dim3((Kmax + 3) / 4, F), 128, 0, st>>>(d, A, (d.box - 1) / 2);
-  return cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  return sl2_launch_kernel(smoe_argmin_kernel, dim3((Kmax + 3) / 4, F), dim3(128), 0, q, false, d, A, (d.box - 1) / 2);
 }

@@ -161,22 +161,21 @@ int snap_chunks(const Sl2Dev &d) { return (d.ld + 2 * SNAP_WARPS - 1) / (2 * SNA
 
 }  // namespace
 
-cudaError_t sl2_launch_pack(const Sl2Dev &d, int lo, int cnt, uint8_t *buf, size_t stride, cudaStream_t st) {
+cudaError_t sl2_launch_pack(const Sl2Dev &d, int lo, int cnt, uint8_t *buf, size_t stride, Sl2Queue q) {
   if (cnt <= 0) return cudaSuccess;
-  pack_streams_kernel<<<dim3(cnt, snap_chunks(d)), SNAP_THREADS, 0, st>>>(d, lo, buf, stride);
-  return cudaGetLastError();
+  return sl2_launch_kernel(pack_streams_kernel, dim3(cnt, snap_chunks(d)), dim3(SNAP_THREADS), 0, q, false, d, lo, buf,
+                           stride);
 }
 
 cudaError_t sl2_launch_snap_check(const Sl2Dev &d, int cnt, const Sl2SnapLoad *ld_dev, const uint8_t *buf,
-                                  size_t stride, int *bad, cudaStream_t st) {
+                                  size_t stride, int *bad, Sl2Queue q) {
   if (cnt <= 0) return cudaSuccess;
-  snap_check_kernel<<<cnt, SNAP_THREADS, 0, st>>>(d, ld_dev, buf, stride, bad);
-  return cudaGetLastError();
+  return sl2_launch_kernel(snap_check_kernel, dim3(cnt), dim3(SNAP_THREADS), 0, q, false, d, ld_dev, buf, stride, bad);
 }
 
 cudaError_t sl2_launch_unpack(const Sl2Dev &d, int cnt, const Sl2SnapLoad *ld_dev, const uint8_t *buf, size_t stride,
-                              cudaStream_t st) {
+                              Sl2Queue q) {
   if (cnt <= 0) return cudaSuccess;
-  unpack_streams_kernel<<<dim3(cnt, snap_chunks(d)), SNAP_THREADS, 0, st>>>(d, ld_dev, buf, stride);
-  return cudaGetLastError();
+  return sl2_launch_kernel(unpack_streams_kernel, dim3(cnt, snap_chunks(d)), dim3(SNAP_THREADS), 0, q, false, d, ld_dev,
+                           buf, stride);
 }

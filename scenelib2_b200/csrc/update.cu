@@ -1481,11 +1481,10 @@ cudaError_t sl2_configure_update(const Sl2Dev &d) {
 cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, int staged_m,
                               const int *st_feat, const double *st_Hxv, const double *st_Hy,
                               const double *st_R, const double *st_nu, int only_normalise,
-                              cudaStream_t st, cudaEvent_t *ev6, int *launches) {
+                              Sl2Queue q, cudaEvent_t *ev6) {
   if (stream_cnt <= 0) return cudaSuccess;
   cudaError_t e;
-  int nl = 0;
-  auto mark = [&](int i) { return ev6 ? cudaEventRecord(ev6[i], st) : cudaSuccess; };
+  auto mark = [&](int i) { return ev6 ? cudaEventRecord(ev6[i], q.stream) : cudaSuccess; };
   if ((e = mark(0)) != cudaSuccess) return e;
   // row blocks of H P / S per stream: spread over CTAs unless the batch already fills the GPU with two streams per SM
   // (then one CTA per stream is fastest: every CTA rebuilds the measurement list and H tables)
@@ -1500,17 +1499,15 @@ cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, in
     auto *k13 = piped ? upd_hp2_kernel<13> : upd_hp_kernel<13>;
     auto *k7 = piped ? upd_hp2_kernel<7> : upd_hp_kernel<7>;
     const size_t smem = hp_layout(d.kmax, d.ld, piped ? kd : 0).bytes;
-    e = sl2_launch_kernel(kd == 13 ? k13 : k7, grid, dim3(HP_THREADS), smem, st, pdl, d, stream_lo, staged_m,
+    e = sl2_launch_kernel(kd == 13 ? k13 : k7, grid, dim3(HP_THREADS), smem, q, pdl, d, stream_lo, staged_m,
                           st_feat, st_Hxv, st_Hy, st_R, st_nu);
     if (e != cudaSuccess) return e;
-    ++nl;
   }
   if ((e = mark(1)) != cudaSuccess) return e;
   if (!only_normalise) {
-    e = sl2_launch_kernel(upd_chol_kernel, dim3(stream_cnt), dim3(UPD_THREADS), sl2_update_smem_bytes(d), st, pdl, d,
+    e = sl2_launch_kernel(upd_chol_kernel, dim3(stream_cnt), dim3(UPD_THREADS), sl2_update_smem_bytes(d), q, pdl, d,
                           stream_lo);
     if (e != cudaSuccess) return e;
-    ++nl;
   }
   if ((e = mark(2)) != cudaSuccess) return e;
   if (!only_normalise) {
@@ -1521,10 +1518,9 @@ cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, in
     // stream, groups walked inside), a small one spreads a stream over nslab CTAs (latency)
     const bool walk = solve.np <= 13 && stream_cnt >= d.nsm;
     if (walk) warps = SOLVE_MAX_WARPS;
-    e = sl2_launch_kernel(solve.kern, dim3(walk ? 1 : nslab, stream_cnt), dim3(64 * warps), solve.smem, st, pdl, d,
+    e = sl2_launch_kernel(solve.kern, dim3(walk ? 1 : nslab, stream_cnt), dim3(64 * warps), solve.smem, q, pdl, d,
                           stream_lo);
     if (e != cudaSuccess) return e;
-    ++nl;
   }
   if ((e = mark(3)) != cudaSuccess) return e;
   if (!only_normalise) {
@@ -1532,16 +1528,13 @@ cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, in
     // third resident CTA per SM)
     const int nt = (SL2_NXV + 3 * d.Nmax + 1 + 63) / 64;
     e = sl2_launch_kernel(upd_syrk_kernel<32, 2>, dim3(nt * (nt + 1) / 2, stream_cnt), dim3(SYRK_THREADS), SYRK_SMEM,
-                          st, pdl, d, stream_lo);
+                          q, pdl, d, stream_lo);
     if (e != cudaSuccess) return e;
-    ++nl;
   }
   if ((e = mark(4)) != cudaSuccess) return e;
-  e = sl2_launch_kernel(upd_finish_kernel, dim3(stream_cnt), dim3(UPD_THREADS), 0, st, pdl, d, stream_lo,
+  e = sl2_launch_kernel(upd_finish_kernel, dim3(stream_cnt), dim3(UPD_THREADS), 0, q, pdl, d, stream_lo,
                         (int)(staged_m >= 0), only_normalise);
   if (e != cudaSuccess) return e;
-  ++nl;
   if ((e = mark(5)) != cudaSuccess) return e;
-  if (launches) *launches += nl;
   return cudaGetLastError();
 }
