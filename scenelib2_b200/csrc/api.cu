@@ -281,7 +281,7 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   if (!selection_fits(cfg->max_features, cfg->number_of_features_to_select))
     return fail(nullptr, SL2_ERR_ARG,
                 "number_of_features_to_select must be <= SL2_MAX_MEASURED (128) when max_features > 128");
-  if (cfg->boxsize != 11 && cfg->boxsize != 15)
+  if (!sl2_box_supported(cfg->boxsize))
     return fail(nullptr, SL2_ERR_ARG, "boxsize must be 11 or 15");
   if (cfg->width < cfg->boxsize || cfg->height < cfg->boxsize)
     return fail(nullptr, SL2_ERR_ARG, "frame smaller than the patch");

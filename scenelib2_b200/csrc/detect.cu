@@ -201,18 +201,10 @@ cudaError_t sl2_launch_detect(const Sl2Dev &d, int stream, int slot, int n, cons
   double *part_ev = reinterpret_cast<double *>(scratch_dev);
   int *part_idx = reinterpret_cast<int *>(part_ev + (size_t)n * max_tiles);
   const dim3 grid(max_tiles, n);
-  cudaError_t e;
-  switch (d.box) {
-    case 11:
-      e = sl2_launch_kernel(detect_tiles_kernel<11>, grid, dim3(DTHREADS), 0, q, false, d, stream, slot, regions_dev,
-                            max_tiles, part_ev, part_idx);
-      break;
-    case 15:
-      e = sl2_launch_kernel(detect_tiles_kernel<15>, grid, dim3(DTHREADS), 0, q, false, d, stream, slot, regions_dev,
-                            max_tiles, part_ev, part_idx);
-      break;
-    default: return cudaErrorInvalidValue;
-  }
+  const cudaError_t e = sl2_with_box(d.box, [&](auto box) {
+    return sl2_launch_kernel(detect_tiles_kernel<decltype(box)::value>, grid, dim3(DTHREADS), 0, q, false, d, stream,
+                             slot, regions_dev, max_tiles, part_ev, part_idx);
+  });
   if (e != cudaSuccess) return e;
   return sl2_launch_kernel(detect_reduce_kernel, dim3(n), dim3(128), 0, q, false, d, stream, regions_dev,
                            (d.box - 1) / 2, max_tiles, part_ev, part_idx, out_uv_dev, out_ev_dev);

@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "../../include/sl2b200.h"  // SL2_MAX_FEATURES, SL2_MAX_MEASURED
 
 #define SL2_NXV 13          // vehicle state size (motion_model.cpp:44)
@@ -164,6 +166,20 @@ inline cudaError_t sl2_launch_kernel(void (*kern)(KArgs...), dim3 grid, dim3 blo
   return e;
 }
 #endif
+
+// The BOXSIZEs the patch kernels are built for: f(std::integral_constant<int, BOX>{}) for a supported box,
+// cudaErrorInvalidValue otherwise
+template <typename F>
+inline cudaError_t sl2_with_box(int box, F &&f) {
+  switch (box) {
+    case 11: return f(std::integral_constant<int, 11>{});
+    case 15: return f(std::integral_constant<int, 15>{});
+    default: return cudaErrorInvalidValue;
+  }
+}
+inline bool sl2_box_supported(int box) {
+  return sl2_with_box(box, [](auto) { return cudaSuccess; }) == cudaSuccess;
+}
 
 // launchers (defined in search.cu / ekf.cu / update.cu), called from api.cu
 struct SearchLaunch {
