@@ -95,13 +95,44 @@ int sl2_get_stream_config(sl2_ctx *ctx, int32_t stream_id, sl2_stream_config *sc
 /* The frame ring keeps the context's width x height per stream.  A stream whose image is smaller
  * (sl2_set_stream_config) occupies the top-left width_s x height_s of its block; the rest of the block
  * is never read into a result. */
-/* one stream, one slot: copies the stream's width_s x height_s image; `stride` = bytes between image rows */
+/* one stream, one slot: copies the stream's width_s x height_s image, or its raw frame when the stream has a source
+ * (below); `stride` = bytes between image (raw) rows */
 int sl2_set_frame(sl2_ctx *ctx, int32_t stream_id, int32_t slot, const uint8_t *gray, size_t stride);
-/* all streams of a slot at once: gray is [num_streams][height][width] contiguous, in the context's size (pinned
- * memory makes the copy asynchronous) */
+/* all streams of a slot at once: gray is the frame set of sl2_frame_set_layout, which is [num_streams][height][width]
+ * contiguous, in the context's size, while every stream has the default source (pinned memory makes the copy
+ * asynchronous) */
 int sl2_set_frames(sl2_ctx *ctx, int32_t slot, const uint8_t *gray);
 /* device-resident producer: copy device -> device, same layout as sl2_set_frames */
 int sl2_set_frames_dev(sl2_ctx *ctx, int32_t slot, const uint8_t *gray_dev);
+
+/* ---- live cameras: per-stream raw frame sources (framegrabber/usbcamgrabber.cpp:75-113) --------------------------
+ * The reference's camera grabber takes a raw RGB24 or YUV422 (UYVY) frame, converts it with cv::cvtColor(CV_RGB2GRAY
+ * / CV_YUV2GRAY_Y422) and, when it is not the cfg's image size, cv::resize(..., CV_INTER_LINEAR)s it.  A stream with a
+ * source takes that raw frame and the device does both: the host only copies bytes.
+ *   SL2_SRC_GRAY_RING (width = height = 0, the default): the stream contributes the context's width x height gray
+ *     block to a frame set, exactly as without sources.  A context whose streams all have it runs no extra kernel.
+ *   otherwise: the stream's raw frame is width x height x bpp bytes, rows contiguous.  The device converts it to gray
+ *     and, when width x height differs from the stream's image (sl2_stream_config width_s x height_s), resizes it
+ *     (OpenCV's 8-bit INTER_LINEAR, bit for bit) into the stream's block of the ring slot being written.
+ * Frame sets (sl2_set_frames[_dev], sl2_step_host[_async]) hold the streams' frames back to back, in stream order;
+ * sl2_frame_set_layout gives the byte offset of each (offsets[num_streams] = the total).
+ * Ordering: like sl2_set_stream_config (frames copied after the call use the new source); joins both step groups and
+ * synchronises when it has to grow the device staging of the raw frames (slots x the raw bytes of a frame set).
+ * SL2_ERR_ARG, with the source unchanged, for: a bad stream_id or NULL src; an unknown format; reserved != 0; the
+ * default format with a non-zero size; another format with a dimension outside [1, SL2_MAX_SOURCE_DIM]; an odd UYVY
+ * width.  A source belongs to the stream slot, like the frame ring: snapshots do not carry it and a load leaves it. */
+#define SL2_SRC_GRAY_RING 0 /* default */
+#define SL2_SRC_GRAY8 1     /* 1 B/px gray at the source size */
+#define SL2_SRC_RGB24 2     /* 3 B/px, R G B: cvtColor(CV_RGB2GRAY) of OpenCV 2.4 */
+#define SL2_SRC_UYVY 3      /* 2 B/px, U Y0 V Y1: cvtColor(CV_YUV2GRAY_Y422) (Y422 == UYVY in OpenCV) */
+#define SL2_MAX_SOURCE_DIM 4096
+typedef struct sl2_stream_source {
+  int32_t format, width, height, reserved;
+} sl2_stream_source;
+int sl2_set_stream_source(sl2_ctx *ctx, int32_t stream_id, const sl2_stream_source *src);
+int sl2_get_stream_source(sl2_ctx *ctx, int32_t stream_id, sl2_stream_source *src);
+/* offsets: num_streams + 1 entries */
+int sl2_frame_set_layout(sl2_ctx *ctx, size_t *offsets);
 
 /* ---- map and state (Feature::y_/xp_org_/patch_, feature.cpp:108-149; MonoSLAM::xv_/Pxx_ and the
  *      per-feature Pxy_/Pyy_/matrix_block_list_ blocks held as ONE dense P, layout of
@@ -240,11 +271,11 @@ int sl2_normalise_state(sl2_ctx *ctx, int32_t stream_id);
  *      the context: predict -> select -> measure -> update -> normalise -> cull -> symmetrise.
  *      Everything stays on the device; no host round trip inside the frame. */
 int sl2_step(sl2_ctx *ctx, int32_t slot);
-/* end-to-end form: host frames in ([num_streams][height][width], the layout of sl2_set_frames), camera states out
+/* end-to-end form: host frames in (the frame set of sl2_set_frames), camera states out
  * (xv_out: [num_streams][13], may be NULL).  Copies run on the context's stream. */
 int sl2_step_host(sl2_ctx *ctx, int32_t slot, const uint8_t *gray, double *xv_out);
 /* asynchronous end-to-end form for a frame ring: enqueues the H2D copy of `gray` into `slot` on a
- * copy stream, the fused step, and the D2H of the camera states into xv_out, then returns. gray and
+ * copy stream (with the conversion of the streams that have a source), the fused step, and the D2H of the camera states into xv_out, then returns. gray and
  * xv_out must be pinned and stay valid until sl2_wait_slot(ctx, slot) (or sl2_sync) returns.
  * Consecutive calls should use different slots: the copy of frame t+1 then overlaps the kernels of
  * frame t (the producer side of FrameGrabber::GetFrame, framegrabber.cpp:73-104). */
@@ -309,7 +340,9 @@ int64_t sl2_launch_count(const sl2_ctx *ctx);
  * The rule for what goes in: every per-stream array of the device state that an entry point reads before a later
  * kernel overwrites it.  Out: scratch of one update, the frame ring, and the context-wide settings (boxsize, search
  * tile radius, minimum_attempted_measurements_of_feature, successful_match_fraction, search_override), which belong
- * to the receiving context.  The format is canonical: a blob saved, loaded anywhere and saved again is
+ * to the receiving context; the stream's frame source (sl2_set_stream_source) stays with the stream slot, like the
+ * frame ring, and a load leaves the slot's source as it was (the loaded camera's image becomes its resize target, as
+ * with sl2_set_stream_config).  The format is canonical: a blob saved, loaded anywhere and saved again is
  * byte-identical. */
 #define SL2_SNAPSHOT_MAGIC 0x53324C53u /* the bytes "SL2S" on a little-endian host */
 #define SL2_SNAPSHOT_VERSION 1

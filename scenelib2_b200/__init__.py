@@ -8,9 +8,9 @@ Layout (hot path only, see DESIGN.md):
 """
 from . import synth  # noqa: F401
 from .lib import (STEP_RECORD_DTYPE, Context, Sl2Config, Sl2Error, Sl2SnapshotHeader, Sl2StepRecord,  # noqa: F401
-                  Sl2StreamConfig, config_for_scene, default_config, load, load_scene, read_snapshot,
+                  Sl2StreamConfig, Sl2StreamSource, config_for_scene, default_config, load, load_scene, read_snapshot,
                   stream_config_for_scene)
 
 __all__ = ["synth", "STEP_RECORD_DTYPE", "Context", "Sl2Config", "Sl2Error", "Sl2SnapshotHeader", "Sl2StepRecord",
-           "Sl2StreamConfig", "config_for_scene", "default_config", "load", "load_scene", "read_snapshot",
+           "Sl2StreamConfig", "Sl2StreamSource", "config_for_scene", "default_config", "load", "load_scene", "read_snapshot",
            "stream_config_for_scene"]

@@ -55,6 +55,15 @@ struct sl2_ctx {
   bool b_pending = false, b_search_valid = false;
   std::vector<cudaEvent_t> ev_cmp_b;  // per frame slot: group B is done with the slot
   int64_t rec_steps = 0;  // fused steps recorded since sl2_enable_records (the ring itself is d.rec)
+  // raw frame sources (sl2_set_stream_source): the host mirror, the frame-set layout, and the device table of the
+  // streams with a non-default source (src_rows, in stream order) with their raw frames' staging
+  std::vector<sl2_stream_source> srcs;  // [B]
+  std::vector<size_t> layout;           // [B + 1] byte offsets of the streams' frames in a frame set
+  std::vector<Sl2Source> src_rows;
+  Sl2Source *src_tab = nullptr;   // [B] device
+  uint8_t *src_stage = nullptr;   // [slots][src_slot_bytes] + 16 bytes of slack for the kernel's aligned loads
+  size_t src_stage_bytes = 0, src_slot_bytes = 0;
+  cudaEvent_t ev_src = nullptr;   // recorded on `stream` behind the last table write
 };
 
 namespace {
@@ -208,11 +217,51 @@ void pack_patch_rows(uint8_t *dst, const uint8_t *src, int n, int box) {
   for (size_t r = 0; r < (size_t)n * box; ++r) memcpy(dst + r * 16, src + r * box, box);
 }
 
-// one frame slot of every stream, [B][H][W] packed, into the frame ring
-cudaError_t copy_slot_frames(const Sl2Dev &d, int slot, const uint8_t *src, cudaMemcpyKind kind, cudaStream_t st) {
-  uint8_t *dst = d.frames + (size_t)slot * d.B * d.H * d.pitch;
-  if (d.pitch == d.W) return cudaMemcpyAsync(dst, src, (size_t)d.B * d.H * d.W, kind, st);
-  return cudaMemcpy2DAsync(dst, d.pitch, src, d.W, d.W, (size_t)d.B * d.H, kind, st);
+// gray blocks of the streams [lo, hi), [hi - lo][H][W] packed, into the frame ring
+cudaError_t copy_gray_blocks(const Sl2Dev &d, int slot, int lo, int hi, const uint8_t *src, cudaMemcpyKind kind,
+                             cudaStream_t st) {
+  uint8_t *dst = d.frames + ((size_t)slot * d.B + lo) * d.H * d.pitch;
+  if (d.pitch == d.W) return cudaMemcpyAsync(dst, src, (size_t)(hi - lo) * d.H * d.W, kind, st);
+  return cudaMemcpy2DAsync(dst, d.pitch, src, d.W, d.W, (size_t)(hi - lo) * d.H, kind, st);
+}
+
+uint8_t *source_stage(const sl2_ctx *c, int slot) { return c->src_stage + (size_t)slot * c->src_slot_bytes; }
+
+// convert the raw frames of source rows [base, base + cnt) of `slot`'s staging into the ring
+cudaError_t ingest(sl2_ctx *c, int slot, int base, int cnt, Sl2Queue q) {
+  int max_dh = 0, max_rb = 0;
+  for (int j = base; j < base + cnt; ++j) {
+    const Sl2Source &r = c->src_rows[j];
+    max_dh = std::max(max_dh, r.dh);
+    max_rb = std::max(max_rb, r.sw * sl2_source_bpp(r.format));
+  }
+  return sl2_launch_ingest(c->d, c->src_tab, base, cnt, max_dh, max_rb, source_stage(c, slot), slot, q);
+}
+
+// One frame slot of every stream, a frame set (sl2_frame_set_layout), into the frame ring: each run of consecutive
+// default streams in one copy to the ring (the whole set when no stream has a source), each run of streams with a
+// source in one copy to the slot's staging, then one conversion launch for all of them.
+cudaError_t copy_slot_frames(sl2_ctx *c, int slot, const uint8_t *src, cudaMemcpyKind kind, Sl2Queue q) {
+  const Sl2Dev &d = c->d;
+  if (c->src_rows.empty()) return copy_gray_blocks(d, slot, 0, d.B, src, kind, q.stream);
+  for (int a = 0; a < d.B;) {
+    const bool raw = c->srcs[a].format != SL2_SRC_GRAY_RING;
+    int b = a + 1;
+    while (b < d.B && (c->srcs[b].format != SL2_SRC_GRAY_RING) == raw) ++b;
+    cudaError_t e;
+    if (raw) {
+      size_t at = 0;  // staging offset of stream a
+      for (const Sl2Source &r : c->src_rows)
+        if (r.stream == a) at = (size_t)r.off;
+      e = cudaMemcpyAsync(source_stage(c, slot) + at, src + c->layout[a], c->layout[b] - c->layout[a], kind,
+                          q.stream);
+    } else {
+      e = copy_gray_blocks(d, slot, a, b, src + c->layout[a], kind, q.stream);
+    }
+    if (e != cudaSuccess) return e;
+    a = b;
+  }
+  return ingest(c, slot, 0, (int)c->src_rows.size(), q);
 }
 
 int device_nfeat(sl2_ctx *c, int s, int *out) {
@@ -346,6 +395,9 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   sc0.delta_t = cfg->delta_t;
   sc0.number_of_features_to_select = cfg->number_of_features_to_select;
   c->cams.assign(d.B, sc0);
+  c->srcs.assign(d.B, sl2_stream_source{});
+  c->layout.resize(d.B + 1);
+  for (int s = 0; s <= d.B; ++s) c->layout[s] = (size_t)s * d.H * d.W;
   const std::vector<Sl2StreamCam> rows(d.B, cam_row(sc0));  // read by the copy below until the final synchronise
 
   const size_t B = d.B, N = d.Nmax;
@@ -437,6 +489,9 @@ void sl2_destroy(sl2_ctx *c) {
     if (e) cudaEventDestroy(e);
   for (void *p : c->allocs) cudaFree(p);
   if (c->d.rec) cudaFree(c->d.rec);
+  if (c->src_tab) cudaFree(c->src_tab);
+  if (c->src_stage) cudaFree(c->src_stage);
+  if (c->ev_src) cudaEventDestroy(c->ev_src);
   if (c->stg_dev) cudaFree(c->stg_dev);
   if (c->smoe_map) cudaFree(c->smoe_map);
   if (c->stg_host) cudaFreeHost(c->stg_host);
@@ -478,12 +533,111 @@ static int check_stream_config(sl2_ctx *c, const sl2_stream_config *sc, const st
   return SL2_OK;
 }
 
+static int install_sources(sl2_ctx *c, const std::vector<sl2_stream_source> &srcs);
+
 int sl2_set_stream_config(sl2_ctx *c, int32_t s, const sl2_stream_config *sc) {
   if (bad_stream(c, s) || !sc) return fail(c, SL2_ERR_ARG, "sl2_set_stream_config: bad argument");
   const int rc = check_stream_config(c, sc, "sl2_set_stream_config");
   if (rc) return rc;
   CU_TRY(c, sl2_launch_kernel(write_cam_row_kernel, dim3(1), dim3(1), 0, queue(c), false, c->d.cams + s, cam_row(*sc)));
+  const sl2_stream_config old = c->cams[s];
   c->cams[s] = *sc;
+  if (c->srcs[s].format != SL2_SRC_GRAY_RING && (old.width != sc->width || old.height != sc->height))
+    return install_sources(c, c->srcs);  // the resize target of the stream's next frame
+  return SL2_OK;
+}
+
+// ---- raw frame sources ------------------------------------------------------------------------------
+static size_t frame_bytes(const sl2_ctx *c, const sl2_stream_source &s) {
+  return s.format == SL2_SRC_GRAY_RING ? (size_t)c->d.H * c->d.W
+                                       : (size_t)s.width * s.height * sl2_source_bpp(s.format);
+}
+
+// Make `srcs` the context's sources (with the cameras in c->cams): layout, table rows, staging and the device table.
+// The table is rewritten on `stream` after every conversion queued so far on the copy stream.
+static int install_sources(sl2_ctx *c, const std::vector<sl2_stream_source> &srcs) {
+  const Sl2Dev &d = c->d;
+  std::vector<size_t> layout(d.B + 1, 0);
+  std::vector<Sl2Source> rows;
+  size_t raw = 0;
+  for (int s = 0; s < d.B; ++s) {
+    layout[s + 1] = layout[s] + frame_bytes(c, srcs[s]);
+    if (srcs[s].format == SL2_SRC_GRAY_RING) continue;
+    rows.push_back({s, srcs[s].format, srcs[s].width, srcs[s].height, c->cams[s].width, c->cams[s].height,
+                    (int64_t)raw});
+    raw += frame_bytes(c, srcs[s]);
+  }
+  const size_t slot_bytes = (raw + 15) & ~(size_t)15;
+  const size_t need = rows.empty() ? 0 : (size_t)d.slots * slot_bytes + 16;
+  // every allocation before anything changes: a failed one leaves the sources, the staging and the table as they were
+  if (need > c->src_stage_bytes) {  // nothing may still read or write the old staging
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    CU_TRY(c, cudaStreamSynchronize(c->copy_stream));
+    uint8_t *stage = nullptr;
+    CU_TRY(c, cudaMalloc((void **)&stage, need));
+    if (c->src_stage) cudaFree(c->src_stage);
+    c->src_stage = stage;
+    c->src_stage_bytes = need;
+  }
+  if (!rows.empty() && !c->src_tab) CU_TRY(c, cudaMalloc((void **)&c->src_tab, sizeof(Sl2Source) * d.B));
+  if (!rows.empty() && !c->ev_src) CU_TRY(c, cudaEventCreateWithFlags(&c->ev_src, cudaEventDisableTiming));
+  if (!rows.empty()) {
+    for (cudaEvent_t e : c->ev_h2d) CU_TRY(c, cudaStreamWaitEvent(c->stream, e, 0));  // conversions in flight
+    for (size_t first = 0; first < rows.size(); first += SL2_SOURCE_CHUNK) {
+      Sl2SourceChunk ch = {};
+      ch.first = (int)first;
+      ch.n = (int)std::min(rows.size() - first, (size_t)SL2_SOURCE_CHUNK);
+      for (int i = 0; i < ch.n; ++i) ch.row[i] = rows[first + i];
+      CU_TRY(c, sl2_launch_source_write(c->src_tab, ch, queue(c)));
+    }
+    CU_TRY(c, cudaEventRecord(c->ev_src, c->stream));
+  }
+  c->srcs = srcs;
+  c->layout = layout;
+  c->src_rows = rows;
+  c->src_slot_bytes = slot_bytes;
+  return SL2_OK;
+}
+
+// A snapshot load gives streams [lo, lo + cnt) the blobs' cameras: a stream with a source then resizes to its new image
+static int loaded_cameras(sl2_ctx *c, int lo, const std::vector<sl2_stream_config> &cams) {
+  bool resized = false;
+  for (size_t i = 0; i < cams.size(); ++i) {
+    const sl2_stream_config &old = c->cams[lo + i];
+    resized = resized || (c->srcs[lo + i].format != SL2_SRC_GRAY_RING &&
+                          (old.width != cams[i].width || old.height != cams[i].height));
+    c->cams[lo + i] = cams[i];
+  }
+  return resized ? install_sources(c, c->srcs) : SL2_OK;
+}
+
+int sl2_set_stream_source(sl2_ctx *c, int32_t s, const sl2_stream_source *src) {
+  if (bad_stream(c, s) || !src) return fail(c, SL2_ERR_ARG, "sl2_set_stream_source: bad argument");
+  const int f = src->format;
+  if (f < SL2_SRC_GRAY_RING || f > SL2_SRC_UYVY || src->reserved != 0)
+    return fail(c, SL2_ERR_ARG, "sl2_set_stream_source: unknown format or non-zero reserved field");
+  if (f == SL2_SRC_GRAY_RING ? (src->width != 0 || src->height != 0)
+                             : (src->width < 1 || src->height < 1 || src->width > SL2_MAX_SOURCE_DIM ||
+                                src->height > SL2_MAX_SOURCE_DIM))
+    return fail(c, SL2_ERR_ARG,
+                "sl2_set_stream_source: size must be 0 x 0 for the default source, else in [1, SL2_MAX_SOURCE_DIM]");
+  if (f == SL2_SRC_UYVY && (src->width & 1))
+    return fail(c, SL2_ERR_ARG, "sl2_set_stream_source: a UYVY frame has an even width");
+  std::vector<sl2_stream_source> srcs = c->srcs;
+  srcs[s] = *src;
+  return install_sources(c, srcs);
+}
+
+int sl2_get_stream_source(sl2_ctx *c, int32_t s, sl2_stream_source *src) {
+  if (bad_stream(c, s) || !src) return fail(c, SL2_ERR_ARG, "sl2_get_stream_source: bad argument");
+  *src = c->srcs[s];
+  return SL2_OK;
+}
+
+int sl2_frame_set_layout(sl2_ctx *c, size_t *offsets) {
+  enter(c);
+  if (!c || !offsets) return fail(c, SL2_ERR_ARG, "sl2_frame_set_layout: bad argument");
+  std::copy(c->layout.begin(), c->layout.end(), offsets);
   return SL2_OK;
 }
 
@@ -497,9 +651,19 @@ int sl2_get_stream_config(sl2_ctx *c, int32_t s, sl2_stream_config *sc) {
 int sl2_set_frame(sl2_ctx *c, int32_t s, int32_t slot, const uint8_t *gray, size_t stride) {
   if (bad_stream(c, s) || bad_slot(c, slot) || !gray) return fail(c, SL2_ERR_ARG, "sl2_set_frame: bad argument");
   const Sl2Dev &d = c->d;
-  uint8_t *dst = d.frames + ((size_t)slot * d.B + s) * d.H * d.pitch;
-  const sl2_stream_config &sc = c->cams[s];  // the stream's image, top-left of its block
-  CU_TRY(c, cudaMemcpy2DAsync(dst, d.pitch, gray, stride, sc.width, sc.height, cudaMemcpyHostToDevice, c->stream));
+  if (c->srcs[s].format != SL2_SRC_GRAY_RING) {  // the raw frame to the slot's staging, then its conversion
+    int j = 0;
+    while (c->src_rows[j].stream != s) ++j;
+    const Sl2Source &r = c->src_rows[j];
+    const size_t rb = (size_t)r.sw * sl2_source_bpp(r.format);
+    CU_TRY(c, cudaMemcpy2DAsync(source_stage(c, slot) + r.off, rb, gray, stride, rb, r.sh, cudaMemcpyHostToDevice,
+                                c->stream));
+    CU_TRY(c, ingest(c, slot, j, 1, queue(c)));
+  } else {
+    uint8_t *dst = d.frames + ((size_t)slot * d.B + s) * d.H * d.pitch;
+    const sl2_stream_config &sc = c->cams[s];  // the stream's image, top-left of its block
+    CU_TRY(c, cudaMemcpy2DAsync(dst, d.pitch, gray, stride, sc.width, sc.height, cudaMemcpyHostToDevice, c->stream));
+  }
   CU_TRY(c, cudaEventRecord(c->ev_cmp[slot], c->stream));  // slot busy until the copy has landed
   return SL2_OK;
 }
@@ -507,7 +671,7 @@ int sl2_set_frame(sl2_ctx *c, int32_t s, int32_t slot, const uint8_t *gray, size
 static int set_frames_any(sl2_ctx *c, int32_t slot, const uint8_t *gray, cudaMemcpyKind kind) {
   enter(c);
   if (!c || bad_slot(c, slot) || !gray) return fail(c, SL2_ERR_ARG, "sl2_set_frames: bad argument");
-  CU_TRY(c, copy_slot_frames(c->d, slot, gray, kind, c->stream));
+  CU_TRY(c, copy_slot_frames(c, slot, gray, kind, queue(c)));
   CU_TRY(c, cudaEventRecord(c->ev_cmp[slot], c->stream));  // slot busy until the copy has landed
   return SL2_OK;
 }
@@ -1086,7 +1250,8 @@ int sl2_step_host_async(sl2_ctx *c, int32_t slot, const uint8_t *gray, double *x
   // Work on OTHER slots is not waited for: the copy of frame t+1 overlaps the kernels of frame t.
   CU_TRY(c, cudaStreamWaitEvent(cs, c->ev_cmp[slot], 0));
   CU_TRY(c, cudaStreamWaitEvent(cs, c->ev_cmp_b[slot], 0));
-  CU_TRY(c, copy_slot_frames(d, slot, gray, cudaMemcpyHostToDevice, cs));
+  if (!c->src_rows.empty()) CU_TRY(c, cudaStreamWaitEvent(cs, c->ev_src, 0));  // the current source table
+  CU_TRY(c, copy_slot_frames(c, slot, gray, cudaMemcpyHostToDevice, {cs, &c->launches}));
   CU_TRY(c, cudaEventRecord(c->ev_h2d[slot], cs));
   CU_TRY(c, cudaStreamWaitEvent(c->stream, c->ev_h2d[slot], 0));
   CU_TRY(c, cudaStreamWaitEvent(c->stream, c->ev_out[slot], 0));  // staging buffer of this slot is free
@@ -1358,8 +1523,7 @@ int sl2_load_streams(sl2_ctx *c, int32_t lo, int32_t cnt, const void *buf, size_
                                 queue(c)));
   }
   CU_TRY(c, cudaStreamSynchronize(c->stream));
-  for (int i = 0; i < cnt; ++i) c->cams[lo + i] = cams[i];
-  return SL2_OK;
+  return loaded_cameras(c, lo, cams);
 }
 
 int sl2_load_streams_dev(sl2_ctx *c, int32_t lo, int32_t cnt, const void *buf_dev, size_t stride) {
@@ -1396,8 +1560,7 @@ int sl2_load_streams_dev(sl2_ctx *c, int32_t lo, int32_t cnt, const void *buf_de
   if (bad) return fail(c, SL2_ERR_ARG, "sl2_load_streams_dev: sel_rank or job_feat out of range");
   CU_TRY(c, sl2_launch_unpack(c->d, cnt, q_dev, in, stride, queue(c)));
   CU_TRY(c, cudaStreamSynchronize(c->stream));
-  for (int i = 0; i < cnt; ++i) c->cams[lo + i] = cams[i];
-  return SL2_OK;
+  return loaded_cameras(c, lo, cams);
 }
 
 // ---- step records -------------------------------------------------------------------------------

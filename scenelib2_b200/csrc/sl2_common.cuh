@@ -233,6 +233,26 @@ size_t sl2_detect_scratch_bytes(const Sl2Dev &d, int n);
 cudaError_t sl2_launch_detect(const Sl2Dev &d, int stream, int slot, int n, const int *regions_dev,
                               int *out_uv_dev, double *out_ev_dev, void *scratch_dev, Sl2Queue q);
 
+// ---- raw frame sources (ingest.cu): one row per stream with a non-default sl2_stream_source, in stream order -------
+struct Sl2Source {
+  int stream, format;  // camera stream, SL2_SRC_*
+  int sw, sh;          // raw frame size
+  int dw, dh;          // the stream's image (sl2_stream_config width_s x height_s): the resize target
+  int64_t off;         // byte offset of the raw frame in a slot of the staging area
+};
+#define SL2_SOURCE_CHUNK 64  // rows one table write carries as its kernel parameter
+struct Sl2SourceChunk {
+  int first, n;
+  Sl2Source row[SL2_SOURCE_CHUNK];
+};
+inline int sl2_source_bpp(int format) { return format == SL2_SRC_RGB24 ? 3 : format == SL2_SRC_UYVY ? 2 : 1; }
+// table[first .. first + n) = the chunk's rows, ordered on the queue like any other launch
+cudaError_t sl2_launch_source_write(Sl2Source *table, const Sl2SourceChunk &chunk, Sl2Queue q);
+// convert (and resize) the raw frames of table rows [base, base + cnt) from one slot of the staging area into the
+// ring slot `slot`; max_row_bytes = the largest sw * bpp of those rows
+cudaError_t sl2_launch_ingest(const Sl2Dev &d, const Sl2Source *table, int base, int cnt, int max_dh,
+                              int max_row_bytes, const uint8_t *stage_slot, int slot, Sl2Queue q);
+
 // ---- stream snapshots (snapshot.cu): the blob format of include/sl2b200.h --------------------------------------
 // Section field[k] of a blob is the stream's first nfeat records of array k of SL2_STREAM_ARRAYS (x, P and the
 // templates are laid out separately).

@@ -46,10 +46,21 @@ class Sl2StreamConfig(C.Structure):
     ]
 
 
+class Sl2StreamSource(C.Structure):
+    """sl2_stream_source: the raw frame format and size a camera stream takes (SL2_SRC_*; 0 x 0 for the default)."""
+    _fields_ = [("format", C.c_int32), ("width", C.c_int32), ("height", C.c_int32), ("reserved", C.c_int32)]
+
+
+SL2_SRC_GRAY_RING, SL2_SRC_GRAY8, SL2_SRC_RGB24, SL2_SRC_UYVY = 0, 1, 2, 3
+SL2_MAX_SOURCE_DIM = 4096
+SOURCE_BPP = {SL2_SRC_GRAY8: 1, SL2_SRC_RGB24: 3, SL2_SRC_UYVY: 2}
+
+
 # every symbol include/sl2b200.h declares (checked by tests/test_abi.py)
 EXPORTS = [
     "sl2_default_config", "sl2_create", "sl2_destroy", "sl2_last_error", "sl2_sync", "sl2_version",
-    "sl2_set_stream_config", "sl2_get_stream_config", "sl2_set_frame", "sl2_set_frames", "sl2_set_frames_dev", "sl2_set_features",
+    "sl2_set_stream_config", "sl2_get_stream_config", "sl2_set_frame", "sl2_set_frames", "sl2_set_frames_dev",
+    "sl2_set_stream_source", "sl2_get_stream_source", "sl2_frame_set_layout", "sl2_set_features",
     "sl2_num_features", "sl2_state_size", "sl2_set_state", "sl2_get_state", "sl2_delete_feature", "sl2_append_feature",
     "sl2_patch_search", "sl2_score_map", "sl2_smoe_search", "sl2_find_best_patch", "sl2_ekf_predict",
     "sl2_predict_measurements", "sl2_make_measurements", "sl2_ekf_update",
@@ -186,6 +197,9 @@ def load():
         L.sl2_set_frame.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_size_t]
         L.sl2_set_frames.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
         L.sl2_set_frames_dev.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
+        L.sl2_set_stream_source.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamSource)]
+        L.sl2_get_stream_source.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamSource)]
+        L.sl2_frame_set_layout.argtypes = [C.c_void_p, C.POINTER(C.c_size_t)]
         L.sl2_step.argtypes = [C.c_void_p, C.c_int32]
         L.sl2_step_host.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
         L.sl2_step_host_async.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
@@ -281,15 +295,43 @@ class Context:
         return sc
 
     # ---- frames -------------------------------------------------------------------------------
+    def set_stream_source(self, stream_id, format, width=0, height=0):
+        """sl2_set_stream_source: the stream takes raw `format` frames of width x height (SL2_SRC_*), converted to
+        gray and resized to its image on the device; SL2_SRC_GRAY_RING with 0 x 0 restores the default."""
+        src = Sl2StreamSource(format, width, height, 0)
+        self._ck(self.L.sl2_set_stream_source(self.h, stream_id, C.byref(src)))
+        self._sources = None
+
+    def stream_source(self, stream_id):
+        src = Sl2StreamSource()
+        self._ck(self.L.sl2_get_stream_source(self.h, stream_id, C.byref(src)))
+        return src
+
+    def frame_set_layout(self):
+        """Byte offsets of the streams' frames in a frame set, and the total (num_streams + 1 entries)."""
+        out = (C.c_size_t * (self.cfg.num_streams + 1))()
+        self._ck(self.L.sl2_frame_set_layout(self.h, out))
+        return [int(v) for v in out]
+
+    def _has_sources(self):
+        if getattr(self, "_sources", None) is None:
+            self._sources = any(self.stream_source(s).format for s in range(self.cfg.num_streams))
+        return self._sources
+
     def set_frame(self, stream_id, slot, gray):
+        """One stream's image (H_s, W_s) or, with a source, its raw frame (height, width[, bpp])."""
         gray = np.ascontiguousarray(gray, np.uint8)
         self._ck(self.L.sl2_set_frame(self.h, stream_id, slot, gray.ctypes.data, gray.strides[0]))
         self._ck(self.L.sl2_sync(self.h))
 
     def set_frames(self, slot, gray):
-        """gray: (num_streams, H, W) u8 host array."""
+        """gray: (num_streams, H, W) u8 host array, or, when a stream has a source, the packed frame set of
+        frame_set_layout() (any u8 array of that many bytes)."""
         gray = np.ascontiguousarray(gray, np.uint8)
-        assert gray.shape == (self.cfg.num_streams, self.cfg.height, self.cfg.width)
+        if self._has_sources():
+            assert gray.nbytes == self.frame_set_layout()[-1]
+        else:
+            assert gray.shape == (self.cfg.num_streams, self.cfg.height, self.cfg.width)
         self._ck(self.L.sl2_set_frames(self.h, slot, gray.ctypes.data))
         self._ck(self.L.sl2_sync(self.h))
 
