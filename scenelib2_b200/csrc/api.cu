@@ -7,7 +7,9 @@
 #include <cstdlib>
 #include <cstring>
 #include <initializer_list>
+#include <memory>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/sl2b200.h"
@@ -17,58 +19,99 @@ namespace {
 
 thread_local std::string g_create_error;
 
+// Owning handles of the CUDA resources a context creates: a handle releases what it holds when it is reset, assigned
+// or destroyed, so deleting the context releases everything it created, whatever point its creation reached.
+struct DevFree { void operator()(void *p) const { cudaFree(p); } };
+struct HostFree { void operator()(void *p) const { cudaFreeHost(p); } };
+struct EventFree { void operator()(cudaEvent_t e) const { cudaEventDestroy(e); } };
+struct StreamFree { void operator()(cudaStream_t s) const { cudaStreamDestroy(s); } };
+template <typename T> using DevPtr = std::unique_ptr<T, DevFree>;    // device memory
+template <typename T> using HostPtr = std::unique_ptr<T, HostFree>;  // pinned host memory
+using Event = std::unique_ptr<CUevent_st, EventFree>;
+using Stream = std::unique_ptr<CUstream_st, StreamFree>;
+
+// each fills its handle only when the creation succeeds
+template <typename T> cudaError_t cuda_malloc(DevPtr<T> &h, size_t bytes) {
+  void *p = nullptr;
+  const cudaError_t e = cudaMalloc(&p, bytes);
+  if (e == cudaSuccess) h.reset(static_cast<T *>(p));
+  return e;
+}
+template <typename T> cudaError_t cuda_malloc_host(HostPtr<T> &h, size_t bytes) {
+  void *p = nullptr;
+  const cudaError_t e = cudaMallocHost(&p, bytes);
+  if (e == cudaSuccess) h.reset(static_cast<T *>(p));
+  return e;
+}
+cudaError_t cuda_event_create(Event &h, unsigned flags) {
+  cudaEvent_t ev = nullptr;
+  const cudaError_t e = cudaEventCreateWithFlags(&ev, flags);
+  if (e == cudaSuccess) h.reset(ev);
+  return e;
+}
+cudaError_t cuda_stream_create(Stream &h) {
+  cudaStream_t st = nullptr;
+  const cudaError_t e = cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking);
+  if (e == cudaSuccess) h.reset(st);
+  return e;
+}
+
+// the events of one frame slot: its frames have landed (h2d), the context's stream or group B is done with it (cmp,
+// cmp_b), its camera states have been copied to the host (out)
+struct SlotEvents { Event h2d, cmp, cmp_b, out; };
+
 }  // namespace
 
 struct sl2_ctx {
   sl2_config cfg;
   Sl2Dev d;
   std::vector<sl2_stream_config> cams;  // host mirror of d.cams, updated with it
-  cudaStream_t stream = nullptr;
-  bool own_stream = false;
+  cudaStream_t stream = nullptr;        // cfg.cuda_stream, else owned_stream
+  Stream owned_stream;                  // set only when the context created its stream
   CUtensorMap tmap;
   std::string err;
-  std::vector<void *> allocs;
+  std::vector<DevPtr<void>> allocs;  // behind the Sl2Dev arrays and xv_stage
   // staging
-  uint8_t *stg_dev = nullptr;   // device scratch for staged API calls
+  DevPtr<uint8_t> stg_dev;   // device scratch for staged API calls
   size_t stg_bytes = 0;
-  uint8_t *stg_host = nullptr;  // pinned
-  double *smoe_map = nullptr;   // [features of the call][W][H] score cache of the SMOE kernels (lazily sized)
+  HostPtr<uint8_t> stg_host;
+  DevPtr<double> smoe_map;   // [features of the call][W][H] score cache of the SMOE kernels (lazily sized)
   size_t smoe_map_bytes = 0;
   int64_t launches = 0;  // kernels launched: counted by sl2_launch_kernel through every Sl2Queue of the context
   bool timing = false;
   // timing mode: ev[0..4] bracket predict / search / update / cull, evu[0..5] the five update kernels
-  cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-  cudaEvent_t evu[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  Event ev[5], evu[6];
   // asynchronous end-to-end path: frames of step t+1 are copied while step t computes
-  cudaStream_t copy_stream = nullptr;  // H2D of the frames
-  cudaStream_t out_stream = nullptr;   // D2H of the results (own stream: must not block the next H2D)
-  std::vector<cudaEvent_t> ev_h2d, ev_cmp, ev_out;  // per frame slot
-  double *xv_stage = nullptr;                        // [slots][B][13] device
+  Stream copy_stream;  // H2D of the frames
+  Stream out_stream;   // D2H of the results (own stream: must not block the next H2D)
+  std::vector<SlotEvents> ev_slot;  // [slots]
+  double *xv_stage = nullptr;       // [slots][B][13] device
   // Fused step as two staggered groups of camera streams: group A (first half) on `stream`, group B on
   // `stream_b`; B's predict+search wait for A's search of the same step and A's next step waits for
   // B's search, so the integer-bound search of one group runs under the FP64-bound update of the other
   // and the two update kernels are half a step out of phase.  Results are identical to the serial order
   // (the groups share nothing); every other entry point joins the two streams first (enter()).
   int step_groups = 1;  // off by default: with two streams per SM the update would lose its second CTA per SM
-  cudaStream_t stream_b = nullptr;
-  cudaEvent_t ev_main = nullptr, ev_a_search = nullptr, ev_b_search = nullptr, ev_b_done = nullptr;
+  Stream stream_b;
+  Event ev_main, ev_a_search, ev_b_search, ev_b_done;
   bool b_pending = false, b_search_valid = false;
-  std::vector<cudaEvent_t> ev_cmp_b;  // per frame slot: group B is done with the slot
-  int64_t rec_steps = 0;  // fused steps recorded since sl2_enable_records (the ring itself is d.rec)
+  DevPtr<sl2_step_record> rec;  // the ring d.rec points into
+  int64_t rec_steps = 0;        // fused steps recorded since sl2_enable_records
   // raw frame sources (sl2_set_stream_source): the host mirror, the frame-set layout, and the device table of the
   // streams with a non-default source (src_rows, in stream order) with their raw frames' staging
   std::vector<sl2_stream_source> srcs;  // [B]
   std::vector<size_t> layout;           // [B + 1] byte offsets of the streams' frames in a frame set
   std::vector<Sl2Source> src_rows;
-  Sl2Source *src_tab = nullptr;   // [B] device
-  uint8_t *src_stage = nullptr;   // [slots][src_slot_bytes] + 16 bytes of slack for the kernel's aligned loads
+  DevPtr<Sl2Source> src_tab;    // [B]
+  DevPtr<uint8_t> src_stage;    // [slots][src_slot_bytes] + 16 bytes of slack for the kernel's aligned loads
   size_t src_stage_bytes = 0, src_slot_bytes = 0;
-  cudaEvent_t ev_src = nullptr;   // recorded on `stream` behind the last table write
+  Event ev_src;                 // recorded on `stream` behind the last table write
 };
 
 namespace {
 
 int fail(sl2_ctx *c, int code, const std::string &msg) {
+  if (code == SL2_ERR_CUDA) cudaGetLastError();  // reported once: sl2_launch_update returns the runtime's last error
   if (c) c->err = msg;
   else g_create_error = msg;
   return code;
@@ -84,10 +127,11 @@ int fail(sl2_ctx *c, int code, const std::string &msg) {
 
 template <typename T>
 cudaError_t dev_alloc(sl2_ctx *c, T **p, size_t count, bool zero = true) {
-  void *q = nullptr;
-  cudaError_t e = cudaMalloc(&q, count * sizeof(T) + 256);
+  DevPtr<void> h;
+  cudaError_t e = cuda_malloc(h, count * sizeof(T) + 256);
   if (e != cudaSuccess) return e;
-  c->allocs.push_back(q);
+  void *q = h.get();
+  c->allocs.push_back(std::move(h));
   if (zero) {
     e = cudaMemsetAsync(q, 0, count * sizeof(T) + 256, c->stream);
     if (e != cudaSuccess) return e;
@@ -129,7 +173,7 @@ inline void enter(sl2_ctx *c, bool join = true) {
   if (!c) return;
   cudaSetDevice(c->cfg.device);
   if (join && c->b_pending) {  // the second stream group's step work becomes visible to `stream`
-    cudaStreamWaitEvent(c->stream, c->ev_b_done, 0);
+    cudaStreamWaitEvent(c->stream, c->ev_b_done.get(), 0);
     c->b_pending = false;
     c->b_search_valid = false;
   }
@@ -140,20 +184,25 @@ bool bad_stream(sl2_ctx *c, int s) {
 }
 bool bad_slot(sl2_ctx *c, int s) { return s < 0 || s >= c->cfg.frame_slots; }
 
-int stage_reserve(sl2_ctx *c, size_t bytes) {
-  if (bytes <= c->stg_bytes) return SL2_OK;
-  if (c->stg_dev) {
-    CU_TRY(c, cudaStreamSynchronize(c->stream));
-    cudaFree(c->stg_dev);
-    cudaFreeHost(c->stg_host);
-    c->stg_dev = nullptr;
-    c->stg_host = nullptr;
-  }
-  bytes = (bytes + 4095) & ~(size_t)4095;
-  CU_TRY(c, cudaMalloc((void **)&c->stg_dev, bytes));
-  CU_TRY(c, cudaMallocHost((void **)&c->stg_host, bytes));
-  c->stg_bytes = bytes;
+// Grows a scratch buffer, whose contents never outlive a call, to `bytes`: the old one is released once the context's
+// stream is done with it (and before the new allocation, so the peak stays one buffer), then the device buffer and its
+// pinned twin, if any, are allocated.  `size` is recorded only when both exist: after a failed grow the buffer is
+// empty and the next call allocates again.
+template <typename T>
+int grow_scratch(sl2_ctx *c, size_t bytes, size_t &size, DevPtr<T> &dev, HostPtr<T> *host = nullptr) {
+  if (bytes <= size) return SL2_OK;
+  if (dev) CU_TRY(c, cudaStreamSynchronize(c->stream));
+  size = 0;
+  dev.reset();
+  if (host) host->reset();
+  CU_TRY(c, cuda_malloc(dev, bytes));
+  if (host) CU_TRY(c, cuda_malloc_host(*host, bytes));
+  size = bytes;
   return SL2_OK;
+}
+
+int stage_reserve(sl2_ctx *c, size_t bytes) {
+  return grow_scratch(c, (bytes + 4095) & ~(size_t)4095, c->stg_bytes, c->stg_dev, &c->stg_host);
 }
 
 // One section of a staged call's buffers.  STAGE_IN sections go to the device before the launches (from `src`, or
@@ -190,20 +239,20 @@ int staged_call(sl2_ctx *c, std::initializer_list<Stage *> secs, Pack &&pack, La
   const size_t h2d = end[STAGE_INOUT], d2h = end[STAGE_OUT] - end[STAGE_IN];
   if (h2d) CU_TRY(c, cudaStreamSynchronize(c->stream));
   for (Stage *x : secs) {
-    x->h = c->stg_host + x->at;
-    x->d = c->stg_dev + x->at;
+    x->h = c->stg_host.get() + x->at;
+    x->d = c->stg_dev.get() + x->at;
     if (x->dir <= STAGE_INOUT) {
       if (x->src) memcpy(x->h, x->src, x->bytes);
       else memset(x->h, 0, x->bytes);
     }
   }
   pack();
-  if (h2d) CU_TRY(c, cudaMemcpyAsync(c->stg_dev, c->stg_host, h2d, cudaMemcpyHostToDevice, c->stream));
+  if (h2d) CU_TRY(c, cudaMemcpyAsync(c->stg_dev.get(), c->stg_host.get(), h2d, cudaMemcpyHostToDevice, c->stream));
   rc = launch();
   if (rc) return rc;
   if (d2h)
-    CU_TRY(c, cudaMemcpyAsync(c->stg_host + end[STAGE_IN], c->stg_dev + end[STAGE_IN], d2h, cudaMemcpyDeviceToHost,
-                              c->stream));
+    CU_TRY(c, cudaMemcpyAsync(c->stg_host.get() + end[STAGE_IN], c->stg_dev.get() + end[STAGE_IN], d2h,
+                              cudaMemcpyDeviceToHost, c->stream));
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   return SL2_OK;
 }
@@ -225,7 +274,7 @@ cudaError_t copy_gray_blocks(const Sl2Dev &d, int slot, int lo, int hi, const ui
   return cudaMemcpy2DAsync(dst, d.pitch, src, d.W, d.W, (size_t)(hi - lo) * d.H, kind, st);
 }
 
-uint8_t *source_stage(const sl2_ctx *c, int slot) { return c->src_stage + (size_t)slot * c->src_slot_bytes; }
+uint8_t *source_stage(const sl2_ctx *c, int slot) { return c->src_stage.get() + (size_t)slot * c->src_slot_bytes; }
 
 // convert the raw frames of source rows [base, base + cnt) of `slot`'s staging into the ring
 cudaError_t ingest(sl2_ctx *c, int slot, int base, int cnt, Sl2Queue q) {
@@ -235,7 +284,7 @@ cudaError_t ingest(sl2_ctx *c, int slot, int base, int cnt, Sl2Queue q) {
     max_dh = std::max(max_dh, r.dh);
     max_rb = std::max(max_rb, r.sw * sl2_source_bpp(r.format));
   }
-  return sl2_launch_ingest(c->d, c->src_tab, base, cnt, max_dh, max_rb, source_stage(c, slot), slot, q);
+  return sl2_launch_ingest(c->d, c->src_tab.get(), base, cnt, max_dh, max_rb, source_stage(c, slot), slot, q);
 }
 
 // One frame slot of every stream, a frame set (sl2_frame_set_layout), into the frame ring: each run of consecutive
@@ -351,15 +400,18 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
 
   sl2_ctx *c = new sl2_ctx();
   c->cfg = *cfg;
+  // what exists is held by c's handles: a failure releases it through sl2_destroy
+  const auto failed = [c](int rc, const std::string &msg) {
+    g_create_error = msg;
+    sl2_destroy(c);
+    return rc;
+  };
   if (cfg->cuda_stream) {
     c->stream = static_cast<cudaStream_t>(cfg->cuda_stream);
   } else {
-    e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
-    if (e != cudaSuccess) {
-      delete c;
-      return fail(nullptr, SL2_ERR_CUDA, cudaGetErrorString(e));
-    }
-    c->own_stream = true;
+    e = cuda_stream_create(c->owned_stream);
+    if (e != cudaSuccess) return failed(SL2_ERR_CUDA, cudaGetErrorString(e));
+    c->stream = c->owned_stream.get();
   }
   Sl2Dev &d = c->d;
   memset(&d, 0, sizeof d);
@@ -400,12 +452,15 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   for (int s = 0; s <= d.B; ++s) c->layout[s] = (size_t)s * d.H * d.W;
   const std::vector<Sl2StreamCam> rows(d.B, cam_row(sc0));  // read by the copy below until the final synchronise
 
+  const auto alloc_failed = [&] {
+    return failed(SL2_ERR_CUDA, std::string("cudaMalloc failed: ") + cudaGetErrorString(cudaGetLastError()));
+  };
   const size_t B = d.B, N = d.Nmax;
-  bool ok = true;
-#define ALLOC(ptr, count) ok = ok && (dev_alloc(c, &(ptr), (count)) == cudaSuccess)
+#define ALLOC(ptr, count) \
+  if (dev_alloc(c, &(ptr), (count)) != cudaSuccess) return alloc_failed()
   ALLOC(d.cams, B);
-  ok = ok && cudaMemcpyAsync(d.cams, rows.data(), B * sizeof(Sl2StreamCam), cudaMemcpyHostToDevice, c->stream) ==
-                 cudaSuccess;
+  if (cudaMemcpyAsync(d.cams, rows.data(), B * sizeof(Sl2StreamCam), cudaMemcpyHostToDevice, c->stream) != cudaSuccess)
+    return alloc_failed();
   ALLOC(d.frames, (size_t)d.slots * B * d.H * d.pitch);
   ALLOC(d.patches, (B * N + SL2_MAX_PARTIAL) * d.box * 16);  // + scratch templates (partially-initialised features)
   ALLOC(d.x, B * d.ld);
@@ -423,46 +478,26 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   ALLOC(d.Wp, B * SL2_MAX_PANELS * 256);
   ALLOC(c->xv_stage, (size_t)d.slots * B * SL2_NXV);
 #undef ALLOC
-  if (!ok) {
-    const std::string m = std::string("cudaMalloc failed: ") + cudaGetErrorString(cudaGetLastError());
-    sl2_destroy(c);
-    return fail(nullptr, SL2_ERR_CUDA, m);
-  }
   int rc = make_tensor_map(c);
-  if (rc == SL2_OK && (sl2_configure_search(d) != cudaSuccess || sl2_configure_update(d) != cudaSuccess))
-    rc = fail(c, SL2_ERR_CUDA, std::string("kernel configuration failed: ") + cudaGetErrorString(cudaGetLastError()));
-  if (rc == SL2_OK) rc = stage_reserve(c, 1 << 20);
-  if (rc == SL2_OK) {
-    for (int i = 0; i < 5 && rc == SL2_OK; ++i)
-      if (cudaEventCreate(&c->ev[i]) != cudaSuccess) rc = SL2_ERR_CUDA;
-    for (int i = 0; i < 6 && rc == SL2_OK; ++i)
-      if (cudaEventCreate(&c->evu[i]) != cudaSuccess) rc = SL2_ERR_CUDA;
-    if (cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking) != cudaSuccess) rc = SL2_ERR_CUDA;
-    if (cudaStreamCreateWithFlags(&c->out_stream, cudaStreamNonBlocking) != cudaSuccess) rc = SL2_ERR_CUDA;
-    if (cudaStreamCreateWithFlags(&c->stream_b, cudaStreamNonBlocking) != cudaSuccess) rc = SL2_ERR_CUDA;
-    for (cudaEvent_t *e : {&c->ev_main, &c->ev_a_search, &c->ev_b_search, &c->ev_b_done})
-      if (cudaEventCreateWithFlags(e, cudaEventDisableTiming) != cudaSuccess) rc = SL2_ERR_CUDA;
-    for (int i = 0; i < d.slots && rc == SL2_OK; ++i) {
-      cudaEvent_t e1, e2, e3, e4;
-      if (cudaEventCreateWithFlags(&e1, cudaEventDisableTiming) != cudaSuccess ||
-          cudaEventCreateWithFlags(&e2, cudaEventDisableTiming) != cudaSuccess ||
-          cudaEventCreateWithFlags(&e3, cudaEventDisableTiming) != cudaSuccess ||
-          cudaEventCreateWithFlags(&e4, cudaEventDisableTiming) != cudaSuccess) {
-        rc = SL2_ERR_CUDA;
-        break;
-      }
-      c->ev_h2d.push_back(e1);
-      c->ev_cmp.push_back(e2);
-      c->ev_out.push_back(e3);
-      c->ev_cmp_b.push_back(e4);
-    }
-  }
-  if (rc == SL2_OK && cudaStreamSynchronize(c->stream) != cudaSuccess) rc = SL2_ERR_CUDA;
-  if (rc != SL2_OK) {
-    g_create_error = c->err.empty() ? "context initialisation failed" : c->err;
-    sl2_destroy(c);
-    return rc;
-  }
+  if (rc) return failed(rc, c->err);
+  if (sl2_configure_search(d) != cudaSuccess || sl2_configure_update(d) != cudaSuccess)
+    return failed(SL2_ERR_CUDA, std::string("kernel configuration failed: ") + cudaGetErrorString(cudaGetLastError()));
+  rc = stage_reserve(c, 1 << 20);
+  if (rc) return failed(rc, c->err);
+  const auto init_failed = [&] { return failed(SL2_ERR_CUDA, "context initialisation failed"); };
+  // the step-time events ev / evu keep the default (timing) flags; every other event only orders work
+  for (Event &e : c->ev)
+    if (cuda_event_create(e, cudaEventDefault) != cudaSuccess) return init_failed();
+  for (Event &e : c->evu)
+    if (cuda_event_create(e, cudaEventDefault) != cudaSuccess) return init_failed();
+  for (Stream *s : {&c->copy_stream, &c->out_stream, &c->stream_b})
+    if (cuda_stream_create(*s) != cudaSuccess) return init_failed();
+  c->ev_slot.resize(d.slots);
+  std::vector<Event *> untimed = {&c->ev_main, &c->ev_a_search, &c->ev_b_search, &c->ev_b_done};
+  for (SlotEvents &s : c->ev_slot) untimed.insert(untimed.end(), {&s.h2d, &s.cmp, &s.cmp_b, &s.out});
+  for (Event *e : untimed)
+    if (cuda_event_create(*e, cudaEventDisableTiming) != cudaSuccess) return init_failed();
+  if (cudaStreamSynchronize(c->stream) != cudaSuccess) return init_failed();
   *out = c;
   return SL2_OK;
 }
@@ -470,45 +505,17 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
 void sl2_destroy(sl2_ctx *c) {
   if (!c) return;
   enter(c);
-  if (c->stream) cudaStreamSynchronize(c->stream);
-  if (c->copy_stream) {
-    cudaStreamSynchronize(c->copy_stream);
-    cudaStreamDestroy(c->copy_stream);
-  }
-  if (c->out_stream) {
-    cudaStreamSynchronize(c->out_stream);
-    cudaStreamDestroy(c->out_stream);
-  }
-  if (c->stream_b) {
-    cudaStreamSynchronize(c->stream_b);
-    cudaStreamDestroy(c->stream_b);
-  }
-  for (auto &v : {c->ev_h2d, c->ev_cmp, c->ev_out, c->ev_cmp_b})
-    for (cudaEvent_t e : v) cudaEventDestroy(e);
-  for (cudaEvent_t e : {c->ev_main, c->ev_a_search, c->ev_b_search, c->ev_b_done})
-    if (e) cudaEventDestroy(e);
-  for (void *p : c->allocs) cudaFree(p);
-  if (c->d.rec) cudaFree(c->d.rec);
-  if (c->src_tab) cudaFree(c->src_tab);
-  if (c->src_stage) cudaFree(c->src_stage);
-  if (c->ev_src) cudaEventDestroy(c->ev_src);
-  if (c->stg_dev) cudaFree(c->stg_dev);
-  if (c->smoe_map) cudaFree(c->smoe_map);
-  if (c->stg_host) cudaFreeHost(c->stg_host);
-  for (auto &e : c->ev)
-    if (e) cudaEventDestroy(e);
-  for (auto &e : c->evu)
-    if (e) cudaEventDestroy(e);
-  if (c->own_stream && c->stream) cudaStreamDestroy(c->stream);
-  delete c;
+  for (cudaStream_t s : {c->stream, c->copy_stream.get(), c->out_stream.get(), c->stream_b.get()})
+    if (s) cudaStreamSynchronize(s);
+  delete c;  // its handles release everything it created
 }
 
 int sl2_sync(sl2_ctx *c) {
   if (!c) return SL2_ERR_ARG;
   enter(c);
   CU_TRY(c, cudaStreamSynchronize(c->stream));
-  if (c->copy_stream) CU_TRY(c, cudaStreamSynchronize(c->copy_stream));
-  if (c->out_stream) CU_TRY(c, cudaStreamSynchronize(c->out_stream));
+  if (c->copy_stream) CU_TRY(c, cudaStreamSynchronize(c->copy_stream.get()));
+  if (c->out_stream) CU_TRY(c, cudaStreamSynchronize(c->out_stream.get()));
   return SL2_OK;
 }
 
@@ -570,27 +577,29 @@ static int install_sources(sl2_ctx *c, const std::vector<sl2_stream_source> &src
   const size_t slot_bytes = (raw + 15) & ~(size_t)15;
   const size_t need = rows.empty() ? 0 : (size_t)d.slots * slot_bytes + 16;
   // every allocation before anything changes: a failed one leaves the sources, the staging and the table as they were
+  DevPtr<uint8_t> stage;
   if (need > c->src_stage_bytes) {  // nothing may still read or write the old staging
     CU_TRY(c, cudaStreamSynchronize(c->stream));
-    CU_TRY(c, cudaStreamSynchronize(c->copy_stream));
-    uint8_t *stage = nullptr;
-    CU_TRY(c, cudaMalloc((void **)&stage, need));
-    if (c->src_stage) cudaFree(c->src_stage);
-    c->src_stage = stage;
+    CU_TRY(c, cudaStreamSynchronize(c->copy_stream.get()));
+    CU_TRY(c, cuda_malloc(stage, need));
+  }
+  if (!rows.empty() && !c->src_tab) CU_TRY(c, cuda_malloc(c->src_tab, sizeof(Sl2Source) * d.B));
+  if (!rows.empty() && !c->ev_src) CU_TRY(c, cuda_event_create(c->ev_src, cudaEventDisableTiming));
+  if (stage) {
+    c->src_stage = std::move(stage);
     c->src_stage_bytes = need;
   }
-  if (!rows.empty() && !c->src_tab) CU_TRY(c, cudaMalloc((void **)&c->src_tab, sizeof(Sl2Source) * d.B));
-  if (!rows.empty() && !c->ev_src) CU_TRY(c, cudaEventCreateWithFlags(&c->ev_src, cudaEventDisableTiming));
   if (!rows.empty()) {
-    for (cudaEvent_t e : c->ev_h2d) CU_TRY(c, cudaStreamWaitEvent(c->stream, e, 0));  // conversions in flight
+    for (const SlotEvents &e : c->ev_slot)  // conversions in flight
+      CU_TRY(c, cudaStreamWaitEvent(c->stream, e.h2d.get(), 0));
     for (size_t first = 0; first < rows.size(); first += SL2_SOURCE_CHUNK) {
       Sl2SourceChunk ch = {};
       ch.first = (int)first;
       ch.n = (int)std::min(rows.size() - first, (size_t)SL2_SOURCE_CHUNK);
       for (int i = 0; i < ch.n; ++i) ch.row[i] = rows[first + i];
-      CU_TRY(c, sl2_launch_source_write(c->src_tab, ch, queue(c)));
+      CU_TRY(c, sl2_launch_source_write(c->src_tab.get(), ch, queue(c)));
     }
-    CU_TRY(c, cudaEventRecord(c->ev_src, c->stream));
+    CU_TRY(c, cudaEventRecord(c->ev_src.get(), c->stream));
   }
   c->srcs = srcs;
   c->layout = layout;
@@ -664,7 +673,7 @@ int sl2_set_frame(sl2_ctx *c, int32_t s, int32_t slot, const uint8_t *gray, size
     const sl2_stream_config &sc = c->cams[s];  // the stream's image, top-left of its block
     CU_TRY(c, cudaMemcpy2DAsync(dst, d.pitch, gray, stride, sc.width, sc.height, cudaMemcpyHostToDevice, c->stream));
   }
-  CU_TRY(c, cudaEventRecord(c->ev_cmp[slot], c->stream));  // slot busy until the copy has landed
+  CU_TRY(c, cudaEventRecord(c->ev_slot[slot].cmp.get(), c->stream));  // slot busy until the copy has landed
   return SL2_OK;
 }
 
@@ -672,7 +681,7 @@ static int set_frames_any(sl2_ctx *c, int32_t slot, const uint8_t *gray, cudaMem
   enter(c);
   if (!c || bad_slot(c, slot) || !gray) return fail(c, SL2_ERR_ARG, "sl2_set_frames: bad argument");
   CU_TRY(c, copy_slot_frames(c, slot, gray, kind, queue(c)));
-  CU_TRY(c, cudaEventRecord(c->ev_cmp[slot], c->stream));  // slot busy until the copy has landed
+  CU_TRY(c, cudaEventRecord(c->ev_slot[slot].cmp.get(), c->stream));  // slot busy until the copy has landed
   return SL2_OK;
 }
 int sl2_set_frames(sl2_ctx *c, int32_t slot, const uint8_t *gray) {
@@ -859,15 +868,8 @@ static int partial_features(sl2_ctx *c, int32_t s, int32_t slot, const PartialIO
       if (io.feat_index[f] < 0 || io.feat_index[f] >= nf)
         return fail(c, SL2_ERR_ARG, std::string(who) + ": feature index out of range");
   }
-  const size_t map_bytes = sl2_smoe_map_bytes(d, F);
-  if (map_bytes > c->smoe_map_bytes) {
-    CU_TRY(c, cudaStreamSynchronize(c->stream));
-    if (c->smoe_map) cudaFree(c->smoe_map);
-    c->smoe_map = nullptr;
-    c->smoe_map_bytes = 0;
-    CU_TRY(c, cudaMalloc(&c->smoe_map, map_bytes));
-    c->smoe_map_bytes = map_bytes;
-  }
+  const int grown = grow_scratch(c, sl2_smoe_map_bytes(d, F), c->smoe_map_bytes, c->smoe_map);
+  if (grown) return grown;
   // h / Sinv3 / detS: outputs of the prediction, else inputs; prob: rewritten by the re-weighting
   const size_t n = (size_t)F * Kmax, nF = F;
   Stage K{STAGE_IN, 4 * nF, io.K}, ft{STAGE_IN, 4 * nF}, ypi{STAGE_IN, 48 * nF, io.ypi},
@@ -892,7 +894,7 @@ static int partial_features(sl2_ctx *c, int32_t s, int32_t slot, const PartialIO
                                                 Sinv3.dev<double>(), detS.dev<double>(), queue(c)));
         // measure_feature_with_multiple_priors (monoslam.cpp:1408-1438): ellipses (SInv_k, h_k), one template per feature
         CU_TRY(c, sl2_launch_smoe(d, s, slot, F, Kmax, K.dev<int>(), ft.dev<int>(), h.dev<double>(), Sinv3.dev<double>(),
-                                  c->smoe_map, uv.dev<int>(), found.d, nullptr, queue(c)));
+                                  c->smoe_map.get(), uv.dev<int>(), found.d, nullptr, queue(c)));
         if (reweight)
           CU_TRY(c, sl2_launch_particles(F, Kmax, K.dev<int>(), h.dev<double>(), Sinv3.dev<double>(),
                                          detS.dev<double>(), lam.dev<double>(), uv.dev<int>(), found.d, io.prune,
@@ -1152,9 +1154,9 @@ int sl2_normalise_state(sl2_ctx *c, int32_t s) {
 static int step_group(sl2_ctx *c, int32_t slot, int lo, int cnt, Sl2Queue q, cudaEvent_t after_search, bool t) {
   const Sl2Dev &d = c->d;
   const cudaStream_t st = q.stream;
-  if (t) CU_TRY(c, cudaEventRecord(c->ev[0], st));
+  if (t) CU_TRY(c, cudaEventRecord(c->ev[0].get(), st));
   CU_TRY(c, sl2_launch_predict(d, lo, cnt, nullptr, 1, 1, q));
-  if (t) CU_TRY(c, cudaEventRecord(c->ev[1], st));
+  if (t) CU_TRY(c, cudaEventRecord(c->ev[1].get(), st));
   SearchLaunch L = {};
   // job arrays are indexed by the stream number local to the launch
   L.job_feat = d.job_feat + (size_t)lo * d.Nmax;
@@ -1166,12 +1168,14 @@ static int step_group(sl2_ctx *c, int32_t slot, int lo, int cnt, Sl2Queue q, cud
   L.slot = slot;
   L.scatter_to_features = 1;
   CU_TRY(c, sl2_launch_search(d, c->tmap, L, q));
-  if (t) CU_TRY(c, cudaEventRecord(c->ev[2], st));
+  if (t) CU_TRY(c, cudaEventRecord(c->ev[2].get(), st));
   if (after_search) CU_TRY(c, cudaEventRecord(after_search, st));
-  CU_TRY(c, sl2_launch_update(d, lo, cnt, -1, nullptr, nullptr, nullptr, nullptr, nullptr, 0, q, t ? c->evu : nullptr));
-  if (t) CU_TRY(c, cudaEventRecord(c->ev[3], st));
+  cudaEvent_t evu[6];
+  for (int i = 0; i < 6; ++i) evu[i] = c->evu[i].get();
+  CU_TRY(c, sl2_launch_update(d, lo, cnt, -1, nullptr, nullptr, nullptr, nullptr, nullptr, 0, q, t ? evu : nullptr));
+  if (t) CU_TRY(c, cudaEventRecord(c->ev[3].get(), st));
   CU_TRY(c, sl2_launch_cull(d, lo, cnt, -1, q));
-  if (t) CU_TRY(c, cudaEventRecord(c->ev[4], st));
+  if (t) CU_TRY(c, cudaEventRecord(c->ev[4].get(), st));
   if (d.rec_depth)  // after ev[4]: the step times keep their meaning
     CU_TRY(c, sl2_launch_records(d, lo, cnt, c->rec_steps, q));
   return SL2_OK;
@@ -1190,16 +1194,16 @@ static int step_enqueue_groups(sl2_ctx *c, int32_t slot, bool serial) {
     return step_group(c, slot, 0, d.B, queue(c), nullptr, c->timing);
   }
   // group B sees everything `stream` has done so far (uploads, staged calls, the frame copy)
-  CU_TRY(c, cudaEventRecord(c->ev_main, c->stream));
-  CU_TRY(c, cudaStreamWaitEvent(c->stream_b, c->ev_main, 0));
-  if (c->b_search_valid) CU_TRY(c, cudaStreamWaitEvent(c->stream, c->ev_b_search, 0));
-  int rc = step_group(c, slot, 0, BA, queue(c), c->ev_a_search, false);
+  CU_TRY(c, cudaEventRecord(c->ev_main.get(), c->stream));
+  CU_TRY(c, cudaStreamWaitEvent(c->stream_b.get(), c->ev_main.get(), 0));
+  if (c->b_search_valid) CU_TRY(c, cudaStreamWaitEvent(c->stream, c->ev_b_search.get(), 0));
+  int rc = step_group(c, slot, 0, BA, queue(c), c->ev_a_search.get(), false);
   if (rc) return rc;
-  CU_TRY(c, cudaStreamWaitEvent(c->stream_b, c->ev_a_search, 0));
-  rc = step_group(c, slot, BA, d.B - BA, {c->stream_b, &c->launches}, c->ev_b_search, false);
+  CU_TRY(c, cudaStreamWaitEvent(c->stream_b.get(), c->ev_a_search.get(), 0));
+  rc = step_group(c, slot, BA, d.B - BA, {c->stream_b.get(), &c->launches}, c->ev_b_search.get(), false);
   if (rc) return rc;
   c->b_search_valid = true;
-  CU_TRY(c, cudaEventRecord(c->ev_b_done, c->stream_b));
+  CU_TRY(c, cudaEventRecord(c->ev_b_done.get(), c->stream_b.get()));
   c->b_pending = true;
   return SL2_OK;
 }
@@ -1212,8 +1216,8 @@ static int step_enqueue(sl2_ctx *c, int32_t slot, bool serial = false) {
 
 // the slot's frames are busy until everything queued so far on the step stream(s) has run
 static int mark_slot_busy(sl2_ctx *c, int32_t slot) {
-  CU_TRY(c, cudaEventRecord(c->ev_cmp[slot], c->stream));
-  if (c->b_pending) CU_TRY(c, cudaEventRecord(c->ev_cmp_b[slot], c->stream_b));
+  CU_TRY(c, cudaEventRecord(c->ev_slot[slot].cmp.get(), c->stream));
+  if (c->b_pending) CU_TRY(c, cudaEventRecord(c->ev_slot[slot].cmp_b.get(), c->stream_b.get()));
   return SL2_OK;
 }
 
@@ -1243,18 +1247,18 @@ int sl2_step_host_async(sl2_ctx *c, int32_t slot, const uint8_t *gray, double *x
   enter(c, false);
   if (!c || bad_slot(c, slot) || !gray) return fail(c, SL2_ERR_ARG, "sl2_step_host_async: bad argument");
   const Sl2Dev &d = c->d;
-  cudaStream_t cs = c->copy_stream;
+  cudaStream_t cs = c->copy_stream.get();
   // the frame slot may still be in use by work queued earlier on it: ev_cmp[slot] / ev_cmp_b[slot] are recorded
   // behind EVERY operation that reads or writes the slot (fused steps of either stream group, sl2_set_frame(s));
   // the remaining slot users (staged searches, detector, particles) synchronise the stream before they return.
   // Work on OTHER slots is not waited for: the copy of frame t+1 overlaps the kernels of frame t.
-  CU_TRY(c, cudaStreamWaitEvent(cs, c->ev_cmp[slot], 0));
-  CU_TRY(c, cudaStreamWaitEvent(cs, c->ev_cmp_b[slot], 0));
-  if (!c->src_rows.empty()) CU_TRY(c, cudaStreamWaitEvent(cs, c->ev_src, 0));  // the current source table
+  CU_TRY(c, cudaStreamWaitEvent(cs, c->ev_slot[slot].cmp.get(), 0));
+  CU_TRY(c, cudaStreamWaitEvent(cs, c->ev_slot[slot].cmp_b.get(), 0));
+  if (!c->src_rows.empty()) CU_TRY(c, cudaStreamWaitEvent(cs, c->ev_src.get(), 0));  // the current source table
   CU_TRY(c, copy_slot_frames(c, slot, gray, cudaMemcpyHostToDevice, {cs, &c->launches}));
-  CU_TRY(c, cudaEventRecord(c->ev_h2d[slot], cs));
-  CU_TRY(c, cudaStreamWaitEvent(c->stream, c->ev_h2d[slot], 0));
-  CU_TRY(c, cudaStreamWaitEvent(c->stream, c->ev_out[slot], 0));  // staging buffer of this slot is free
+  CU_TRY(c, cudaEventRecord(c->ev_slot[slot].h2d.get(), cs));
+  CU_TRY(c, cudaStreamWaitEvent(c->stream, c->ev_slot[slot].h2d.get(), 0));
+  CU_TRY(c, cudaStreamWaitEvent(c->stream, c->ev_slot[slot].out.get(), 0));  // staging buffer of this slot is free
   int rc = step_enqueue(c, slot);
   if (rc) return rc;
   // camera states of this step -> per-slot staging (each group on its own stream) -> host
@@ -1263,20 +1267,20 @@ int sl2_step_host_async(sl2_ctx *c, int32_t slot, const uint8_t *gray, double *x
   const int nA = BA ? BA : d.B;
   CU_TRY(c, cudaMemcpy2DAsync(stage, sizeof(double) * SL2_NXV, d.x, sizeof(double) * d.ld,
                               sizeof(double) * SL2_NXV, nA, cudaMemcpyDeviceToDevice, c->stream));
-  CU_TRY(c, cudaEventRecord(c->ev_cmp[slot], c->stream));
-  CU_TRY(c, cudaStreamWaitEvent(c->out_stream, c->ev_cmp[slot], 0));
+  CU_TRY(c, cudaEventRecord(c->ev_slot[slot].cmp.get(), c->stream));
+  CU_TRY(c, cudaStreamWaitEvent(c->out_stream.get(), c->ev_slot[slot].cmp.get(), 0));
   if (BA) {
     CU_TRY(c, cudaMemcpy2DAsync(stage + (size_t)BA * SL2_NXV, sizeof(double) * SL2_NXV,
                                 d.x + (size_t)BA * d.ld, sizeof(double) * d.ld, sizeof(double) * SL2_NXV,
-                                d.B - BA, cudaMemcpyDeviceToDevice, c->stream_b));
-    CU_TRY(c, cudaEventRecord(c->ev_cmp_b[slot], c->stream_b));
-    CU_TRY(c, cudaEventRecord(c->ev_b_done, c->stream_b));
-    CU_TRY(c, cudaStreamWaitEvent(c->out_stream, c->ev_cmp_b[slot], 0));
+                                d.B - BA, cudaMemcpyDeviceToDevice, c->stream_b.get()));
+    CU_TRY(c, cudaEventRecord(c->ev_slot[slot].cmp_b.get(), c->stream_b.get()));
+    CU_TRY(c, cudaEventRecord(c->ev_b_done.get(), c->stream_b.get()));
+    CU_TRY(c, cudaStreamWaitEvent(c->out_stream.get(), c->ev_slot[slot].cmp_b.get(), 0));
   }
   if (xv_out)
     CU_TRY(c, cudaMemcpyAsync(xv_out, stage, sizeof(double) * SL2_NXV * d.B, cudaMemcpyDeviceToHost,
-                              c->out_stream));
-  CU_TRY(c, cudaEventRecord(c->ev_out[slot], c->out_stream));
+                              c->out_stream.get()));
+  CU_TRY(c, cudaEventRecord(c->ev_slot[slot].out.get(), c->out_stream.get()));
   return SL2_OK;
 }
 
@@ -1296,7 +1300,7 @@ int sl2_set_step_groups(sl2_ctx *c, int32_t groups) {
 int sl2_wait_slot(sl2_ctx *c, int32_t slot) {
   enter(c);
   if (!c || bad_slot(c, slot)) return fail(c, SL2_ERR_ARG, "sl2_wait_slot: bad slot");
-  CU_TRY(c, cudaEventSynchronize(c->ev_out[slot]));
+  CU_TRY(c, cudaEventSynchronize(c->ev_slot[slot].out.get()));
   return SL2_OK;
 }
 
@@ -1311,8 +1315,8 @@ int sl2_last_step_times(sl2_ctx *c, float *ms4) {
   enter(c);
   if (!c || !ms4) return SL2_ERR_ARG;
   if (!c->timing) return fail(c, SL2_ERR_STATE, "timing not enabled");
-  CU_TRY(c, cudaEventSynchronize(c->ev[4]));
-  for (int i = 0; i < 4; ++i) CU_TRY(c, cudaEventElapsedTime(&ms4[i], c->ev[i], c->ev[i + 1]));
+  CU_TRY(c, cudaEventSynchronize(c->ev[4].get()));
+  for (int i = 0; i < 4; ++i) CU_TRY(c, cudaEventElapsedTime(&ms4[i], c->ev[i].get(), c->ev[i + 1].get()));
   return SL2_OK;
 }
 
@@ -1349,8 +1353,8 @@ int sl2_last_update_times(sl2_ctx *c, float *ms5) {
   enter(c);
   if (!c || !ms5) return SL2_ERR_ARG;
   if (!c->timing) return fail(c, SL2_ERR_STATE, "timing not enabled");
-  CU_TRY(c, cudaEventSynchronize(c->evu[5]));
-  for (int i = 0; i < 5; ++i) CU_TRY(c, cudaEventElapsedTime(&ms5[i], c->evu[i], c->evu[i + 1]));
+  CU_TRY(c, cudaEventSynchronize(c->evu[5].get()));
+  for (int i = 0; i < 5; ++i) CU_TRY(c, cudaEventElapsedTime(&ms5[i], c->evu[i].get(), c->evu[i + 1].get()));
   return SL2_OK;
 }
 
@@ -1466,13 +1470,13 @@ int sl2_save_streams(sl2_ctx *c, int32_t lo, int32_t cnt, void *buf, size_t stri
   CU_TRY(c, cudaStreamSynchronize(c->stream));  // staging buffer reuse
   for (int i0 = 0; i0 < cnt; i0 += g) {
     const int k = std::min(g, cnt - i0);
-    CU_TRY(c, sl2_launch_pack(c->d, lo + i0, k, c->stg_dev, sb, queue(c)));
-    CU_TRY(c, cudaMemcpyAsync(c->stg_host, c->stg_dev, (size_t)k * sb, cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(c, sl2_launch_pack(c->d, lo + i0, k, c->stg_dev.get(), sb, queue(c)));
+    CU_TRY(c, cudaMemcpyAsync(c->stg_host.get(), c->stg_dev.get(), (size_t)k * sb, cudaMemcpyDeviceToHost, c->stream));
     CU_TRY(c, cudaStreamSynchronize(c->stream));
     for (int i = 0; i < k; ++i) {
       sl2_snapshot_header h;
-      memcpy(&h, c->stg_host + (size_t)i * sb, sizeof h);
-      memcpy(static_cast<uint8_t *>(buf) + (size_t)(i0 + i) * stride, c->stg_host + (size_t)i * sb, h.total_bytes);
+      memcpy(&h, c->stg_host.get() + (size_t)i * sb, sizeof h);
+      memcpy(static_cast<uint8_t *>(buf) + (size_t)(i0 + i) * stride, c->stg_host.get() + (size_t)i * sb, h.total_bytes);
       if (sizes) sizes[i0 + i] = h.total_bytes;
     }
   }
@@ -1511,16 +1515,16 @@ int sl2_load_streams(sl2_ctx *c, int32_t lo, int32_t cnt, const void *buf, size_
   for (int i0 = 0; i0 < cnt; i0 += g) {
     const int k = std::min(g, cnt - i0);
     CU_TRY(c, cudaStreamSynchronize(c->stream));  // the previous group's unpack has read the staging buffer
-    memcpy(c->stg_host, q.data() + i0, (size_t)k * sizeof(Sl2SnapLoad));
+    memcpy(c->stg_host.get(), q.data() + i0, (size_t)k * sizeof(Sl2SnapLoad));
     size_t end = 0;
     for (int i = 0; i < k; ++i) {
       const size_t tb = sl2_snap_layout(q[i0 + i].nfeat, c->cfg.boxsize).total;
-      memcpy(c->stg_host + pb + (size_t)i * sb, in + (size_t)(i0 + i) * stride, tb);
+      memcpy(c->stg_host.get() + pb + (size_t)i * sb, in + (size_t)(i0 + i) * stride, tb);
       end = pb + (size_t)i * sb + tb;
     }
-    CU_TRY(c, cudaMemcpyAsync(c->stg_dev, c->stg_host, end, cudaMemcpyHostToDevice, c->stream));
-    CU_TRY(c, sl2_launch_unpack(c->d, k, reinterpret_cast<const Sl2SnapLoad *>(c->stg_dev), c->stg_dev + pb, sb,
-                                queue(c)));
+    CU_TRY(c, cudaMemcpyAsync(c->stg_dev.get(), c->stg_host.get(), end, cudaMemcpyHostToDevice, c->stream));
+    CU_TRY(c, sl2_launch_unpack(c->d, k, reinterpret_cast<const Sl2SnapLoad *>(c->stg_dev.get()),
+                                c->stg_dev.get() + pb, sb, queue(c)));
   }
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   return loaded_cameras(c, lo, cams);
@@ -1538,21 +1542,21 @@ int sl2_load_streams_dev(sl2_ctx *c, int32_t lo, int32_t cnt, const void *buf_de
   int rc = stage_reserve(c, o_h + (size_t)cnt * hb);
   if (rc) return rc;
   CU_TRY(c, cudaStreamSynchronize(c->stream));
-  CU_TRY(c, cudaMemcpy2DAsync(c->stg_host + o_h, hb, in, stride, hb, cnt, cudaMemcpyDeviceToHost, c->stream));
+  CU_TRY(c, cudaMemcpy2DAsync(c->stg_host.get() + o_h, hb, in, stride, hb, cnt, cudaMemcpyDeviceToHost, c->stream));
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   std::vector<Sl2SnapLoad> q(cnt);
   std::vector<sl2_stream_config> cams(cnt);
   for (int i = 0; i < cnt; ++i) {
-    const uint8_t *h = c->stg_host + o_h + (size_t)i * hb;
+    const uint8_t *h = c->stg_host.get() + o_h + (size_t)i * hb;
     rc = snap_validate(c, h, stride, false, lo + i, &q[i], "sl2_load_streams_dev");
     if (rc) return rc;
     memcpy(&cams[i], h + offsetof(sl2_snapshot_header, cam), sizeof(sl2_stream_config));
   }
-  memcpy(c->stg_host, q.data(), (size_t)cnt * sizeof(Sl2SnapLoad));
-  memset(c->stg_host + o_bad, 0, sizeof(int));
-  CU_TRY(c, cudaMemcpyAsync(c->stg_dev, c->stg_host, o_bad + sizeof(int), cudaMemcpyHostToDevice, c->stream));
-  const Sl2SnapLoad *q_dev = reinterpret_cast<const Sl2SnapLoad *>(c->stg_dev);
-  int *bad_dev = reinterpret_cast<int *>(c->stg_dev + o_bad);
+  memcpy(c->stg_host.get(), q.data(), (size_t)cnt * sizeof(Sl2SnapLoad));
+  memset(c->stg_host.get() + o_bad, 0, sizeof(int));
+  CU_TRY(c, cudaMemcpyAsync(c->stg_dev.get(), c->stg_host.get(), o_bad + sizeof(int), cudaMemcpyHostToDevice, c->stream));
+  const Sl2SnapLoad *q_dev = reinterpret_cast<const Sl2SnapLoad *>(c->stg_dev.get());
+  int *bad_dev = reinterpret_cast<int *>(c->stg_dev.get() + o_bad);
   CU_TRY(c, sl2_launch_snap_check(c->d, cnt, q_dev, in, stride, bad_dev, queue(c)));
   int bad = 0;
   CU_TRY(c, cudaMemcpyAsync(&bad, bad_dev, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
@@ -1570,24 +1574,18 @@ int sl2_enable_records(sl2_ctx *c, int32_t depth) {
   if (depth < 0 || depth > SL2_MAX_RECORDS)
     return fail(c, SL2_ERR_ARG, "sl2_enable_records: depth outside [0, SL2_MAX_RECORDS]");
   // the new ring first, so that a failed allocation leaves the old one in place
-  sl2_step_record *ring = nullptr;
+  DevPtr<sl2_step_record> ring;
+  cudaError_t e = cudaSuccess;
   if (depth) {
     const size_t bytes = (size_t)c->d.B * depth * sizeof(sl2_step_record);
-    CU_TRY(c, cudaMalloc((void **)&ring, bytes));
-    const cudaError_t e = cudaMemsetAsync(ring, 0, bytes, c->stream);
-    if (e != cudaSuccess) {
-      cudaFree(ring);
-      return fail(c, SL2_ERR_CUDA, std::string("sl2_enable_records: ") + cudaGetErrorString(e));
-    }
+    CU_TRY(c, cuda_malloc(ring, bytes));
+    e = cudaMemsetAsync(ring.get(), 0, bytes, c->stream);
   }
   // steps queued before the call (either group: enter() joined them) have written the old ring
-  const cudaError_t e = cudaStreamSynchronize(c->stream);
-  if (e != cudaSuccess) {
-    if (ring) cudaFree(ring);
-    return fail(c, SL2_ERR_CUDA, std::string("sl2_enable_records: ") + cudaGetErrorString(e));
-  }
-  if (c->d.rec) cudaFree(c->d.rec);
-  c->d.rec = ring;
+  if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+  if (e != cudaSuccess) return fail(c, SL2_ERR_CUDA, std::string("sl2_enable_records: ") + cudaGetErrorString(e));
+  c->rec = std::move(ring);
+  c->d.rec = c->rec.get();
   c->d.rec_depth = depth;
   c->rec_steps = 0;
   return SL2_OK;
