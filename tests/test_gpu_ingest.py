@@ -6,31 +6,14 @@ import numpy as np
 import pytest
 
 import ingest_ref as ir
-from gpu_util import ctx_from_scenes, sl2, synth
+from gpu_util import assert_same_bytes, ctx_from_scenes, ring_block, sl2, stream_result, synth
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 G8, RGB, UYVY = ir.SRC_GRAY8, ir.SRC_RGB24, ir.SRC_UYVY
 
 
-def _ring(img, H, W, rng):
-    """A ring block of H x W with the image top-left and fresh noise everywhere else."""
-    out = rng.integers(0, 256, (H, W), dtype=np.uint8)
-    out[:img.shape[0], :img.shape[1]] = img
-    return out
-
-
 def _frame_set(blocks):
     return np.concatenate([np.ascontiguousarray(b, np.uint8).ravel() for b in blocks])
-
-
-def _state(ctx, s):
-    x, P = ctx.get_state(s)
-    return dict(x=x, P=P, **ctx.features(s))
-
-
-def _assert_same(a, b, where):
-    for k in a:
-        assert a[k].tobytes() == b[k].tobytes(), (where, k)
 
 
 def _fixture_contexts(rng):
@@ -89,7 +72,7 @@ def test_fixture_frames_give_the_restatements_ring_bytes():
     raws = [z["raw_%d" % k] for k in range(n)]
     grays = [z["gray_%d" % k] for k in range(n)]
     a.set_frames(0, _frame_set(raws))
-    b.set_frames(0, np.stack([_ring(g, H, W, rng) for g in grays]))
+    b.set_frames(0, np.stack([ring_block(g, H, W, rng) for g in grays]))
     _compare_ring(a, b, cases, 0, rng)
     for s in range(n):  # one stream at a time, raw rows 7 bytes apart more than their length
         r = raws[s]
@@ -97,7 +80,7 @@ def test_fixture_frames_give_the_restatements_ring_bytes():
         padded[:, :r.shape[1]] = r
         assert a.L.sl2_set_frame(a.h, s, 1, padded.ctypes.data, padded.strides[0]) == 0
     a.sync()
-    b.set_frames(1, np.stack([_ring(g, H, W, rng) for g in grays]))
+    b.set_frames(1, np.stack([ring_block(g, H, W, rng) for g in grays]))
     _compare_ring(a, b, cases, 1, rng)
     a.close()
     b.close()
@@ -127,7 +110,7 @@ def test_camera_sizes_and_the_widest_rows():
                     rng.integers(0, 256, (sh, sw * ir.BPP[fmt]), dtype=np.uint8))
         grays.append(ir.ingest(fmt, raws[-1], sw, sh, dw, dh))
     a.set_frames(0, _frame_set(raws))
-    b.set_frames(0, np.stack([_ring(g, 240, 320, rng) for g in grays]))
+    b.set_frames(0, np.stack([ring_block(g, 240, 320, rng) for g in grays]))
     _compare_ring(a, b, cases, 0, rng)
     a.close()
     b.close()
@@ -163,14 +146,14 @@ def test_a_load_changes_the_resize_target():
         for c in (host, dev):
             c.set_frames(0, raw)
             c.step(0)
-        ref.set_frames(0, _ring(ir.ingest(RGB, raw, 640, 480, 288, 224), 240, 320, rng)[None])
+        ref.set_frames(0, ring_block(ir.ingest(RGB, raw, 640, 480, 288, 224), 240, 320, rng)[None])
         if t == 1:  # the ring itself, whether or not the tracker finds its features in the resized image
             for c in (host, dev):
                 _compare_ring(c, ref, [(RGB, 640, 480, 288, 224)], 0, rng)
         ref.step(0)
-        want = _state(ref, 0)
-        _assert_same(_state(host, 0), want, ("host", t))
-        _assert_same(_state(dev, 0), want, ("dev", t))
+        want = stream_result(ref, 0)
+        assert_same_bytes(stream_result(host, 0), want, ("host", t))
+        assert_same_bytes(stream_result(dev, 0), want, ("dev", t))
     for c in (host, dev, ref):
         c.close()
 
@@ -236,9 +219,9 @@ def test_whole_step_with_mixed_sources_equals_the_gray_path():
     rec = ref.records()
     assert rec.shape == (nS, T)
     for s in range(nS):
-        want = _state(ref, s)
+        want = stream_result(ref, s)
         for k, c in runs.items():
-            _assert_same(_state(c, s), want, (k, s))
+            assert_same_bytes(stream_result(c, s), want, (k, s))
     for k, c in runs.items():
         assert c.records().tobytes() == rec.tobytes(), k
     assert xv[(T - 1) % 3].numpy().tobytes() == np.stack([ref.get_state(s)[0][:13] for s in range(nS)]).tobytes()
@@ -288,7 +271,7 @@ def test_source_change_mid_run_and_resize_target_change():
         c.set_frames(0, sets[t])
         c.step(0)
     for s in range(2):
-        _assert_same(_state(a, s), _state(c, s), s)
+        assert_same_bytes(stream_result(a, s), stream_result(c, s), s)
     for x in (a, r, c):
         x.close()
     # the resize target follows sl2_set_stream_config
@@ -303,10 +286,10 @@ def test_source_change_mid_run_and_resize_target_change():
         raw = ir.raw_like(RGB, ir.upsample2(sc.frames[t]), rng)
         dw, dh = (320, 240) if t < 2 else (288, 224)
         d.set_frames(0, raw)
-        e.set_frames(0, _ring(ir.ingest(RGB, raw, 640, 480, dw, dh), 240, 320, rng)[None])
+        e.set_frames(0, ring_block(ir.ingest(RGB, raw, 640, 480, dw, dh), 240, 320, rng)[None])
         d.step(0)
         e.step(0)
-        _assert_same(_state(d, 0), _state(e, 0), t)
+        assert_same_bytes(stream_result(d, 0), stream_result(e, 0), t)
     d.close()
     e.close()
 

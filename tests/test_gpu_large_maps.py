@@ -11,13 +11,13 @@ import subprocess
 import numpy as np
 import pytest
 
-from gpu_util import (assert_state_close, check_streams_against_oracle, ctx_from_scenes, oracle_slam_from_scene,
-                      synth)
-from test_gpu_update_shapes import RESULT_KEYS, T, Replay, _assert_same, _result, record_oracle
+from gpu_util import (assert_same_bytes, assert_state_close, ctx_from_scenes, large_variant, oracle_slam_from_scene,
+                      random_measurements, record_oracle, run_regimes, step_frames, stream_result, synth)
 
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+T = 12           # frames per run; the bad features are culled by the 10th step
 N_SELECT = 128   # SL2_MAX_MEASURED: the largest selection a map above 128 features may ask for
 
 # capacity -> variants (nf, in view, bad, the edge the variant exists for).  Features from index `in view` on are
@@ -44,25 +44,6 @@ VARIANTS = {
 }
 
 
-def large_variant(nf, in_view, bad=0, stream_id=0, n_frames=T, n_select=N_SELECT):
-    """C4-sized scene of nf features; features >= in_view moved to the side of the view, `bad` templates (spread over
-    the features in view) replaced by random bytes."""
-    sc = synth.make_scene("C4", stream_id=stream_id, n_frames=n_frames, n_features=nf)
-    sc.n_select = n_select
-    if bad:
-        idx = np.linspace(0, in_view - 1, bad).round().astype(int)
-        assert len(set(idx)) == bad
-        patches = sc.patches.copy()
-        rng = np.random.default_rng(2000 + stream_id)
-        patches[idx] = rng.integers(0, 256, patches[idx].shape, dtype=np.uint8)
-        sc.patches = patches
-    if in_view < nf:
-        sc.x0 = sc.x0.copy()
-        sc.x0[13 + 3 * in_view:] += np.tile([3.0, 0.0, 0.0], nf - in_view)
-    sc.meta["variant"] = (nf, in_view, bad)
-    return sc
-
-
 def designed(v):
     """(K, nf before the cull, nf after it)."""
     nf, vis, bad, _ = v
@@ -71,10 +52,6 @@ def designed(v):
 
 def variant_scenes(cap):
     return [large_variant(nf, vis, bad, stream_id=i) for i, (nf, vis, bad, _) in enumerate(VARIANTS[cap])]
-
-
-def variant_of(s, U):
-    return (s * 5) % U
 
 
 def regimes(nsm, U):
@@ -90,45 +67,15 @@ def test_large_map_update_shapes_against_oracle(oracle, cap):
     import torch
     nsm = torch.cuda.get_device_properties(0).multi_processor_count
     scenes = variant_scenes(cap)
-    U = len(scenes)
-    traj = record_oracle(oracle, scenes)
+    traj = record_oracle(oracle, scenes, T)
     for v, rec in zip(VARIANTS[cap], traj):                  # the run is the designed one
         K, nf0, nf1 = designed(v)
         assert int(((rec[0]["f"]["flags"] & 3) == 3).sum()) == K, v
         assert rec[0]["nf"] == nf0 and rec[-1]["nf"] == nf1, v
-    snaps, names = {}, []
-    for name, B, groups in regimes(nsm, U):
-        names.append(name)
-        scene_of = lambda s: scenes[variant_of(s, U)]  # noqa: E731
-        first = {}
-        for s in range(B):
-            first.setdefault(variant_of(s, U), s)
-        picks = sorted(({0, nsm - 1, nsm, B - 1} & set(range(B))) | set(first.values()))
-        ctx = ctx_from_scenes([scene_of(s) for s in range(B)], frame_slots=2, max_features=cap)
-        try:
-            if groups > 1:
-                ctx.set_step_groups(groups)
-            replays = {s: Replay(traj[variant_of(s, U)]) for s in picks}
-            worst = (0.0, 0.0)
-            for t in range(T):
-                ctx.set_frames(t % 2, np.stack([scene_of(s).frames[t] for s in range(B)]))
-                ctx.step(t % 2)
-                ctx.sync()
-                w = check_streams_against_oracle(ctx, replays, picks, scene_of, t)
-                worst = (max(worst[0], w[0]), max(worst[1], w[1]))
-                if t in (8, T - 1):
-                    snaps[name, t] = {u: _result(ctx, s) for u, s in first.items()}
-            for s in range(B):
-                u = variant_of(s, U)
-                if s != first[u]:
-                    _assert_same(_result(ctx, s), snaps[name, T - 1][u], (name, "stream", s, VARIANTS[cap][u][:3]))
-        finally:
-            ctx.close()
-        print("\ncap %3d %-7s B = %3d  worst state %.2e  covariance %.2e" % (cap, name, B, worst[0], worst[1]))
-    for name in names[1:]:
-        for t in (8, T - 1):
-            for u in range(U):
-                _assert_same(snaps[name, t][u], snaps[names[0], t][u], (name, "step", t, VARIANTS[cap][u][:3]))
+    regs = regimes(nsm, len(scenes))
+    _, worst = run_regimes(scenes, cap, regs, T, (8, T - 1), traj)
+    for name, B, _ in regs:
+        print("\ncap %3d %-7s B = %3d  worst state %.2e  covariance %.2e" % (cap, name, B, *worst[name]))
 
 
 @pytest.mark.parametrize("name, nf", [("C4", 100), ("C4", 128), ("C1", 20)])
@@ -143,13 +90,10 @@ def test_capacity_does_not_change_results(name, nf):
     try:
         for t in range(6):
             for c in (small, large):
-                c.set_frames(0, np.stack([sc.frames[t] for sc in scenes]))
-                c.step(0)
-                c.sync()
+                step_frames(c, np.stack([sc.frames[t] for sc in scenes]))
             for s in range(len(scenes)):
-                _assert_same(_result(large, s), _result(small, s), (name, nf, "step", t, "stream", s))
-                Ja, Jb = large.feature_jacobians(s), small.feature_jacobians(s)
-                assert all(np.array_equal(a, b) for a, b in zip(Ja, Jb)), (name, nf, t, s)
+                assert_same_bytes(stream_result(large, s, jacobians=True), stream_result(small, s, jacobians=True),
+                                  (name, nf, "step", t, "stream", s))
     finally:
         small.close()
         large.close()
@@ -170,9 +114,7 @@ def _oracle_from_ctx(oracle, ctx, s, sc):
 
 
 def _step_both(ctx, o, frame):
-    ctx.set_frames(0, frame[None])
-    ctx.step(0)
-    ctx.sync()
+    step_frames(ctx, frame[None])
     o.step(frame)
     fg, fo = ctx.features(0), o.features()
     assert ctx.num_features(0) == o.num_features
@@ -214,7 +156,7 @@ def test_map_grows_and_shrinks_through_128(oracle):
         for c in (a, b):
             c.set_frames(0, full.frames[t][None])
             c.step(0)
-        _assert_same(_result(a, 0), _result(b, 0), ("grown vs whole", t))
+        assert_same_bytes(stream_result(a, 0), stream_result(b, 0), ("grown vs whole", t))
     a.close()
     b.close()
 
@@ -263,7 +205,6 @@ def test_map_grows_and_shrinks_through_128(oracle):
 def test_staged_path_at_capacity_256(oracle):
     """sl2_predict_measurements -> sl2_make_measurements -> sl2_ekf_update_measured on a 256-feature map, and
     sl2_ekf_update with host rows at m = 256 on n = 781 against the dense update of kalman.cpp; m = 258 is refused."""
-    from test_gpu_ekf import _random_measurements
     sc = large_variant(256, 128, stream_id=3, n_frames=3)
     ctx = ctx_from_scenes([sc], max_features=256)
     o = oracle_slam_from_scene(oracle, sc)
@@ -290,7 +231,7 @@ def test_staged_path_at_capacity_256(oracle):
     rng = np.random.default_rng(256128)
     n = sc.n
     assert n == 781
-    feats, Hxv, Hy, R, nu, H, Rfull = _random_measurements(rng, n, 256, 128)
+    feats, Hxv, Hy, R, nu, H, Rfull = random_measurements(rng, n, 256, 128)
     ctx.ekf_update(0, feats, Hxv, Hy, R, nu)
     xg, Pg = ctx.get_state(0)
     xo, Po = oracle.kalman_update_dense(sc.x0, sc.P0, H, Rfull, nu)
@@ -301,7 +242,7 @@ def test_staged_path_at_capacity_256(oracle):
     ex, eP = assert_state_close(xg, Pg, xo, Po)
     assert np.abs(Pg - Pg.T).max() == 0.0
     print("update n=781 m=256: state err %.2e cov err %.2e" % (ex, eP))
-    f2, Hx2, Hy2, R2, nu2, _, _ = _random_measurements(rng, n, 256, 129)
+    f2, Hx2, Hy2, R2, nu2, _, _ = random_measurements(rng, n, 256, 129)
     with pytest.raises(Exception) as e:
         ctx.ekf_update(0, f2, Hx2, Hy2, R2, nu2)
     assert "bad m" in str(e.value)

@@ -6,7 +6,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from gpu_util import ctx_from_scenes, sl2, synth
+from gpu_util import ctx_from_scenes, patch_snapshot_field, random_measurements, sl2, synth
 
 ERR_ARG, ERR_STATE = -1, -3
 STEP = 8  # kernels of one step group
@@ -75,9 +75,8 @@ def test_staged_entry_points():
     assert _launches(ctx, lambda: ctx.ekf_predict(0, [0.01, 0.0, 0.0]))[1] == 1
     assert _launches(ctx, lambda: ctx.predict_measurements(0))[1] == 1
     assert _launches(ctx, lambda: ctx.make_measurements(0, 0))[1] == 1
-    from test_gpu_ekf import _random_measurements
     n = ctx.state_size(0)
-    fi, Hxv, Hy, R, nu, _, _ = _random_measurements(np.random.default_rng(3), n, (n - 13) // 3, 4)
+    fi, Hxv, Hy, R, nu, _, _ = random_measurements(np.random.default_rng(3), n, (n - 13) // 3, 4)
     assert _launches(ctx, lambda: ctx.ekf_update(0, fi, Hxv, Hy, R, nu))[1] == 5
     assert _launches(ctx, lambda: ctx.ekf_update_measured(0))[1] == 5
     assert _launches(ctx, lambda: ctx.normalise_state(0))[1] == 1
@@ -183,7 +182,6 @@ def test_snapshots():
     """The device save is one launch and the device load two (check, unpack); a device blob the check kernel refuses
     costs that one launch.  The host forms launch once per staging group of streams."""
     import torch
-    from test_gpu_snapshot import _patch_field
     ctx, _ = _scene_ctx()
     ctx.step(0)
     ctx.sync()
@@ -194,7 +192,7 @@ def test_snapshots():
     assert _launches(ctx, lambda: ctx.load_streams_dev(0, 2, dev.data_ptr(), sb))[1] == 2
     good = ctx.save_streams()
     nf = sl2.read_snapshot(good[0])["nfeat"]
-    bad = np.frombuffer(_patch_field(good[0], "job_feat", 0, nf), np.uint8)
+    bad = np.frombuffer(patch_snapshot_field(good[0], "job_feat", 0, nf), np.uint8)
     ctx.sync()
     dev[:bad.size] = torch.from_numpy(bad.copy()).cuda()
     torch.cuda.synchronize()

@@ -12,7 +12,7 @@ import pytest
 
 import model_cases as mc
 from gpu_util import (RTOL_TEST, check_streams_against_oracle, ctx_from_scenes, oracle_slam_from_scene,
-                      rigid_transform_scene, sl2, state_err, synth, untransform_state)
+                      rigid_transform_scene, sl2, state_err, step_frames, synth, untransform_state)
 from ref_golden import Reference
 
 # motion-model entries that contain sin/cos: device sin/cos may differ from glibc by 1-2 ulp (SURVEY H2); on an H100
@@ -477,9 +477,7 @@ def test_fused_step_culls_compact_xp_org(oracle):
     ctx = ctx_from_scenes(scenes)
     oracles = [oracle_slam_from_scene(oracle, sc) for sc in scenes]
     for t in range(12):
-        ctx.set_frames(0, np.stack([sc.frames[t] for sc in scenes]))
-        ctx.step(0)
-        ctx.sync()
+        step_frames(ctx, np.stack([sc.frames[t] for sc in scenes]))
         check_streams_against_oracle(ctx, oracles, range(len(scenes)), lambda s: scenes[s], t)
     assert [ctx.num_features(s) for s in range(3)] == [27, 27, 28]
     for s in range(3):
@@ -512,9 +510,7 @@ def test_rotated_world_fused_run(oracle):
         oracles = [oracle_slam_from_scene(oracle, sc) for sc in scenes]
         worst, late, late_discrete = [0.0, 0.0, 0.0], [0.0, 0.0, 0.0], 0
         for t in range(12):
-            ctx.set_frames(0, np.stack([sc.frames[t] for sc in scenes]))
-            ctx.step(0)
-            ctx.sync()
+            step_frames(ctx, np.stack([sc.frames[t] for sc in scenes]))
             check_streams_against_oracle(ctx, oracles, range(len(scenes)), lambda s: scenes[s], t)
             if not override:
                 continue

@@ -2,71 +2,22 @@
 trajectory point, the map counts, NIS = nu^T S^-1 nu and log det S of the step's update, and the camera block of x and
 P.  Records are off by default and never change what the step computes; their values are checked against an
 independent NumPy computation of S from the staged path, against the oracle's counts and against the getters."""
-import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
-from gpu_util import ctx_from_scenes, oracle_slam_from_scene, sl2, synth, update_variant
+from gpu_util import (CAMS_320, assert_same_bytes, ctx_from_scenes, large_variant, oracle_slam_from_scene,
+                      random_measurements, ring_block, sl2, step_frames, stream_result, synth, update_variant)
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 G = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 ERR_ARG, ERR_STATE = -1, -3
-RECORD_FIELDS = ("step", "nfeat", "nvisible", "nsel", "nmeas", "nculled", "m", "nis", "logdet_s", "xv", "pxx_diag")
 # NIS relative and log det S absolute, record vs NumPy on the staged path's S (m up to 256)
 NIS_RTOL, LOGDET_ATOL = 1e-9, 1e-9
 WORST = {"nis": 0.0, "logdet": 0.0}
 
 
-# ---- CPU ------------------------------------------------------------------------------------------------------------
-def test_step_record_layout_matches_header(tmp_path):
-    """sizeof / offsetof of every sl2_step_record field, as the host C compiler lays it out, equal the ctypes mirror and
-    the NumPy dtype; SL2_MAX_RECORDS equals lib.py's."""
-    R, D = sl2.Sl2StepRecord, sl2.STEP_RECORD_DTYPE
-    src = tmp_path / "layout.c"
-    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "sl2b200.h"', "int main(void) {",
-             '  printf("sizeof %zu\\n", sizeof(sl2_step_record));',
-             '  printf("MAX %d\\n", SL2_MAX_RECORDS);']
-    lines += ['  printf("%s %%zu %%zu\\n", offsetof(sl2_step_record, %s), sizeof(((sl2_step_record *)0)->%s));'
-              % (f, f, f) for f in RECORD_FIELDS]
-    lines += ["  return 0;", "}"]
-    src.write_text("\n".join(lines) + "\n")
-    exe = tmp_path / "layout"
-    subprocess.check_call([os.environ.get("CC", "cc"), "-std=c99", "-I", os.path.join(ROOT, "include"), "-o",
-                           str(exe), str(src)])
-    out = dict((l.split()[0], [int(v) for v in l.split()[1:]])
-               for l in subprocess.check_output([str(exe)], text=True).splitlines())
-    assert out.pop("sizeof") == [C.sizeof(R)] == [D.itemsize] == [256]
-    assert out.pop("MAX") == [sl2.lib.SL2_MAX_RECORDS] == [4096]
-    assert [f for f, _ in R._fields_] == list(RECORD_FIELDS) == list(D.names)
-    for f, t in R._fields_:
-        assert out[f] == [getattr(R, f).offset, C.sizeof(t)] == [D.fields[f][1], D.fields[f][0].itemsize], f
-
-
 # ---- helpers --------------------------------------------------------------------------------------------------------
-def _step(ctx, frames, slot=0):
-    ctx.set_frames(slot, frames)
-    ctx.step(slot)
-    ctx.sync()
-
-
-def _result(ctx, s):
-    """Everything the getters show of one stream after a step."""
-    x, P = ctx.get_state(s)
-    out = dict(x=x, P=P, **ctx.features(s))
-    for k, a in zip(("dh_dxv", "dh_dy", "R", "nu"), ctx.feature_jacobians(s)):
-        out[k] = a
-    return out
-
-
-def _assert_same(a, b, where):
-    assert a.keys() == b.keys(), where
-    for k in a:
-        assert a[k].shape == b[k].shape and a[k].tobytes() == b[k].tobytes(), (where, k)
-
-
 def _twin(sc, max_features):
     """A one-stream context that runs the staged path on a copy of a stream."""
     return sl2.Context(sl2.config_for_scene(sc, num_streams=1, max_features=max_features))
@@ -144,7 +95,7 @@ def _run_checked(oracle, scenes, steps, cap=None, slots=2, depth=64):
         for t in range(steps):
             k = t % scenes[0].frames.shape[0]
             want = [_expected(ctx, s, twin, sc.frames[k]) for s, sc in enumerate(scenes)]
-            _step(ctx, np.stack([sc.frames[k] for sc in scenes]), t % slots)
+            step_frames(ctx, np.stack([sc.frames[k] for sc in scenes]), t % slots)
             recs = ctx.records(max=1)
             for s, sc in enumerate(scenes):
                 rec = recs[s, 0]
@@ -176,11 +127,11 @@ def test_records_off_by_default_and_the_step_unchanged(B):
     for t in range(10):
         frames = np.stack([sc.frames[t] for sc in scenes])
         l0, l1 = off.launch_count(), on.launch_count()
-        _step(off, frames, t % 2)
-        _step(on, frames, t % 2)
+        step_frames(off, frames, t % 2)
+        step_frames(on, frames, t % 2)
         assert on.launch_count() - l1 == off.launch_count() - l0 + 1, t
     for s in range(B):
-        _assert_same(_result(on, s), _result(off, s), s)
+        assert_same_bytes(stream_result(on, s, jacobians=True), stream_result(off, s, jacobians=True), s)
     got = on.records()
     assert got.shape == (B, 10) and (got["step"] == np.arange(10)).all()
     assert off.L.sl2_get_records(off.h, 0, 1, 1, rec.ctypes.data) == ERR_STATE
@@ -216,7 +167,6 @@ def test_cull_step_records(oracle):
 def test_capacity_256_with_m_256(oracle):
     """A 256-feature map measuring 128 features (m = 256, n = 781) and a 256-feature map with nothing in view
     (m = 0: nis = logdet_s = 0, nothing of the update scratch is read)."""
-    from test_gpu_large_maps import large_variant
     scenes = [large_variant(256, 128, stream_id=3, n_frames=3), large_variant(256, 0, stream_id=4, n_frames=3)]
     recs = _run_checked(oracle, scenes, 3, cap=256)
     assert (recs[0]["m"] == 256).all() and (recs[1]["m"] == 0).all()
@@ -228,16 +178,15 @@ def test_staged_update_between_fused_steps_does_not_leak():
     """A staged sl2_ekf_update (host rows, another m) between two fused steps writes no record, and the next record
     describes the fused step's own update; on a stream whose features are all out of view the staged update fills
     the update scratch and the next fused step still records m = 0, nis = logdet_s = 0."""
-    from test_gpu_ekf import _random_measurements
     scenes = [synth.make_scene("C4", n_frames=3), update_variant(100, 100, out_of_view=True, stream_id=1, n_frames=3)]
     ctx = ctx_from_scenes(scenes, frame_slots=2)
     ctx.enable_records(8)
     twin = _twin(scenes[0], 100)
-    _step(ctx, np.stack([sc.frames[0] for sc in scenes]))
+    step_frames(ctx, np.stack([sc.frames[0] for sc in scenes]))
     before = ctx.records()
     rng = np.random.default_rng(7)
     for s in (0, 1):
-        feats, Hxv, Hy, R, nu, _, _ = _random_measurements(rng, 313, 100, 5)
+        feats, Hxv, Hy, R, nu, _, _ = random_measurements(rng, 313, 100, 5)
         ctx.ekf_update(s, feats, Hxv, Hy, R, nu)
     for s in (0, 1):  # the other staged entry points write no record either
         ctx.ekf_predict(s)
@@ -246,7 +195,7 @@ def test_staged_update_between_fused_steps_does_not_leak():
     after = ctx.records()
     assert after.shape == (2, 1) and after.tobytes() == before.tobytes()
     want = [_expected(ctx, s, twin, scenes[s].frames[1]) for s in (0, 1)]
-    _step(ctx, np.stack([sc.frames[1] for sc in scenes]), 1)
+    step_frames(ctx, np.stack([sc.frames[1] for sc in scenes]), 1)
     recs = ctx.records(max=1)
     for s in (0, 1):
         assert recs[s, 0]["step"] == 1
@@ -268,7 +217,7 @@ def test_ring_order_wrap_max_and_reenable():
     ctx.enable_records(8)
     hist = []
     for t in range(20):
-        _step(ctx, np.stack([sc.frames[t] for sc in scenes]), t % 2)
+        step_frames(ctx, np.stack([sc.frames[t] for sc in scenes]), t % 2)
         hist.append(ctx.records(max=1)[:, 0].copy())
         if t == 4:  # not wrapped yet: everything so far
             early = ctx.records()
@@ -291,11 +240,11 @@ def test_ring_order_wrap_max_and_reenable():
         assert (dev[:, k:] == 0xAB).all(), (lo, cnt, mx)
     ctx.enable_records(8)
     assert ctx.records().shape == (3, 0)
-    _step(ctx, np.stack([sc.frames[0] for sc in scenes]))
+    step_frames(ctx, np.stack([sc.frames[0] for sc in scenes]))
     assert ctx.records().shape == (3, 1) and (ctx.records()["step"] == 0).all()
     ctx.enable_records(3)
     for t in range(4):
-        _step(ctx, np.stack([sc.frames[t] for sc in scenes]), t % 2)
+        step_frames(ctx, np.stack([sc.frames[t] for sc in scenes]), t % 2)
     assert (ctx.records()["step"] == np.array([1, 2, 3])).all()
     ctx.enable_records(0)
     with pytest.raises(sl2.Sl2Error):
@@ -310,7 +259,6 @@ def test_bench_shape_records_do_not_depend_on_the_batch():
     step groups and sl2_step_host_async over two slots give byte-identical records, every two streams of the same
     scene and camera give byte-identical records, and records add exactly one launch per step group."""
     import torch
-    from test_gpu_stream_configs import CAMS_320, _ring
     nS, T = 264, 3
     cache = {}
 
@@ -327,7 +275,7 @@ def test_bench_shape_records_do_not_depend_on_the_batch():
 
     scenes = [scene_of(s) for s in range(nS)]
     rng = np.random.default_rng(264)
-    frames = [np.stack([_ring(sc.frames[t], 240, 320, rng) for sc in scenes]) for t in range(T)]
+    frames = [np.stack([ring_block(sc.frames[t], 240, 320, rng) for sc in scenes]) for t in range(T)]
 
     def context(groups):
         ctx = ctx_from_scenes(scenes, frame_slots=2)
@@ -341,7 +289,7 @@ def test_bench_shape_records_do_not_depend_on_the_batch():
     for name, groups in (("serial", 1), ("groups", 2)):
         ctx = context(groups)
         for t in range(T):
-            _step(ctx, frames[t], t % 2)
+            step_frames(ctx, frames[t], t % 2)
         runs[name] = ctx
     ctx = context(2)
     host = torch.empty((T, nS, 240, 320), dtype=torch.uint8, pin_memory=True)
@@ -365,11 +313,11 @@ def test_bench_shape_records_do_not_depend_on_the_batch():
     for name, groups in (("serial", 1), ("groups", 2)):
         c = runs[name]
         l0 = c.launch_count()
-        _step(c, frames[0])
+        step_frames(c, frames[0])
         with_rec = c.launch_count() - l0
         c.enable_records(0)
         l0 = c.launch_count()
-        _step(c, frames[0])
+        step_frames(c, frames[0])
         assert with_rec == c.launch_count() - l0 + groups, name
     for c in runs.values():
         c.close()
@@ -386,7 +334,7 @@ def test_rejections_and_entry_points_that_write_no_record():
     ctx = ctx_from_scenes(scenes, frame_slots=2, max_features=32)
     ctx.enable_records(4)
     for t in range(3):
-        _step(ctx, np.stack([sc.frames[t] for sc in scenes]), t % 2)
+        step_frames(ctx, np.stack([sc.frames[t] for sc in scenes]), t % 2)
     L, h = ctx.L, ctx.h
     recs, blobs = ctx.records(), ctx.save_streams()
     out = np.zeros((2, 4), sl2.STEP_RECORD_DTYPE)
@@ -412,7 +360,7 @@ def test_rejections_and_entry_points_that_write_no_record():
     ctx.delete_feature(1, idx)
     assert ctx.records().tobytes() == recs.tobytes()
     assert ctx.save_streams(0, 1) == blobs[:1]
-    _step(ctx, np.stack([sc.frames[3] for sc in scenes]), 1)
+    step_frames(ctx, np.stack([sc.frames[3] for sc in scenes]), 1)
     assert (ctx.records()["step"] == np.arange(4)).all()
     assert ctx.records()[:, :3].tobytes() == recs.tobytes()
     ctx.enable_records(0)

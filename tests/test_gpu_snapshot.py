@@ -2,54 +2,24 @@
 loaded into any stream id of another (other stream count, capacity, frame size, device) continues bit for bit, the
 blob round-trips byte for byte, and every malformed blob is refused before anything is written."""
 import ctypes as C
+import functools
 import os
 import subprocess
 
 import numpy as np
 import pytest
 
-from gpu_util import check_streams_against_oracle, ctx_from_scenes, oracle_slam_from_scene, sl2, synth, update_variant
+from gpu_util import (assert_same_bytes, check_streams_against_oracle, ctx_from_scenes, oracle_slam_from_scene,
+                      patch_snapshot_field, ring_block, sl2, step_frames, stream_result, synth, update_variant)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HOST = os.path.join(ROOT, "scenelib2_b200", "host")
-HEADER_FIELDS = ("magic", "version", "header_bytes", "reserved0", "total_bytes", "boxsize", "nfeat", "n", "reserved1",
-                 "cam", "nsel", "nvisible", "nmeas", "ncull")
 ERR_ARG, ERR_STATE = -1, -3
+# everything of a stream that a snapshot carries, as the getters show it
+_carried = functools.partial(stream_result, jacobians=True, camera=True)
 
 
 # ---- helpers --------------------------------------------------------------------------------------------------------
-def _result(ctx, s):
-    """Everything the getters show of one stream."""
-    x, P = ctx.get_state(s)
-    out = dict(x=x, P=P, **ctx.features(s))
-    for k, a in zip(("dh_dxv", "dh_dy", "R", "nu"), ctx.feature_jacobians(s)):
-        out[k] = a
-    sc = ctx.stream_config(s)
-    out["cam"] = np.array([getattr(sc, k) for k, _ in sl2.Sl2StreamConfig._fields_], np.float64)
-    out["nf"] = np.array([ctx.num_features(s)])
-    return out
-
-
-def _assert_same(a, b, where):
-    assert a.keys() == b.keys(), where
-    for k in a:
-        assert a[k].shape == b[k].shape and a[k].tobytes() == b[k].tobytes(), (where, k)
-
-
-def _step(ctx, frames, slot=0):
-    """One fused step of every stream; frames: (num_streams, H, W)."""
-    ctx.set_frames(slot, frames)
-    ctx.step(slot)
-    ctx.sync()
-
-
-def _ring(img, H, W, rng):
-    """An H x W ring block with the stream's image in its top-left and fresh noise everywhere else."""
-    out = rng.integers(0, 256, (H, W), dtype=np.uint8)
-    out[:img.shape[0], :img.shape[1]] = img
-    return out
-
-
 def _blank_ctx(sc, num_streams, **kw):
     return sl2.Context(sl2.config_for_scene(sc, num_streams=num_streams, frame_slots=2, **kw))
 
@@ -65,42 +35,7 @@ def _patch_header(blob, **fields):
     return bytes(h) + blob[C.sizeof(h):]
 
 
-def _patch_field(blob, name, index, value):
-    """The blob with element `index` of per-feature section `name` replaced."""
-    h = sl2.read_snapshot(blob)
-    layout, _ = sl2.lib.snapshot_layout(h["nfeat"], h["boxsize"])
-    off, _, dt = layout[name]
-    b = bytearray(blob)
-    b[off + index * np.dtype(dt).itemsize:off + (index + 1) * np.dtype(dt).itemsize] = np.array([value], dt).tobytes()
-    return bytes(b)
-
-
 # ---- CPU ------------------------------------------------------------------------------------------------------------
-def test_snapshot_header_layout_matches_header(tmp_path):
-    """sizeof / offsetof of every sl2_snapshot_header field, as the host C compiler lays it out, equal the ctypes
-    mirror, and the header's constants equal lib.py's."""
-    H = sl2.Sl2SnapshotHeader
-    src = tmp_path / "layout.c"
-    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "sl2b200.h"', "int main(void) {",
-             '  printf("sizeof %zu\\n", sizeof(sl2_snapshot_header));',
-             '  printf("MAGIC %u\\n", (unsigned)SL2_SNAPSHOT_MAGIC);',
-             '  printf("VERSION %d\\n", SL2_SNAPSHOT_VERSION);']
-    lines += ['  printf("%s %%zu %%zu\\n", offsetof(sl2_snapshot_header, %s), sizeof(((sl2_snapshot_header *)0)->%s));'
-              % (f, f, f) for f in HEADER_FIELDS]
-    lines += ["  return 0;", "}"]
-    src.write_text("\n".join(lines) + "\n")
-    exe = tmp_path / "layout"
-    subprocess.check_call([os.environ.get("CC", "cc"), "-std=c99", "-I", os.path.join(ROOT, "include"), "-o",
-                           str(exe), str(src)])
-    out = dict((l.split()[0], [int(v) for v in l.split()[1:]])
-               for l in subprocess.check_output([str(exe)], text=True).splitlines())
-    assert out.pop("sizeof") == [C.sizeof(H)] == [128]
-    assert out.pop("MAGIC") == [sl2.lib.SL2_SNAPSHOT_MAGIC] and out.pop("VERSION") == [sl2.lib.SL2_SNAPSHOT_VERSION]
-    assert [f for f, _ in H._fields_] == list(HEADER_FIELDS)
-    for f, t in H._fields_:
-        assert out[f] == [getattr(H, f).offset, C.sizeof(t)], f
-
-
 def _hand_blob(nfeat=5, box=11, seed=0):
     """A blob of the documented format built field by field in NumPy, and the arrays that went into it."""
     rng = np.random.default_rng(seed)
@@ -177,12 +112,12 @@ def test_round_trip_eight_c4_streams():
     scenes = _c4_scenes(8, 8)
     a = ctx_from_scenes(scenes, frame_slots=2)
     for t in range(3):
-        _step(a, np.stack([sc.frames[t] for sc in scenes]), t % 2)
+        step_frames(a, np.stack([sc.frames[t] for sc in scenes]), t % 2)
     blobs = a.save_streams()
     assert len(blobs) == 8 and all(len(b) <= a.snapshot_bytes() for b in blobs)
     assert a.save_streams(2, 3) == blobs[2:5] and a.save_stream(7) == blobs[7]
     for s, (sc, blob) in enumerate(zip(scenes, blobs)):
-        r, snap = _result(a, s), sl2.read_snapshot(blob)
+        r, snap = _carried(a, s), sl2.read_snapshot(blob)
         assert snap["x"].tobytes() == r["x"].tobytes() and snap["P"].tobytes() == r["P"].tobytes()
         for k in ("attempted", "successful"):
             assert (snap[k] == r[k]).all()
@@ -209,12 +144,12 @@ def test_round_trip_eight_c4_streams():
     b = _blank_ctx(scenes[0], 8)
     b.load_streams(blobs)
     for s in range(8):
-        _assert_same(_result(b, s), _result(a, s), ("loaded", s))
+        assert_same_bytes(_carried(b, s), _carried(a, s), ("loaded", s))
     for t in range(3, 8):
         for c in (a, b):
-            _step(c, np.stack([sc.frames[t] for sc in scenes]), t % 2)
+            step_frames(c, np.stack([sc.frames[t] for sc in scenes]), t % 2)
         for s in range(8):
-            _assert_same(_result(b, s), _result(a, s), ("step", t, s))
+            assert_same_bytes(_carried(b, s), _carried(a, s), ("step", t, s))
     assert b.save_streams() == a.save_streams()
     b.load_streams(b.save_streams())  # loading a context's own blobs changes nothing
     assert b.save_streams() == a.save_streams()
@@ -234,7 +169,7 @@ def test_migration_from_the_bench_shape(oracle):
     src = ctx_from_scenes([scene_of(s) for s in range(B)], frame_slots=2)
     picks = (0, 131, 132, 263)
     for t in range(T0):
-        _step(src, np.stack([scene_of(s).frames[t] for s in range(B)]), t % 2)
+        step_frames(src, np.stack([scene_of(s).frames[t] for s in range(B)]), t % 2)
     blobs = {s: src.save_stream(s) for s in picks}
     sc0 = uniq[0]
     nf = sc0.n_features
@@ -260,16 +195,16 @@ def test_migration_from_the_bench_shape(oracle):
                 o.step(scene_of(s).frames[t])
             oracles[name][d] = o
     for t in range(T0, T0 + T1):
-        _step(src, np.stack([scene_of(s).frames[t] for s in range(B)]), t % 2)
+        step_frames(src, np.stack([scene_of(s).frames[t] for s in range(B)]), t % 2)
         for name, ctx, m, (H, W) in dests:
             frames = np.zeros((ctx.cfg.num_streams, H, W), np.uint8)
             for d in range(ctx.cfg.num_streams):
                 img = scene_of(m[d]).frames[t] if d in m else uniq[0].frames[t]
-                frames[d] = _ring(img, H, W, rng)
-            _step(ctx, frames, t % 2)
+                frames[d] = ring_block(img, H, W, rng)
+            step_frames(ctx, frames, t % 2)
             check_streams_against_oracle(ctx, oracles[name], sorted(m), lambda d: scene_of(m[d]), t)
             for d, s in m.items():
-                _assert_same(_result(ctx, d), _result(src, s), (name, t, d, s))
+                assert_same_bytes(_carried(ctx, d), _carried(src, s), (name, t, d, s))
     for _, ctx, _, _ in dests:
         ctx.close()
     src.close()
@@ -287,7 +222,7 @@ def test_counters_survive_and_the_cull_happens_on_time(oracle):
     a = ctx_from_scenes([sc], frame_slots=2)
     o_a = {0: oracle_slam_from_scene(oracle, sc)}
     for t in range(7):
-        _step(a, sc.frames[t][None], t % 2)
+        step_frames(a, sc.frames[t][None], t % 2)
         check_streams_against_oracle(a, o_a, (0,), lambda s: sc, t)
     blob = a.save_stream(0)
     x7, P7 = a.get_state(0)
@@ -299,11 +234,11 @@ def test_counters_survive_and_the_cull_happens_on_time(oracle):
     r.set_features(0, x7[13:].reshape(-1, 3), snap["xp_org"], snap["templates"])
     r.set_state(0, x7, P7)
     for t in range(7, 12):
-        _step(a, sc.frames[t][None], t % 2)
+        step_frames(a, sc.frames[t][None], t % 2)
         check_streams_against_oracle(a, o_a, (0,), lambda s: sc, t)
-        _step(b, np.stack([sc.frames[t]] * 2), t % 2)
-        _step(r, sc.frames[t][None], t % 2)
-        _assert_same(_result(b, 1), _result(a, 0), ("step", t))
+        step_frames(b, np.stack([sc.frames[t]] * 2), t % 2)
+        step_frames(r, sc.frames[t][None], t % 2)
+        assert_same_bytes(_carried(b, 1), _carried(a, 0), ("step", t))
         if t + 1 == 10:
             assert a.num_features(0) == nf - bad
     assert b.num_features(1) == nf - bad
@@ -328,10 +263,10 @@ def _save_load_continue(src, s, frame_of, steps, where):
     assert dst.save_stream(2) == dst.save_stream(0) == blob, where
     for t in range(steps):
         fr = frame_of(t)
-        _step(src, np.stack([fr] * src.cfg.num_streams), t % 2)
-        _step(dst, np.stack([fr] * 3), t % 2)
+        step_frames(src, np.stack([fr] * src.cfg.num_streams), t % 2)
+        step_frames(dst, np.stack([fr] * 3), t % 2)
         for d in (2, 0):
-            _assert_same(_result(dst, d), _result(src, s), (where, t, d))
+            assert_same_bytes(_carried(dst, d), _carried(src, s), (where, t, d))
     assert dst.save_stream(2) == src.save_stream(s), where
     dst.close()
     return blob
@@ -348,7 +283,7 @@ def test_states_left_by_a_cull_a_delete_and_a_rebuild():
     sc = update_variant(cap, nf, bad=bad, n_frames=13)
     a = ctx_from_scenes([sc], frame_slots=2)
     for t in range(10):
-        _step(a, sc.frames[t][None], t % 2)
+        step_frames(a, sc.frames[t][None], t % 2)
     h = sl2.read_snapshot(a.save_stream(0))
     assert h["nfeat"] == nf - bad and h["nvisible"] == nf and h["ncull"] == bad, (h["nfeat"], h["nvisible"], h["ncull"])
     _save_load_continue(a, 0, lambda t: sc.frames[10 + t], 3, "cull")
@@ -357,7 +292,7 @@ def test_states_left_by_a_cull_a_delete_and_a_rebuild():
     scenes = _c4_scenes(1, 5, first=3)
     b = ctx_from_scenes(scenes, frame_slots=2)
     for t in range(2):
-        _step(b, scenes[0].frames[t][None], t % 2)
+        step_frames(b, scenes[0].frames[t][None], t % 2)
     b.delete_feature(0, 5)
     h = sl2.read_snapshot(b.save_stream(0))
     assert h["nvisible"] > h["nfeat"] == scenes[0].n_features - 1
@@ -367,7 +302,7 @@ def test_states_left_by_a_cull_a_delete_and_a_rebuild():
     c2 = synth.make_scene("C2", stream_id=4, n_frames=5, n_features=24)
     c = ctx_from_scenes([c2], frame_slots=2)
     for t in range(2):
-        _step(c, c2.frames[t][None], t % 2)
+        step_frames(c, c2.frames[t][None], t % 2)
     x, P = c.get_state(0)
     k = 10
     c.set_features(0, x[13:13 + 3 * k].reshape(k, 3), c2.xp_org[:k], c2.patches[:k])
@@ -395,43 +330,43 @@ def test_device_rollback_clone_and_reset():
     frames = lambda t, clone=False: np.stack([scenes[1 if clone and s == 3 else s].frames[t] for s in range(4)])
     a = ctx_from_scenes(scenes, frame_slots=2)
     for t in range(2):
-        _step(a, frames(t), t % 2)
+        step_frames(a, frames(t), t % 2)
     buf, stride = _dev_buf(a, 4), a.snapshot_bytes()
     a.save_streams_dev(0, 4, buf.data_ptr(), stride)
     first = []
     for t in range(2, 5):
-        _step(a, frames(t), t % 2)
-        first.append([_result(a, s) for s in range(4)])
+        step_frames(a, frames(t), t % 2)
+        first.append([_carried(a, s) for s in range(4)])
     a.load_streams_dev(0, 4, buf.data_ptr(), stride)
     for j, t in enumerate(range(2, 5)):
-        _step(a, frames(t), t % 2)
+        step_frames(a, frames(t), t % 2)
         for s in range(4):
-            _assert_same(_result(a, s), first[j][s], ("rollback", t, s))
+            assert_same_bytes(_carried(a, s), first[j][s], ("rollback", t, s))
     # clone 1 -> 3, then step on; the reference context never clones
     ref = ctx_from_scenes(scenes, frame_slots=2)
     for t in range(5):
-        _step(ref, frames(t), t % 2)
+        step_frames(ref, frames(t), t % 2)
     a.save_streams_dev(1, 1, buf.data_ptr(), stride)
     a.load_streams_dev(3, 1, buf.data_ptr(), stride)
     for t in range(5, 8):
-        _step(a, frames(t, clone=True), t % 2)
-        _step(ref, frames(t), t % 2)
-        _assert_same(_result(a, 3), _result(a, 1), ("clone", t))
+        step_frames(a, frames(t, clone=True), t % 2)
+        step_frames(ref, frames(t), t % 2)
+        assert_same_bytes(_carried(a, 3), _carried(a, 1), ("clone", t))
         for s in range(3):
-            _assert_same(_result(a, s), _result(ref, s), ("others", t, s))
+            assert_same_bytes(_carried(a, s), _carried(ref, s), ("others", t, s))
     # a 30-feature blob into a slot that held a 100-feature map == into a fresh context
     small = synth.make_scene("C4", stream_id=9, n_frames=3, n_features=30)
     c = ctx_from_scenes([small], frame_slots=2, max_features=100)
-    _step(c, small.frames[0][None])
+    step_frames(c, small.frames[0][None])
     blob = c.save_stream(0)
     fresh = _blank_ctx(small, 4, max_features=100)
     a.load_stream(2, blob)
     fresh.load_stream(2, blob)
     for t in (1, 2):
         fr = np.stack([small.frames[t]] * 4)
-        _step(a, fr, t % 2)
-        _step(fresh, fr, t % 2)
-        _assert_same(_result(a, 2), _result(fresh, 2), ("reset", t))
+        step_frames(a, fr, t % 2)
+        step_frames(fresh, fr, t % 2)
+        assert_same_bytes(_carried(a, 2), _carried(fresh, 2), ("reset", t))
     assert a.save_stream(2) == fresh.save_stream(2)
     for x in (a, ref, c, fresh):
         x.close()
@@ -444,7 +379,7 @@ def test_save_between_staged_calls():
     finished in the saving and in the receiving context gives identical results."""
     sc = synth.make_scene("C2", stream_id=3, n_frames=3, n_features=24)
     a = ctx_from_scenes([sc], frame_slots=1)
-    _step(a, sc.frames[0][None])
+    step_frames(a, sc.frames[0][None])
     a.ekf_predict(0)
     nv = a.predict_measurements(0)
     assert nv > 0
@@ -457,7 +392,7 @@ def test_save_between_staged_calls():
     assert b.make_measurements(1, 0) == a.make_measurements(0, 0) > 0
     a.ekf_update_measured(0)
     b.ekf_update_measured(1)
-    _assert_same(_result(b, 1), _result(a, 0), "staged")
+    assert_same_bytes(_carried(b, 1), _carried(a, 0), "staged")
     assert b.save_stream(1) == a.save_stream(0)
     a.close()
     b.close()
@@ -475,7 +410,7 @@ def test_ordering_with_two_step_groups():
     ref = ctx_from_scenes(scenes, frame_slots=2)
     after = []
     for t in range(2):
-        _step(ref, host[t].numpy(), t % 2)
+        step_frames(ref, host[t].numpy(), t % 2)
         after.append(ref.save_streams())
     a = ctx_from_scenes(scenes, frame_slots=2)
     a.set_step_groups(2)
@@ -505,7 +440,7 @@ def test_large_maps_round_trip_and_move():
     for s, sc in enumerate(scenes):
         a.set_stream_config(s, sl2.stream_config_for_scene(sc))
     for t in range(3):
-        _step(a, np.stack([sc.frames[t] for sc in scenes]), t % 2)
+        step_frames(a, np.stack([sc.frames[t] for sc in scenes]), t % 2)
     blobs = a.save_streams()
     assert [sl2.read_snapshot(b)["n"] for b in blobs] == [781, 781]
     assert len(blobs[0]) == a.snapshot_bytes()
@@ -515,12 +450,12 @@ def test_large_maps_round_trip_and_move():
     other.load_streams(blobs, lo=3)
     for t in range(3, 6):
         fr = np.stack([sc.frames[t] for sc in scenes])
-        _step(a, fr, t % 2)
-        _step(same, fr, t % 2)
-        _step(other, np.concatenate([fr[:1]] * 3 + [fr]), t % 2)
+        step_frames(a, fr, t % 2)
+        step_frames(same, fr, t % 2)
+        step_frames(other, np.concatenate([fr[:1]] * 3 + [fr]), t % 2)
         for s in range(2):
-            _assert_same(_result(same, s), _result(a, s), ("same", t, s))
-            _assert_same(_result(other, 3 + s), _result(a, s), ("other", t, s))
+            assert_same_bytes(_carried(same, s), _carried(a, s), ("same", t, s))
+            assert_same_bytes(_carried(other, 3 + s), _carried(a, s), ("other", t, s))
     assert same.save_streams() == a.save_streams() == other.save_streams(3, 2)
     for c in (a, same, other):
         c.close()
@@ -551,12 +486,13 @@ def _bad_blobs(good, nsel):
            ("nvisible above 256", _patch_header(good, nvisible=257)),
            ("ncull above 256", _patch_header(good, ncull=257)),
            ("boxsize", _patch_header(good, boxsize=15)),
-           ("job_feat past the map", _patch_field(good, "job_feat", 0, nf)),
-           ("job_feat below -1", _patch_field(good, "job_feat", 0, -2)),
-           ("job_feat after nsel", _patch_field(good, "job_feat", nsel, 0)),
-           ("sel_rank at nsel", _patch_field(good, "sel_rank", job, nsel)),
-           ("sel_rank at nfeat below nsel", _patch_field(_patch_header(good, nsel=nf + 5), "sel_rank", job, nf)),
-           ("sel_rank below -1", _patch_field(good, "sel_rank", job, -2)),
+           ("job_feat past the map", patch_snapshot_field(good, "job_feat", 0, nf)),
+           ("job_feat below -1", patch_snapshot_field(good, "job_feat", 0, -2)),
+           ("job_feat after nsel", patch_snapshot_field(good, "job_feat", nsel, 0)),
+           ("sel_rank at nsel", patch_snapshot_field(good, "sel_rank", job, nsel)),
+           ("sel_rank at nfeat below nsel",
+            patch_snapshot_field(_patch_header(good, nsel=nf + 5), "sel_rank", job, nf)),
+           ("sel_rank below -1", patch_snapshot_field(good, "sel_rank", job, -2)),
            ("image wider than the frame", _patch_header(good, **{"cam.width": 321})),
            ("image below the box", _patch_header(good, **{"cam.height": 15})),
            ("fku", _patch_header(good, **{"cam.fku": 0.0})),
@@ -574,7 +510,7 @@ def test_rejections_leave_every_stream_unchanged():
     for sc in scenes:
         sc.n_select = 10
     ctx = ctx_from_scenes(scenes)
-    _step(ctx, np.stack([sc.frames[0] for sc in scenes]))
+    step_frames(ctx, np.stack([sc.frames[0] for sc in scenes]))
     good = ctx.save_streams()
     nsel = sl2.read_snapshot(good[0])["nsel"]
     assert 0 < nsel < 24
@@ -687,13 +623,13 @@ def test_move_between_devices():
     scenes = _c4_scenes(3, 5)
     a = ctx_from_scenes(scenes, frame_slots=2, device=0)
     for t in range(2):
-        _step(a, np.stack([sc.frames[t] for sc in scenes]), t % 2)
+        step_frames(a, np.stack([sc.frames[t] for sc in scenes]), t % 2)
     b = sl2.Context(sl2.config_for_scene(scenes[0], num_streams=3, frame_slots=2, device=1))
     b.load_streams(a.save_streams())
     for t in range(2, 5):
         for c in (a, b):
-            _step(c, np.stack([sc.frames[t] for sc in scenes]), t % 2)
+            step_frames(c, np.stack([sc.frames[t] for sc in scenes]), t % 2)
         for s in range(3):
-            _assert_same(_result(b, s), _result(a, s), ("device 1", t, s))
+            assert_same_bytes(_carried(b, s), _carried(a, s), ("device 1", t, s))
     a.close()
     b.close()

@@ -6,7 +6,7 @@ import numpy as np
 import pytest
 
 from gpu_util import (RTOL_NORTH_STAR, assert_state_close, check_streams_against_oracle, ctx_from_scenes,
-                      oracle_slam_from_scene, sl2, state_err, synth)
+                      oracle_slam_from_scene, sl2, state_err, step_frames, synth)
 
 pytestmark = pytest.mark.gpu
 G = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -18,24 +18,9 @@ def _run(oracle, scenes, steps, slots=2):
     worst = (0.0, 0.0)
     for t in range(steps):
         k = t % scenes[0].frames.shape[0]
-        ctx.set_frames(t % slots, np.stack([sc.frames[k] for sc in scenes]))
-        ctx.step(t % slots)
-        ctx.sync()
-        for s, (sc, o) in enumerate(zip(scenes, oracles)):
-            o.step(sc.frames[k])
-            fg, fo = ctx.features(s), o.features()
-            assert ctx.num_features(s) == o.num_features
-            assert (fg["select_rank"] == fo["select_rank"]).all(), (t, s)
-            assert (fg["flags"] == fo["flags"]).all(), (t, s)
-            ok = (fo["flags"] & 2) > 0
-            assert (fg["z"][ok] == fo["z"][ok]).all(), (t, s)     # bit-exact match positions
-            assert (fg["attempted"] == fo["attempted"]).all()
-            assert (fg["successful"] == fo["successful"]).all()
-            xg, Pg = ctx.get_state(s)
-            xo, Po = o.get_state()
-            e = assert_state_close(xg, Pg, xo, Po)
-            worst = (max(worst[0], e[0]), max(worst[1], e[1]))
-            assert np.abs(Pg - Pg.T).max() == 0.0
+        step_frames(ctx, np.stack([sc.frames[k] for sc in scenes]), t % slots)
+        w = check_streams_against_oracle(ctx, oracles, range(len(scenes)), lambda s: scenes[s], k)
+        worst = (max(worst[0], w[0]), max(worst[1], w[1]))
     ctx.close()
     return worst
 
@@ -135,9 +120,7 @@ def test_empty_map_and_invisible_features(oracle):
     ctx.set_state(2, x2, np.eye(13) * 1e-4)
     o0, o1 = oracle_slam_from_scene(oracle, sc), oracle_slam_from_scene(oracle, far)
     for t in range(2):
-        ctx.set_frames(0, np.stack([sc.frames[t], far.frames[t], sc.frames[t]]))
-        ctx.step(0)
-        ctx.sync()
+        step_frames(ctx, np.stack([sc.frames[t], far.frames[t], sc.frames[t]]))
         o0.step(sc.frames[t])
         o1.step(far.frames[t])
     assert_state_close(*ctx.get_state(0), *o0.get_state())
@@ -166,9 +149,7 @@ def test_c4_many_streams_ground_truth_properties():
     ctx = ctx_from_scenes(scenes, frame_slots=2)
     tr_prev = [np.trace(sc.P0[13:, 13:]) for sc in scenes]
     for t in range(T):
-        ctx.set_frames(t % 2, np.stack([sc.frames[t] for sc in scenes]))
-        ctx.step(t % 2)
-        ctx.sync()
+        step_frames(ctx, np.stack([sc.frames[t] for sc in scenes]), t % 2)
         for s in (0, 7, 18, 36) if t < T - 1 else range(B):
             sc = scenes[s]
             f = ctx.features(s)
@@ -206,9 +187,7 @@ def test_long_run_does_not_drift_from_oracle(oracle):
     worst = 0.0
     for t in range(40):
         k = t % 8
-        ctx.set_frames(t % 2, sc.frames[k][None])
-        ctx.step(t % 2)
-        ctx.sync()
+        step_frames(ctx, sc.frames[k][None], t % 2)
         o.step(sc.frames[k])
         fg, fo = ctx.features(0), o.features()
         assert ctx.num_features(0) == o.num_features
@@ -365,9 +344,7 @@ def test_c4_bench_shape_264_streams_against_oracle(oracle):
     assert len({(s * 5) % U for s in picks}) == 4
     oracles = {s: oracle_slam_from_scene(oracle, scene_of(s)) for s in picks}
     for t in range(T):
-        cfg_ctx.set_frames(t % 2, np.stack([scene_of(s).frames[t] for s in range(B)]))
-        cfg_ctx.step(t % 2)
-        cfg_ctx.sync()
+        step_frames(cfg_ctx, np.stack([scene_of(s).frames[t] for s in range(B)]), t % 2)
         check_streams_against_oracle(cfg_ctx, oracles, picks, scene_of, t)
         for s in range(0, B, 7):
             sc = scene_of(s)
@@ -393,9 +370,7 @@ def test_c3_four_streams_four_frames_against_oracle(oracle):
     ctx = ctx_from_scenes(scenes, frame_slots=2)
     oracles = {s: oracle_slam_from_scene(oracle, scenes[s]) for s in range(B)}
     for t in range(T):
-        ctx.set_frames(t % 2, np.stack([sc.frames[t] for sc in scenes]))
-        ctx.step(t % 2)
-        ctx.sync()
+        step_frames(ctx, np.stack([sc.frames[t] for sc in scenes]), t % 2)
         check_streams_against_oracle(ctx, oracles, range(B), lambda s: scenes[s], t)
     ctx.close()
 
@@ -445,9 +420,7 @@ def test_h2_ellipse_boundary_flips_are_counted(oracle):
         ellipses = cands = flips = bit_diff = 0
         for t in range(steps):
             k = t % sc.frames.shape[0]
-            ctx.set_frames(0, sc.frames[k][None])
-            ctx.step(0)
-            ctx.sync()
+            step_frames(ctx, sc.frames[k][None])
             o.step(sc.frames[k])
             fg, fo = ctx.features(0), o.features()
             assert (fg["select_rank"] == fo["select_rank"]).all() and (fg["flags"] == fo["flags"]).all()

@@ -4,46 +4,20 @@ The frame ring keeps the context's size; the ring bytes outside a smaller stream
 frame, so any read past the stream's image would show up in the results."""
 import ctypes as C
 import hashlib
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-from gpu_util import (assert_state_close, check_streams_against_oracle, ctx_from_scenes, oracle_slam_from_scene,
-                      sl2, synth)
+from gpu_util import (CAMS_320, assert_same_bytes, assert_state_close, camera, check_streams_against_oracle,
+                      ctx_from_scenes, oracle_slam_from_scene, ring_block, sl2, step_frames, stream_result, synth)
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 STREAM_FIELDS = ("width", "height", "fku", "fkv", "u0", "v0", "kd1", "sd", "delta_t", "number_of_features_to_select")
-
-
-def _cam(width, height, focal=1.0, shift=(0.0, 0.0), kd1=1.0, sd=1.0):
-    """A calibration derived from the reference's (synth.camera_params) for a width x height image."""
-    c = synth.camera_params(width, height)
-    c[2:4] *= focal
-    c[4] += shift[0]
-    c[5] += shift[1]
-    c[6] *= kd1
-    c[7] = sd
-    return c
-
-
 # the four calibrations of the mixed-camera tests: a full 640x480 camera, two 320x240 ones (the second with a shifted
 # principal point, 1.3x the focal length and 3x the radial distortion) and a 400x300 one with twice the pixel noise
-CAMS_640 = [_cam(640, 480), _cam(320, 240), _cam(320, 240, focal=1.3, shift=(9.0, -7.0), kd1=3.0),
-            _cam(400, 300, sd=2.0)]
-# calibrations that fit a 320x240 ring (the benchmark's C4 shape)
-CAMS_320 = [_cam(320, 240), _cam(320, 240, focal=1.3, shift=(9.0, -7.0), kd1=3.0), _cam(288, 224, focal=0.9),
-            _cam(320, 240, sd=2.0)]
+CAMS_640 = [camera(640, 480), camera(320, 240), camera(320, 240, focal=1.3, shift=(9.0, -7.0), kd1=3.0),
+            camera(400, 300, sd=2.0)]
 DTS = (1.0 / 60, 1.0 / 30, 1.0 / 15)
 NSEL = (10, 50, 100)
-
-
-def _ring(img, H, W, rng):
-    """A ring block of the context's H x W with the stream's image top-left and fresh noise everywhere else."""
-    out = rng.integers(0, 256, (H, W), dtype=np.uint8)
-    out[:img.shape[0], :img.shape[1]] = img
-    return out
 
 
 def _stream_cfg(ctx, s):
@@ -81,41 +55,7 @@ def _mixed_context(scenes, W, H, frame_slots=1, groups=1, **kw):
     return ctx
 
 
-def _snapshot(ctx, s):
-    x, P = ctx.get_state(s)
-    return dict(x=x, P=P, **ctx.features(s))
-
-
-def _assert_same_bits(a, b, keys, where):
-    for k in keys:
-        assert a[k].shape == b[k].shape and a[k].tobytes() == b[k].tobytes(), (where, k)
-
-
-ALL_KEYS = ("x", "P", "h", "z", "S", "flags", "attempted", "successful", "select_rank")
-
-
 # ---- CPU ------------------------------------------------------------------------------------------------------------
-def test_stream_config_layout_matches_header(tmp_path):
-    """sizeof / offsetof of every sl2_stream_config field, as the host C compiler lays it out, equal the ctypes mirror."""
-    from scenelib2_b200.lib import Sl2StreamConfig
-    src = tmp_path / "layout.c"
-    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "sl2b200.h"', "int main(void) {",
-             '  printf("sizeof %zu\\n", sizeof(sl2_stream_config));']
-    lines += ['  printf("%s %%zu %%zu\\n", offsetof(sl2_stream_config, %s), sizeof(((sl2_stream_config *)0)->%s));'
-              % (f, f, f) for f in STREAM_FIELDS]
-    lines += ["  return 0;", "}"]
-    src.write_text("\n".join(lines) + "\n")
-    exe = tmp_path / "layout"
-    cc = os.environ.get("CC", "cc")
-    subprocess.check_call([cc, "-std=c99", "-I", os.path.join(ROOT, "include"), "-o", str(exe), str(src)])
-    out = dict((l.split()[0], [int(v) for v in l.split()[1:]])
-               for l in subprocess.check_output([str(exe)], text=True).splitlines())
-    assert out.pop("sizeof") == [C.sizeof(Sl2StreamConfig)]
-    assert [f for f, _ in Sl2StreamConfig._fields_] == list(STREAM_FIELDS)
-    for f, t in Sl2StreamConfig._fields_:
-        assert out[f] == [getattr(Sl2StreamConfig, f).offset, C.sizeof(t)], f
-
-
 # sha256 (first 32 hex digits) of every output of make_scene(name, stream_id=s, n_frames=3) before the camera and
 # delta_t arguments existed: the default scenes, and so every recorded result that uses them, must not move
 DEFAULT_SCENE_DIGESTS = {
@@ -168,13 +108,11 @@ def _run_mixed(scenes, W, H, steps, groups=1, oracles=None, picks=(), seed=0, sn
     rng = np.random.default_rng(seed)
     snaps = []
     for t in range(steps):
-        ctx.set_frames(t % 2, np.stack([_ring(sc.frames[t], H, W, rng) for sc in scenes]))
-        ctx.step(t % 2)
-        ctx.sync()
+        step_frames(ctx, np.stack([ring_block(sc.frames[t], H, W, rng) for sc in scenes]), t % 2)
         if oracles is not None:
             check_streams_against_oracle(ctx, oracles, picks, lambda s: scenes[s], t)
         if snap:
-            snaps.append([_snapshot(ctx, s) for s in range(len(scenes))])
+            snaps.append([stream_result(ctx, s) for s in range(len(scenes))])
     return ctx, snaps
 
 
@@ -182,9 +120,8 @@ def _run_alone(sc, steps):
     ctx = ctx_from_scenes([sc], frame_slots=2)
     snaps = []
     for t in range(steps):
-        ctx.set_frames(t % 2, sc.frames[t][None])
-        ctx.step(t % 2)
-        snaps.append(_snapshot(ctx, 0))
+        step_frames(ctx, sc.frames[t][None], t % 2)
+        snaps.append(stream_result(ctx, 0))
     ctx.close()
     return snaps
 
@@ -206,7 +143,7 @@ def test_mixed_cameras_fused_step_against_oracle_and_dedicated_contexts(oracle):
     for s, sc in enumerate(scenes):
         alone = _run_alone(sc, 6)
         for t in range(6):
-            _assert_same_bits(snaps[t][s], alone[t], ALL_KEYS, (s, t))
+            assert_same_bytes(snaps[t][s], alone[t], (s, t))
 
 
 @pytest.mark.gpu
@@ -230,11 +167,11 @@ def test_noop_setter_and_getter():
     for t in range(4):
         for s in range(8):  # before every step, and between the upload and the step
             b.set_stream_config(s, b.stream_config(s))
-        b.set_frames(t % 2, np.stack([_ring(sc.frames[t], 480, 640, rng) for sc in scenes]))
+        b.set_frames(t % 2, np.stack([ring_block(sc.frames[t], 480, 640, rng) for sc in scenes]))
         b.set_stream_config(t % 8, sl2.stream_config_for_scene(scenes[t % 8]))
         b.step(t % 2)
         for s in range(8):
-            _assert_same_bits(sa[t][s], _snapshot(b, s), ALL_KEYS, (s, t))
+            assert_same_bytes(sa[t][s], stream_result(b, s), (s, t))
     a.close()
     b.close()
 
@@ -243,7 +180,7 @@ def _switch_scene():
     """A 24-feature C2 scene on the default 320x240 camera, and a second camera B: a smaller 288x224 image, another
     calibration, frame period and selection count."""
     sc = synth.make_scene("C2", stream_id=5, n_frames=7, n_features=24, override=False)
-    cam_b = _cam(288, 224, focal=1.1, shift=(-6.0, 4.0), kd1=2.0, sd=1.5)
+    cam_b = camera(288, 224, focal=1.1, shift=(-6.0, 4.0), kd1=2.0, sd=1.5)
     b = sl2.Sl2StreamConfig()
     b.width, b.height = 288, 224
     b.fku, b.fkv, b.u0, b.v0, b.kd1, b.sd = [float(v) for v in cam_b[2:8]]
@@ -268,7 +205,7 @@ def _ctx_for_camera(sc, b, x, P):
 def _assert_switch_matches(a, b, where):
     """x, P, h, S, the selection and the matches of the selected features: bit-identical (counters and the flags of
     unselected features carry the history before the switch)."""
-    _assert_same_bits(a, b, ("x", "P", "h", "S", "select_rank"), where)
+    assert_same_bytes(a, b, where, keys=("x", "P", "h", "S", "select_rank"))
     sel = b["select_rank"] >= 0
     assert sel.any(), where
     assert a["z"][sel].tobytes() == b["z"][sel].tobytes() and (a["flags"][sel] == b["flags"][sel]).all(), where
@@ -283,7 +220,7 @@ def test_camera_change_mid_run():
     import torch
     sc, cam_b = _switch_scene()
     rng = np.random.default_rng(11)
-    frames = np.stack([_ring(sc.frames[t], 240, 320, rng) for t in range(7)])
+    frames = np.stack([ring_block(sc.frames[t], 240, 320, rng) for t in range(7)])
     a = ctx_from_scenes([sc], frame_slots=2)
     for t in range(3):
         a.set_frames(t % 2, frames[t][None])
@@ -297,9 +234,9 @@ def test_camera_change_mid_run():
         a.step(t % 2)
         ref.set_frames(t % 2, np.ascontiguousarray(sc.frames[t][:224, :288])[None])
         ref.step(t % 2)
-        _assert_switch_matches(_snapshot(a, 0), _snapshot(ref, 0), t)
+        _assert_switch_matches(stream_result(a, 0), stream_result(ref, 0), t)
     assert ref.features(0)["attempted"].max() < 10
-    final = _snapshot(ref, 0)
+    final = stream_result(ref, 0)
     a.close()
     ref.close()
     # the same switch between two asynchronous steps
@@ -312,7 +249,7 @@ def test_camera_change_mid_run():
             c.set_stream_config(0, cam_b)
         c.step_host_async(t % 2, host[t].data_ptr(), xv[t].data_ptr())
     c.sync()
-    _assert_switch_matches(_snapshot(c, 0), final, "async")
+    _assert_switch_matches(stream_result(c, 0), final, "async")
     assert xv[6].numpy().tobytes() == final["x"][:13].tobytes()
     c.close()
 
@@ -330,7 +267,7 @@ def test_staged_path_and_score_map_on_a_smaller_stream(oracle):
     o = oracle_slam_from_scene(oracle, sc)
     rng = np.random.default_rng(5)
     for t in range(3):
-        ctx.set_frames(0, np.stack([_ring(scn.frames[t], 480, 640, rng) for scn in scenes]))
+        ctx.set_frames(0, np.stack([ring_block(scn.frames[t], 480, 640, rng) for scn in scenes]))
         ctx.set_frame(s, 0, sc.frames[t])  # copies the stream's 320 x 240 image only
         ctx.ekf_predict(s)
         ctx.predict_measurements(s)
@@ -379,7 +316,7 @@ def test_partial_features_and_detector_on_a_smaller_stream(oracle):
     sc.fku, sc.fkv, sc.u0, sc.v0, sc.kd1, sc.sd = [float(v) for v in cam8[2:8]]
     sc.delta_t, sc.number_of_features_to_select = 1.0 / 30, 10
     ctx.set_stream_config(s, sc)
-    ring = np.stack([_ring(img, 480, 640, rng) for _ in range(3)])
+    ring = np.stack([ring_block(img, 480, 640, rng) for _ in range(3)])
     ctx.set_frames(0, ring)
     xv = np.zeros(13)
     xv[:3] = [0.02, -0.01, 0.01]
@@ -505,9 +442,7 @@ def test_capacity_256_per_stream_selection(oracle):
         sl2.load_scene(ctx, s, sc)
     oracles = {s: oracle_slam_from_scene(oracle, sc) for s, sc in enumerate(scenes)}
     for t in range(4):
-        ctx.set_frames(t % 2, np.stack([sc.frames[t] for sc in scenes]))
-        ctx.step(t % 2)
-        ctx.sync()
+        step_frames(ctx, np.stack([sc.frames[t] for sc in scenes]), t % 2)
         check_streams_against_oracle(ctx, oracles, (0, 1), lambda s: scenes[s], t)
     assert (ctx.features(0)["select_rank"] >= 0).sum() == 128 and (ctx.features(1)["select_rank"] >= 0).sum() == 10
     before = _stream_cfg(ctx, 0)

@@ -10,10 +10,9 @@ every launch regime, and compared with the CPU oracle at every step; results mus
 """
 import math
 
-import numpy as np
 import pytest
 
-from gpu_util import check_streams_against_oracle, ctx_from_scenes, oracle_slam_from_scene, update_variant
+from gpu_util import record_oracle, run_regimes, update_variant
 
 T = 12              # frames per run; the bad features are culled by the 10th step
 SNAP_STEPS = (8, T - 1)   # compared across regimes: the last step before the cull, and the last step
@@ -75,10 +74,6 @@ def designed(v):
 def variant_scenes(cap):
     return [update_variant(cap, nf, bad, out, stream_id=i, n_frames=T)
             for i, (nf, bad, out, _) in enumerate(VARIANTS[cap])]
-
-
-def variant_of(s, U):
-    return (s * 5) % U              # neighbouring streams hold different variants (U coprime to 5)
 
 
 # ---- Python mirror of sl2_launch_update's decisions -----------------------------------------------------------
@@ -170,41 +165,6 @@ def coverage(nsm):
     return rows, hits
 
 
-# ---- the oracle, stepped once per capacity ------------------------------------------------------------------
-def record_oracle(oracle, scenes, states=True):
-    """One oracle per variant stepped over the T frames (threads across variants); per variant and step: map size,
-    features, and (states) x and P."""
-    slams = [oracle_slam_from_scene(oracle, sc) for sc in scenes]
-    nthreads = max(1, min(len(slams), oracle.usable_cpus()))
-    traj = [[] for _ in slams]
-    for t in range(T):
-        oracle.run_slams(slams, [sc.frames[t][None] for sc in scenes], 1, nthreads)
-        for rec, o in zip(traj, slams):
-            rec.append(dict(nf=o.num_features, f=o.features(), xP=o.get_state() if states else None))
-    return traj
-
-
-class Replay:
-    """A recorded oracle trajectory with the surface check_streams_against_oracle uses (each step() advances one
-    recorded step; the frames are those the trajectory was recorded on)."""
-
-    def __init__(self, steps):
-        self.steps, self.t = steps, -1
-
-    def step(self, frame):
-        self.t += 1
-
-    @property
-    def num_features(self):
-        return self.steps[self.t]["nf"]
-
-    def features(self):
-        return self.steps[self.t]["f"]
-
-    def get_state(self):
-        return self.steps[self.t]["xP"]
-
-
 # ---- CPU: the variants still reach their edges ---------------------------------------------------------------
 def test_variants_reach_every_update_shape(oracle):
     """Each variant has its designed K at every step and loses exactly its bad features at the 10th step, and the
@@ -215,7 +175,7 @@ def test_variants_reach_every_update_shape(oracle):
         assert max(v[0] for v in vs) == cap, cap            # some stream fills the capacity
         if 13 + 3 * cap <= 320:                              # every hp2 ragged-block case
             assert {designed(v)[0] % 4 for v in vs if designed(v)[0]} == {0, 1, 2, 3}, cap
-        traj = record_oracle(oracle, variant_scenes(cap), states=False)
+        traj = record_oracle(oracle, variant_scenes(cap), T, states=False)
         for v, rec in zip(vs, traj):
             K, nf0, nf1 = designed(v)
             sel = [int((r["f"]["flags"] & 1).sum()) for r in rec]
@@ -236,21 +196,9 @@ def test_variants_reach_every_update_shape(oracle):
         assert not missing, (nsm, missing)
 
 
+
+
 # ---- GPU: every regime against the oracle and against each other ---------------------------------------------
-RESULT_KEYS = ("z", "flags", "attempted", "successful", "select_rank", "h", "S")
-
-
-def _result(ctx, s):
-    x, P = ctx.get_state(s)
-    f = ctx.features(s)
-    return dict(x=x, P=P, **{k: f[k].copy() for k in RESULT_KEYS})
-
-
-def _assert_same(a, b, what):
-    for k in a:
-        assert a[k].shape == b[k].shape and np.array_equal(a[k], b[k]), (what, k)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("cap", sorted(VARIANTS))
 def test_update_shapes_against_oracle(oracle, cap):
@@ -263,45 +211,12 @@ def test_update_shapes_against_oracle(oracle, cap):
     scenes = variant_scenes(cap)
     U = len(scenes)
     assert U < nsm
-    traj = record_oracle(oracle, scenes)
+    traj = record_oracle(oracle, scenes, T)
     for v, rec in zip(VARIANTS[cap], traj):                  # the run is the designed one
         assert int(((rec[0]["f"]["flags"] & 3) == 3).sum()) == designed(v)[0], v
-    snaps = {}
-    names = []
-    for name, B, groups, launches in regimes(cap, nsm, U):
-        names.append(name)
-        scene_of = lambda s: scenes[variant_of(s, U)]  # noqa: E731
-        first = {}
-        for s in range(B):
-            first.setdefault(variant_of(s, U), s)
-        assert len(first) == U
-        picks = sorted(({0, nsm - 1, nsm, B - 1} & set(range(B))) | set(first.values()))
-        ctx = ctx_from_scenes([scene_of(s) for s in range(B)], frame_slots=2, max_features=cap)
-        try:
-            if groups > 1:
-                ctx.set_step_groups(groups)
-            replays = {s: Replay(traj[variant_of(s, U)]) for s in picks}
-            worst = (0.0, 0.0)
-            for t in range(T):
-                ctx.set_frames(t % 2, np.stack([scene_of(s).frames[t] for s in range(B)]))
-                ctx.step(t % 2)
-                ctx.sync()
-                w = check_streams_against_oracle(ctx, replays, picks, scene_of, t)
-                worst = (max(worst[0], w[0]), max(worst[1], w[1]))
-                if t in SNAP_STEPS:
-                    snaps[name, t] = {u: _result(ctx, s) for u, s in first.items()}
-            last = snaps[name, T - 1]
-            for s in range(B):
-                u = variant_of(s, U)
-                if s != first[u]:
-                    _assert_same(_result(ctx, s), last[u], (name, "stream", s, "variant", VARIANTS[cap][u][:3]))
-        finally:
-            ctx.close()
+    regs = regimes(cap, nsm, U)
+    _, worst = run_regimes(scenes, cap, [r[:3] for r in regs], T, SNAP_STEPS, traj)
+    for name, B, _, launches in regs:
         labels = sorted({shape_label(launch_shape(cap, cnt, nsm)) for _, cnt in launches})
         print("\ncap %3d %-11s B = %3d  %-44s worst state %.2e  covariance %.2e"
-              % (cap, name, B, " | ".join(labels), worst[0], worst[1]))
-    for name in names[1:]:
-        for t in SNAP_STEPS:
-            for u in range(U):
-                _assert_same(snaps[name, t][u], snaps[names[0], t][u],
-                             (name, "vs", names[0], "step", t, "variant", VARIANTS[cap][u][:3]))
+              % (cap, name, B, " | ".join(labels), *worst[name]))

@@ -3,12 +3,7 @@
 A stream holds up to SL2_MAX_FEATURES = 256 map features (n <= 781); one step measures at most SL2_MAX_MEASURED =
 128 of them (m <= 256).  sl2_create validates both before it looks for a device, so the rules hold on any machine.
 """
-import os
-import re
-
 import pytest
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
@@ -34,13 +29,6 @@ def _create_rc(lib, cfg):
     if rc == 0:
         L.sl2_destroy(h)
     return rc, L.sl2_last_error(None).decode()
-
-
-def test_lib_constants_match_header(lib):
-    hdr = open(os.path.join(ROOT, "include", "sl2b200.h")).read()
-    consts = dict(re.findall(r"#define\s+(SL2_MAX_FEATURES|SL2_MAX_MEASURED)\s+(\d+)", hdr))
-    assert int(consts["SL2_MAX_FEATURES"]) == lib.lib.SL2_MAX_FEATURES == 256
-    assert int(consts["SL2_MAX_MEASURED"]) == lib.lib.SL2_MAX_MEASURED == 128
 
 
 @pytest.mark.parametrize("max_features, n_select, rule", [
