@@ -9,13 +9,18 @@
 //     tensor = [slot*stream][H][W] u8) that completes on a per-warp mbarrier; windows larger
 //     than the tile are walked tile by tile.  The TMA unit needs a 16-byte aligned box start
 //     so the box is loaded from x & ~15 and is 15 B wider.
-//   * while the TMA is in flight the warp evaluates the exact FP64 ellipse predicate for every
-//     candidate of the tile and compacts the non-empty vertical strips (SL2_STRIP candidates of
-//     one column) into a task list with ballots, so later rounds run with full lanes.
+//   * while the TMA is in flight the warp reads the template and forms its constants (first tile
+//     only), evaluates the exact FP64 ellipse predicate for every candidate of the tile and
+//     compacts the non-empty vertical strips (candidates of one column) into a task list with
+//     ballots, so later rounds run with full lanes.
 //   * integer phase, per lane = one strip: every image row is read once from shared memory as
 //     aligned 32-bit words, byte-aligned with funnel shifts, and feeds all strip candidates that
-//     overlap it: Sg0g1 by IDP.4A against the template held in registers, Sg1 / Sg1sq by IDP.4A
-//     against 0x01010101 / itself.  All sums are exact int32 like the reference's.
+//     overlap it: Sg0g1 by IDP.4A against the template held in registers, the row's Sg1 / Sg1sq
+//     by IDP.4A against 0x01010101 / itself.  All sums are exact int32 like the reference's.
+//     The filtered kernel runs strips of filter_strip(BOX) candidates and forms each candidate's
+//     Sg1 / Sg1sq as the difference of two running sums over the strip's rows; it scores a
+//     candidate as soon as its last row is in, so only the candidates whose rows are still
+//     being read hold integer sums.
 //   * FP64 phase: the score of improc.cpp:99-133 op-for-op with __d*_rn (no FMA contraction,
 //     IEEE div / sqrt) so that scores are bit-identical to the x86-64 SSE2 reference build.
 //   * arg-min with the reference's tie-break (`corr <= corrmax` => the LAST candidate in
@@ -68,14 +73,55 @@ struct DumpPtrs {
   int cap;
 };
 
+// One image row of a candidate's window: NW + 1 aligned words from the tile, byte-aligned by `sh` bits, bytes past BOX
+// cleared.
+template <int BOX>
+__device__ __forceinline__ void window_row(const uint32_t *wp, int sh, uint32_t (&sw)[(BOX + 3) / 4]) {
+  constexpr int NW = (BOX + 3) / 4;
+  constexpr uint32_t LASTMASK = (BOX % 4 == 0) ? 0xffffffffu : ((1u << (8 * (BOX % 4))) - 1u);
+  uint32_t w[NW + 1];
+#pragma unroll
+  for (int k = 0; k <= NW; ++k) w[k] = wp[k];
+#pragma unroll
+  for (int k = 0; k < NW; ++k) sw[k] = __funnelshift_r(w[k], w[k + 1], sh);
+  sw[NW - 1] &= LASTMASK;
+}
+
+// The filter's approximate score 2 - 2 rho from the exact integer moments (rho in FP32): +inf when the window's sigma
+// is below 10 (never accepted), -3e38 on the knife edge sigma == 10 (the exact chain decides).
+template <int BOX>
+__device__ __forceinline__ float approx_score(uint32_t ax, uint32_t a1, uint32_t a2, int Sg0, float V0f) {
+  constexpr uint32_t NN = BOX * BOX, T100u = 100u * NN * NN;
+  const uint32_t V1u = NN * a2 - a1 * a1;
+  if (V1u > T100u) {
+    float num;
+    if constexpr (BOX <= 11) {
+      // n^2 var = n Sxx - Sx^2 and n Sxy - Sx0 Sx1 fit 32-bit integers for n <= 121
+      // (n^2 255^2 < 2^31): exact in the integer pipe, one conversion each to FP32
+      num = (float)((int)NN * (int)ax - Sg0 * (int)a1);
+    } else {
+      // n = 225: n Sxx, Sx^2 and both terms of n Sxy - Sx0 Sx1 still fit 32 unsigned bits
+      // (225 * 225 * 255^2 < 2^32); only the last difference needs 64: exact in the integer pipe
+      // (the FP64 pipe runs at half rate and every candidate paid 2 conversions + 2 DFMA + DSETP)
+      num = (float)((long long)NN * (long long)ax - (long long)Sg0 * (long long)a1);
+    }
+    const float rho = num * rsqrtf(V0f * (float)V1u);
+    return fmaf(-2.0f, rho, 2.0f);
+  }
+  return V1u == T100u ? -3.0e38f : __int_as_float(0x7f800000);
+}
+
+// Candidates per strip task of the filtered search, per template size, from measurements on an H100 (BASELINE.md §6):
+// 8 at 11 x 11 (18 image rows per strip), 16 at 15 x 15 (30 rows: 1.9 instead of 2.75 row reads per candidate).
+__host__ __device__ constexpr int filter_strip(int box) { return box <= 11 ? 8 : 16; }
+
 template <int BOX, bool FILTER>
 __global__ void __launch_bounds__(SL2_SEARCH_WARPS * 32, FILTER ? (BOX <= 11 ? 4 : 3) : 2)
     search_kernel(const __grid_constant__ CUtensorMap tmap, const Sl2Dev d, const SearchLaunch L,
                   const DumpPtrs dump) {
   constexpr int NW = (BOX + 3) / 4;             // 32-bit words per template row
   constexpr int HALF = (BOX - 1) / 2;
-  constexpr int V = SL2_STRIP;
-  constexpr uint32_t LASTMASK = (BOX % 4 == 0) ? 0xffffffffu : ((1u << (8 * (BOX % 4))) - 1u);
+  constexpr int V = FILTER ? filter_strip(BOX) : SL2_STRIP;  // candidates per strip
   extern __shared__ __align__(128) uint8_t smem[];
   pdl_prologue();
 
@@ -85,7 +131,11 @@ __global__ void __launch_bounds__(SL2_SEARCH_WARPS * 32, FILTER ? (BOX <= 11 ? 4
   const int r = (blockIdx.x % groups) * SL2_SEARCH_WARPS + warp;  // job of this warp
   if (r >= L.jobs_per_stream) return;
   const int job = sl * L.jobs_per_stream + r;
+  // the job's ellipse is read with its feature index (an empty job's values are never used)
   const int feat = L.job_feat[job];
+  const double P00 = L.job_puinv[job * 3 + 0], P01 = L.job_puinv[job * 3 + 1],
+               P11 = L.job_puinv[job * 3 + 2];
+  const double cx = L.job_centre[job * 2 + 0], cy = L.job_centre[job * 2 + 1];
   if (feat < 0) return;
   const int s = L.stream_lo + sl;
 
@@ -105,6 +155,29 @@ __global__ void __launch_bounds__(SL2_SEARCH_WARPS * 32, FILTER ? (BOX <= 11 ? 4
     fence_proxy_async();
   }
   __syncwarp();
+
+  // ---- search box around the rounded centre ----------------------------------------------------
+  const int uc = __double2int_rz(add_(cx, 0.5));
+  const int vc = __double2int_rz(add_(cy, 0.5));
+  // clamped to the stream's own image, so no window reads past it (the tile loads may: those bytes feed nothing)
+  const SearchBox sb = search_box(P00, P01, P11, uc, vc, stream_width(d.cams[s]), stream_height(d.cams[s]), HALF);
+  const Ellipse ell = make_ellipse(P00, P01, P11);
+  const int CW = sb.cols(), CH = sb.rows();
+  const int x0 = uc + sb.us - HALF, y0 = vc + sb.vs - HALF;
+  if (!FILTER && lane == 0) {
+    dump.box[0] = sb.us; dump.box[1] = sb.uf; dump.box[2] = sb.vs; dump.box[3] = sb.vf;
+    dump.box[4] = uc; dump.box[5] = vc;
+  }
+
+  // the first tile's TMA goes out before the template is read and its constants are formed: both overlap the load
+  const int img = L.slot * d.B + s;
+  const auto stage = [&](int tx0, int ty0) {
+    if (lane == 0) {
+      mbar_expect_tx(bar, (uint32_t)(TW * TH));
+      tma_load_3d(tile_s, &tmap, bar, (x0 + tx0) & ~15, y0 + ty0, img);
+    }
+  };
+  if (CW > 0 && CH > 0) stage(0, 0);
 
   // ---- template into registers, rows zero-padded to 16 bytes in HBM --------------------------
   uint32_t T[BOX][NW];
@@ -131,35 +204,15 @@ __global__ void __launch_bounds__(SL2_SEARCH_WARPS * 32, FILTER ? (BOX <= 11 ? 4
   const bool patch_ok = !(pconst.sigmag0 < 10.0);  // kCorrelationSigmaThreshold_ gate on the template
   float bmin = 3.0e38f;                            // running minimum of the approximate score
 
-  // ---- search box around the rounded centre ----------------------------------------------------
-  const double P00 = L.job_puinv[job * 3 + 0], P01 = L.job_puinv[job * 3 + 1],
-               P11 = L.job_puinv[job * 3 + 2];
-  const double cx = L.job_centre[job * 2 + 0], cy = L.job_centre[job * 2 + 1];
-  const int uc = __double2int_rz(add_(cx, 0.5));
-  const int vc = __double2int_rz(add_(cy, 0.5));
-  // clamped to the stream's own image, so no window reads past it (the tile loads may: those bytes feed nothing)
-  const SearchBox sb = search_box(P00, P01, P11, uc, vc, stream_width(d.cams[s]), stream_height(d.cams[s]), HALF);
-  const Ellipse ell = make_ellipse(P00, P01, P11);
-  const int CW = sb.cols(), CH = sb.rows();
-  const int x0 = uc + sb.us - HALF, y0 = vc + sb.vs - HALF;
-  if (!FILTER && lane == 0) {
-    dump.box[0] = sb.us; dump.box[1] = sb.uf; dump.box[2] = sb.vs; dump.box[3] = sb.vf;
-    dump.box[4] = uc; dump.box[5] = vc;
-  }
-
   ScanBest best;
   uint32_t phase = 0;
-  const int img = L.slot * d.B + s;
 
   if (CW > 0 && CH > 0) {
     for (int ty0 = 0; ty0 < CH; ty0 += TCH) {
       for (int tx0 = 0; tx0 < CW; tx0 += TCW) {
         const int tcw = min(TCW, CW - tx0), tch = min(TCH, CH - ty0);
-        const int xa = (x0 + tx0) & ~15, xoff = (x0 + tx0) & 15;
-        if (lane == 0) {
-          mbar_expect_tx(bar, (uint32_t)(TW * TH));
-          tma_load_3d(tile_s, &tmap, bar, xa, y0 + ty0, img);
-        }
+        const int xoff = (x0 + tx0) & 15;
+        if (tx0 != 0 || ty0 != 0) stage(tx0, ty0);
         // ---- task list while the TMA is in flight ------------------------------------------
         const int nstrips = (tch + V - 1) / V;
         const int ntask = tcw * nstrips;
@@ -174,15 +227,18 @@ __global__ void __launch_bounds__(SL2_SEARCH_WARPS * 32, FILTER ? (BOX <= 11 ? 4
           // three rows around the vertex); a column that does not settle in a few moves is scanned row by row.
           // ~5 exact evaluations per column instead of one per candidate.
           const int vbase = sb.vs + ty0;
+          // the estimate's 1 / (2 P11), once per tile instead of one FP64 and one FP32 division per column
+          const double r2p11 = 1.0 / (2.0 * P11);
+          const float r2p11f = (float)r2p11;
           for (int cu = lane; cu < tcw; cu += 32) {
             const Ellipse::Col col = ell.col((double)(sb.us + tx0 + cu));
             auto inside = [&](int cv) { return ell.inside(col, (double)(vbase + cv)); };
             int lo, hi;
             bool scan = !(P11 > 1e-7) || !(P11 < 1e7);  // degenerate ellipse (or NaN): no shortcut
             if (!scan) {
-              const double vx = -col.b / (2.0 * P11);                   // vertex (approximate arithmetic from here)
+              const double vx = -col.b * r2p11;                         // vertex (approximate arithmetic from here)
               const double disc = col.b * col.b - 4.0 * P11 * (col.a - 9.0);
-              const float r = disc > 0.0 ? __fsqrt_rn((float)disc) / (float)(2.0 * P11) : 0.0f;
+              const float r = disc > 0.0 ? __fsqrt_rn((float)disc) * r2p11f : 0.0f;
               const float lo_f = fminf(fmaxf(ceilf((float)vx - r) - (float)vbase, -1.0f), (float)tch);
               const float hi_f = fminf(fmaxf(floorf((float)vx + r) - (float)vbase, -1.0f), (float)tch);
               lo = max(0, min(tch - 1, (int)lo_f));
@@ -228,6 +284,7 @@ __global__ void __launch_bounds__(SL2_SEARCH_WARPS * 32, FILTER ? (BOX <= 11 ? 4
                 const short2 rg = colrange[cu];
                 const int jlo = max((int)rg.x - st * V, 0), jhi = min(min((int)rg.y - st * V, V - 1), tch - 1 - st * V);
                 if (jlo <= jhi) {
+                  // bits 16..31: the strip's candidates inside the ellipse
                   const uint32_t mask = ((1u << (jhi + 1)) - 1u) & ~((1u << jlo) - 1u);
                   entry = (uint32_t)cu | ((uint32_t)st << 8) | (mask << 16);
                 }
@@ -278,36 +335,113 @@ __global__ void __launch_bounds__(SL2_SEARCH_WARPS * 32, FILTER ? (BOX <= 11 ? 4
         phase ^= 1;
 
         // ---- strips ------------------------------------------------------------------------
-        for (int l0 = 0; l0 < nlist; l0 += 32) {
-          const bool has_task = l0 + lane < nlist;
-          uint32_t ax[V], a1[V], a2[V];
-          float cap[V];           // FILTER: approximate scores of the strip
-          int cand0 = 0;          // scan index of candidate j = 0 of the strip
+        const int tw4 = TW >> 2;
+        if constexpr (FILTER) {
+          // The reference's score equals 2 - 2*rho (rho = normalised cross-correlation) up to
+          // FP64 rounding (<= 1e-9 for sigma >= 10).  rho is evaluated in FP32 from the EXACT
+          // integer moments; only candidates whose approximate score is within kWindow of the
+          // running minimum can be the reference's arg-min (or tie with it), and only those go
+          // through the exact FP64 chain.  window 1e-5 >= 2 * (FP32 error 1.1e-6 + 1e-9).
+          // pass 1: approximate scores of the strip (no FP64 div/sqrt), each candidate scored as
+          // soon as its last row is in; pass 2, after the warp has agreed on the running minimum:
+          // the survivors' integer sums again from the tile, and the exact chain.
+          static_assert(V <= 16, "the task entry holds a 16-bit candidate mask");
+          static_assert(V >= SL2_STRIP, "the task list is sized for strips of SL2_STRIP candidates");
+          for (int l0 = 0; l0 < nlist; l0 += 32) {
+            float cap[V];  // approximate scores of the strip, +inf: not a candidate
 #pragma unroll
-          for (int j = 0; j < V; ++j) {
-            ax[j] = a1[j] = a2[j] = 0;
-            cap[j] = __int_as_float(0x7f800000);  // +inf: not a candidate
+            for (int j = 0; j < V; ++j) cap[j] = __int_as_float(0x7f800000);
+            int cv0 = 0, cand0 = 0;  // strip's first candidate row in the tile, its scan index
+            int sh = 0;
+            const uint32_t *wbase = nullptr;
+            if (l0 + lane < nlist && patch_ok) {
+              const uint32_t e = list[l0 + lane];
+              const int cu = e & 0xff, st = (e >> 8) & 0xff;
+              const uint32_t m_in = e >> 16;
+              cv0 = st * V;
+              cand0 = (tx0 + cu) * CH + (ty0 + cv0);
+              const int cx = cu + xoff;  // byte column of the candidate's window inside the tile
+              sh = (cx & 3) * 8;
+              wbase = reinterpret_cast<const uint32_t *>(tile) + (cx >> 2);
+              // candidate j: Sg1 = s1 - h1[j], Sg1sq = s2 - h2[j], with s the running sums of the rows read so far
+              // and h their values before row j (every true sum < 2^31: exact in uint32 arithmetic)
+              uint32_t ax[V], h1[V], h2[V], s1 = 0, s2 = 0;
+              float lmin = bmin;
+#pragma unroll
+              for (int j = 0; j < V; ++j) ax[j] = 0;
+#pragma unroll
+              for (int rr = 0; rr < V + BOX - 1; ++rr) {
+                uint32_t sw[NW];
+                window_row<BOX>(wbase + min(cv0 + rr, TH - 1) * tw4, sh, sw);
+                if (rr < V) {
+                  h1[rr] = s1;
+                  h2[rr] = s2;
+                }
+#pragma unroll
+                for (int k = 0; k < NW; ++k) {
+                  s1 = __dp4a(sw[k], 0x01010101u, s1);
+                  s2 = __dp4a(sw[k], sw[k], s2);
+                }
+#pragma unroll
+                for (int j = 0; j < V; ++j) {
+                  const int t = rr - j;  // template row seen by candidate j in this image row
+                  if (t >= 0 && t < BOX) {
+#pragma unroll
+                    for (int k = 0; k < NW; ++k) ax[j] = __dp4a(sw[k], T[t][k], ax[j]);
+                  }
+                }
+                const int j = rr - (BOX - 1);  // the candidate whose last row this is
+                if (j >= 0 && ((m_in >> j) & 1u)) {
+                  cap[j] = approx_score<BOX>(ax[j], s1 - h1[j], s2 - h2[j], Sg0, V0f);
+                  if (cap[j] > -1.0e38f) lmin = fminf(lmin, cap[j]);
+                }
+              }
+              bmin = lmin;
+            }
+            // the warp agrees on the running minimum, then only the survivors take the exact chain
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) bmin = fminf(bmin, __shfl_xor_sync(0xffffffffu, bmin, o));
+            const float thr = bmin + 1.0e-5f;  // kWindow, see above
+            uint32_t surv = 0;
+#pragma unroll
+            for (int j = 0; j < V; ++j) surv |= (cap[j] <= thr ? 1u : 0u) << j;
+            while (surv) {
+              const int j = __ffs(surv) - 1;
+              surv &= surv - 1;
+              uint32_t ax = 0, a1 = 0, a2 = 0;
+#pragma unroll
+              for (int t = 0; t < BOX; ++t) {
+                uint32_t sw[NW];
+                window_row<BOX>(wbase + (cv0 + j + t) * tw4, sh, sw);
+#pragma unroll
+                for (int k = 0; k < NW; ++k) {
+                  ax = __dp4a(sw[k], T[t][k], ax);
+                  a1 = __dp4a(sw[k], 0x01010101u, a1);
+                  a2 = __dp4a(sw[k], sw[k], a2);
+                }
+              }
+              double sg1;
+              const double corr = exact_score_fn(pconst, (double)(int)a1, (double)(int)a2, (double)(int)ax, &sg1);
+              if (!(sg1 < 10.0)) best.offer(corr, cand0 + j);
+            }
           }
-          if (has_task) {
+        } else {
+          for (int l0 = 0; l0 < nlist; l0 += 32) {
+            if (l0 + lane >= nlist) continue;
+            uint32_t ax[V], a1[V], a2[V];
+#pragma unroll
+            for (int j = 0; j < V; ++j) ax[j] = a1[j] = a2[j] = 0;
             const uint32_t e = list[l0 + lane];
             const int cu = e & 0xff, st = (e >> 8) & 0xff;
             const uint32_t m_in = (e >> 16) & 0xff, m_all = m_in | ((e >> 24) & 0xff);
             const int cv0 = st * V;
-            cand0 = (tx0 + cu) * CH + (ty0 + cv0);
             const int cx = cu + xoff;  // byte column of the candidate's window inside the tile
             const int sh = (cx & 3) * 8;
             const uint32_t *wbase = reinterpret_cast<const uint32_t *>(tile) + (cx >> 2);
-            const int tw4 = TW >> 2;
 #pragma unroll
             for (int rr = 0; rr < V + BOX - 1; ++rr) {
-              const int row = min(cv0 + rr, TH - 1);
-              const uint32_t *wp = wbase + row * tw4;
-              uint32_t w[NW + 1], sw[NW];
-#pragma unroll
-              for (int k = 0; k <= NW; ++k) w[k] = wp[k];
-#pragma unroll
-              for (int k = 0; k < NW; ++k) sw[k] = __funnelshift_r(w[k], w[k + 1], sh);
-              sw[NW - 1] &= LASTMASK;
+              uint32_t sw[NW];
+              window_row<BOX>(wbase + min(cv0 + rr, TH - 1) * tw4, sh, sw);
               uint32_t rs = 0, rq = 0;
 #pragma unroll
               for (int k = 0; k < NW; ++k) {
@@ -326,84 +460,22 @@ __global__ void __launch_bounds__(SL2_SEARCH_WARPS * 32, FILTER ? (BOX <= 11 ? 4
               }
             }
             // ---- FP64 score, improc.cpp:99-133 ------------------------------------------------
-            if constexpr (FILTER) {
-              // The reference's score equals 2 - 2*rho (rho = normalised cross-correlation) up to
-              // FP64 rounding (<= 1e-9 for sigma >= 10).  rho is evaluated in FP32 from the EXACT
-              // integer moments; only candidates whose approximate score is within kWindow of the
-              // running minimum can be the reference's arg-min (or tie with it), and only those go
-              // through the exact FP64 chain.  window 1e-5 >= 2 * (FP32 error 1.1e-6 + 1e-9).
-              // pass 1: approximate scores of the strip (no FP64 div/sqrt); pass 2, after the warp
-              // has agreed on the running minimum: exact chain for the survivors only.
-              if (patch_ok) {
-                float lmin = bmin;
-#pragma unroll
-                for (int j = 0; j < V; ++j) {
-                  if ((m_in >> j) & 1u) {
-                    if constexpr (BOX <= 11) {
-                      // n^2 var = n Sxx - Sx^2 and n Sxy - Sx0 Sx1 fit 32-bit integers for n <= 121
-                      // (n^2 255^2 < 2^31): exact in the integer pipe, one conversion each to FP32
-                      constexpr uint32_t NN = BOX * BOX, T100u = 100u * NN * NN;
-                      const uint32_t V1u = NN * a2[j] - a1[j] * a1[j];
-                      if (V1u > T100u) {
-                        const int N01i = (int)NN * (int)ax[j] - Sg0 * (int)a1[j];
-                        const float rho = (float)N01i * rsqrtf(V0f * (float)V1u);
-                        cap[j] = fmaf(-2.0f, rho, 2.0f);
-                        lmin = fminf(lmin, cap[j]);
-                      } else if (V1u == T100u) {
-                        cap[j] = -3.0e38f;  // knife edge of sdimage >= 10: the exact chain decides
-                      }
-                    } else {
-                      // n = 225: n Sxx, Sx^2 and both terms of n Sxy - Sx0 Sx1 still fit 32 unsigned bits
-                      // (225 * 225 * 255^2 < 2^32); only the last difference needs 64: exact in the integer pipe
-                      // (the FP64 pipe runs at half rate and every candidate paid 2 conversions + 2 DFMA + DSETP)
-                      constexpr uint32_t NN = BOX * BOX, T100u = 100u * NN * NN;
-                      const uint32_t V1u = NN * a2[j] - a1[j] * a1[j];
-                      if (V1u > T100u) {
-                        const long long N01 = (long long)NN * (long long)ax[j] - (long long)Sg0 * (long long)a1[j];
-                        const float rho = (float)N01 * rsqrtf(V0f * (float)V1u);
-                        cap[j] = fmaf(-2.0f, rho, 2.0f);
-                        lmin = fminf(lmin, cap[j]);
-                      } else if (V1u == T100u) {
-                        cap[j] = -3.0e38f;  // knife edge of sdimage >= 10: the exact chain decides
-                      }
-                    }
-                  }
-                }
-                bmin = lmin;
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < V; ++j) {
-                if ((m_all >> j) & 1u) {
-                  const double Sg1d = (double)(int)a1[j], Sg1sqd = (double)(int)a2[j],
-                               Sg0g1d = (double)(int)ax[j];
-                  double sigmag1;
-                  const double corr = exact_score_fn(pconst, Sg1d, Sg1sqd, Sg0g1d, &sigmag1);
-                  const int ui = tx0 + cu, vi = ty0 + cv0 + j;
-                  const int idx = ui * CH + vi;  // scan index
-                  const bool inside = (m_in >> j) & 1u;
-                  if (idx < dump.cap) {
-                    dump.corr[idx] = corr;
-                    dump.sd[idx] = sigmag1;
-                    dump.inside[idx] = inside ? 1 : 0;
-                  }
-                  if (inside && patch_ok && !(sigmag1 < 10.0)) best.offer(corr, idx);
-                }
-              }
-            }
-          }
-          if constexpr (FILTER) {
-            // the warp agrees on the running minimum, then only the survivors take the exact chain
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) bmin = fminf(bmin, __shfl_xor_sync(0xffffffffu, bmin, o));
-            const float thr = bmin + 1.0e-5f;  // kWindow, see above
 #pragma unroll
             for (int j = 0; j < V; ++j) {
-              if (cap[j] <= thr) {
-                double sg1;
-                const double corr = exact_score_fn(pconst, (double)(int)a1[j], (double)(int)a2[j],
-                                                   (double)(int)ax[j], &sg1);
-                if (!(sg1 < 10.0)) best.offer(corr, cand0 + j);
+              if ((m_all >> j) & 1u) {
+                const double Sg1d = (double)(int)a1[j], Sg1sqd = (double)(int)a2[j],
+                             Sg0g1d = (double)(int)ax[j];
+                double sigmag1;
+                const double corr = exact_score_fn(pconst, Sg1d, Sg1sqd, Sg0g1d, &sigmag1);
+                const int ui = tx0 + cu, vi = ty0 + cv0 + j;
+                const int idx = ui * CH + vi;  // scan index
+                const bool inside = (m_in >> j) & 1u;
+                if (idx < dump.cap) {
+                  dump.corr[idx] = corr;
+                  dump.sd[idx] = sigmag1;
+                  dump.inside[idx] = inside ? 1 : 0;
+                }
+                if (inside && patch_ok && !(sigmag1 < 10.0)) best.offer(corr, idx);
               }
             }
           }
