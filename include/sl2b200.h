@@ -91,6 +91,33 @@ const char *sl2_version(void);
 int sl2_set_stream_config(sl2_ctx *ctx, int32_t stream_id, const sl2_stream_config *sc);
 int sl2_get_stream_config(sl2_ctx *ctx, int32_t stream_id, sl2_stream_config *sc);
 
+/* ---- match consensus: keep wrong matches out of the EKF update (no reference counterpart) ----------------------
+ * The reference trusts every match its patch search accepts.  A stream with an inlier radius tau > 0 px runs a
+ * one-point RANSAC over the step's matches between the search and the update (Civera, Grasa, Davison, Montiel,
+ * "1-Point RANSAC for EKF Filtering", J. Field Robotics 2010), without its rescue stage:
+ *   M = the selected features whose match succeeded, in selection-rank order; k = |M|.
+ *   Every i in M is a hypothesis (exhaustive, no random sampling: a stream's result never depends on its batch
+ *   position, the step groups or the launch path).  Hypothesis i is the state-only partial update from i alone:
+ *   w_i = S_i^-1 nu_i (nu_i = z_i - h_i, S_i^-1 as the search forms it), a_i = dh_dxp_i^T w_i, b_i = dh_dy_i^T w_i,
+ *   dx_p = P[0:7, 0:7] a_i + P[0:7, y_i] b_i, dy_j = P[y_j, 0:7] a_i + P[y_j, y_i] b_i, with the predicted x and P.
+ *   Match j is an inlier of i when the camera model maps y_j + dy_j, seen from x_p + dx_p (q not renormalised), to a
+ *   point in front of the camera whose squared distance to z_j is <= fl(tau * tau); a NaN distance never is.  The
+ *   support of i counts its inliers (i included).  The winner has the largest support, ties going to the lowest
+ *   selection rank.  When its support is >= 2, every match of M outside its inlier set is rejected; otherwise (no
+ *   two matches agree) nothing is.
+ *   A rejected match keeps z and its score and gets found = 2 (sl2_get_features flags bit 2): it does not enter the
+ *   update, and it counts as an attempted, unsuccessful measurement, so a feature that keeps matching the wrong place
+ *   is culled by delete_bad_features' rule (minimum_attempted_measurements_of_feature, successful_match_fraction).
+ *   A step record's nmeas, m, nis and logdet_s describe the rows that entered the update.
+ * Every operation is a correctly rounded FP64 operation in the order written in the kernel (csrc/ekf.cu,
+ * consensus_kernel), so decisions are reproducible bit for bit.
+ * inlier_px = 0 (the default) is off: a context where no stream has it on runs exactly the path without it.
+ * Ordering like sl2_set_stream_config.  The setting belongs to the stream slot, like the frame source: snapshots do
+ * not carry it and a load leaves it.  SL2_ERR_ARG, with the setting unchanged, for a bad stream_id, a negative, NaN
+ * or infinite inlier_px, or (get) a NULL inlier_px. */
+int sl2_set_stream_consensus(sl2_ctx *ctx, int32_t stream_id, double inlier_px);
+int sl2_get_stream_consensus(sl2_ctx *ctx, int32_t stream_id, double *inlier_px);
+
 /* ---- frames (replaces the cv::Mat `frame` argument of MonoSLAM::GoOneStep, monoslam.cpp:108) */
 /* The frame ring keeps the context's width x height per stream.  A stream whose image is smaller
  * (sl2_set_stream_config) occupies the top-left width_s x height_s of its block; the rest of the block
@@ -252,7 +279,8 @@ int sl2_ekf_predict(sl2_ctx *ctx, int32_t stream_id, const double *u3);
  * Returns the number of visible features (>= 0) or a negative error. */
 int sl2_predict_measurements(sl2_ctx *ctx, int32_t stream_id);
 /* MonoSLAM::make_measurements (monoslam.cpp:336-359) for the features selected by
- * sl2_predict_measurements; returns the number of successful measurements. */
+ * sl2_predict_measurements, followed by the stream's match consensus when it is on; returns the number of
+ * successful measurements after the consensus. */
 int sl2_make_measurements(sl2_ctx *ctx, int32_t stream_id, int32_t slot);
 /* Kalman::KalmanFilterUpdate (kalman.cpp:72-119) with host-supplied measurement rows, in the
  * order of construct_total_measurement_stuff (monoslam.cpp:548-572): row pair k belongs to
@@ -292,7 +320,9 @@ int sl2_join(sl2_ctx *ctx);
 
 /* ---- read-back of per-feature results (Feature::h_/z_/S_/flags/counters, feature.h:96-140) */
 int sl2_get_features(sl2_ctx *ctx, int32_t stream_id, double *h /* n x 2 */, double *z /* n x 2 */,
-                     double *S /* n x 4 col-major */, uint8_t *flags /* bit0 selected, bit1 successful */,
+                     double *S /* n x 4 col-major */,
+                     uint8_t *flags /* bit0 selected, bit1 successful, bit2 matched and rejected by the match
+                                       consensus (sl2_set_stream_consensus) */,
                      int32_t *attempted, int32_t *successful, int32_t *select_rank);
 /* Feature::dh_by_dxv_ (2x13), dh_by_dy_ (2x3), R_ (2x2), nu_ (2) of the last prediction /
  * measurement, all column-major like the Eigen members (feature.h:104-112). Arrays may be NULL. */
@@ -331,7 +361,8 @@ int64_t sl2_launch_count(const sl2_ctx *ctx);
  *    dh_dy      double[nfeat][2][3]        row-major
  *    sel_rank   int32[nfeat]               rank in the selected list, -1 = not selected
  *    z_uv       int32[nfeat][2]            last match
- *    found      uint8[nfeat]               1 = the last measurement of the feature succeeded
+ *    found      uint8[nfeat]               1 = the last measurement of the feature succeeded, 2 = it matched and the
+ *                                          match consensus rejected it, 0 = it failed
  *    best       double[nfeat]              last correlation score
  *    job_feat   int32[nfeat]               feature of measurement job r (-1 = none): only jobs r < nsel hold one
  *    job_centre double[nfeat][2]           search centre of job r
@@ -426,7 +457,7 @@ typedef struct sl2_step_record { /* 256 bytes, no padding */
   int32_t nvisible;     /* visible features of the step's prediction */
   int32_t nsel;         /* features of the step's selection still in the map after the cull (the reference's
                            selected_feature_list_ after GoOneStep) */
-  int32_t nmeas;        /* successful measurements (= rows m / 2 of the update) */
+  int32_t nmeas;        /* successful measurements (= rows m / 2 of the update; after the match consensus) */
   int32_t nculled;      /* features the step's cull deleted */
   int32_t m;            /* rows of S; 0 when nothing was measured */
   double nis;           /* nu^T S^-1 nu of the step's update; 0 when m == 0 */

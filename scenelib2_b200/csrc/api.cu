@@ -106,6 +106,10 @@ struct sl2_ctx {
   DevPtr<uint8_t> src_stage;    // [slots][src_slot_bytes] + 16 bytes of slack for the kernel's aligned loads
   size_t src_stage_bytes = 0, src_slot_bytes = 0;
   Event ev_src;                 // recorded on `stream` behind the last table write
+  // match consensus (sl2_set_stream_consensus): the host mirror of every stream's inlier radius (0 = off) and the
+  // device array of the squared radii the consensus kernel reads
+  std::vector<double> cons_tau;  // [B]
+  double *cons_tau2 = nullptr;   // [B] device
 };
 
 namespace {
@@ -336,6 +340,14 @@ Sl2StreamCam cam_row(const sl2_stream_config &sc) {
 
 // the row travels as a kernel parameter, so the write is ordered on the stream like any other launch
 __global__ void write_cam_row_kernel(Sl2StreamCam *dst, const Sl2StreamCam row) { *dst = row; }
+__global__ void write_double_kernel(double *dst, const double v) { *dst = v; }
+
+// whether some stream of [lo, lo + cnt) has the match consensus on
+bool consensus_on(const sl2_ctx *c, int lo, int cnt) {
+  for (int s = lo; s < lo + cnt; ++s)
+    if (c->cons_tau[s] > 0.0) return true;
+  return false;
+}
 
 }  // namespace
 
@@ -477,6 +489,8 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   ALLOC(d.upd_m, B);
   ALLOC(d.Wp, B * SL2_MAX_PANELS * 256);
   ALLOC(c->xv_stage, (size_t)d.slots * B * SL2_NXV);
+  ALLOC(c->cons_tau2, B);
+  c->cons_tau.assign(B, 0.0);
 #undef ALLOC
   int rc = make_tensor_map(c);
   if (rc) return failed(rc, c->err);
@@ -653,6 +667,23 @@ int sl2_frame_set_layout(sl2_ctx *c, size_t *offsets) {
 int sl2_get_stream_config(sl2_ctx *c, int32_t s, sl2_stream_config *sc) {
   if (bad_stream(c, s) || !sc) return fail(c, SL2_ERR_ARG, "sl2_get_stream_config: bad argument");
   *sc = c->cams[s];
+  return SL2_OK;
+}
+
+// ---- match consensus ----------------------------------------------------------------------------
+int sl2_set_stream_consensus(sl2_ctx *c, int32_t s, double inlier_px) {
+  if (bad_stream(c, s)) return fail(c, SL2_ERR_ARG, "sl2_set_stream_consensus: bad stream");
+  if (!std::isfinite(inlier_px) || inlier_px < 0.0)
+    return fail(c, SL2_ERR_ARG, "sl2_set_stream_consensus: the inlier radius must be finite and >= 0");
+  const double tau = inlier_px == 0.0 ? 0.0 : inlier_px;  // -0 is off like +0
+  CU_TRY(c, sl2_launch_kernel(write_double_kernel, dim3(1), dim3(1), 0, queue(c), false, c->cons_tau2 + s, tau * tau));
+  c->cons_tau[s] = tau;
+  return SL2_OK;
+}
+
+int sl2_get_stream_consensus(sl2_ctx *c, int32_t s, double *inlier_px) {
+  if (bad_stream(c, s) || !inlier_px) return fail(c, SL2_ERR_ARG, "sl2_get_stream_consensus: bad argument");
+  *inlier_px = c->cons_tau[s];
   return SL2_OK;
 }
 
@@ -1096,6 +1127,7 @@ int sl2_make_measurements(sl2_ctx *c, int32_t s, int32_t slot) {
   L.slot = slot;
   L.scatter_to_features = 1;
   CU_TRY(c, sl2_launch_search(d, c->tmap, L, queue(c)));
+  if (c->cons_tau[s] > 0.0) CU_TRY(c, sl2_launch_consensus(d, s, 1, c->cons_tau2, queue(c)));
   // successful measurements of THIS step only: found[] keeps the flag of features that were not
   // selected this frame (Feature::successful_measurement_flag_), so count over the job list
   std::vector<uint8_t> f(d.Nmax);
@@ -1107,7 +1139,7 @@ int sl2_make_measurements(sl2_ctx *c, int32_t s, int32_t slot) {
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   int cnt = 0;
   for (int r = 0; r < nsel && r < d.Nmax; ++r)
-    if (jf[r] >= 0 && jf[r] < d.Nmax && f[jf[r]]) ++cnt;
+    if (jf[r] >= 0 && jf[r] < d.Nmax && f[jf[r]] == 1) ++cnt;
   return cnt;
 }
 
@@ -1168,6 +1200,8 @@ static int step_group(sl2_ctx *c, int32_t slot, int lo, int cnt, Sl2Queue q, cud
   L.slot = slot;
   L.scatter_to_features = 1;
   CU_TRY(c, sl2_launch_search(d, c->tmap, L, q));
+  if (consensus_on(c, lo, cnt))  // part of the search's time: the update times still sum to ev[2] .. ev[3]
+    CU_TRY(c, sl2_launch_consensus(d, lo, cnt, c->cons_tau2, q));
   if (t) CU_TRY(c, cudaEventRecord(c->ev[2].get(), st));
   if (after_search) CU_TRY(c, cudaEventRecord(after_search, st));
   cudaEvent_t evu[6];
@@ -1382,7 +1416,7 @@ int sl2_get_features(sl2_ctx *c, int32_t s, double *h, double *z, double *S, uin
     if (h) { h[2 * i] = hh[2 * i]; h[2 * i + 1] = hh[2 * i + 1]; }
     if (z) { z[2 * i] = (double)zz[2 * i]; z[2 * i + 1] = (double)zz[2 * i + 1]; }
     if (S) for (int k = 0; k < 4; ++k) S[4 * i + k] = SS[4 * i + k];
-    if (flags) flags[i] = (uint8_t)((rk[i] >= 0 ? 1 : 0) | (fd[i] ? 2 : 0));
+    if (flags) flags[i] = (uint8_t)((rk[i] >= 0 ? 1 : 0) | (fd[i] == 1 ? 2 : 0) | (fd[i] == 2 ? 4 : 0));
     if (attempted) attempted[i] = at[i];
     if (successful) successful[i] = su[i];
     if (select_rank) select_rank[i] = rk[i];

@@ -45,7 +45,7 @@ enum { SL2_BY_FEATURE, SL2_BY_JOB };
   X(double,  dh_dy,       6, SL2_BY_FEATURE, 0)  /* [2][3] row-major */                                         \
   X(int,     sel_rank,    1, SL2_BY_FEATURE, -1) /* rank in the selected list or -1 */                          \
   X(int,     z_uv,        2, SL2_BY_FEATURE, 0)                                                                 \
-  X(uint8_t, found,       1, SL2_BY_FEATURE, 0)  /* 1 = successful measurement this step */                     \
+  X(uint8_t, found,       1, SL2_BY_FEATURE, 0)  /* 1 = successful, 2 = matched but rejected by the consensus */ \
   X(double,  best,        1, SL2_BY_FEATURE, 0)                                                                 \
   /* per step, per job (rank order = measurement order) */                                                      \
   X(int,     job_feat,    1, SL2_BY_JOB,     -1) /* feature index of job r, -1 = none */                        \
@@ -202,6 +202,9 @@ cudaError_t sl2_launch_score_map(const Sl2Dev &d, const CUtensorMap &tmap, int s
                                  double *corr_dev, double *sd_dev, uint8_t *inside_dev, int cap, Sl2Queue q);
 cudaError_t sl2_launch_predict(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *u3_dev,
                                int do_predict, int do_measure, Sl2Queue q);
+// match consensus of the streams [stream_lo, stream_lo + stream_cnt) between the search and the update; tau2_dev[s] =
+// the squared inlier radius of stream s, 0 = off (ekf.cu)
+cudaError_t sl2_launch_consensus(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *tau2_dev, Sl2Queue q);
 // EKF update = 5 kernels (hp, chol, solve, syrk, finish); ev6 (optional) = 6 events recorded around them
 cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, int staged_m,
                               const int *st_feat, const double *st_Hxv, const double *st_Hy,

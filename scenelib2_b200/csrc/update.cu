@@ -229,7 +229,7 @@ __device__ __forceinline__ int hp_tables(const Sl2Dev &d, const HpSmem &sm, int 
     int feat = -1;
     if (tid < d.Nmax && tid < nsel) {
       const int i = d.job_feat[fb + tid];
-      if (i >= 0 && d.found[fb + i]) feat = i;
+      if (i >= 0 && d.found[fb + i] == 1) feat = i;
     }
     const unsigned bal = __ballot_sync(0xffffffffu, feat >= 0);
     if (lane == 0) sm.wcount[warp] = __popc(bal);
@@ -1414,7 +1414,7 @@ __global__ void __launch_bounds__(UPD_THREADS) upd_finish_kernel(const Sl2Dev d,
       int att = d.attempted[fb + i], suc = d.successful[fb + i];
       if (d.sel_rank[fb + i] >= 0) {
         att += 1;
-        if (d.found[fb + i]) suc += 1;
+        if (d.found[fb + i] == 1) suc += 1;  // a match the consensus rejected (2) is an unsuccessful attempt
         d.attempted[fb + i] = att;
         d.successful[fb + i] = suc;
       }

@@ -59,7 +59,8 @@ SOURCE_BPP = {SL2_SRC_GRAY8: 1, SL2_SRC_RGB24: 3, SL2_SRC_UYVY: 2}
 # every symbol include/sl2b200.h declares (checked by tests/test_abi.py)
 EXPORTS = [
     "sl2_default_config", "sl2_create", "sl2_destroy", "sl2_last_error", "sl2_sync", "sl2_version",
-    "sl2_set_stream_config", "sl2_get_stream_config", "sl2_set_frame", "sl2_set_frames", "sl2_set_frames_dev",
+    "sl2_set_stream_config", "sl2_get_stream_config", "sl2_set_stream_consensus", "sl2_get_stream_consensus",
+    "sl2_set_frame", "sl2_set_frames", "sl2_set_frames_dev",
     "sl2_set_stream_source", "sl2_get_stream_source", "sl2_frame_set_layout", "sl2_set_features",
     "sl2_num_features", "sl2_state_size", "sl2_set_state", "sl2_get_state", "sl2_delete_feature", "sl2_append_feature",
     "sl2_patch_search", "sl2_score_map", "sl2_smoe_search", "sl2_find_best_patch", "sl2_ekf_predict",
@@ -194,6 +195,8 @@ def load():
         L.sl2_default_config.restype = None
         L.sl2_set_stream_config.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamConfig)]
         L.sl2_get_stream_config.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamConfig)]
+        L.sl2_set_stream_consensus.argtypes = [C.c_void_p, C.c_int32, C.c_double]
+        L.sl2_get_stream_consensus.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_double)]
         L.sl2_set_frame.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_size_t]
         L.sl2_set_frames.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
         L.sl2_set_frames_dev.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
@@ -293,6 +296,17 @@ class Context:
         sc = Sl2StreamConfig()
         self._ck(self.L.sl2_get_stream_config(self.h, stream_id, C.byref(sc)))
         return sc
+
+    # ---- match consensus ----------------------------------------------------------------------
+    def set_stream_consensus(self, stream_id, inlier_px):
+        """sl2_set_stream_consensus: reject the step's matches that disagree with the best one-point hypothesis by
+        more than inlier_px pixels before the EKF update (0 = off, the default)."""
+        self._ck(self.L.sl2_set_stream_consensus(self.h, stream_id, float(inlier_px)))
+
+    def stream_consensus(self, stream_id):
+        v = C.c_double()
+        self._ck(self.L.sl2_get_stream_consensus(self.h, stream_id, C.byref(v)))
+        return v.value
 
     # ---- frames -------------------------------------------------------------------------------
     def set_stream_source(self, stream_id, format, width=0, height=0):
