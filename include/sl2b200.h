@@ -478,6 +478,63 @@ int sl2_enable_records(sl2_ctx *ctx, int32_t depth);
 int sl2_get_records(sl2_ctx *ctx, int32_t lo, int32_t cnt, int32_t max, sl2_step_record *out);
 int sl2_get_records_dev(sl2_ctx *ctx, int32_t lo, int32_t cnt, int32_t max, void *out_dev);
 
+/* ---- relocalisation: put a lost camera stream back on its own map (no reference counterpart) --------------------
+ * Williams, Klein, Reid, "Real-Time SLAM Relocalisation", ICCV 2007: find the map's features anywhere in the frame,
+ * estimate the camera pose from those 2-D / 3-D matches with a three-point consensus, and restart the filter there.
+ * For each listed stream s, in the frame of ring slot `slot`:
+ *   1. Full-image search.  Every map feature i < nfeat is searched with the rules of sl2_patch_search (search box,
+ *      ellipse test, sigma gates, scan-order arg-min, corrmax <= 0.40) with one job centred on ((w - 1) / 2,
+ *      (h - 1) / 2) with PuInv = diag(eps, eps), eps = 9 / (w^2 + h^2) of the stream's w x h image: an ellipse that
+ *      holds every window position.  M = the features whose search succeeded, in feature-index order; k = |M|.
+ *   2. Bearings.  z_j (the match pixel) -> Camera::Unproject (camera.cpp:133-157) -> divided by its norm.
+ *   3. Hypotheses.  Hypothesis h in [0, SL2_RELOC_HYPOTHESES) takes the matches (M[i0], M[i1], M[i2]) with
+ *      a = g(3h), b = g(3h + 1), c = g(3h + 2), g(x) = splitmix64 (Steele, Lea, Flood 2014) of state x, i.e. the
+ *      finaliser applied to x + 0x9E3779B97F4A7C15:  i0 = a mod k;  i1 = b mod (k - 1), then + 1 if >= i0;
+ *      i2 = c mod (k - 2), then + 1 if >= min(i0, i1), then + 1 if >= max(i0, i1).  k < 3: no hypothesis.
+ *      Each triple goes through Kneip, Scaramuzza, Siegwart's P3P (CVPR 2011): up to 4 poses, in the order of the
+ *      real roots of its quartic.  Collinear or coincident points or bearings, and any non-finite pose, give none.
+ *   4. Support of a pose xp = (r, q): match j is an inlier when the camera model (pose_RRW, zeroed_point,
+ *      project_point in csrc/ekf.cu) maps y_j to a point in front of the camera whose squared distance to z_j is
+ *      <= fl(tau * tau); a NaN distance never is.  The winner has the largest support; ties go to the lowest
+ *      (hypothesis, pose) index.
+ *   5. Refinement: SL2_RELOC_GN_ITERS Gauss-Newton steps over the position and a body-frame rotation increment on the
+ *      winner's inliers (stopping early when the 6 x 6 normal matrix is not positive definite); the inliers are then
+ *      counted again with the refined pose.
+ *   6. Acceptance iff that count >= min_inliers.  Then and only then the stream's state is written: x[0:3] = r,
+ *      x[3:7] = q, x[7:10] = v, x[10:13] = omega, P[0:13, 0:13] = Pxx, P[0:13, 13:n] = P[13:n, 0:13] = 0.  Nothing
+ *      else of the stream changes (Pyy, templates, counters, per-feature results, job slots, records).
+ * A stream's results and writes depend only on its state, its frame and the arguments (not on the list, its order,
+ * the stream id, the capacity or the step groups).  Unlisted streams are not touched.  Joins both step groups like
+ * every entry point, is ordered with queued work and synchronises; writes no step record.  Two kernel launches per
+ * call with cnt >= 1 (the search and the pose kernel); cnt = 0 does nothing.
+ * out[i] describes stream_ids[i]; z_uv[i][f] is the search's best position of feature f ((-1, -1) when no candidate
+ * was scored or f >= nfeat), flags[i][f] bit0 = matched (f in M), bit1 = inlier of the refined pose.
+ * SL2_ERR_ARG, with nothing changed, for: cnt < 0; a NULL stream_ids (cnt > 0), p, Pxx or out; a bad or repeated
+ * stream id; a bad slot; tau <= 0 or not finite; min_inliers < 4; reserved != 0; a non-finite v or omega, or
+ * |omega| = 0; a Pxx that is not finite, not exactly symmetric, or has an eigenvalue below -1e-12 times its largest
+ * eigenvalue magnitude (not positive semi-definite). */
+#define SL2_RELOC_HYPOTHESES 1024 /* three-point hypotheses per stream and call */
+#define SL2_RELOC_GN_ITERS 5      /* Gauss-Newton steps of the refinement */
+typedef struct sl2_reloc_params {
+  double inlier_px;      /* tau > 0: a match agrees with a pose when its reprojection is within tau px */
+  int32_t min_inliers;   /* >= 4: inliers the refined pose needs to be accepted */
+  int32_t reserved;      /* 0 */
+  double v[3], omega[3]; /* velocity state written on acceptance; |omega| > 0 (omega = 0 makes the motion model's F
+                            NaN) */
+} sl2_reloc_params;
+typedef struct sl2_reloc_result {
+  int32_t status;  /* 1 = accepted and written, 0 = the stream is unchanged */
+  int32_t matches; /* k: features whose full-image search succeeded */
+  int32_t support; /* inliers of the winning hypothesis (0 when no hypothesis exists) */
+  int32_t inliers; /* inliers of the refined pose (0 when no hypothesis exists) */
+  double rms_px;   /* RMS reprojection error over those inliers (NaN when there are none) */
+  double pose[7];  /* r (3), q (w, x, y, z; unit, w >= 0) of the refined pose; NaN when no hypothesis exists */
+} sl2_reloc_result;
+int sl2_relocalise(sl2_ctx *ctx, const int32_t *stream_ids, int32_t cnt, int32_t slot, const sl2_reloc_params *p,
+                   const double *Pxx /* 13 x 13 column-major */, sl2_reloc_result *out /* cnt */,
+                   int32_t *z_uv /* cnt x max_features x 2, may be NULL */,
+                   uint8_t *flags /* cnt x max_features, may be NULL */);
+
 #ifdef __cplusplus
 }
 #endif

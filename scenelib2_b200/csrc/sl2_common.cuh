@@ -205,6 +205,11 @@ cudaError_t sl2_launch_predict(const Sl2Dev &d, int stream_lo, int stream_cnt, c
 // match consensus of the streams [stream_lo, stream_lo + stream_cnt) between the search and the update; tau2_dev[s] =
 // the squared inlier radius of stream s, 0 = off (ekf.cu)
 cudaError_t sl2_launch_consensus(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *tau2_dev, Sl2Queue q);
+// relocalisation of the cnt streams ids_dev[] from the full-image search's results by job (job = (stream - stream_lo) *
+// Nmax + feature): pose consensus, refinement and, on acceptance, the state write (ekf.cu reloc_kernel)
+cudaError_t sl2_launch_reloc(const Sl2Dev &d, int cnt, const int *ids_dev, int stream_lo, const int *search_uv,
+                             const uint8_t *search_found, const sl2_reloc_params *prm_dev, const double *Pxx_dev,
+                             sl2_reloc_result *res_dev, int *zuv_dev, uint8_t *flags_dev, Sl2Queue q);
 // EKF update = 5 kernels (hp, chol, solve, syrk, finish); ev6 (optional) = 6 events recorded around them
 cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, int staged_m,
                               const int *st_feat, const double *st_Hxv, const double *st_Hy,

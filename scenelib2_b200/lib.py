@@ -70,8 +70,28 @@ EXPORTS = [
     "sl2_smoe_search_patch", "sl2_measure_partial_features",
     "sl2_get_features", "sl2_get_feature_jacobians", "sl2_enable_timing", "sl2_last_step_times", "sl2_last_update_times", "sl2_launch_count",
     "sl2_snapshot_layout", "sl2_snapshot_bytes", "sl2_save_streams", "sl2_load_streams", "sl2_save_streams_dev", "sl2_load_streams_dev",
-    "sl2_enable_records", "sl2_get_records", "sl2_get_records_dev",
+    "sl2_enable_records", "sl2_get_records", "sl2_get_records_dev", "sl2_relocalise",
 ]
+
+SL2_RELOC_HYPOTHESES = 1024   # three-point hypotheses per stream and sl2_relocalise call
+SL2_RELOC_GN_ITERS = 5        # Gauss-Newton steps of the refinement
+
+
+class Sl2RelocParams(C.Structure):
+    """sl2_reloc_params: inlier radius, acceptance count and the velocity state of a relocalisation."""
+    _fields_ = [("inlier_px", C.c_double), ("min_inliers", C.c_int32), ("reserved", C.c_int32),
+                ("v", C.c_double * 3), ("omega", C.c_double * 3)]
+
+
+class Sl2RelocResult(C.Structure):
+    """sl2_reloc_result: what sl2_relocalise found for one stream."""
+    _fields_ = [("status", C.c_int32), ("matches", C.c_int32), ("support", C.c_int32), ("inliers", C.c_int32),
+                ("rms_px", C.c_double), ("pose", C.c_double * 7)]
+
+
+# the same result as a NumPy structured dtype: Context.relocalise returns an array of it
+RELOC_RESULT_DTYPE = np.dtype([("status", np.int32), ("matches", np.int32), ("support", np.int32),
+                               ("inliers", np.int32), ("rms_px", np.float64), ("pose", np.float64, (7,))])
 
 SL2_SNAPSHOT_MAGIC = 0x53324C53
 SL2_SNAPSHOT_VERSION = 1
@@ -229,6 +249,8 @@ def load():
         L.sl2_enable_records.argtypes = [C.c_void_p, C.c_int32]
         L.sl2_get_records.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
         L.sl2_get_records_dev.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
+        L.sl2_relocalise.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(Sl2RelocParams),
+                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib = L
     return _lib
 
@@ -656,6 +678,28 @@ class Context:
         """sl2_get_records_dev: the same records into device memory at dev_ptr (record i * max + j, 8-byte aligned),
         asynchronous on the context's stream.  Returns k."""
         return self._ck(self.L.sl2_get_records_dev(self.h, lo, cnt, max, dev_ptr))
+
+    # ---- relocalisation -------------------------------------------------------------------------
+    def relocalise(self, stream_ids, slot, inlier_px, min_inliers, v, omega, Pxx, reserved=0):
+        """sl2_relocalise: search every map feature of each listed stream over its whole frame in `slot`, estimate
+        the camera pose with a three-point consensus and, when at least min_inliers matches agree with the refined
+        pose, restart the stream's filter there (x[7:13] = v, omega; Pxx; the camera-map correlations zero).
+        Returns (results, z_uv, flags): a RELOC_RESULT_DTYPE array (cnt,), int32 (cnt, max_features, 2) and uint8
+        (cnt, max_features) (bit0 matched, bit1 inlier of the refined pose)."""
+        ids = np.ascontiguousarray(stream_ids, np.int32).reshape(-1)
+        cnt = ids.size
+        prm = Sl2RelocParams()
+        prm.inlier_px, prm.min_inliers, prm.reserved = float(inlier_px), int(min_inliers), int(reserved)
+        for i in range(3):
+            prm.v[i], prm.omega[i] = float(v[i]), float(omega[i])
+        Pxx = np.asfortranarray(np.asarray(Pxx, np.float64).reshape(13, 13))
+        N = self.cfg.max_features
+        res = np.zeros(max(cnt, 1), RELOC_RESULT_DTYPE)
+        z = np.zeros((max(cnt, 1), N, 2), np.int32)
+        fl = np.zeros((max(cnt, 1), N), np.uint8)
+        self._ck(self.L.sl2_relocalise(self.h, ids.ctypes.data, cnt, slot, C.byref(prm), Pxx.ctypes.data,
+                                       res.ctypes.data, z.ctypes.data, fl.ctypes.data))
+        return res[:cnt], z[:cnt], fl[:cnt]
 
 
 def config_for_scene(sc, num_streams=1, frame_slots=1, device=0, max_features=None,
