@@ -109,7 +109,7 @@ int sl2_get_stream_config(sl2_ctx *ctx, int32_t stream_id, sl2_stream_config *sc
  *   update, and it counts as an attempted, unsuccessful measurement, so a feature that keeps matching the wrong place
  *   is culled by delete_bad_features' rule (minimum_attempted_measurements_of_feature, successful_match_fraction).
  *   A step record's nmeas, m, nis and logdet_s describe the rows that entered the update.
- * Every operation is a correctly rounded FP64 operation in the order written in the kernel (csrc/ekf.cu,
+ * Every operation is a correctly rounded FP64 operation in the order written in the kernel (csrc/consensus.cu,
  * consensus_kernel), so decisions are reproducible bit for bit.
  * inlier_px = 0 (the default) is off: a context where no stream has it on runs exactly the path without it.
  * Ordering like sl2_set_stream_config.  The setting belongs to the stream slot, like the frame source: snapshots do
@@ -494,7 +494,7 @@ int sl2_get_records_dev(sl2_ctx *ctx, int32_t lo, int32_t cnt, int32_t max, void
  *      Each triple goes through Kneip, Scaramuzza, Siegwart's P3P (CVPR 2011): up to 4 poses, in the order of the
  *      real roots of its quartic.  Collinear or coincident points or bearings, and any non-finite pose, give none.
  *   4. Support of a pose xp = (r, q): match j is an inlier when the camera model (pose_RRW, zeroed_point,
- *      project_point in csrc/ekf.cu) maps y_j to a point in front of the camera whose squared distance to z_j is
+ *      project_point in csrc/sl2_model.cuh) maps y_j to a point in front of the camera whose squared distance to z_j is
  *      <= fl(tau * tau); a NaN distance never is.  The winner has the largest support; ties go to the lowest
  *      (hypothesis, pose) index.
  *   5. Refinement: SL2_RELOC_GN_ITERS Gauss-Newton steps over the position and a body-frame rotation increment on the

@@ -3,10 +3,11 @@ import os
 import subprocess
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-SOURCES = ["csrc/api.cu", "csrc/search.cu", "csrc/ekf.cu", "csrc/update.cu", "csrc/detect.cu", "csrc/particles.cu", "csrc/smoe.cu",
-           "csrc/snapshot.cu", "csrc/records.cu", "csrc/ingest.cu"]
-HEADERS = ["csrc/sl2_common.cuh", "csrc/sl2_ptx.cuh", "csrc/sl2_score.cuh", "../include/sl2b200.h", "host/scenelib2_b200.cpp",
-           "host/scenelib2_b200.h", "host/sl2_compat.h", "host/sl2_headless.cpp", "host/png_decode.h", "host/jpeg_decode.h", "host/bmp_decode.h"]
+SOURCES = ["csrc/api.cu", "csrc/search.cu", "csrc/ekf.cu", "csrc/consensus.cu", "csrc/reloc.cu", "csrc/update.cu",
+           "csrc/detect.cu", "csrc/particles.cu", "csrc/smoe.cu", "csrc/snapshot.cu", "csrc/records.cu", "csrc/ingest.cu"]
+HEADERS = ["csrc/sl2_common.cuh", "csrc/sl2_model.cuh", "csrc/sl2_ptx.cuh", "csrc/sl2_score.cuh", "../include/sl2b200.h",
+           "host/scenelib2_b200.cpp", "host/scenelib2_b200.h", "host/sl2_compat.h", "host/sl2_headless.cpp",
+           "host/png_decode.h", "host/jpeg_decode.h", "host/bmp_decode.h"]
 LIB = os.path.join(HERE, "libsl2b200.so")
 
 

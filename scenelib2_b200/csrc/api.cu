@@ -1,6 +1,6 @@
 // api.cu — context management and the extern "C" surface declared in include/sl2b200.h.
 // Host side only orchestrates: every arithmetic step of the hot path runs in the sm_90a
-// kernels of search.cu / ekf.cu.  There is deliberately no CPU fallback.
+// kernels of search.cu / ekf.cu / consensus.cu / reloc.cu / update.cu.  There is deliberately no CPU fallback.
 #include <algorithm>
 #include <cmath>
 #include <cstdio>

@@ -1,6 +1,6 @@
 // particles.cu — depth particles of partially-initialised features (SURVEY N2): the re-weighting of
-// sl2_measure_partial_features / sl2_measure_particles.  Their prediction (particle_predict_kernel) is in ekf.cu, with
-// the measurement models it shares with map features.
+// sl2_measure_partial_features / sl2_measure_particles.  Their prediction (particle_predict_kernel) is in ekf.cu, built
+// from the measurement models it shares with map features (sl2_model.cuh).
 //   particle_kernel   MonoSLAM::update_partially_initialised_feature_probabilities (monoslam.cpp:1447-1493, body for
 //                     one FeatureInitInfo) + FeatureInitInfo::normalise_particle_vector_and_calculate_cumulative /
 //                     prune_particle_vector / calculate_mean_and_covariance (feature_init_info.cpp:95-172), after the

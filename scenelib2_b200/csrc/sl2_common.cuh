@@ -133,6 +133,23 @@ __device__ __forceinline__ void pdl_prologue() {
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 }
+
+// The ordered gather of a block: the values v >= 0 of its threads, in thread order, into out[0 .. count); returns count
+// and sets *at (if given) to this thread's index in out, -1 for v < 0.  wcount: scratch for the first nwarps warps,
+// which hold every thread with a value.  All threads call; out is complete after the caller's next __syncthreads().
+__device__ __forceinline__ int block_gather(int v, int *out, int *wcount, int nwarps, int *at = nullptr) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const unsigned bal = __ballot_sync(0xffffffffu, v >= 0);
+  if (lane == 0) wcount[warp] = __popc(bal);
+  __syncthreads();
+  int base = 0, count = 0;
+  for (int w = 0; w < nwarps; ++w) { base += w < warp ? wcount[w] : 0; count += wcount[w]; }
+  const int j = base + __popc(bal & ((1u << lane) - 1u));
+  if (v >= 0) out[j] = v;
+  if (at) *at = v >= 0 ? j : -1;
+  return count;
+}
+
 // PDL when the launch covers fewer camera streams than SL2_PDL_AUTO_STREAMS: a single camera stream is a chain of 8
 // short kernels bound by launch-to-launch latency, which PDL shortens; a full batch fills the GPU and PDL only adds
 // resident waiting CTAs.
@@ -181,7 +198,7 @@ inline bool sl2_box_supported(int box) {
   return sl2_with_box(box, [](auto) { return cudaSuccess; }) == cudaSuccess;
 }
 
-// launchers (defined in search.cu / ekf.cu / update.cu), called from api.cu
+// launchers (defined in search.cu / ekf.cu / consensus.cu / reloc.cu / update.cu), called from api.cu
 struct SearchLaunch {
   // job arrays may be the context's own (fused step) or temporaries (staged API)
   const int *job_feat;       // [njobs_per_stream * B] or [n]
@@ -203,10 +220,10 @@ cudaError_t sl2_launch_score_map(const Sl2Dev &d, const CUtensorMap &tmap, int s
 cudaError_t sl2_launch_predict(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *u3_dev,
                                int do_predict, int do_measure, Sl2Queue q);
 // match consensus of the streams [stream_lo, stream_lo + stream_cnt) between the search and the update; tau2_dev[s] =
-// the squared inlier radius of stream s, 0 = off (ekf.cu)
+// the squared inlier radius of stream s, 0 = off (consensus.cu)
 cudaError_t sl2_launch_consensus(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *tau2_dev, Sl2Queue q);
 // relocalisation of the cnt streams ids_dev[] from the full-image search's results by job (job = (stream - stream_lo) *
-// Nmax + feature): pose consensus, refinement and, on acceptance, the state write (ekf.cu reloc_kernel)
+// Nmax + feature): pose consensus, refinement and, on acceptance, the state write (reloc.cu reloc_kernel)
 cudaError_t sl2_launch_reloc(const Sl2Dev &d, int cnt, const int *ids_dev, int stream_lo, const int *search_uv,
                              const uint8_t *search_found, const sl2_reloc_params *prm_dev, const double *Pxx_dev,
                              sl2_reloc_result *res_dev, int *zuv_dev, uint8_t *flags_dev, Sl2Queue q);

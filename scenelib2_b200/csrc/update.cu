@@ -217,7 +217,7 @@ __device__ __forceinline__ HpSmem hp_carve(uint8_t *base, int kmax, int ld) {
 __device__ __forceinline__ int hp_tables(const Sl2Dev &d, const HpSmem &sm, int s, int rows_per_block, int staged_m,
                                          const int *st_feat, const double *st_Hxv, const double *st_Hy,
                                          const double *st_R, const double *st_nu) {
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const size_t fb = (size_t)s * d.Nmax;
   // ---- measurement list in selected order, successful only (monoslam.cpp:556-571) --------------
   int K;
@@ -231,16 +231,8 @@ __device__ __forceinline__ int hp_tables(const Sl2Dev &d, const HpSmem &sm, int 
       const int i = d.job_feat[fb + tid];
       if (i >= 0 && d.found[fb + i] == 1) feat = i;
     }
-    const unsigned bal = __ballot_sync(0xffffffffu, feat >= 0);
-    if (lane == 0) sm.wcount[warp] = __popc(bal);
-    __syncthreads();
-    int base = 0, total = 0;
-    for (int w = 0; w < (SL2_MAX_MEASURED + 31) / 32; ++w) {  // nsel <= kmax: later warps select nothing
-      if (w < warp) base += sm.wcount[w];
-      total += sm.wcount[w];
-    }
-    if (feat >= 0) sm.mfeat[base + __popc(bal & ((1u << lane) - 1u))] = feat;
-    K = total;
+    // nsel <= kmax: the warps beyond the first (SL2_MAX_MEASURED + 31) / 32 select nothing
+    K = block_gather(feat, sm.mfeat, sm.wcount, (SL2_MAX_MEASURED + 31) / 32);
   }
   const int m = 2 * K;
   if (blockIdx.x == 0 && tid == 0) {

@@ -1,5 +1,5 @@
 // TEST INFRASTRUCTURE ONLY.  The match consensus (include/sl2b200.h, sl2_set_stream_consensus) on top of the CPU
-// oracle (oracle/slam.hpp, used as it is): the consensus as a pure function in the operation order of csrc/ekf.cu
+// oracle (oracle/slam.hpp, used as it is): the consensus as a pure function in the operation order of csrc/consensus.cu
 // consensus_kernel, and a whole step that runs it between the oracle's measure and update.  Compiled by
 // tests/consensus_oracle.py with the oracle's flags (-O3 -ffp-contract=off).
 #include <cstring>

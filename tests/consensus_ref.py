@@ -1,36 +1,11 @@
 """The match consensus (include/sl2b200.h, sl2_set_stream_consensus) restated in Python floats, independently of
-the oracle: the operation order of csrc/ekf.cu consensus_kernel, one IEEE double operation at a time."""
+the oracle: the operation order of csrc/consensus.cu consensus_kernel, one IEEE double operation at a time; the camera
+model is camera_ref's."""
 import math
 
 import numpy as np
 
-
-def _quat_to_R(w, x, y, z):
-    tx, ty, tz = 2.0 * x, 2.0 * y, 2.0 * z
-    twx, twy, twz = tx * w, ty * w, tz * w
-    txx, txy, txz = tx * x, ty * x, tz * x
-    tyy, tyz, tzz = ty * y, tz * y, tz * z
-    return [[1.0 - (tyy + tzz), txy - twz, txz + twy],
-            [txy + twz, 1.0 - (txx + tzz), tyz - twx],
-            [txz - twy, tyz + twx, 1.0 - (txx + tyy)]]
-
-
-def _rrw(xp):
-    w, x, y, z = (float(v) for v in xp[3:7])
-    n2 = w * w + x * x + y * y + z * z
-    if n2 > 0.0:
-        w, x, y, z = w / n2, (-x) / n2, (-y) / n2, (-z) / n2
-    else:
-        w = x = y = z = 0.0
-    return _quat_to_R(w, x, y, z)
-
-
-def _project(cam8, zc):
-    fku, fkv, u0, v0, kd1 = (float(v) for v in cam8[2:7])
-    uc = (-fku) * zc[0] / zc[2]
-    vc = (-fkv) * zc[1] / zc[2]
-    factor = math.sqrt(1.0 + 2.0 * kd1 * (uc * uc + vc * vc))
-    return uc / factor + u0, vc / factor + v0
+from camera_ref import reprojection_d2
 
 
 def _sinv(S):
@@ -55,8 +30,6 @@ def restated(cam8, x, P, pos, z, h, S, dxp, dy, tau):
         a.append([float(dxp[j, 0, c]) * w0 + float(dxp[j, 1, c]) * w1 for c in range(7)])
         b.append([float(dy[j, 0, c]) * w0 + float(dy[j, 1, c]) * w1 for c in range(3)])
     d2 = np.full((k, k), np.nan)
-    support = np.zeros(k, np.int32)
-    inl = np.zeros((k, k), bool)
     for i in range(k):
         xp = []
         for r in range(7):
@@ -66,29 +39,18 @@ def restated(cam8, x, P, pos, z, h, S, dxp, dy, tau):
             for c in range(3):
                 s = s + float(P[r, pos[i] + c]) * b[i][c]
             xp.append(float(x[r]) + s)
-        R = _rrw(xp)
+        y = np.empty((k, 3))
         for j in range(k):
-            y = []
             for r in range(3):
                 s = 0.0
                 for c in range(7):
                     s = s + float(P[pos[j] + r, c]) * a[i][c]
                 for c in range(3):
                     s = s + float(P[pos[j] + r, pos[i] + c]) * b[i][c]
-                y.append(float(x[pos[j] + r]) + s)
-            dd = [y[r] - xp[r] for r in range(3)]
-            zc = []
-            for r in range(3):
-                s = 0.0
-                for c in range(3):
-                    s = s + R[r][c] * dd[c]
-                zc.append(s)
-            if zc[2] > 0.0:
-                g = _project(cam8, zc)
-                du, dv = float(z[j, 0]) - g[0], float(z[j, 1]) - g[1]
-                d2[i, j] = du * du + dv * dv
-                inl[i, j] = d2[i, j] <= tau2
-        support[i] = int(inl[i].sum())
+                y[j, r] = float(x[pos[j] + r]) + s
+        d2[i] = reprojection_d2(cam8, xp, y, z)
+    inl = d2 <= tau2  # NaN: never
+    support = inl.sum(axis=1).astype(np.int32)
     win = int(np.argmax(support)) if k else -1
     if k == 0 or support[win] < 2:
         return np.ones(k, bool), support, -1, d2

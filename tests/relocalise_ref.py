@@ -1,13 +1,14 @@
-"""Relocalisation (include/sl2b200.h, sl2_relocalise) restated in NumPy, steps 2-6, in the order of csrc/ekf.cu
+"""Relocalisation (include/sl2b200.h, sl2_relocalise) restated in NumPy, steps 2-6, in the order of csrc/reloc.cu
 reloc_kernel: bearings, the splitmix64 hypothesis sequence, Kneip's P3P, support, winner, Gauss-Newton refinement,
-recount.  The inlier tests run the camera model one IEEE double operation at a time in the kernel's order (NumPy's
-element-wise operations are correctly rounded and never fused); the P3P, whose cube roots and trigonometry differ
-between libraries in the last bits, is followed up to rounding.  Fed the device's matches, it gives the device's
-decisions whenever no squared distance lies within reach of a last-bit difference of fl(tau * tau): `margin` says
-how far the closest one was."""
+recount.  The inlier tests run the camera model of camera_ref one IEEE double operation at a time in the kernel's
+order; the P3P, whose cube roots and trigonometry differ between libraries in the last bits, is followed up to
+rounding.  Fed the device's matches, it gives the device's decisions whenever no squared distance lies within reach of
+a last-bit difference of fl(tau * tau): `margin` says how far the closest one was."""
 import math
 
 import numpy as np
+
+from camera_ref import camera_points, reprojection_d2, rrw
 
 HYPOTHESES = 1024
 GN_ITERS = 5
@@ -203,43 +204,6 @@ def p3p(Pw, fb):
     return out
 
 
-def _rrw(xp):
-    w, x, y, z = (float(v) for v in xp[3:7])
-    n2 = w * w + x * x + y * y + z * z
-    if n2 > 0.0:
-        w, x, y, z = w / n2, (-x) / n2, (-y) / n2, (-z) / n2
-    else:
-        w = x = y = z = 0.0
-    tx, ty, tz = 2.0 * x, 2.0 * y, 2.0 * z
-    twx, twy, twz = tx * w, ty * w, tz * w
-    txx, txy, txz = tx * x, ty * x, tz * x
-    tyy, tyz, tzz = ty * y, tz * y, tz * z
-    return [[1.0 - (tyy + tzz), txy - twz, txz + twy],
-            [txy + twz, 1.0 - (txx + tzz), tyz - twx],
-            [txz - twy, tyz + twx, 1.0 - (txx + tyy)]]
-
-
-def camera_points(xp, y):
-    """zeroed_point of every y (k, 3) seen from xp: RRW (y - r), rows summed from 0.0 in ascending order."""
-    R = _rrw(xp)
-    d = [y[:, i] - float(xp[i]) for i in range(3)]
-    return np.stack([((0.0 + R[i][0] * d[0]) + R[i][1] * d[1]) + R[i][2] * d[2] for i in range(3)], axis=1)
-
-
-def reprojection_d2(cam8, xp, y, z):
-    """Squared distance of project_point(zeroed_point(y)) to z, NaN behind the camera (the kernel's reloc_inlier)."""
-    fku, fkv, u0, v0, kd1 = (float(v) for v in cam8[2:7])
-    zc = camera_points(xp, y)
-    with np.errstate(all="ignore"):
-        uc = ((-fku) * zc[:, 0]) / zc[:, 2]
-        vc = ((-fkv) * zc[:, 1]) / zc[:, 2]
-        factor = np.sqrt(1.0 + (2.0 * kd1) * (uc * uc + vc * vc))
-        du = z[:, 0] - (uc / factor + u0)
-        dv = z[:, 1] - (vc / factor + v0)
-        d2 = du * du + dv * dv
-    return np.where(zc[:, 2] > 0.0, d2, np.nan)
-
-
 def project(cam8, xp, y):
     """h and dh/dz (Camera::ProjectionJacobian) of the points y (k, 3) seen from xp, for the refinement."""
     fku, fkv, u0, v0, kd1 = (float(v) for v in cam8[2:7])
@@ -271,7 +235,7 @@ def refine(cam8, xp, y, z):
     xp = [float(v) for v in xp]
     for _ in range(GN_ITERS):
         h, J, zc = project(cam8, xp, y)
-        RRW = np.array(_rrw(xp))
+        RRW = np.array(rrw(xp))
         Zx = np.zeros((len(y), 3, 3))
         Zx[:, 0, 1], Zx[:, 0, 2] = -zc[:, 2], zc[:, 1]
         Zx[:, 1, 0], Zx[:, 1, 2] = zc[:, 2], -zc[:, 0]

@@ -9,7 +9,8 @@ import numpy as np
 import pytest
 
 import consensus_oracle as co
-from consensus_ref import _project, _quat_to_R, restated
+from camera_ref import project_point, quat_to_R
+from consensus_ref import restated
 from oracle import pyoracle as po
 from scenelib2_b200 import synth
 
@@ -32,7 +33,7 @@ def make_case(rng, k, nf=None, outliers=(), offset=(9.0, -6.0), P=None, camera_p
     if camera_pts is None:
         d = rng.uniform(0.5, 1.5, nf)
         camera_pts = np.stack([rng.uniform(-0.35, 0.35, nf) * d, rng.uniform(-0.25, 0.25, nf) * d, d], axis=1)
-    R = np.array(_quat_to_R(*xv[3:7]))
+    R = np.array(quat_to_R(*xv[3:7]))
     x = np.concatenate([xv, (xv[:3] + camera_pts @ R.T).ravel()])
     if P is None:
         P = synth.make_prior_covariance(rng, n, sig_y=0.01)
@@ -122,14 +123,14 @@ def test_point_behind_the_camera_is_never_an_inlier():
     # exactly that mirrored projection
     p = case["pos"][2]
     xv = case["x"][:13]
-    R = np.array(_quat_to_R(*xv[3:7]))
+    R = np.array(quat_to_R(*xv[3:7]))
     c = R.T @ (case["x"][p:p + 3] - xv[:3])
     case["x"][p:p + 3] = xv[:3] + R @ (c * [1.0, 1.0, -1.0])
     case["P"][p:p + 3, :] = 0.0
     case["P"][:, p:p + 3] = 0.0
     case["P"][p:p + 3, p:p + 3] = np.eye(3) * 1e-4
     zc = R.T @ (case["x"][p:p + 3] - xv[:3])
-    case["z"][2] = np.round(_project(CAM8, zc))
+    case["z"][2] = np.round(project_point(CAM8, zc)[0])
     keep, sup, win, d2 = both(case, 1000.0)  # a radius that takes every point in front of the camera
     assert np.isnan(d2[:, 2]).all()
     assert win >= 0 and not keep[2] and keep[np.arange(k) != 2].all()

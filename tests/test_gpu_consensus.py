@@ -1,4 +1,4 @@
-"""The match consensus on the device (sl2_set_stream_consensus, csrc/ekf.cu consensus_kernel) on scenes with
+"""The match consensus on the device (sl2_set_stream_consensus, csrc/consensus.cu consensus_kernel) on scenes with
 distractors: a feature's template pasted at a fixed offset inside its search ellipse while its true location is
 occluded, so that the patch search returns a confident wrong match.  A match is correct iff z = pix + shift[t]."""
 import math

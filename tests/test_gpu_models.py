@@ -24,7 +24,7 @@ TRANSFORMS = [([1e-3, 0.48, -0.6, 0.64], [0.7, -1.3, 2.1]),      # near-180 degr
               ([0.2, -0.1, 0.9, -0.4], [3.0, 0.0, -1.0])]
 GENERAL_OMEGA = [0.05, -0.08, 0.03]
 # The moved world is equivariant only while |q| = 1: the reference never renormalises q in x (quirk Q1), so after an
-# update |q| - 1 is ~1e-6 .. 1e-4, and for q = s u its rotation matrix (math_util / ekf.cu quat_to_R) is
+# update |q| - 1 is ~1e-6 .. 1e-4, and for q = s u its rotation matrix (math_util / sl2_model.cuh quat_to_R) is
 # (1 - s^2) I + s^2 R(u), whose (1 - s^2) I part acts in world axes.  h then moves by 1e-4 px after the second step
 # and ~5e-3 px after the twelfth, enough to reorder two features of nearly equal trace S.  So the moved and unmoved
 # runs are compared on the first step only; later steps are compared with the oracle, stream by stream.

@@ -1,4 +1,4 @@
-"""Relocalisation on the device (sl2_relocalise; csrc/ekf.cu reloc_kernel after the full-image patch search) on
+"""Relocalisation on the device (sl2_relocalise; csrc/reloc.cu reloc_kernel after the full-image patch search) on
 kidnapped scenes: a stream tracks a synth scene for 5 steps, then its camera jumps to a ground-truth pose the
 prediction cannot reach.  The new frame is a fresh texture with every template pasted at the rounded projection of
 its map point under that pose; three fused steps confirm the loss, then the stream is relocalised."""
