@@ -1,7 +1,7 @@
 // consensus.cu — the match consensus on sm_90a, between the patch search and the EKF update of the fused step.
 // One-point RANSAC with exhaustive hypotheses (Civera, Grasa, Davison, Montiel, J. Field Robotics 2010), one CTA per
 // camera stream of the launch; streams whose tau2[s] (= fl(tau * tau), 0 = off) is not > 0 return at once.
-// Semantics: include/sl2b200.h, sl2_set_stream_consensus.
+// Semantics: include/sl2b200.h, sl2_set_stream_consensus (which, with sl2_get_stream_consensus, ends this file).
 //
 // M = the job slots r < nsel whose feature has found == 1, in rank order (match j, k = |M| <= SL2_MAX_MEASURED);
 // x, P are the predicted state and covariance.  Every operation is one correctly rounded, never-fused op (rd), in
@@ -20,7 +20,12 @@
 // Shape: warp w takes hypotheses w, w + CONS_WARPS, ...; its lanes take the matches j = lane + 32 c and count the
 // support (warp_support).  The per-match terms and P[yj, 0:7] sit in shared memory, P[0:7, yi] and the 3x3 blocks
 // P[yj, yi] are read from L2.
+#include <cmath>
+
+#include "sl2_context.cuh"
 #include "sl2_model.cuh"
+
+using namespace sl2;
 
 namespace {
 
@@ -130,6 +135,8 @@ __global__ void __launch_bounds__(32 * CONS_WARPS) consensus_kernel(const Sl2Dev
     if (!((mask[win][j >> 5] >> (j & 31)) & 1u)) d.found[fb + mf[j]] = 2;
 }
 
+__global__ void write_double_kernel(double *dst, const double v) { *dst = v; }
+
 }  // namespace
 
 cudaError_t sl2_launch_consensus(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *tau2_dev, Sl2Queue q) {
@@ -137,3 +144,23 @@ cudaError_t sl2_launch_consensus(const Sl2Dev &d, int stream_lo, int stream_cnt,
   return sl2_launch_kernel(consensus_kernel, dim3(stream_cnt), dim3(32 * CONS_WARPS), 0, q, sl2_use_pdl(stream_cnt), d,
                            stream_lo, tau2_dev);
 }
+
+extern "C" {
+
+int sl2_set_stream_consensus(sl2_ctx *c, int32_t s, double inlier_px) {
+  if (bad_stream(c, s)) return fail(c, SL2_ERR_ARG, "sl2_set_stream_consensus: bad stream");
+  if (!std::isfinite(inlier_px) || inlier_px < 0.0)
+    return fail(c, SL2_ERR_ARG, "sl2_set_stream_consensus: the inlier radius must be finite and >= 0");
+  const double tau = inlier_px == 0.0 ? 0.0 : inlier_px;  // -0 is off like +0
+  CU_TRY(c, sl2_launch_kernel(write_double_kernel, dim3(1), dim3(1), 0, queue(c), false, c->cons_tau2 + s, tau * tau));
+  c->cons_tau[s] = tau;
+  return SL2_OK;
+}
+
+int sl2_get_stream_consensus(sl2_ctx *c, int32_t s, double *inlier_px) {
+  if (bad_stream(c, s) || !inlier_px) return fail(c, SL2_ERR_ARG, "sl2_get_stream_consensus: bad argument");
+  *inlier_px = c->cons_tau[s];
+  return SL2_OK;
+}
+
+}  // extern "C"

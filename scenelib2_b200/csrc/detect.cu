@@ -16,7 +16,10 @@
 // then along columns: (BOX + BOX) adds per position instead of the BOX^2 gradient evaluations and 3 BOX^2
 // multiply-adds of a per-position scan, and each pixel is read from global memory once per tile instead of
 // once per position that covers it.  A second small kernel takes the best of the tiles of each region.
-#include "sl2_common.cuh"
+// Entry point: sl2_find_best_patch.
+#include "sl2_context.cuh"
+
+using namespace sl2;
 
 namespace {
 
@@ -186,8 +189,6 @@ __global__ void __launch_bounds__(128) detect_reduce_kernel(const Sl2Dev d, int 
   }
 }
 
-}  // namespace
-
 // bytes of device scratch the launch needs for n regions of a W x H frame (per-tile partial results)
 size_t sl2_detect_scratch_bytes(const Sl2Dev &d, int n) {
   const int max_tiles = ((d.W + DT - 1) / DT) * ((d.H + DT - 1) / DT);
@@ -209,3 +210,31 @@ cudaError_t sl2_launch_detect(const Sl2Dev &d, int stream, int slot, int n, cons
   return sl2_launch_kernel(detect_reduce_kernel, dim3(n), dim3(128), 0, q, false, d, stream, regions_dev,
                            (d.box - 1) / 2, max_tiles, part_ev, part_idx, out_uv_dev, out_ev_dev);
 }
+
+}  // namespace
+
+extern "C" {
+
+int sl2_find_best_patch(sl2_ctx *c, int32_t s, int32_t slot, int32_t n, const int32_t *regions,
+                        int32_t *ubest, int32_t *vbest, double *evbest) {
+  if (bad_stream(c, s) || bad_slot(c, slot) || n < 0 || (n && (!regions || !evbest)))
+    return fail(c, SL2_ERR_ARG, "sl2_find_best_patch: bad argument");
+  if (n == 0) return SL2_OK;
+  Stage rg{STAGE_IN, 16 * (size_t)n, regions}, uv{STAGE_OUT, 8 * (size_t)n}, ev{STAGE_OUT, 8 * (size_t)n},
+      scratch{STAGE_DEV, sl2_detect_scratch_bytes(c->d, n)};
+  const int rc = staged_call(c, {&rg, &uv, &ev, &scratch}, [] {}, [&] {
+    CU_TRY(c, sl2_launch_detect(c->d, s, slot, n, rg.dev<int>(), uv.dev<int>(), ev.dev<double>(), scratch.d, queue(c)));
+    return SL2_OK;
+  });
+  if (rc) return rc;
+  for (int i = 0; i < n; ++i) {
+    evbest[i] = ev.host<double>()[i];
+    if (uv.host<int>()[2 * i] >= 0) {
+      if (ubest) ubest[i] = uv.host<int>()[2 * i];
+      if (vbest) vbest[i] = uv.host<int>()[2 * i + 1];
+    }
+  }
+  return SL2_OK;
+}
+
+}  // extern "C"

@@ -9,12 +9,16 @@
 //   MonoSLAM::predict_partially_initialised_feature_measurements   monoslam.cpp:1347-1400
 //                                          (+ part_feature_model.cpp:80-143, 231-265, feature_init_info.cpp:57-65)
 // Map features and depth particles share the camera and feature models of sl2_model.cuh.
+// Entry points of one stream: sl2_ekf_predict, sl2_predict_measurements, sl2_append_feature, sl2_delete_feature.
 //
 // State layout in HBM: ONE dense column-major P (ld x ld) per stream in the order of
 // construct_total_covariance (monoslam.cpp:518-546): [xv(13) | y_0 | y_1 | ...], with both
 // triangles kept bit-consistent (the reference rebuilds the lower triangle from the upper blocks
 // on every gather, so P is exactly block-symmetric whenever it is read).
+#include "sl2_context.cuh"
 #include "sl2_model.cuh"
+
+using namespace sl2;
 
 namespace {
 
@@ -545,13 +549,13 @@ __global__ void __launch_bounds__(256) append_kernel(const Sl2Dev d, int s, cons
   if (tid == 0) d.nfeat[s] = nf + 1;
 }
 
-}  // namespace
-
 cudaError_t sl2_launch_append(const Sl2Dev &d, int s, const double *y3_dev, const double *xp7_dev,
                               const uint8_t *patch_rows16_dev, const double *Pcol_dev, Sl2Queue q) {
   return sl2_launch_kernel(append_kernel, dim3(1), dim3(256), 0, q, false, d, s, y3_dev, xp7_dev, patch_rows16_dev,
                            Pcol_dev);
 }
+
+}  // namespace
 
 cudaError_t sl2_launch_predict(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *u3_dev,
                                int do_predict, int do_measure, Sl2Queue q) {
@@ -577,3 +581,54 @@ cudaError_t sl2_launch_cull(const Sl2Dev &d, int stream_lo, int stream_cnt, int 
   return sl2_launch_kernel(cull_kernel, dim3(stream_cnt), dim3(256), 0, q, sl2_use_pdl(stream_cnt), d,
                            stream_lo, force_index);
 }
+
+extern "C" {
+
+int sl2_ekf_predict(sl2_ctx *c, int32_t s, const double *u3) {
+  if (bad_stream(c, s)) return fail(c, SL2_ERR_ARG, "bad stream");
+  Stage u{STAGE_IN, u3 ? (size_t)24 : 0, u3};
+  return staged_call(c, {&u}, [] {}, [&] {
+    CU_TRY(c, sl2_launch_predict(c->d, s, 1, u3 ? u.dev<double>() : nullptr, 1, 0, queue(c)));
+    return SL2_OK;
+  });
+}
+
+int sl2_predict_measurements(sl2_ctx *c, int32_t s) {
+  if (bad_stream(c, s)) return fail(c, SL2_ERR_ARG, "bad stream");
+  CU_TRY(c, sl2_launch_predict(c->d, s, 1, nullptr, 0, 1, queue(c)));
+  int nv = 0;
+  CU_TRY(c, cudaMemcpyAsync(&nv, c->d.nvisible + s, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  return nv;
+}
+
+int sl2_delete_feature(sl2_ctx *c, int32_t s, int32_t index) {
+  if (bad_stream(c, s)) return fail(c, SL2_ERR_ARG, "bad stream");
+  const int n = sl2_num_features(c, s);
+  if (n < 0) return n;
+  if (index < 0 || index >= n) return fail(c, SL2_ERR_ARG, "sl2_delete_feature: bad index");
+  CU_TRY(c, sl2_launch_cull(c->d, s, 1, index, queue(c)));
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  return SL2_OK;
+}
+
+int sl2_append_feature(sl2_ctx *c, int32_t s, const double *y, const double *xp_org, const uint8_t *patch,
+                       const double *Pcol) {
+  if (bad_stream(c, s) || !y || !xp_org || !patch) return fail(c, SL2_ERR_ARG, "sl2_append_feature: bad argument");
+  const int nf = sl2_num_features(c, s);
+  if (nf < 0) return nf;
+  if (nf >= c->cfg.max_features) return fail(c, SL2_ERR_STATE, "sl2_append_feature: the map is full (max_features)");
+  const int box = c->d.box, n3 = SL2_NXV + 3 * nf + 3;
+  Stage ys{STAGE_IN, 24, y}, xs{STAGE_IN, 56, xp_org}, pc{STAGE_IN, Pcol ? 8 * 3 * (size_t)n3 : 0, Pcol},
+      rows{STAGE_IN, (size_t)box * 16};
+  const int rc = staged_call(
+      c, {&ys, &xs, &pc, &rows}, [&] { pack_patch_rows(rows.h, patch, 1, box); },
+      [&] {
+        CU_TRY(c, sl2_launch_append(c->d, s, ys.dev<double>(), xs.dev<double>(), rows.d,
+                                    Pcol ? pc.dev<double>() : nullptr, queue(c)));
+        return SL2_OK;
+      });
+  return rc ? rc : nf;  // index of the new feature
+}
+
+}  // extern "C"

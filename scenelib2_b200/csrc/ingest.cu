@@ -23,7 +23,21 @@
 // One launch covers the streams of a frame copy: block (band, row) converts output rows [band * ROWS, ...) of table
 // row base + blockIdx.y.  The raw source rows an output row needs are loaded once into shared memory with aligned
 // 16-byte loads and converted there (gray is recomputed per use, which is exact); consecutive output rows reuse them.
-#include "sl2_common.cuh"
+//
+// Host side: sl2_set_stream_source builds the table of streams with a source and their raw frames' staging
+// (install_sources); sl2_set_frame / sl2_set_frames* and the asynchronous step copy a frame set into the ring or the
+// staging (copy_slot_frames), then convert.
+#include <algorithm>
+
+#include "sl2_context.cuh"
+
+using namespace sl2;
+
+#define SL2_SOURCE_CHUNK 64  // rows one table write carries as its kernel parameter
+struct Sl2SourceChunk {
+  int first, n;
+  Sl2Source row[SL2_SOURCE_CHUNK];
+};
 
 namespace {
 
@@ -131,12 +145,15 @@ __global__ void __launch_bounds__(INGEST_THREADS) ingest_kernel(const Sl2Source 
   }
 }
 
-}  // namespace
+int sl2_source_bpp(int format) { return format == SL2_SRC_RGB24 ? 3 : format == SL2_SRC_UYVY ? 2 : 1; }
 
+// table[first .. first + n) = the chunk's rows, ordered on the queue like any other launch
 cudaError_t sl2_launch_source_write(Sl2Source *table, const Sl2SourceChunk &chunk, Sl2Queue q) {
   return sl2_launch_kernel(source_write_kernel, dim3(1), dim3(SL2_SOURCE_CHUNK), 0, q, false, table, chunk);
 }
 
+// convert (and resize) the raw frames of table rows [base, base + cnt) from one slot of the staging area into the
+// ring slot `slot`; max_row_bytes = the largest sw * bpp of those rows
 cudaError_t sl2_launch_ingest(const Sl2Dev &d, const Sl2Source *table, int base, int cnt, int max_dh,
                               int max_row_bytes, const uint8_t *stage_slot, int slot, Sl2Queue q) {
   if (cnt <= 0) return cudaSuccess;
@@ -146,3 +163,189 @@ cudaError_t sl2_launch_ingest(const Sl2Dev &d, const Sl2Source *table, int base,
   return sl2_launch_kernel(ingest_kernel, grid, dim3(INGEST_THREADS), 2 * (size_t)row_cap, q, false, table, base,
                            stage_slot, ring_slot, d.H, d.pitch, row_cap);
 }
+
+// gray blocks of the streams [lo, hi), [hi - lo][H][W] packed, into the frame ring
+cudaError_t copy_gray_blocks(const Sl2Dev &d, int slot, int lo, int hi, const uint8_t *src, cudaMemcpyKind kind,
+                             cudaStream_t st) {
+  uint8_t *dst = d.frames + ((size_t)slot * d.B + lo) * d.H * d.pitch;
+  if (d.pitch == d.W) return cudaMemcpyAsync(dst, src, (size_t)(hi - lo) * d.H * d.W, kind, st);
+  return cudaMemcpy2DAsync(dst, d.pitch, src, d.W, d.W, (size_t)(hi - lo) * d.H, kind, st);
+}
+
+uint8_t *source_stage(const sl2_ctx *c, int slot) { return c->src_stage.get() + (size_t)slot * c->src_slot_bytes; }
+
+// convert the raw frames of source rows [base, base + cnt) of `slot`'s staging into the ring
+cudaError_t ingest(sl2_ctx *c, int slot, int base, int cnt, Sl2Queue q) {
+  int max_dh = 0, max_rb = 0;
+  for (int j = base; j < base + cnt; ++j) {
+    const Sl2Source &r = c->src_rows[j];
+    max_dh = std::max(max_dh, r.dh);
+    max_rb = std::max(max_rb, r.sw * sl2_source_bpp(r.format));
+  }
+  return sl2_launch_ingest(c->d, c->src_tab.get(), base, cnt, max_dh, max_rb, source_stage(c, slot), slot, q);
+}
+
+size_t frame_bytes(const sl2_ctx *c, const sl2_stream_source &s) {
+  return s.format == SL2_SRC_GRAY_RING ? (size_t)c->d.H * c->d.W
+                                       : (size_t)s.width * s.height * sl2_source_bpp(s.format);
+}
+
+}  // namespace
+
+namespace sl2 {
+
+// Make `srcs` the context's sources (with the cameras in c->cams): layout, table rows, staging and the device table.
+// The table is rewritten on `stream` after every conversion queued so far on the copy stream.
+int install_sources(sl2_ctx *c, const std::vector<sl2_stream_source> &srcs) {
+  const Sl2Dev &d = c->d;
+  std::vector<size_t> layout(d.B + 1, 0);
+  std::vector<Sl2Source> rows;
+  size_t raw = 0;
+  for (int s = 0; s < d.B; ++s) {
+    layout[s + 1] = layout[s] + frame_bytes(c, srcs[s]);
+    if (srcs[s].format == SL2_SRC_GRAY_RING) continue;
+    rows.push_back({s, srcs[s].format, srcs[s].width, srcs[s].height, c->cams[s].width, c->cams[s].height,
+                    (int64_t)raw});
+    raw += frame_bytes(c, srcs[s]);
+  }
+  const size_t slot_bytes = (raw + 15) & ~(size_t)15;
+  const size_t need = rows.empty() ? 0 : (size_t)d.slots * slot_bytes + 16;
+  // every allocation before anything changes: a failed one leaves the sources, the staging and the table as they were
+  DevPtr<uint8_t> stage;
+  if (need > c->src_stage_bytes) {  // nothing may still read or write the old staging
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    CU_TRY(c, cudaStreamSynchronize(c->copy_stream.get()));
+    CU_TRY(c, cuda_malloc(stage, need));
+  }
+  if (!rows.empty() && !c->src_tab) CU_TRY(c, cuda_malloc(c->src_tab, sizeof(Sl2Source) * d.B));
+  if (!rows.empty() && !c->ev_src) CU_TRY(c, cuda_event_create(c->ev_src, cudaEventDisableTiming));
+  if (stage) {
+    c->src_stage = std::move(stage);
+    c->src_stage_bytes = need;
+  }
+  if (!rows.empty()) {
+    for (const SlotEvents &e : c->ev_slot)  // conversions in flight
+      CU_TRY(c, cudaStreamWaitEvent(c->stream, e.h2d.get(), 0));
+    for (size_t first = 0; first < rows.size(); first += SL2_SOURCE_CHUNK) {
+      Sl2SourceChunk ch = {};
+      ch.first = (int)first;
+      ch.n = (int)std::min(rows.size() - first, (size_t)SL2_SOURCE_CHUNK);
+      for (int i = 0; i < ch.n; ++i) ch.row[i] = rows[first + i];
+      CU_TRY(c, sl2_launch_source_write(c->src_tab.get(), ch, queue(c)));
+    }
+    CU_TRY(c, cudaEventRecord(c->ev_src.get(), c->stream));
+  }
+  c->srcs = srcs;
+  c->layout = layout;
+  c->src_rows = rows;
+  c->src_slot_bytes = slot_bytes;
+  return SL2_OK;
+}
+
+// A snapshot load gives streams [lo, lo + cnt) the blobs' cameras: a stream with a source then resizes to its new image
+int loaded_cameras(sl2_ctx *c, int lo, const std::vector<sl2_stream_config> &cams) {
+  bool resized = false;
+  for (size_t i = 0; i < cams.size(); ++i) {
+    const sl2_stream_config &old = c->cams[lo + i];
+    resized = resized || (c->srcs[lo + i].format != SL2_SRC_GRAY_RING &&
+                          (old.width != cams[i].width || old.height != cams[i].height));
+    c->cams[lo + i] = cams[i];
+  }
+  return resized ? install_sources(c, c->srcs) : SL2_OK;
+}
+
+// One frame slot of every stream, a frame set (sl2_frame_set_layout), into the frame ring: each run of consecutive
+// default streams in one copy to the ring (the whole set when no stream has a source), each run of streams with a
+// source in one copy to the slot's staging, then one conversion launch for all of them.
+cudaError_t copy_slot_frames(sl2_ctx *c, int slot, const uint8_t *src, cudaMemcpyKind kind, Sl2Queue q) {
+  const Sl2Dev &d = c->d;
+  if (c->src_rows.empty()) return copy_gray_blocks(d, slot, 0, d.B, src, kind, q.stream);
+  for (int a = 0; a < d.B;) {
+    const bool raw = c->srcs[a].format != SL2_SRC_GRAY_RING;
+    int b = a + 1;
+    while (b < d.B && (c->srcs[b].format != SL2_SRC_GRAY_RING) == raw) ++b;
+    cudaError_t e;
+    if (raw) {
+      size_t at = 0;  // staging offset of stream a
+      for (const Sl2Source &r : c->src_rows)
+        if (r.stream == a) at = (size_t)r.off;
+      e = cudaMemcpyAsync(source_stage(c, slot) + at, src + c->layout[a], c->layout[b] - c->layout[a], kind,
+                          q.stream);
+    } else {
+      e = copy_gray_blocks(d, slot, a, b, src + c->layout[a], kind, q.stream);
+    }
+    if (e != cudaSuccess) return e;
+    a = b;
+  }
+  return ingest(c, slot, 0, (int)c->src_rows.size(), q);
+}
+
+}  // namespace sl2
+
+extern "C" {
+
+int sl2_set_stream_source(sl2_ctx *c, int32_t s, const sl2_stream_source *src) {
+  if (bad_stream(c, s) || !src) return fail(c, SL2_ERR_ARG, "sl2_set_stream_source: bad argument");
+  const int f = src->format;
+  if (f < SL2_SRC_GRAY_RING || f > SL2_SRC_UYVY || src->reserved != 0)
+    return fail(c, SL2_ERR_ARG, "sl2_set_stream_source: unknown format or non-zero reserved field");
+  if (f == SL2_SRC_GRAY_RING ? (src->width != 0 || src->height != 0)
+                             : (src->width < 1 || src->height < 1 || src->width > SL2_MAX_SOURCE_DIM ||
+                                src->height > SL2_MAX_SOURCE_DIM))
+    return fail(c, SL2_ERR_ARG,
+                "sl2_set_stream_source: size must be 0 x 0 for the default source, else in [1, SL2_MAX_SOURCE_DIM]");
+  if (f == SL2_SRC_UYVY && (src->width & 1))
+    return fail(c, SL2_ERR_ARG, "sl2_set_stream_source: a UYVY frame has an even width");
+  std::vector<sl2_stream_source> srcs = c->srcs;
+  srcs[s] = *src;
+  return install_sources(c, srcs);
+}
+
+int sl2_get_stream_source(sl2_ctx *c, int32_t s, sl2_stream_source *src) {
+  if (bad_stream(c, s) || !src) return fail(c, SL2_ERR_ARG, "sl2_get_stream_source: bad argument");
+  *src = c->srcs[s];
+  return SL2_OK;
+}
+
+int sl2_frame_set_layout(sl2_ctx *c, size_t *offsets) {
+  enter(c);
+  if (!c || !offsets) return fail(c, SL2_ERR_ARG, "sl2_frame_set_layout: bad argument");
+  std::copy(c->layout.begin(), c->layout.end(), offsets);
+  return SL2_OK;
+}
+
+int sl2_set_frame(sl2_ctx *c, int32_t s, int32_t slot, const uint8_t *gray, size_t stride) {
+  if (bad_stream(c, s) || bad_slot(c, slot) || !gray) return fail(c, SL2_ERR_ARG, "sl2_set_frame: bad argument");
+  const Sl2Dev &d = c->d;
+  if (c->srcs[s].format != SL2_SRC_GRAY_RING) {  // the raw frame to the slot's staging, then its conversion
+    int j = 0;
+    while (c->src_rows[j].stream != s) ++j;
+    const Sl2Source &r = c->src_rows[j];
+    const size_t rb = (size_t)r.sw * sl2_source_bpp(r.format);
+    CU_TRY(c, cudaMemcpy2DAsync(source_stage(c, slot) + r.off, rb, gray, stride, rb, r.sh, cudaMemcpyHostToDevice,
+                                c->stream));
+    CU_TRY(c, ingest(c, slot, j, 1, queue(c)));
+  } else {
+    uint8_t *dst = d.frames + ((size_t)slot * d.B + s) * d.H * d.pitch;
+    const sl2_stream_config &sc = c->cams[s];  // the stream's image, top-left of its block
+    CU_TRY(c, cudaMemcpy2DAsync(dst, d.pitch, gray, stride, sc.width, sc.height, cudaMemcpyHostToDevice, c->stream));
+  }
+  CU_TRY(c, cudaEventRecord(c->ev_slot[slot].cmp.get(), c->stream));  // slot busy until the copy has landed
+  return SL2_OK;
+}
+
+static int set_frames_any(sl2_ctx *c, int32_t slot, const uint8_t *gray, cudaMemcpyKind kind) {
+  enter(c);
+  if (!c || bad_slot(c, slot) || !gray) return fail(c, SL2_ERR_ARG, "sl2_set_frames: bad argument");
+  CU_TRY(c, copy_slot_frames(c, slot, gray, kind, queue(c)));
+  CU_TRY(c, cudaEventRecord(c->ev_slot[slot].cmp.get(), c->stream));  // slot busy until the copy has landed
+  return SL2_OK;
+}
+int sl2_set_frames(sl2_ctx *c, int32_t slot, const uint8_t *gray) {
+  return set_frames_any(c, slot, gray, cudaMemcpyHostToDevice);
+}
+int sl2_set_frames_dev(sl2_ctx *c, int32_t slot, const uint8_t *gray_dev) {
+  return set_frames_any(c, slot, gray_dev, cudaMemcpyDeviceToDevice);
+}
+
+}  // extern "C"

@@ -10,7 +10,12 @@
 //                 Sl2Dev::Wp for the solve, and nothing else writes Wp: its diagonal holds the reciprocal pivots
 //                 W_ii = 1 / U_ii the solve applied.  log det S = 2 sum log U_ii = -2 sum log W_ii.
 // When m == 0 the update wrote neither G nor Wp (they hold another update's values) and the kernel reads neither.
-#include "sl2_common.cuh"
+// Entry points: sl2_enable_records (the ring) and sl2_get_records* (the most recent records, oldest first).
+#include <algorithm>
+
+#include "sl2_context.cuh"
+
+using namespace sl2;
 
 namespace {
 
@@ -67,3 +72,62 @@ cudaError_t sl2_launch_records(const Sl2Dev &d, int stream_lo, int stream_cnt, i
   return sl2_launch_kernel(record_kernel, dim3(stream_cnt), dim3(REC_THREADS), 0, q, sl2_use_pdl(stream_cnt), d,
                            stream_lo, (long long)step);
 }
+
+extern "C" {
+
+int sl2_enable_records(sl2_ctx *c, int32_t depth) {
+  if (!c) return SL2_ERR_ARG;
+  enter(c);
+  if (depth < 0 || depth > SL2_MAX_RECORDS)
+    return fail(c, SL2_ERR_ARG, "sl2_enable_records: depth outside [0, SL2_MAX_RECORDS]");
+  // the new ring first, so that a failed allocation leaves the old one in place
+  DevPtr<sl2_step_record> ring;
+  cudaError_t e = cudaSuccess;
+  if (depth) {
+    const size_t bytes = (size_t)c->d.B * depth * sizeof(sl2_step_record);
+    CU_TRY(c, cuda_malloc(ring, bytes));
+    e = cudaMemsetAsync(ring.get(), 0, bytes, c->stream);
+  }
+  // steps queued before the call (either group: enter() joined them) have written the old ring
+  if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+  if (e != cudaSuccess) return fail(c, SL2_ERR_CUDA, std::string("sl2_enable_records: ") + cudaGetErrorString(e));
+  c->rec = std::move(ring);
+  c->d.rec = c->rec.get();
+  c->d.rec_depth = depth;
+  c->rec_steps = 0;
+  return SL2_OK;
+}
+
+// The most recent k records of streams [lo, lo + cnt), oldest first, as one or two 2-D copies (two when the k rows
+// wrap around the end of the ring): row pitch `depth` records in the ring, `mx` records in the output.
+static int get_records(sl2_ctx *c, int32_t lo, int32_t cnt, int32_t mx, void *out, cudaMemcpyKind kind,
+                       const char *who) {
+  if (bad_range(c, lo, cnt) || !out || mx < 1 ||
+      (kind == cudaMemcpyDeviceToDevice && ((uintptr_t)out & 7)))
+    return fail(c, SL2_ERR_ARG, std::string(who) + ": bad argument");
+  const int64_t depth = c->d.rec_depth;
+  if (!depth) return fail(c, SL2_ERR_STATE, std::string(who) + ": records are off (sl2_enable_records)");
+  const int k = (int)std::min<int64_t>(std::min<int64_t>(mx, c->rec_steps), depth);
+  if (k == 0 || cnt == 0) return k;
+  const size_t R = sizeof(sl2_step_record);
+  const int r0 = (int)((c->rec_steps - k) % depth);  // ring row of the oldest record returned
+  const int k1 = (int)std::min<int64_t>(k, depth - r0);
+  const sl2_step_record *src = c->d.rec + (size_t)lo * depth;
+  uint8_t *dst = static_cast<uint8_t *>(out);
+  CU_TRY(c, cudaMemcpy2DAsync(dst, (size_t)mx * R, src + r0, (size_t)depth * R, (size_t)k1 * R, cnt, kind, c->stream));
+  if (k1 < k)
+    CU_TRY(c, cudaMemcpy2DAsync(dst + (size_t)k1 * R, (size_t)mx * R, src, (size_t)depth * R, (size_t)(k - k1) * R,
+                                cnt, kind, c->stream));
+  if (kind == cudaMemcpyDeviceToHost) CU_TRY(c, cudaStreamSynchronize(c->stream));
+  return k;
+}
+
+int sl2_get_records(sl2_ctx *c, int32_t lo, int32_t cnt, int32_t max, sl2_step_record *out) {
+  return get_records(c, lo, cnt, max, out, cudaMemcpyDeviceToHost, "sl2_get_records");
+}
+
+int sl2_get_records_dev(sl2_ctx *c, int32_t lo, int32_t cnt, int32_t max, void *out_dev) {
+  return get_records(c, lo, cnt, max, out_dev, cudaMemcpyDeviceToDevice, "sl2_get_records_dev");
+}
+
+}  // extern "C"

@@ -1,8 +1,15 @@
 // reloc.cu — relocalisation on sm_90a (Williams, Klein, Reid, ICCV 2007): after the full-image search, the camera pose
-// of a lost stream from its matches with a three-point consensus.  Semantics: include/sl2b200.h, sl2_relocalise.
+// of a lost stream from its matches with a three-point consensus.  Semantics: include/sl2b200.h, sl2_relocalise, whose
+// entry point (argument checks, the full-image search through sl2_launch_search, then reloc_kernel) ends this file.
 #include <math_constants.h>
 
+#include <algorithm>
+#include <cmath>
+
+#include "sl2_context.cuh"
 #include "sl2_model.cuh"
+
+using namespace sl2;
 
 namespace {
 
@@ -504,8 +511,8 @@ __global__ void __launch_bounds__(RELOC_THREADS) reloc_kernel(const Sl2Dev d, co
   }
 }
 
-}  // namespace
-
+// relocalisation of the cnt streams ids_dev[] from the full-image search's results by job (job = (stream - stream_lo) *
+// Nmax + feature): pose consensus, refinement and, on acceptance, the state write
 cudaError_t sl2_launch_reloc(const Sl2Dev &d, int cnt, const int *ids_dev, int stream_lo, const int *search_uv,
                              const uint8_t *search_found, const sl2_reloc_params *prm_dev, const double *Pxx_dev,
                              sl2_reloc_result *res_dev, int *zuv_dev, uint8_t *flags_dev, Sl2Queue q) {
@@ -516,3 +523,129 @@ cudaError_t sl2_launch_reloc(const Sl2Dev &d, int cnt, const int *ids_dev, int s
   return sl2_launch_kernel(reloc_kernel, dim3(cnt), dim3(RELOC_THREADS), sizeof(RelocSmem), q, false, d, ids_dev,
                            stream_lo, search_uv, search_found, prm_dev, Pxx_dev, res_dev, zuv_dev, flags_dev);
 }
+
+// whether the symmetric 13 x 13 matrix A (column-major) is positive semi-definite: cyclic Jacobi eigenvalues, the
+// smallest >= -1e-12 times the largest magnitude
+bool psd13(const double *A0) {
+  double A[13][13];
+  double scale = 0.0;
+  for (int i = 0; i < 13; ++i)
+    for (int j = 0; j < 13; ++j) {
+      A[i][j] = A0[i + 13 * j];
+      scale += A[i][j] * A[i][j];
+    }
+  for (int sweep = 0; sweep < 100; ++sweep) {
+    double off = 0.0;
+    for (int p = 0; p < 13; ++p)
+      for (int q = p + 1; q < 13; ++q) off += A[p][q] * A[p][q];
+    if (off <= 1e-34 * scale) break;
+    for (int p = 0; p < 13; ++p)
+      for (int q = p + 1; q < 13; ++q) {
+        if (A[p][q] == 0.0) continue;
+        const double th = (A[q][q] - A[p][p]) / (2.0 * A[p][q]);
+        const double t = (th >= 0.0 ? 1.0 : -1.0) / (std::fabs(th) + std::sqrt(th * th + 1.0));
+        const double c = 1.0 / std::sqrt(t * t + 1.0), s = t * c;
+        for (int k = 0; k < 13; ++k) {
+          const double akp = A[k][p], akq = A[k][q];
+          A[k][p] = c * akp - s * akq;
+          A[k][q] = s * akp + c * akq;
+        }
+        for (int k = 0; k < 13; ++k) {
+          const double apk = A[p][k], aqk = A[q][k];
+          A[p][k] = c * apk - s * aqk;
+          A[q][k] = s * apk + c * aqk;
+        }
+      }
+  }
+  double lo = 0.0, hi = 0.0;
+  for (int i = 0; i < 13; ++i) {
+    lo = std::min(lo, A[i][i]);
+    hi = std::max(hi, std::fabs(A[i][i]));
+  }
+  return lo >= -1e-12 * hi;
+}
+
+}  // namespace
+
+extern "C" {
+
+int sl2_relocalise(sl2_ctx *c, const int32_t *ids, int32_t cnt, int32_t slot, const sl2_reloc_params *p,
+                   const double *Pxx, sl2_reloc_result *out, int32_t *z_uv, uint8_t *flags) {
+  enter(c);
+  if (!c || cnt < 0 || (cnt > 0 && !ids) || bad_slot(c, slot) || !p || !Pxx || !out)
+    return fail(c, SL2_ERR_ARG, "sl2_relocalise: bad argument");
+  const Sl2Dev &d = c->d;
+  std::vector<char> seen(d.B, 0);
+  int lo = d.B, hi = -1;
+  for (int i = 0; i < cnt; ++i) {
+    const int s = ids[i];
+    if (s < 0 || s >= d.B || seen[s]) return fail(c, SL2_ERR_ARG, "sl2_relocalise: bad or repeated stream id");
+    seen[s] = 1;
+    lo = std::min(lo, s);
+    hi = std::max(hi, s);
+  }
+  if (!(p->inlier_px > 0.0) || !std::isfinite(p->inlier_px))
+    return fail(c, SL2_ERR_ARG, "sl2_relocalise: inlier_px must be finite and > 0");
+  if (p->min_inliers < 4 || p->reserved != 0)
+    return fail(c, SL2_ERR_ARG, "sl2_relocalise: min_inliers must be >= 4 and reserved 0");
+  for (int i = 0; i < 3; ++i)
+    if (!std::isfinite(p->v[i]) || !std::isfinite(p->omega[i]))
+      return fail(c, SL2_ERR_ARG, "sl2_relocalise: v and omega must be finite");
+  if (!(std::sqrt(p->omega[0] * p->omega[0] + p->omega[1] * p->omega[1] + p->omega[2] * p->omega[2]) > 0.0))
+    return fail(c, SL2_ERR_ARG, "sl2_relocalise: |omega| must be > 0");
+  for (int i = 0; i < 13; ++i)
+    for (int j = 0; j < 13; ++j)
+      if (!std::isfinite(Pxx[i + 13 * j]) || Pxx[i + 13 * j] != Pxx[j + 13 * i])
+        return fail(c, SL2_ERR_ARG, "sl2_relocalise: Pxx must be finite and symmetric");
+  if (!psd13(Pxx)) return fail(c, SL2_ERR_ARG, "sl2_relocalise: Pxx is not positive semi-definite");
+  if (cnt == 0) return SL2_OK;
+  // one search job per feature of every listed stream over the id range [lo, hi], empty jobs elsewhere
+  const int R = hi - lo + 1;
+  std::vector<int> nf(R);
+  CU_TRY(c, cudaMemcpyAsync(nf.data(), d.nfeat + lo, sizeof(int) * R, cudaMemcpyDeviceToHost, c->stream));
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  const size_t nj = (size_t)R * d.Nmax, nc = cnt, no = nc * d.Nmax;
+  Stage is{STAGE_IN, 4 * nc, ids}, ps{STAGE_IN, sizeof(sl2_reloc_params), p}, px{STAGE_IN, 8 * 169, Pxx},
+      jf{STAGE_IN, 4 * nj}, jc{STAGE_IN, 16 * nj}, jp{STAGE_IN, 24 * nj}, rs{STAGE_OUT, sizeof(sl2_reloc_result) * nc},
+      zo{STAGE_OUT, 8 * no}, fo{STAGE_OUT, no}, su{STAGE_DEV, 8 * nj}, sf{STAGE_DEV, nj};
+  auto pack = [&] {
+    for (int r = 0; r < R; ++r) {
+      const int s = lo + r;
+      const sl2_stream_config &sc = c->cams[s];
+      const double eps = 9.0 / ((double)sc.width * sc.width + (double)sc.height * sc.height);
+      for (int f = 0; f < d.Nmax; ++f) {
+        const size_t j = (size_t)r * d.Nmax + f;
+        jf.host<int>()[j] = seen[s] && f < nf[r] ? f : -1;
+        jc.host<double>()[2 * j] = 0.5 * (sc.width - 1);
+        jc.host<double>()[2 * j + 1] = 0.5 * (sc.height - 1);
+        jp.host<double>()[3 * j] = eps;
+        jp.host<double>()[3 * j + 1] = 0.0;
+        jp.host<double>()[3 * j + 2] = eps;
+      }
+    }
+  };
+  const int rc = staged_call(c, {&is, &ps, &px, &jf, &jc, &jp, &rs, &zo, &fo, &su, &sf}, pack, [&] {
+    SearchLaunch L = {};
+    L.job_feat = jf.dev<int>();
+    L.job_centre = jc.dev<double>();
+    L.job_puinv = jp.dev<double>();
+    L.jobs_per_stream = d.Nmax;
+    L.stream_lo = lo;
+    L.stream_cnt = R;
+    L.slot = slot;
+    L.out_uv = su.dev<int>();
+    L.out_found = sf.d;
+    L.scatter_to_features = 0;
+    CU_TRY(c, sl2_launch_search(d, c->tmap, L, queue(c)));
+    CU_TRY(c, sl2_launch_reloc(d, cnt, is.dev<int>(), lo, su.dev<int>(), sf.d, ps.dev<sl2_reloc_params>(),
+                               px.dev<double>(), rs.dev<sl2_reloc_result>(), zo.dev<int>(), fo.d, queue(c)));
+    return SL2_OK;
+  });
+  if (rc) return rc;
+  memcpy(out, rs.h, rs.bytes);
+  if (z_uv) memcpy(z_uv, zo.h, zo.bytes);
+  if (flags) memcpy(flags, fo.h, fo.bytes);
+  return SL2_OK;
+}
+
+}  // extern "C"

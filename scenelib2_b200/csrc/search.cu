@@ -26,9 +26,12 @@
 //   * arg-min with the reference's tie-break (`corr <= corrmax` => the LAST candidate in
 //     urel-major / vrel-minor scan order wins) carried as (score, scan index) through a
 //     warp-shuffle reduction.
-#include "sl2_common.cuh"
+// Entry points: sl2_patch_search (the staged search of one stream's jobs) and sl2_score_map (one job's scores).
+#include "sl2_context.cuh"
 #include "sl2_ptx.cuh"
 #include "sl2_score.cuh"
+
+using namespace sl2;
 
 namespace {
 
@@ -543,9 +546,10 @@ cudaError_t sl2_launch_search(const Sl2Dev &d, const CUtensorMap &tmap, const Se
 }
 
 // one job (centre, puinv, feature index: device arrays of 2, 3 and 1) with every candidate's score dumped
-cudaError_t sl2_launch_score_map(const Sl2Dev &d, const CUtensorMap &tmap, int stream_id, int slot,
-                                 const double *centre_dev, const double *puinv_dev, const int *feat_dev, int *box_dev,
-                                 double *corr_dev, double *sd_dev, uint8_t *inside_dev, int cap, Sl2Queue q) {
+static cudaError_t sl2_launch_score_map(const Sl2Dev &d, const CUtensorMap &tmap, int stream_id, int slot,
+                                        const double *centre_dev, const double *puinv_dev, const int *feat_dev,
+                                        int *box_dev, double *corr_dev, double *sd_dev, uint8_t *inside_dev, int cap,
+                                        Sl2Queue q) {
   SearchLaunch L = {};
   L.job_centre = centre_dev;
   L.job_puinv = puinv_dev;
@@ -557,3 +561,68 @@ cudaError_t sl2_launch_score_map(const Sl2Dev &d, const CUtensorMap &tmap, int s
   const DumpPtrs dump = {corr_dev, sd_dev, inside_dev, box_dev, cap};
   return launch<false>(d, tmap, L, dump, q);
 }
+
+extern "C" {
+
+int sl2_patch_search(sl2_ctx *c, int32_t s, int32_t slot, int32_t n, const int32_t *feat_index,
+                     const double *centre, const double *PuInv3, int32_t *u, int32_t *v,
+                     uint8_t *found, double *best) {
+  if (n > 0 && !feat_index) return fail(c, SL2_ERR_ARG, "sl2_patch_search: feat_index is null");
+  if (bad_stream(c, s) || bad_slot(c, slot) || n < 0 || !centre || !PuInv3)
+    return fail(c, SL2_ERR_ARG, "patch search: bad argument");
+  if (n == 0) return SL2_OK;
+  int rc = check_feature_indices(c, s, feat_index, n, "patch search: feature index out of range");
+  if (rc) return rc;
+  const size_t N = n;
+  Stage ce{STAGE_IN, 16 * N, centre}, pu{STAGE_IN, 24 * N, PuInv3}, fe{STAGE_IN, 4 * N, feat_index},
+      uv{STAGE_OUT, 8 * N}, fd{STAGE_OUT, N}, be{STAGE_OUT, 8 * N};
+  rc = staged_call(c, {&ce, &pu, &fe, &uv, &fd, &be}, [] {}, [&] {
+    SearchLaunch L = {};
+    L.job_centre = ce.dev<double>();
+    L.job_puinv = pu.dev<double>();
+    L.job_feat = fe.dev<int>();
+    L.jobs_per_stream = n;
+    L.stream_lo = s;
+    L.stream_cnt = 1;
+    L.slot = slot;
+    L.out_uv = uv.dev<int>();
+    L.out_found = fd.d;
+    L.out_best = be.dev<double>();
+    L.scatter_to_features = 0;
+    CU_TRY(c, sl2_launch_search(c->d, c->tmap, L, queue(c)));
+    return SL2_OK;
+  });
+  if (rc) return rc;
+  for (int i = 0; i < n; ++i) {
+    if (u) u[i] = uv.host<int>()[2 * i];
+    if (v) v[i] = uv.host<int>()[2 * i + 1];
+    if (found) found[i] = fd.h[i];
+    if (best) best[i] = be.host<double>()[i];
+  }
+  return SL2_OK;
+}
+
+int sl2_score_map(sl2_ctx *c, int32_t s, int32_t slot, int32_t feat, const double *centre,
+                  const double *PuInv3, int32_t *box6, double *corr, double *sd_image,
+                  uint8_t *inside, size_t cap) {
+  if (bad_stream(c, s) || bad_slot(c, slot) || !centre || !PuInv3 || !box6)
+    return fail(c, SL2_ERR_ARG, "sl2_score_map: bad argument");
+  int rc = check_feature_indices(c, s, &feat, 1, "sl2_score_map: bad feature index");
+  if (rc) return rc;
+  Stage ce{STAGE_IN, 16, centre}, pu{STAGE_IN, 24, PuInv3}, fe{STAGE_IN, 4, &feat}, bx{STAGE_OUT, 24},
+      co{STAGE_OUT, 8 * cap}, sd{STAGE_OUT, 8 * cap}, in{STAGE_OUT, cap};
+  rc = staged_call(c, {&ce, &pu, &fe, &bx, &co, &sd, &in}, [] {}, [&] {
+    CU_TRY(c, cudaMemsetAsync(bx.d, 0xff, in.d + cap - bx.d, c->stream));  // NaN / 0xff fill of every output
+    CU_TRY(c, sl2_launch_score_map(c->d, c->tmap, s, slot, ce.dev<double>(), pu.dev<double>(), fe.dev<int>(),
+                                   bx.dev<int>(), co.dev<double>(), sd.dev<double>(), in.d, (int)cap, queue(c)));
+    return SL2_OK;
+  });
+  if (rc) return rc;
+  memcpy(box6, bx.h, 24);
+  if (corr) memcpy(corr, co.h, 8 * cap);
+  if (sd_image) memcpy(sd_image, sd.h, 8 * cap);
+  if (inside) memcpy(inside, in.h, cap);
+  return SL2_OK;
+}
+
+}  // extern "C"

@@ -23,6 +23,30 @@ struct Sl2StreamCam {
   int pad_;
 };
 static_assert(sizeof(Sl2StreamCam) % sizeof(double) == 0, "rows are copied as doubles");
+// The row of a stream's sl2_stream_config, or of an sl2_config (whose camera fields every stream starts with)
+template <typename Config>
+__host__ __device__ inline Sl2StreamCam sl2_cam_row(const Config &sc) {
+  Sl2StreamCam r = {};
+  const double cam[8] = {(double)sc.width, (double)sc.height, sc.fku, sc.fkv, sc.u0, sc.v0, sc.kd1, sc.sd};
+  for (int i = 0; i < 8; ++i) r.cam[i] = cam[i];
+  r.dt = sc.delta_t;
+  r.n_select = sc.number_of_features_to_select;
+  return r;
+}
+// and back: the fields are assigned one by one, so the padding of *sc keeps the bytes it had (the zeros of a
+// snapshot header)
+__host__ __device__ inline void sl2_cam_config(const Sl2StreamCam &r, sl2_stream_config *sc) {
+  sc->width = (int32_t)r.cam[0];
+  sc->height = (int32_t)r.cam[1];
+  sc->fku = r.cam[2];
+  sc->fkv = r.cam[3];
+  sc->u0 = r.cam[4];
+  sc->v0 = r.cam[5];
+  sc->kd1 = r.cam[6];
+  sc->sd = r.cam[7];
+  sc->delta_t = r.dt;
+  sc->number_of_features_to_select = r.n_select;
+}
 __device__ __forceinline__ int stream_width(const Sl2StreamCam &c) { return (int)c.cam[0]; }
 __device__ __forceinline__ int stream_height(const Sl2StreamCam &c) { return (int)c.cam[1]; }
 
@@ -198,7 +222,8 @@ inline bool sl2_box_supported(int box) {
   return sl2_with_box(box, [](auto) { return cudaSuccess; }) == cudaSuccess;
 }
 
-// launchers (defined in search.cu / ekf.cu / consensus.cu / reloc.cu / update.cu), called from api.cu
+// launchers that files other than their own call (defined in search.cu / ekf.cu / consensus.cu / update.cu /
+// records.cu / particles.cu)
 struct SearchLaunch {
   // job arrays may be the context's own (fused step) or temporaries (staged API)
   const int *job_feat;       // [njobs_per_stream * B] or [n]
@@ -214,31 +239,20 @@ struct SearchLaunch {
 };
 
 cudaError_t sl2_launch_search(const Sl2Dev &d, const CUtensorMap &tmap, const SearchLaunch &L, Sl2Queue q);
-cudaError_t sl2_launch_score_map(const Sl2Dev &d, const CUtensorMap &tmap, int stream_id, int slot,
-                                 const double *centre_dev, const double *puinv_dev, const int *feat_dev, int *box_dev,
-                                 double *corr_dev, double *sd_dev, uint8_t *inside_dev, int cap, Sl2Queue q);
 cudaError_t sl2_launch_predict(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *u3_dev,
                                int do_predict, int do_measure, Sl2Queue q);
 // match consensus of the streams [stream_lo, stream_lo + stream_cnt) between the search and the update; tau2_dev[s] =
 // the squared inlier radius of stream s, 0 = off (consensus.cu)
 cudaError_t sl2_launch_consensus(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *tau2_dev, Sl2Queue q);
-// relocalisation of the cnt streams ids_dev[] from the full-image search's results by job (job = (stream - stream_lo) *
-// Nmax + feature): pose consensus, refinement and, on acceptance, the state write (reloc.cu reloc_kernel)
-cudaError_t sl2_launch_reloc(const Sl2Dev &d, int cnt, const int *ids_dev, int stream_lo, const int *search_uv,
-                             const uint8_t *search_found, const sl2_reloc_params *prm_dev, const double *Pxx_dev,
-                             sl2_reloc_result *res_dev, int *zuv_dev, uint8_t *flags_dev, Sl2Queue q);
 // EKF update = 5 kernels (hp, chol, solve, syrk, finish); ev6 (optional) = 6 events recorded around them
 cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, int staged_m,
                               const int *st_feat, const double *st_Hxv, const double *st_Hy,
                               const double *st_R, const double *st_nu, int only_normalise,
                               Sl2Queue q, cudaEvent_t *ev6 = nullptr);
 cudaError_t sl2_launch_cull(const Sl2Dev &d, int stream_lo, int stream_cnt, int force_index, Sl2Queue q);
-cudaError_t sl2_launch_append(const Sl2Dev &d, int s, const double *y3_dev, const double *xp7_dev,
-                              const uint8_t *patch_rows16_dev, const double *Pcol_dev, Sl2Queue q);
 // one step record per stream of [stream_lo, stream_lo + stream_cnt) into ring row step % d.rec_depth; launched after
 // the cull of the fused step (records.cu)
 cudaError_t sl2_launch_records(const Sl2Dev &d, int stream_lo, int stream_cnt, int64_t step, Sl2Queue q);
-size_t sl2_update_smem_bytes(const Sl2Dev &d);
 cudaError_t sl2_configure_search(const Sl2Dev &d);  // per context: dynamic smem opt-in
 cudaError_t sl2_configure_update(const Sl2Dev &d);
 // partially-initialised features (ekf.cu, smoe.cu, particles.cu): F features x Kmax particle slots (K_dev[f] used)
@@ -246,75 +260,7 @@ cudaError_t sl2_launch_particle_predict(const Sl2Dev &d, int s, int F, int Kmax,
                                         const double *ypi, const double *Pxy, const double *Pyy,
                                         const double *lambda, double *h, double *sinv3, double *detS,
                                         Sl2Queue q);
-size_t sl2_smoe_map_bytes(const Sl2Dev &d, int F);
-cudaError_t sl2_launch_smoe(const Sl2Dev &d, int s, int slot, int F, int Kmax, const int *K_dev, const int *feat_dev,
-                            const double *centre_dev, const double *puinv_dev, double *map_dev, int *out_uv_dev,
-                            uint8_t *out_found_dev, double *out_best_dev, Sl2Queue q);
 cudaError_t sl2_launch_particles(int F, int Kmax, const int *K_dev, const double *h, const double *sinv3,
                                  const double *detS, const double *lambda, const int *z_uv, const uint8_t *found,
                                  double prune_threshold, double *prob, uint8_t *keep, double *cumulative,
                                  double *mean_var, int *left_out, Sl2Queue q);
-size_t sl2_detect_scratch_bytes(const Sl2Dev &d, int n);
-cudaError_t sl2_launch_detect(const Sl2Dev &d, int stream, int slot, int n, const int *regions_dev,
-                              int *out_uv_dev, double *out_ev_dev, void *scratch_dev, Sl2Queue q);
-
-// ---- raw frame sources (ingest.cu): one row per stream with a non-default sl2_stream_source, in stream order -------
-struct Sl2Source {
-  int stream, format;  // camera stream, SL2_SRC_*
-  int sw, sh;          // raw frame size
-  int dw, dh;          // the stream's image (sl2_stream_config width_s x height_s): the resize target
-  int64_t off;         // byte offset of the raw frame in a slot of the staging area
-};
-#define SL2_SOURCE_CHUNK 64  // rows one table write carries as its kernel parameter
-struct Sl2SourceChunk {
-  int first, n;
-  Sl2Source row[SL2_SOURCE_CHUNK];
-};
-inline int sl2_source_bpp(int format) { return format == SL2_SRC_RGB24 ? 3 : format == SL2_SRC_UYVY ? 2 : 1; }
-// table[first .. first + n) = the chunk's rows, ordered on the queue like any other launch
-cudaError_t sl2_launch_source_write(Sl2Source *table, const Sl2SourceChunk &chunk, Sl2Queue q);
-// convert (and resize) the raw frames of table rows [base, base + cnt) from one slot of the staging area into the
-// ring slot `slot`; max_row_bytes = the largest sw * bpp of those rows
-cudaError_t sl2_launch_ingest(const Sl2Dev &d, const Sl2Source *table, int base, int cnt, int max_dh,
-                              int max_row_bytes, const uint8_t *stage_slot, int slot, Sl2Queue q);
-
-// ---- stream snapshots (snapshot.cu): the blob format of include/sl2b200.h --------------------------------------
-// Section field[k] of a blob is the stream's first nfeat records of array k of SL2_STREAM_ARRAYS (x, P and the
-// templates are laid out separately).
-struct Sl2SnapLayout {
-  size_t x, P, field[SL2_SNAPSHOT_FIELDS], templates, total;  // byte offsets in the blob, total size
-};
-__host__ __device__ inline size_t sl2_snap_align8(size_t b) { return (b + 7) & ~(size_t)7; }
-__host__ __device__ inline Sl2SnapLayout sl2_snap_layout(int nfeat, int box) {
-  Sl2SnapLayout L;
-  const size_t n = SL2_NXV + 3 * (size_t)nfeat;
-  size_t o = sizeof(sl2_snapshot_header);
-  L.x = o;
-  o += sl2_snap_align8(8 * n);
-  L.P = o;
-  o += 8 * n * n;
-#define SL2_SECTION(T, name, per, by, reset) \
-  L.field[SL2_FIELD_##name] = o;             \
-  o += sl2_snap_align8((size_t)nfeat * per * sizeof(T));
-  SL2_STREAM_ARRAYS(SL2_SECTION)
-#undef SL2_SECTION
-  L.templates = o;
-  o += sl2_snap_align8((size_t)nfeat * box * box);
-  L.total = o;
-  return L;
-}
-
-// what the host validated for one blob of a load: the kernels take sizes and counts from here, never from the blob
-struct Sl2SnapLoad {
-  Sl2StreamCam cam;
-  int stream, nfeat, nsel, nvisible, nmeas, ncull;
-  int pad_[2];
-};
-// pack the streams [lo, lo + cnt) into blobs at buf + i * stride (nfeat read on the device, header written)
-cudaError_t sl2_launch_pack(const Sl2Dev &d, int lo, int cnt, uint8_t *buf, size_t stride, Sl2Queue q);
-// adds the number of blobs whose job_feat / sel_rank fail the index rules (with the validated counts) to *bad
-cudaError_t sl2_launch_snap_check(const Sl2Dev &d, int cnt, const Sl2SnapLoad *ld_dev, const uint8_t *buf,
-                                  size_t stride, int *bad, Sl2Queue q);
-// unpack blob i into stream ld_dev[i].stream and reset what the blob does not cover
-cudaError_t sl2_launch_unpack(const Sl2Dev &d, int cnt, const Sl2SnapLoad *ld_dev, const uint8_t *buf, size_t stride,
-                              Sl2Queue q);

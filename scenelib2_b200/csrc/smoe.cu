@@ -13,8 +13,14 @@
 //                       cached value, `corr <= corrmax` => the LAST minimum in (urel, vrel) order wins.
 // The round-1 path ran search_kernel in an "smoe mode" that recomputed the score per ellipse (K = 100 heavily
 // overlapping ellipses: up to ~100x redundant work).
-#include "sl2_common.cuh"
+// Entry points: sl2_smoe_search*, sl2_measure_particles* and sl2_measure_partial_features, each one staged call
+// (partial_features) of [particle prediction ->] both SMOE kernels [-> re-weighting, particles.cu].
+#include <algorithm>
+
+#include "sl2_context.cuh"
 #include "sl2_score.cuh"
+
+using namespace sl2;
 
 namespace {
 
@@ -151,8 +157,6 @@ __global__ void __launch_bounds__(128) smoe_argmin_kernel(const Sl2Dev d, const 
   }
 }
 
-}  // namespace
-
 size_t sl2_smoe_map_bytes(const Sl2Dev &d, int F) { return (size_t)F * d.W * d.H * sizeof(double); }
 
 // F features x up to Kmax ellipses each (K_dev[f] of them used), templates at feat_dev[f] (relative to the
@@ -172,3 +176,192 @@ cudaError_t sl2_launch_smoe(const Sl2Dev &d, int s, int slot, int F, int Kmax, c
   if (e != cudaSuccess) return e;
   return sl2_launch_kernel(smoe_argmin_kernel, dim3((Kmax + 3) / 4, F), dim3(128), 0, q, false, d, A, (d.box - 1) / 2);
 }
+
+// ---- partially-initialised features: F features x Kmax particle slots in one pass ------------------------------
+// One H2D of everything, [particle_predict] -> smoe map -> smoe argmin -> [reweight], one D2H.
+//   feat_index / patches : templates, either map features or raw BOX x BOX templates (scratch slots behind the map)
+//   ypi != NULL          : predict h / Sinv3 / detS on the device (they are outputs), else they are inputs
+//   prob != NULL         : run the re-weighting (lambda, prob, prune threshold), else search only
+struct PartialIO {
+  int F, Kmax;
+  const int32_t *K;
+  const int32_t *feat_index;
+  const uint8_t *patches;
+  const double *ypi, *Pxy, *Pyy;
+  double *h, *Sinv3, *detS;
+  const double *lambda;
+  double prune;
+  double *prob;
+  int32_t *z_uv;
+  uint8_t *found, *keep;
+  double *cumulative, *mean_var;
+  int32_t *left;
+};
+
+int partial_features(sl2_ctx *c, int32_t s, int32_t slot, const PartialIO &io, const char *who) {
+  const Sl2Dev &d = c->d;
+  const int F = io.F, Kmax = io.Kmax;
+  const bool predict = io.ypi != nullptr, reweight = io.prob != nullptr;
+  if (bad_stream(c, s) || bad_slot(c, slot) || F < 0 || F > SL2_MAX_PARTIAL || Kmax < 0 ||
+      Kmax > SL2_MAX_PARTICLES || (F && Kmax && (!io.K || (!io.feat_index && !io.patches) || !io.h || !io.Sinv3)) ||
+      (predict && (!io.Pxy || !io.Pyy || !io.lambda || !io.detS)) || (reweight && (!io.lambda || !io.detS)))
+    return fail(c, SL2_ERR_ARG, std::string(who) + ": bad argument");
+  if (F == 0 || Kmax == 0) return SL2_OK;
+  for (int f = 0; f < F; ++f)
+    if (io.K[f] < 0 || io.K[f] > Kmax) return fail(c, SL2_ERR_ARG, std::string(who) + ": particle count out of range");
+  if (io.feat_index) {
+    const int rc = check_feature_indices(c, s, io.feat_index, F, std::string(who) + ": feature index out of range");
+    if (rc) return rc;
+  }
+  const int grown = grow_scratch(c, sl2_smoe_map_bytes(d, F), c->smoe_map_bytes, c->smoe_map);
+  if (grown) return grown;
+  // h / Sinv3 / detS: outputs of the prediction, else inputs; prob: rewritten by the re-weighting
+  const size_t n = (size_t)F * Kmax, nF = F;
+  Stage K{STAGE_IN, 4 * nF, io.K}, ft{STAGE_IN, 4 * nF}, ypi{STAGE_IN, 48 * nF, io.ypi},
+      Pxy{STAGE_IN, 8 * 78 * nF, io.Pxy}, Pyy{STAGE_IN, 8 * 36 * nF, io.Pyy}, lam{STAGE_IN, 8 * n, io.lambda},
+      tpl{STAGE_IN, nF * d.box * 16}, prob{STAGE_INOUT, 8 * n, io.prob},
+      h{STAGE_INOUT, 16 * n, predict ? nullptr : io.h}, Sinv3{STAGE_INOUT, 24 * n, predict ? nullptr : io.Sinv3},
+      detS{STAGE_INOUT, 8 * n, predict ? nullptr : io.detS}, cum{STAGE_OUT, 8 * n}, mv{STAGE_OUT, 16 * nF},
+      uv{STAGE_OUT, 8 * n}, left{STAGE_OUT, 4 * nF}, found{STAGE_OUT, n}, keep{STAGE_OUT, n};
+  auto pack = [&] {
+    for (int f = 0; f < F; ++f) ft.host<int>()[f] = io.feat_index ? io.feat_index[f] : (d.B - s) * d.Nmax + f;
+    if (io.patches) pack_patch_rows(tpl.h, io.patches, F, d.box);
+  };
+  const int rc = staged_call(
+      c, {&K, &ft, &ypi, &Pxy, &Pyy, &lam, &tpl, &prob, &h, &Sinv3, &detS, &cum, &mv, &uv, &left, &found, &keep}, pack,
+      [&] {
+        if (io.patches)  // raw templates -> the scratch slots behind the map templates
+          CU_TRY(c, cudaMemcpyAsync(d.patches + (size_t)d.B * d.Nmax * d.box * 16, tpl.d, tpl.bytes,
+                                    cudaMemcpyDeviceToDevice, c->stream));
+        if (predict)
+          CU_TRY(c, sl2_launch_particle_predict(d, s, F, Kmax, K.dev<int>(), ypi.dev<double>(), Pxy.dev<double>(),
+                                                Pyy.dev<double>(), lam.dev<double>(), h.dev<double>(),
+                                                Sinv3.dev<double>(), detS.dev<double>(), queue(c)));
+        // measure_feature_with_multiple_priors (monoslam.cpp:1408-1438): ellipses (SInv_k, h_k), one template per feature
+        CU_TRY(c, sl2_launch_smoe(d, s, slot, F, Kmax, K.dev<int>(), ft.dev<int>(), h.dev<double>(), Sinv3.dev<double>(),
+                                  c->smoe_map.get(), uv.dev<int>(), found.d, nullptr, queue(c)));
+        if (reweight)
+          CU_TRY(c, sl2_launch_particles(F, Kmax, K.dev<int>(), h.dev<double>(), Sinv3.dev<double>(),
+                                         detS.dev<double>(), lam.dev<double>(), uv.dev<int>(), found.d, io.prune,
+                                         prob.dev<double>(), keep.d, cum.dev<double>(), mv.dev<double>(),
+                                         left.dev<int>(), queue(c)));
+        return SL2_OK;
+      });
+  if (rc) return rc;
+  if (predict) {
+    memcpy(io.h, h.h, h.bytes);
+    memcpy(io.Sinv3, Sinv3.h, Sinv3.bytes);
+    memcpy(io.detS, detS.h, detS.bytes);
+  }
+  if (reweight) {
+    memcpy(io.prob, prob.h, prob.bytes);
+    if (io.cumulative) memcpy(io.cumulative, cum.h, cum.bytes);
+    if (io.mean_var) memcpy(io.mean_var, mv.h, mv.bytes);
+    if (io.keep) memcpy(io.keep, keep.h, keep.bytes);
+    if (io.left) memcpy(io.left, left.h, left.bytes);
+  }
+  if (io.z_uv) memcpy(io.z_uv, uv.h, uv.bytes);
+  if (io.found) memcpy(io.found, found.h, found.bytes);
+  return SL2_OK;
+}
+
+int smoe_one(sl2_ctx *c, int32_t s, int32_t slot, const int32_t *feat_index, const uint8_t *patch, int32_t K,
+             const double *PuInv3, const double *centres, int32_t *res_u, int32_t *res_v, uint8_t *res_flag,
+             const char *who) {
+  if (K < 0 || (K && (!PuInv3 || !centres))) return fail(c, SL2_ERR_ARG, std::string(who) + ": bad argument");
+  if (K == 0) return SL2_OK;
+  if (K > SL2_MAX_PARTICLES) return fail(c, SL2_ERR_ARG, std::string(who) + ": more than SL2_MAX_PARTICLES ellipses");
+  std::vector<int32_t> uv(2 * (size_t)K);
+  PartialIO io = {};
+  io.F = 1, io.Kmax = K, io.K = &K;
+  io.feat_index = feat_index, io.patches = patch;
+  io.h = const_cast<double *>(centres), io.Sinv3 = const_cast<double *>(PuInv3);  // inputs (no prediction)
+  io.z_uv = uv.data(), io.found = res_flag;
+  const int rc = partial_features(c, s, slot, io, who);
+  if (rc) return rc;
+  for (int i = 0; i < K; ++i) {
+    if (res_u) res_u[i] = uv[2 * i];
+    if (res_v) res_v[i] = uv[2 * i + 1];
+  }
+  return SL2_OK;
+}
+
+int measure_particles(sl2_ctx *c, int32_t s, int32_t slot, const int32_t *feat_index, const uint8_t *patch,
+                      int32_t K, const double *h, const double *Sinv3, const double *detS, const double *lambda,
+                      double prune_probability_threshold, double *prob, int32_t *z_uv, uint8_t *found,
+                      uint8_t *keep, double *cumulative, double *mean_var) {
+  if (K < 0 || (K && (!h || !Sinv3 || !detS || !lambda || !prob)))
+    return fail(c, SL2_ERR_ARG, "sl2_measure_particles: bad argument");
+  if (K == 0) return 0;
+  if (K > SL2_MAX_PARTICLES) return fail(c, SL2_ERR_ARG, "sl2_measure_particles: more than SL2_MAX_PARTICLES particles");
+  int32_t left = 0;
+  PartialIO io = {};
+  io.F = 1, io.Kmax = K, io.K = &K;
+  io.feat_index = feat_index, io.patches = patch;
+  io.h = const_cast<double *>(h), io.Sinv3 = const_cast<double *>(Sinv3), io.detS = const_cast<double *>(detS);
+  io.lambda = lambda, io.prune = prune_probability_threshold, io.prob = prob;
+  io.z_uv = z_uv, io.found = found, io.keep = keep, io.cumulative = cumulative, io.mean_var = mean_var;
+  io.left = &left;
+  const int rc = partial_features(c, s, slot, io, "sl2_measure_particles");
+  return rc ? rc : left;
+}
+
+}  // namespace
+
+extern "C" {
+
+int sl2_smoe_search(sl2_ctx *c, int32_t s, int32_t slot, int32_t feat_index, int32_t K,
+                    const double *PuInv3, const double *centres, int32_t *res_u, int32_t *res_v,
+                    uint8_t *res_flag) {
+  return smoe_one(c, s, slot, &feat_index, nullptr, K, PuInv3, centres, res_u, res_v, res_flag, "sl2_smoe_search");
+}
+
+int sl2_smoe_search_patch(sl2_ctx *c, int32_t s, int32_t slot, const uint8_t *patch, int32_t K,
+                          const double *PuInv3, const double *centres, int32_t *res_u, int32_t *res_v,
+                          uint8_t *res_flag) {
+  if (!patch) return fail(c, SL2_ERR_ARG, "sl2_smoe_search_patch: patch is null");
+  return smoe_one(c, s, slot, nullptr, patch, K, PuInv3, centres, res_u, res_v, res_flag, "sl2_smoe_search_patch");
+}
+
+int sl2_measure_particles(sl2_ctx *c, int32_t s, int32_t slot, int32_t feat_index, int32_t K,
+                          const double *h, const double *Sinv3, const double *detS, const double *lambda,
+                          double prune_probability_threshold, double *prob, int32_t *z_uv, uint8_t *found,
+                          uint8_t *keep, double *cumulative, double *mean_var) {
+  return measure_particles(c, s, slot, &feat_index, nullptr, K, h, Sinv3, detS, lambda,
+                           prune_probability_threshold, prob, z_uv, found, keep, cumulative, mean_var);
+}
+
+int sl2_measure_particles_patch(sl2_ctx *c, int32_t s, int32_t slot, const uint8_t *patch, int32_t K,
+                                const double *h, const double *Sinv3, const double *detS, const double *lambda,
+                                double prune_probability_threshold, double *prob, int32_t *z_uv,
+                                uint8_t *found, uint8_t *keep, double *cumulative, double *mean_var) {
+  if (!patch) return fail(c, SL2_ERR_ARG, "sl2_measure_particles_patch: patch is null");
+  return measure_particles(c, s, slot, nullptr, patch, K, h, Sinv3, detS, lambda, prune_probability_threshold,
+                           prob, z_uv, found, keep, cumulative, mean_var);
+}
+
+int sl2_measure_partial_features(sl2_ctx *c, int32_t s, int32_t slot, int32_t F, int32_t Kmax, const int32_t *K,
+                                 const uint8_t *patches, const double *ypi, const double *Pxy, const double *Pyy,
+                                 const double *lambda, double prune_probability_threshold, double *prob,
+                                 double *h, double *Sinv3, double *detS, int32_t *z_uv, uint8_t *found,
+                                 uint8_t *keep, double *cumulative, double *mean_var, int32_t *left) {
+  if (F > 0 && Kmax > 0 && (!patches || !ypi || !prob))
+    return fail(c, SL2_ERR_ARG, "sl2_measure_partial_features: bad argument");
+  // h / Sinv3 / detS are outputs the caller may not want: they still travel through the staging buffer
+  std::vector<double> th, ts, td;
+  const size_t n = (size_t)std::max(F, 0) * std::max(Kmax, 0);
+  if (!h) th.resize(2 * n), h = th.data();
+  if (!Sinv3) ts.resize(3 * n), Sinv3 = ts.data();
+  if (!detS) td.resize(n), detS = td.data();
+  PartialIO io = {};
+  io.F = F, io.Kmax = Kmax, io.K = K;
+  io.patches = patches;
+  io.ypi = ypi, io.Pxy = Pxy, io.Pyy = Pyy;
+  io.h = h, io.Sinv3 = Sinv3, io.detS = detS;
+  io.lambda = lambda, io.prune = prune_probability_threshold, io.prob = prob;
+  io.z_uv = z_uv, io.found = found, io.keep = keep, io.cumulative = cumulative, io.mean_var = mean_var;
+  io.left = left;
+  return partial_features(c, s, slot, io, "sl2_measure_partial_features");
+}
+
+}  // extern "C"

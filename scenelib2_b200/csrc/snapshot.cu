@@ -3,7 +3,45 @@
 // P dominates the bytes (0.78 MB per stream at n = 313, 4.9 MB at n = 781): it is copied one column per warp, and a
 // column is contiguous on both sides (stride ld in the context, n in the blob), so every load and store of a warp
 // covers 32 consecutive doubles.  The packed columns are only 16-byte aligned when n is even, hence 8-byte accesses.
-#include "sl2_common.cuh"
+// Entry points: sl2_snapshot_bytes / sl2_snapshot_layout, sl2_save_streams* and sl2_load_streams*, which check every
+// blob's header on the host (snap_validate) and its index fields with the rule snap_index_ok states once for both.
+#include <algorithm>
+
+#include "sl2_context.cuh"
+
+using namespace sl2;
+
+// Section field[k] of a blob is the stream's first nfeat records of array k of SL2_STREAM_ARRAYS (x, P and the
+// templates are laid out separately).
+struct Sl2SnapLayout {
+  size_t x, P, field[SL2_SNAPSHOT_FIELDS], templates, total;  // byte offsets in the blob, total size
+};
+__host__ __device__ inline size_t sl2_snap_align8(size_t b) { return (b + 7) & ~(size_t)7; }
+__host__ __device__ inline Sl2SnapLayout sl2_snap_layout(int nfeat, int box) {
+  Sl2SnapLayout L;
+  const size_t n = SL2_NXV + 3 * (size_t)nfeat;
+  size_t o = sizeof(sl2_snapshot_header);
+  L.x = o;
+  o += sl2_snap_align8(8 * n);
+  L.P = o;
+  o += 8 * n * n;
+#define SL2_SECTION(T, name, per, by, reset) \
+  L.field[SL2_FIELD_##name] = o;             \
+  o += sl2_snap_align8((size_t)nfeat * per * sizeof(T));
+  SL2_STREAM_ARRAYS(SL2_SECTION)
+#undef SL2_SECTION
+  L.templates = o;
+  o += sl2_snap_align8((size_t)nfeat * box * box);
+  L.total = o;
+  return L;
+}
+
+// what the host validated for one blob of a load: the kernels take sizes and counts from here, never from the blob
+struct Sl2SnapLoad {
+  Sl2StreamCam cam;
+  int stream, nfeat, nsel, nvisible, nmeas, ncull;
+  int pad_[2];
+};
 
 namespace {
 
@@ -78,17 +116,7 @@ __global__ void __launch_bounds__(SNAP_THREADS) pack_streams_kernel(const Sl2Dev
     u.h.boxsize = box;
     u.h.nfeat = nf;
     u.h.n = n;
-    const Sl2StreamCam &cr = d.cams[s];
-    u.h.cam.width = (int32_t)cr.cam[0];
-    u.h.cam.height = (int32_t)cr.cam[1];
-    u.h.cam.fku = cr.cam[2];
-    u.h.cam.fkv = cr.cam[3];
-    u.h.cam.u0 = cr.cam[4];
-    u.h.cam.v0 = cr.cam[5];
-    u.h.cam.kd1 = cr.cam[6];
-    u.h.cam.sd = cr.cam[7];
-    u.h.cam.delta_t = cr.dt;
-    u.h.cam.number_of_features_to_select = cr.n_select;
+    sl2_cam_config(d.cams[s], &u.h.cam);
     u.h.nsel = d.nsel[s];
     u.h.nvisible = d.nvisible[s];
     u.h.nmeas = d.nmeas[s];
@@ -98,7 +126,14 @@ __global__ void __launch_bounds__(SNAP_THREADS) pack_streams_kernel(const Sl2Dev
   }
 }
 
-// the index rules of a load for blob blockIdx.x, with the host-validated nfeat and nsel (include/sl2b200.h)
+// The index rule of a load for feature f of a blob with nsel selected of nfeat features (include/sl2b200.h): its
+// sel_rank r is -1 or a rank below both; its job_feat j names a feature or, below nsel, may be empty (-1), and is -1
+// above nsel (the cull writes job slot sel_rank)
+__host__ __device__ inline bool snap_index_ok(int f, int r, int j, int nsel, int nfeat) {
+  return (r == -1 || (r >= 0 && r < nsel && r < nfeat)) && (f < nsel ? (j >= -1 && j < nfeat) : j == -1);
+}
+
+// the index rule for blob blockIdx.x, with the host-validated nfeat and nsel
 __global__ void __launch_bounds__(SNAP_THREADS) snap_check_kernel(const Sl2Dev d, const Sl2SnapLoad *ld,
                                                                   const uint8_t *buf, size_t stride, int *bad) {
   const Sl2SnapLoad q = ld[blockIdx.x];
@@ -107,11 +142,7 @@ __global__ void __launch_bounds__(SNAP_THREADS) snap_check_kernel(const Sl2Dev d
   const int *rank = reinterpret_cast<const int *>(blob + L.field[SL2_FIELD_sel_rank]);
   const int *job = reinterpret_cast<const int *>(blob + L.field[SL2_FIELD_job_feat]);
   int ok = 1;
-  for (int f = threadIdx.x; f < q.nfeat; f += blockDim.x) {
-    const int r = rank[f], j = job[f];
-    ok &= (r == -1 || (r >= 0 && r < q.nsel && r < q.nfeat));
-    ok &= f < q.nsel ? (j >= -1 && j < q.nfeat) : (j == -1);
-  }
+  for (int f = threadIdx.x; f < q.nfeat; f += blockDim.x) ok &= snap_index_ok(f, rank[f], job[f], q.nsel, q.nfeat);
   if (!__syncthreads_and(ok) && threadIdx.x == 0) atomicAdd(bad, 1);
 }
 
@@ -159,23 +190,199 @@ __global__ void __launch_bounds__(SNAP_THREADS) unpack_streams_kernel(const Sl2D
 // blocks per stream: about two columns of P per warp at the context's capacity
 int snap_chunks(const Sl2Dev &d) { return (d.ld + 2 * SNAP_WARPS - 1) / (2 * SNAP_WARPS); }
 
-}  // namespace
-
+// pack the streams [lo, lo + cnt) into blobs at buf + i * stride (nfeat read on the device, header written)
 cudaError_t sl2_launch_pack(const Sl2Dev &d, int lo, int cnt, uint8_t *buf, size_t stride, Sl2Queue q) {
   if (cnt <= 0) return cudaSuccess;
   return sl2_launch_kernel(pack_streams_kernel, dim3(cnt, snap_chunks(d)), dim3(SNAP_THREADS), 0, q, false, d, lo, buf,
                            stride);
 }
 
+// adds the number of blobs whose job_feat / sel_rank fail the index rule (with the validated counts) to *bad
 cudaError_t sl2_launch_snap_check(const Sl2Dev &d, int cnt, const Sl2SnapLoad *ld_dev, const uint8_t *buf,
                                   size_t stride, int *bad, Sl2Queue q) {
   if (cnt <= 0) return cudaSuccess;
   return sl2_launch_kernel(snap_check_kernel, dim3(cnt), dim3(SNAP_THREADS), 0, q, false, d, ld_dev, buf, stride, bad);
 }
 
+// unpack blob i into stream ld_dev[i].stream and reset what the blob does not cover
 cudaError_t sl2_launch_unpack(const Sl2Dev &d, int cnt, const Sl2SnapLoad *ld_dev, const uint8_t *buf, size_t stride,
                               Sl2Queue q) {
   if (cnt <= 0) return cudaSuccess;
   return sl2_launch_kernel(unpack_streams_kernel, dim3(cnt, snap_chunks(d)), dim3(SNAP_THREADS), 0, q, false, d, ld_dev,
                            buf, stride);
 }
+
+// Checks the header of one blob (and, with `index`, its job_feat / sel_rank) against this context; fills `q` with
+// the validated counts for stream s.  `blob` is host memory of at least `avail` bytes, any alignment.
+int snap_validate(sl2_ctx *c, const uint8_t *blob, size_t stride, bool index, int s, Sl2SnapLoad *q,
+                  const std::string &who) {
+  sl2_snapshot_header h;
+  memcpy(&h, blob, sizeof h);
+  if (h.magic != SL2_SNAPSHOT_MAGIC || h.version != SL2_SNAPSHOT_VERSION || h.header_bytes != sizeof h)
+    return fail(c, SL2_ERR_ARG, who + ": not a snapshot of this version and byte order");
+  if (h.reserved0 != 0 || h.reserved1 != 0) return fail(c, SL2_ERR_ARG, who + ": reserved header fields are not 0");
+  if (h.total_bytes > stride) return fail(c, SL2_ERR_ARG, who + ": blob larger than the stride");
+  if (h.nfeat < 0 || h.nsel < 0 || h.nvisible < 0 || h.nmeas < 0 || h.ncull < 0)
+    return fail(c, SL2_ERR_ARG, who + ": negative count");
+  if ((int64_t)h.n != SL2_NXV + 3 * (int64_t)h.nfeat) return fail(c, SL2_ERR_ARG, who + ": n != 13 + 3 nfeat");
+  if (h.boxsize != c->cfg.boxsize) return fail(c, SL2_ERR_ARG, who + ": boxsize differs from the context's");
+  if (h.nfeat > c->cfg.max_features) return fail(c, SL2_ERR_STATE, who + ": map larger than max_features");
+  const Sl2SnapLayout L = sl2_snap_layout(h.nfeat, h.boxsize);
+  if (h.total_bytes != L.total) return fail(c, SL2_ERR_ARG, who + ": total size does not match nfeat and boxsize");
+  // the counts are not renewed by a cull, sl2_delete_feature or sl2_set_features, so they are bounded by what any
+  // prediction / update can produce, not by nfeat (include/sl2b200.h)
+  if (h.nsel > SL2_MAX_MEASURED || h.nmeas > SL2_MAX_MEASURED || h.nvisible > SL2_MAX_FEATURES ||
+      h.ncull > SL2_MAX_FEATURES)
+    return fail(c, SL2_ERR_ARG, who + ": count above what a step can produce");
+  const int rc = check_stream_config(c, &h.cam, who);
+  if (rc) return rc;
+  if (index) {
+    for (int f = 0; f < h.nfeat; ++f) {
+      int32_t r, j;
+      memcpy(&r, blob + L.field[SL2_FIELD_sel_rank] + 4 * (size_t)f, 4);
+      memcpy(&j, blob + L.field[SL2_FIELD_job_feat] + 4 * (size_t)f, 4);
+      if (!snap_index_ok(f, r, j, h.nsel, h.nfeat))
+        return fail(c, SL2_ERR_ARG, who + ": sel_rank or job_feat out of range");
+    }
+  }
+  memset(q, 0, sizeof *q);
+  q->cam = sl2_cam_row(h.cam);
+  q->stream = s;
+  q->nfeat = h.nfeat;
+  q->nsel = h.nsel;
+  q->nvisible = h.nvisible;
+  q->nmeas = h.nmeas;
+  q->ncull = h.ncull;
+  return SL2_OK;
+}
+
+// The host forms stage groups of streams of at most this many bytes (at least one stream), so a save or load of a
+// whole large context does not grow the staging buffers to the size of all its blobs.
+const size_t SL2_SNAP_STAGE_BYTES = (size_t)64 << 20;
+int snap_group(size_t sb) { return (int)std::max<size_t>(1, SL2_SNAP_STAGE_BYTES / sb); }
+
+}  // namespace
+
+extern "C" {
+
+size_t sl2_snapshot_bytes(const sl2_ctx *c) { return c ? sl2_snap_layout(c->cfg.max_features, c->cfg.boxsize).total : 0; }
+
+int sl2_snapshot_layout(int32_t nfeat, int32_t boxsize, sl2_snapshot_sections *out) {
+  if (nfeat < 0 || nfeat > SL2_MAX_FEATURES || boxsize <= 0 || !out) return SL2_ERR_ARG;
+  const Sl2SnapLayout L = sl2_snap_layout(nfeat, boxsize);
+  out->x = L.x;
+  out->P = L.P;
+  for (int k = 0; k < SL2_SNAPSHOT_FIELDS; ++k) out->field[k] = L.field[k];
+  out->templates = L.templates;
+  out->total = L.total;
+  return SL2_OK;
+}
+
+int sl2_save_streams(sl2_ctx *c, int32_t lo, int32_t cnt, void *buf, size_t stride, size_t *sizes) {
+  if (bad_range(c, lo, cnt) || (cnt && !buf)) return fail(c, SL2_ERR_ARG, "sl2_save_streams: bad argument");
+  const size_t sb = sl2_snapshot_bytes(c);
+  if (stride < sb) return fail(c, SL2_ERR_ARG, "sl2_save_streams: stride below sl2_snapshot_bytes");
+  if (cnt == 0) return SL2_OK;
+  const int g = std::min(cnt, snap_group(sb));
+  int rc = stage_reserve(c, (size_t)g * sb);
+  if (rc) return rc;
+  CU_TRY(c, cudaStreamSynchronize(c->stream));  // staging buffer reuse
+  for (int i0 = 0; i0 < cnt; i0 += g) {
+    const int k = std::min(g, cnt - i0);
+    CU_TRY(c, sl2_launch_pack(c->d, lo + i0, k, c->stg_dev.get(), sb, queue(c)));
+    CU_TRY(c, cudaMemcpyAsync(c->stg_host.get(), c->stg_dev.get(), (size_t)k * sb, cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    for (int i = 0; i < k; ++i) {
+      sl2_snapshot_header h;
+      memcpy(&h, c->stg_host.get() + (size_t)i * sb, sizeof h);
+      memcpy(static_cast<uint8_t *>(buf) + (size_t)(i0 + i) * stride, c->stg_host.get() + (size_t)i * sb, h.total_bytes);
+      if (sizes) sizes[i0 + i] = h.total_bytes;
+    }
+  }
+  return SL2_OK;
+}
+
+int sl2_save_streams_dev(sl2_ctx *c, int32_t lo, int32_t cnt, void *buf_dev, size_t stride) {
+  if (bad_range(c, lo, cnt) || (cnt && !buf_dev) || ((uintptr_t)buf_dev & 7) || (stride & 7))
+    return fail(c, SL2_ERR_ARG, "sl2_save_streams_dev: bad argument");
+  if (stride < sl2_snapshot_bytes(c)) return fail(c, SL2_ERR_ARG, "sl2_save_streams_dev: stride below sl2_snapshot_bytes");
+  if (cnt == 0) return SL2_OK;
+  CU_TRY(c, sl2_launch_pack(c->d, lo, cnt, static_cast<uint8_t *>(buf_dev), stride, queue(c)));
+  return SL2_OK;
+}
+
+int sl2_load_streams(sl2_ctx *c, int32_t lo, int32_t cnt, const void *buf, size_t stride) {
+  if (bad_range(c, lo, cnt) || (cnt && !buf) || stride < sizeof(sl2_snapshot_header))
+    return fail(c, SL2_ERR_ARG, "sl2_load_streams: bad argument");
+  if (cnt == 0) return SL2_OK;
+  const uint8_t *in = static_cast<const uint8_t *>(buf);
+  std::vector<Sl2SnapLoad> q(cnt);
+  std::vector<sl2_stream_config> cams(cnt);
+  for (int i = 0; i < cnt; ++i) {
+    const int rc = snap_validate(c, in + (size_t)i * stride, stride, true, lo + i, &q[i], "sl2_load_streams");
+    if (rc) return rc;
+    memcpy(&cams[i], in + (size_t)i * stride + offsetof(sl2_snapshot_header, cam), sizeof(sl2_stream_config));
+  }
+  // staging, one group of streams at a time: its load records, then its blobs at the context's snapshot size
+  const size_t sb = sl2_snapshot_bytes(c);
+  const int g = std::min(cnt, snap_group(sb));
+  const size_t pb = ((size_t)g * sizeof(Sl2SnapLoad) + 255) & ~(size_t)255;
+  int rc = stage_reserve(c, pb + (size_t)g * sb);
+  if (rc) return rc;
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  for (int i0 = 0; i0 < cnt; i0 += g) {
+    const int k = std::min(g, cnt - i0);
+    CU_TRY(c, cudaStreamSynchronize(c->stream));  // the previous group's unpack has read the staging buffer
+    memcpy(c->stg_host.get(), q.data() + i0, (size_t)k * sizeof(Sl2SnapLoad));
+    size_t end = 0;
+    for (int i = 0; i < k; ++i) {
+      const size_t tb = sl2_snap_layout(q[i0 + i].nfeat, c->cfg.boxsize).total;
+      memcpy(c->stg_host.get() + pb + (size_t)i * sb, in + (size_t)(i0 + i) * stride, tb);
+      end = pb + (size_t)i * sb + tb;
+    }
+    CU_TRY(c, cudaMemcpyAsync(c->stg_dev.get(), c->stg_host.get(), end, cudaMemcpyHostToDevice, c->stream));
+    CU_TRY(c, sl2_launch_unpack(c->d, k, reinterpret_cast<const Sl2SnapLoad *>(c->stg_dev.get()),
+                                c->stg_dev.get() + pb, sb, queue(c)));
+  }
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  return loaded_cameras(c, lo, cams);
+}
+
+int sl2_load_streams_dev(sl2_ctx *c, int32_t lo, int32_t cnt, const void *buf_dev, size_t stride) {
+  if (bad_range(c, lo, cnt) || (cnt && !buf_dev) || ((uintptr_t)buf_dev & 7) || (stride & 7) ||
+      stride < sizeof(sl2_snapshot_header))
+    return fail(c, SL2_ERR_ARG, "sl2_load_streams_dev: bad argument");
+  if (cnt == 0) return SL2_OK;
+  const uint8_t *in = static_cast<const uint8_t *>(buf_dev);
+  const size_t hb = sizeof(sl2_snapshot_header);
+  // staging: load records | verdict (int) | headers copied down
+  const size_t pb = ((size_t)cnt * sizeof(Sl2SnapLoad) + 255) & ~(size_t)255, o_bad = pb, o_h = pb + 256;
+  int rc = stage_reserve(c, o_h + (size_t)cnt * hb);
+  if (rc) return rc;
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  CU_TRY(c, cudaMemcpy2DAsync(c->stg_host.get() + o_h, hb, in, stride, hb, cnt, cudaMemcpyDeviceToHost, c->stream));
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  std::vector<Sl2SnapLoad> q(cnt);
+  std::vector<sl2_stream_config> cams(cnt);
+  for (int i = 0; i < cnt; ++i) {
+    const uint8_t *h = c->stg_host.get() + o_h + (size_t)i * hb;
+    rc = snap_validate(c, h, stride, false, lo + i, &q[i], "sl2_load_streams_dev");
+    if (rc) return rc;
+    memcpy(&cams[i], h + offsetof(sl2_snapshot_header, cam), sizeof(sl2_stream_config));
+  }
+  memcpy(c->stg_host.get(), q.data(), (size_t)cnt * sizeof(Sl2SnapLoad));
+  memset(c->stg_host.get() + o_bad, 0, sizeof(int));
+  CU_TRY(c, cudaMemcpyAsync(c->stg_dev.get(), c->stg_host.get(), o_bad + sizeof(int), cudaMemcpyHostToDevice, c->stream));
+  const Sl2SnapLoad *q_dev = reinterpret_cast<const Sl2SnapLoad *>(c->stg_dev.get());
+  int *bad_dev = reinterpret_cast<int *>(c->stg_dev.get() + o_bad);
+  CU_TRY(c, sl2_launch_snap_check(c->d, cnt, q_dev, in, stride, bad_dev, queue(c)));
+  int bad = 0;
+  CU_TRY(c, cudaMemcpyAsync(&bad, bad_dev, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  if (bad) return fail(c, SL2_ERR_ARG, "sl2_load_streams_dev: sel_rank or job_feat out of range");
+  CU_TRY(c, sl2_launch_unpack(c->d, cnt, q_dev, in, stride, queue(c)));
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  return loaded_cameras(c, lo, cams);
+}
+
+}  // extern "C"

@@ -37,10 +37,13 @@
 // read once by upd_solve (registers), Y is written once and read by the tiles of the same stream, which run at the
 // same time on neighbouring SMs (L2 hits).  The dense O(n^2 m) parts use ordinary FP64 FMAs / DMMA (tolerance
 // 1e-5 relative, north star); nothing in this file decides which pixels are searched.
+// Entry points of one stream: sl2_ekf_update (a caller's H, R, nu), sl2_ekf_update_measured, sl2_normalise_state.
 #include <type_traits>
 
-#include "sl2_common.cuh"
+#include "sl2_context.cuh"
 #include "sl2_ptx.cuh"
+
+using namespace sl2;
 
 namespace {
 
@@ -1442,11 +1445,11 @@ inline void solve_shape(int Nmax, int &nslab, int &warps) {
 }
 constexpr size_t SYRK_SMEM = (size_t)2 * 2 * 32 * UPD_YS * sizeof(double);  // upd_syrk_kernel<32, 2>
 
-}  // namespace
-
 size_t sl2_update_smem_bytes(const Sl2Dev &d) {  // upd_chol
   return chol_smem_doubles(d.kmax) * sizeof(double);
 }
+
+}  // namespace
 
 cudaError_t sl2_configure_update(const Sl2Dev &d) {
   const SolveKernel solve = solve_kernel(d.kmax);
@@ -1530,3 +1533,46 @@ cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, in
   if ((e = mark(5)) != cudaSuccess) return e;
   return cudaGetLastError();
 }
+
+extern "C" {
+
+int sl2_ekf_update(sl2_ctx *c, int32_t s, int32_t m, const int32_t *feat_index, const double *H_xv,
+                   const double *H_y, const double *R, const double *nu) {
+  if (bad_stream(c, s) || m < 0 || (m & 1) || m > c->d.mmax)
+    return fail(c, SL2_ERR_ARG, "sl2_ekf_update: bad m");
+  if (m == 0) return SL2_OK;
+  if (!feat_index || !H_xv || !H_y || !R || !nu) return fail(c, SL2_ERR_ARG, "sl2_ekf_update: null argument");
+  const int K = m / 2;
+  int nf = 0;
+  int rc = device_nfeat(c, s, &nf);
+  if (rc) return rc;
+  for (int k = 0; k < K; ++k) {
+    if (feat_index[k] < 0 || feat_index[k] >= nf) return fail(c, SL2_ERR_ARG, "sl2_ekf_update: bad feature index");
+    // the full 2x2 block R_k enters S (kalman.cpp:101); a covariance block has to be symmetric
+    if (R[k * 4 + 1] != R[k * 4 + 2]) return fail(c, SL2_ERR_ARG, "sl2_ekf_update: R block is not symmetric");
+  }
+  const size_t k = K;
+  Stage hx{STAGE_IN, 8 * 26 * k, H_xv}, hy{STAGE_IN, 8 * 6 * k, H_y}, r{STAGE_IN, 8 * 4 * k, R},
+      v{STAGE_IN, 8 * 2 * k, nu}, fe{STAGE_IN, 4 * k, feat_index};
+  return staged_call(c, {&hx, &hy, &r, &v, &fe}, [] {}, [&] {
+    CU_TRY(c, sl2_launch_update(c->d, s, 1, m, fe.dev<int>(), hx.dev<double>(), hy.dev<double>(), r.dev<double>(),
+                                v.dev<double>(), 0, queue(c)));
+    return SL2_OK;
+  });
+}
+
+int sl2_ekf_update_measured(sl2_ctx *c, int32_t s) {
+  if (bad_stream(c, s)) return fail(c, SL2_ERR_ARG, "bad stream");
+  CU_TRY(c, sl2_launch_update(c->d, s, 1, -1, nullptr, nullptr, nullptr, nullptr, nullptr, 0, queue(c)));
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  return SL2_OK;
+}
+
+int sl2_normalise_state(sl2_ctx *c, int32_t s) {
+  if (bad_stream(c, s)) return fail(c, SL2_ERR_ARG, "bad stream");
+  CU_TRY(c, sl2_launch_update(c->d, s, 1, -1, nullptr, nullptr, nullptr, nullptr, nullptr, 1, queue(c)));
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  return SL2_OK;
+}
+
+}  // extern "C"
