@@ -23,9 +23,10 @@ def _quat(rng, spread):
     return q / np.linalg.norm(q)
 
 
-def make_case(rng, k, nf=None, outliers=(), offset=(9.0, -6.0), P=None, camera_pts=None, xv=None):
+def make_case(rng, k, nf=None, outliers=(), offset=(9.0, -6.0), P=None, camera_pts=None, xv=None, cam8=CAM8):
     """k matched features of a map of nf, in a random rank order: the oracle's predictions (h, dh/dxv, dh/dy, S) of
-    the predicted state, z = round(h) (+-1 px) and, for the matches in `outliers`, z shifted by `offset`."""
+    the predicted state for the camera cam8, z = round(h) (+-1 px) and, for the matches in `outliers`, z shifted by
+    `offset`."""
     nf = nf or k + 3
     n = 13 + 3 * nf
     if xv is None:
@@ -41,13 +42,13 @@ def make_case(rng, k, nf=None, outliers=(), offset=(9.0, -6.0), P=None, camera_p
     pos = 13 + 3 * feats
     h, S, dxp, dy = np.zeros((k, 2)), np.zeros((k, 2, 2)), np.zeros((k, 2, 7)), np.zeros((k, 2, 3))
     for j, p in enumerate(pos):
-        hj, dxv, dyj, _, Sj = po.predict_feature(CAM8, xv, x[p:p + 3], P[:13, :13], P[:13, p:p + 3],
+        hj, dxv, dyj, _, Sj = po.predict_feature(cam8, xv, x[p:p + 3], P[:13, :13], P[:13, p:p + 3],
                                                  P[p:p + 3, p:p + 3])
         h[j], S[j], dxp[j], dy[j] = hj, Sj, dxv[:, :7], dyj
     z = np.round(h) + rng.integers(-1, 2, (k, 2))
     for j in outliers:
         z[j] += offset
-    return dict(cam8=CAM8, x=x, P=P, pos=pos.astype(np.int32), z=z, h=h, S=S, dh_dxp=dxp, dh_dy=dy)
+    return dict(cam8=cam8, x=x, P=P, pos=pos.astype(np.int32), z=z, h=h, S=S, dh_dxp=dxp, dh_dy=dy)
 
 
 def both(case, tau):
@@ -115,12 +116,10 @@ def test_two_equal_clusters_lowest_rank_wins():
         assert win == 0 and (keep == even).all()
 
 
-def test_point_behind_the_camera_is_never_an_inlier():
-    rng = np.random.default_rng(15)
-    k = 6
+def behind_camera_case(rng, k=6):
+    """Feature of rank 2 moved behind the camera (its prediction stays finite: the projection mirrors), its z set to
+    exactly that mirrored projection."""
     case = make_case(rng, k, nf=k)
-    # feature of rank 2 moved behind the camera (its prediction stays finite: the projection mirrors), its z set to
-    # exactly that mirrored projection
     p = case["pos"][2]
     xv = case["x"][:13]
     R = np.array(quat_to_R(*xv[3:7]))
@@ -131,6 +130,12 @@ def test_point_behind_the_camera_is_never_an_inlier():
     case["P"][p:p + 3, p:p + 3] = np.eye(3) * 1e-4
     zc = R.T @ (case["x"][p:p + 3] - xv[:3])
     case["z"][2] = np.round(project_point(CAM8, zc)[0])
+    return case
+
+
+def test_point_behind_the_camera_is_never_an_inlier():
+    k = 6
+    case = behind_camera_case(np.random.default_rng(15), k)
     keep, sup, win, d2 = both(case, 1000.0)  # a radius that takes every point in front of the camera
     assert np.isnan(d2[:, 2]).all()
     assert win >= 0 and not keep[2] and keep[np.arange(k) != 2].all()

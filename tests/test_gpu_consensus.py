@@ -1,6 +1,7 @@
 """The match consensus on the device (sl2_set_stream_consensus, csrc/consensus.cu consensus_kernel) on scenes with
 distractors: a feature's template pasted at a fixed offset inside its search ellipse while its true location is
 occluded, so that the patch search returns a confident wrong match.  A match is correct iff z = pix + shift[t]."""
+import dataclasses
 import math
 
 import numpy as np
@@ -9,9 +10,12 @@ import pytest
 import consensus_oracle as co
 import scenelib2_b200 as sl2
 from consensus_ref import restated
+from consensus_truth import consensus_truth
 from gpu_util import (CAMS_320, assert_same_bytes, check_streams_against_oracle, ctx_from_scenes, large_variant,
-                      step_frames, stream_result)
+                      oracle_slam_from_scene, step_frames, stream_result)
+from oracle import pyoracle as po
 from scenelib2_b200 import synth
+from scenelib2_b200.lib import SL2_MAX_MEASURED
 
 TAU = 2.5          # px: the synthetic camera moves by whole pixels, correct matches sit within ~1 px of a hypothesis
 OFFSET = (9, -6)   # px: where a distractor pastes the template, inside the 20 px ellipse
@@ -422,3 +426,174 @@ def test_rejected_setter_arguments_change_nothing():
         assert math.copysign(1.0, ctx.stream_consensus(0)) == 1.0
     finally:
         ctx.close()
+
+
+# ---- 10. the device against the consensus from its definition, at the kernel's shape edges --------------------------
+# The device exposes only its rejections: the rejected set must be the complement of the truth winner's inlier set
+# (consensus_truth, np.longdouble) whenever no decision of the step lies within D2_BAND of fl(tau tau), besides equal
+# to the test oracle's bit for bit.  D2_BAND is test_consensus_truth.D2_BOUND, set from the CPU cases.
+D2_BAND = 1e-10
+K_SHAPES = (2, 3, 8, 9, 16, 17, 31, 32, 33, 63, 64, 65)   # CONS_WARPS = 8 hypotheses, 32 matches per word
+
+
+def truth_of(cam8, inp, tau=TAU):
+    return consensus_truth(cam8, inp["x"], inp["P"], inp["pos"], inp["z"], inp["h"], inp["S"], inp["dh_dxp"],
+                           inp["dh_dy"], tau, prec="ld")
+
+
+def staged_inputs(ctx, clone, streams, frame_of):
+    """The consensus inputs of each stream of `streams` on frame_of(s), staged in the one-stream `clone` under that
+    stream's camera and selection count, with the test oracle's decisions and the truth: {s: (inp, keep, truth)}."""
+    out = {}
+    for s in streams:
+        clone.set_stream_config(0, ctx.stream_config(s))
+        inp = staged_clone(clone, ctx.save_stream(s), frame_of(s))
+        cam8 = _cam8(ctx, s)
+        out[s] = (inp, expected(cam8, inp, TAU)[0], truth_of(cam8, inp))
+    return out
+
+
+def check_rejections(ctx, s, inp, keep, tr, where):
+    """-> True when the truth was unambiguous and the device's rejections were held to it."""
+    got = rejected_now(ctx, s)
+    assert got == set(inp["M"][~keep].tolist()), (where, "oracle")
+    if tr.margin <= D2_BAND * max(1.0, TAU * TAU):
+        print("%s: a decision within %.1e px^2 of tau^2; only the oracle compared" % (where, tr.margin))
+        return False
+    assert got == set(inp["M"][~tr.keep].tolist()), (where, "truth", tr.winner, tr.support)
+    return True
+
+
+def matched_count(sc, n_select, t=0):
+    """How many of the n_select features the oracle (and so the device) finds in frame t of the scene."""
+    o = oracle_slam_from_scene(po, dataclasses.replace(sc, n_select=n_select))
+    o.predict()
+    o.select()
+    o.measure(sc.frames[t])
+    f = o.features()
+    return int(((f["select_rank"] >= 0) & ((f["flags"] & 2) > 0)).sum())
+
+
+def shape_scene(k, stream_id=0, n_frames=2):
+    """C4 camera, k + 8 features (at least 12) in view, distractors on every fourth feature (every ninth from k = 64
+    on, where the grid is dense), and the smallest n_select at which exactly k matches are found in frame 0."""
+    nf = max(k + 8, 12)
+    sc = large_variant(nf, nf, stream_id=stream_id, n_frames=n_frames)
+    sc = distractor_scene(None, sc=sc, persistent=range(1, nf, 4 if k < 64 else 9))
+    for n in range(k, min(nf, SL2_MAX_MEASURED) + 1):
+        if matched_count(sc, n) >= k:
+            break
+    assert matched_count(sc, n) == k, (k, n)
+    sc.n_select = n
+    return sc
+
+
+def run_against_truth(scenes, T, max_features=None, tau_streams=None, expect_k=None):
+    """Fused steps of a context of `scenes` with the consensus on, each step held to the oracle and the truth.
+    -> (steps held to the truth, [the k of every step and stream])"""
+    ctx, clone = ctx_from_scenes(scenes, max_features=max_features), ctx_from_scenes(scenes[:1],
+                                                                                     max_features=max_features)
+    held, ks = 0, []
+    try:
+        streams = range(len(scenes))
+        for s in streams:
+            ctx.set_stream_consensus(s, TAU)
+        for t in range(T):
+            staged = staged_inputs(ctx, clone, streams, lambda s: scenes[s].frames[t])
+            step_frames(ctx, np.stack([sc.frames[t] for sc in scenes]))
+            for s, (inp, keep, tr) in staged.items():
+                ks.append(inp["M"].size)
+                if expect_k is not None and t == 0:
+                    assert inp["M"].size == expect_k[s], (s, inp["M"].size, expect_k[s])
+                held += check_rejections(ctx, s, inp, keep, tr, ("step", t, "stream", s, "k", inp["M"].size))
+        return held, ks, ctx.get_state(0)[0]
+    finally:
+        ctx.close()
+        clone.close()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("k", K_SHAPES)
+def test_shapes_against_the_truth(k):
+    sc = shape_scene(k)
+    held, ks, _ = run_against_truth([sc], 2, expect_k=[k])
+    assert held >= 1, ks
+
+
+@pytest.mark.gpu
+def test_rank_order_is_a_permutation_of_map_order():
+    sc = shape_scene(40)
+    ctx, clone = ctx_from_scenes([sc]), ctx_from_scenes([sc])
+    try:
+        inp = staged_clone(clone, ctx.save_stream(0), sc.frames[0])
+        assert (np.diff(inp["M"]) < 0).any() and (inp["M"] != np.sort(inp["M"])).sum() > inp["M"].size // 2
+    finally:
+        ctx.close()
+        clone.close()
+    assert run_against_truth([sc], 2)[0] >= 1
+
+
+@pytest.mark.gpu
+def test_capacity_256_matches_past_index_128():
+    """ld = 784: features 0..127 out of view, 40 of 128..255 measured."""
+    sc = large_variant(256, 256, n_frames=2)
+    sc.x0 = sc.x0.copy()
+    sc.x0[13:13 + 3 * 128] += np.tile([3.0, 0.0, 0.0], 128)
+    sc = distractor_scene(None, sc=sc, persistent=range(129, 256, 5))
+    sc.n_select = next(n for n in range(40, 129) if matched_count(sc, n) >= 40)
+    ctx, clone = ctx_from_scenes([sc], max_features=256), ctx_from_scenes([sc], max_features=256)
+    try:
+        inp = staged_clone(clone, ctx.save_stream(0), sc.frames[0])
+        assert inp["M"].size == 40 and inp["M"].min() >= 128 and inp["P"].shape[0] == 13 + 3 * 256
+    finally:
+        ctx.close()
+        clone.close()
+    assert run_against_truth([sc], 2, max_features=256)[0] >= 1
+
+
+@pytest.mark.gpu
+def test_c3_camera_against_the_truth():
+    """640 x 480, kd1 = 2.25e-6, 15 x 15 templates, 100 features selected."""
+    sc = distractor_scene("C3", n_frames=2, persistent=range(2, 100, 6))
+    held, ks, _ = run_against_truth([sc], 2)
+    assert held >= 1 and max(ks) > 64, ks
+
+
+@pytest.mark.gpu
+def test_non_unit_q_after_fused_steps():
+    """x is never renormalised (quirk Q1): after some fused steps |q| != 1 and the truth's pose model sees it.  Nine
+    steps: the tenth would cull the distractors' features and renumber the map under the comparison."""
+    sc = distractor_scene("C2", n_frames=9, n_features=40, persistent=[4, 17], transient={25: range(2, 6)})
+    held, ks, x = run_against_truth([sc], 9)
+    dq = abs(float(np.linalg.norm(x[3:7])) - 1.0)
+    print("| |q| - 1 | after 9 fused steps: %.3e" % dq)
+    assert dq > 0.0 and held >= 8, (dq, held)
+
+
+@pytest.mark.gpu
+def test_264_streams_each_with_its_own_k():
+    """One C4-camera scene in 264 streams whose selection counts give every k from 2 to 65 that the scene allows, in a
+    scrambled order (no two neighbours alike): each stream's decisions are held to its own k."""
+    B = 264
+    sc = shape_scene(65)
+    n_for = {}
+    for n in range(2, sc.n_select + 1):
+        n_for.setdefault(matched_count(sc, n), n)
+    kv = sorted(k for k in n_for if k >= 2)
+    ks = [kv[(37 * s) % len(kv)] for s in range(B)]
+    assert len(kv) >= 50 and all(a != b for a, b in zip(ks, ks[1:]))
+    ctx, clone = ctx_from_scenes([sc] * B), ctx_from_scenes([sc])
+    held = 0
+    try:
+        for s in range(B):
+            ctx.set_stream_config(s, number_of_features_to_select=n_for[ks[s]])
+            ctx.set_stream_consensus(s, TAU)
+        staged = staged_inputs(ctx, clone, range(B), lambda s: sc.frames[0])
+        step_frames(ctx, np.stack([sc.frames[0]] * B))
+        for s, (inp, keep, tr) in staged.items():
+            assert inp["M"].size == ks[s], (s, inp["M"].size, ks[s])
+            held += check_rejections(ctx, s, inp, keep, tr, ("stream", s, "k", ks[s]))
+    finally:
+        ctx.close()
+        clone.close()
+    assert held >= B - 4, held
