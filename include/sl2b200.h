@@ -218,8 +218,9 @@ int sl2_smoe_search(sl2_ctx *ctx, int32_t stream_id, int32_t slot, int32_t feat_
  * in: h (K x 2), Sinv3 (K x (S00,S01,S11)), detS (K), lambda (K); in/out: prob (K);
  * out (each may be NULL): z_uv (K x 2), found (K), keep (K; 1 = particle survives), cumulative (K; of the
  * survivors in order, 0 for pruned ones), mean_var (2).
- * Returns the number of surviving particles, 0 when every probability is zero (the reference then deletes the
- * feature and leaves prob un-normalised), < 0 on error. */
+ * Returns the number of surviving particles, < 0 on error.  0 has two causes: every probability is zero (the
+ * reference deletes the feature; prob is left un-normalised), or every particle fell below the prune threshold (the
+ * reference keeps the feature with no particles; prob holds the probabilities normalised before the prune). */
 int sl2_measure_particles(sl2_ctx *ctx, int32_t stream_id, int32_t slot, int32_t feat_index, int32_t K,
                           const double *h, const double *Sinv3, const double *detS, const double *lambda,
                           double prune_probability_threshold, double *prob, int32_t *z_uv, uint8_t *found,
@@ -245,13 +246,13 @@ int sl2_measure_particles_patch(sl2_ctx *ctx, int32_t stream_id, int32_t slot, c
  *     SearchMultipleOverlappingEllipses with the score of every image location computed once per feature;
  *   MonoSLAM::update_partially_initialised_feature_probabilities   monoslam.cpp:1447-1493 (see above).
  * F <= SL2_MAX_PARTIAL features, feature f uses K[f] <= Kmax <= SL2_MAX_PARTICLES particles; every per-particle
- * array is F x Kmax (entries k >= K[f] are ignored / left alone).
+ * array is F x Kmax (entries k >= K[f] are ignored on input and left as the caller had them on output).
  * in : patches (F x boxsize x boxsize u8), ypi (F x 6: r, hhat), Pxy (F x 13x6 column-major: covariance between
  *      x_v and the feature's 6 states), Pyy (F x 6x6 column-major), lambda (F x Kmax), prune threshold;
  * in/out: prob (F x Kmax);
  * out (each may be NULL): h (F x Kmax x 2), Sinv3 (F x Kmax x (S00,S01,S11)), detS (F x Kmax), z_uv (F x Kmax x 2),
- *      found, keep (F x Kmax), cumulative (F x Kmax), mean_var (F x 2), left (F: survivors, 0 = the reference
- *      deletes the feature). */
+ *      found, keep (F x Kmax), cumulative (F x Kmax), mean_var (F x 2), left (F: survivors; 0 as for
+ *      sl2_measure_particles: deleted by the reference, or kept with every particle pruned). */
 #define SL2_MAX_PARTIAL 16
 #define SL2_MAX_PARTICLES 256
 int sl2_measure_partial_features(sl2_ctx *ctx, int32_t stream_id, int32_t slot, int32_t F, int32_t Kmax,

@@ -248,20 +248,30 @@ int partial_features(sl2_ctx *c, int32_t s, int32_t slot, const PartialIO &io, c
         return SL2_OK;
       });
   if (rc) return rc;
+  // Per-particle outputs: feature f's first K[f] slots are this call's results; slots k >= K[f] of the caller's
+  // arrays are left as they were (the kernels never write them, so the staging buffer holds whatever an earlier call
+  // left there, or zeros).
+  auto particles_out = [&](void *dst, const Stage &src, size_t per_particle) {
+    if (!dst) return;
+    for (int f = 0; f < F; ++f) {
+      const size_t o = (size_t)f * Kmax * per_particle;
+      memcpy(static_cast<uint8_t *>(dst) + o, src.h + o, (size_t)io.K[f] * per_particle);
+    }
+  };
   if (predict) {
-    memcpy(io.h, h.h, h.bytes);
-    memcpy(io.Sinv3, Sinv3.h, Sinv3.bytes);
-    memcpy(io.detS, detS.h, detS.bytes);
+    particles_out(io.h, h, 16);
+    particles_out(io.Sinv3, Sinv3, 24);
+    particles_out(io.detS, detS, 8);
   }
   if (reweight) {
-    memcpy(io.prob, prob.h, prob.bytes);
-    if (io.cumulative) memcpy(io.cumulative, cum.h, cum.bytes);
+    particles_out(io.prob, prob, 8);
+    particles_out(io.cumulative, cum, 8);
+    particles_out(io.keep, keep, 1);
     if (io.mean_var) memcpy(io.mean_var, mv.h, mv.bytes);
-    if (io.keep) memcpy(io.keep, keep.h, keep.bytes);
     if (io.left) memcpy(io.left, left.h, left.bytes);
   }
-  if (io.z_uv) memcpy(io.z_uv, uv.h, uv.bytes);
-  if (io.found) memcpy(io.found, found.h, found.bytes);
+  particles_out(io.z_uv, uv, 8);
+  particles_out(io.found, found, 1);
   return SL2_OK;
 }
 

@@ -493,11 +493,13 @@ class Context:
             left = self._ck(self.L.sl2_measure_particles_patch(self.h, stream_id, slot, patch.ctypes.data, *args))
         return left, prob, z, found, keep, cum, mv
 
-    def measure_partial_features(self, stream_id, slot, patches, ypi, Pxy, Pyy, lam, prune_threshold, prob, K=None):
+    def measure_partial_features(self, stream_id, slot, patches, ypi, Pxy, Pyy, lam, prune_threshold, prob, K=None,
+                                 out=None):
         """N2 for F partially-initialised features in one call: device prediction of every particle's ellipse
         (monoslam.cpp:1347-1400), SMOE search with one score map per feature, particle re-weighting.
         patches (F,B,B) u8; ypi (F,6); Pxy (F,13,6); Pyy (F,6,6); lam, prob (F,Kmax); K (F,) particle counts
-        (default Kmax).  Returns a dict of arrays."""
+        (default Kmax).  Returns a dict of arrays; `out` may supply any of them (same shape and dtype), which the call
+        then writes in place (slots k >= K[f] keep what they held)."""
         patches = np.ascontiguousarray(patches, np.uint8)
         F = patches.shape[0]
         ypi = np.ascontiguousarray(ypi, np.float64).reshape(F, 6)
@@ -507,10 +509,16 @@ class Context:
         Kmax = lam.shape[1]
         prob = np.array(prob, np.float64).reshape(F, Kmax)
         K = np.full(F, Kmax, np.int32) if K is None else np.ascontiguousarray(K, np.int32)
+        given = out or {}
         out = {"h": np.zeros((F, Kmax, 2)), "Sinv3": np.zeros((F, Kmax, 3)), "detS": np.zeros((F, Kmax)),
                "z": np.zeros((F, Kmax, 2), np.int32), "found": np.zeros((F, Kmax), np.uint8),
                "keep": np.zeros((F, Kmax), np.uint8), "cumulative": np.zeros((F, Kmax)),
                "mean_var": np.zeros((F, 2)), "left": np.zeros(F, np.int32)}
+        for k, a in given.items():
+            if k not in out or a.shape != out[k].shape or a.dtype != out[k].dtype or not a.flags.c_contiguous:
+                raise ValueError("out[%r]: expected a C-contiguous %s array of shape %s" % (k, out[k].dtype,
+                                                                                        out[k].shape))
+            out[k] = a
         self._ck(self.L.sl2_measure_partial_features(
             self.h, stream_id, slot, F, Kmax, _p(K, i32p), C.c_void_p(patches.ctypes.data), _p(ypi, f64p), _p(Pxy, f64p),
             _p(Pyy, f64p), _p(lam, f64p), C.c_double(float(prune_threshold)), _p(prob, f64p), _p(out["h"], f64p),
