@@ -118,6 +118,49 @@ int sl2_get_stream_config(sl2_ctx *ctx, int32_t stream_id, sl2_stream_config *sc
 int sl2_set_stream_consensus(sl2_ctx *ctx, int32_t stream_id, double inlier_px);
 int sl2_get_stream_consensus(sl2_ctx *ctx, int32_t stream_id, double *inlier_px);
 
+/* ---- planar patch warp: match each template at the predicted viewpoint (no reference counterpart) ---------------
+ * The reference searches every feature with the template stored when it was first seen, while the visibility test
+ * admits distance ratios in [0.5, 2], 45 degrees of viewing angle and any roll.  A stream with the warp on searches
+ * each selected feature with its template warped to the predicted viewpoint (Davison, Reid, Molton, Stasse, "MonoSLAM",
+ * PAMI 2007; Molton, Davison, Reid, "Locally Planar Patch Features", BMVC 2004), taking the surface around the feature
+ * as planar with its normal pointing at the camera that first saw it.
+ * Warped template of feature i at the camera pose xp (r, q): with cam = the stream's camera, HALF = (B - 1) / 2,
+ * y = the feature's state, xo = its xp_org,
+ *   h = project_point(zeroed_point(y) from xp) (the prediction's h, bit for bit), ho = the same from xo (the centre of
+ *   the stored template); the plane passes through y with world normal nW = xo[0:3] - y (not normalised);
+ *   output pixel (row a, column b): p = h + (b - HALF, a - HALF); dW = RRW^T unproject_point(p);
+ *   t = (nW . (y - r)) / (nW . dW); X = r + t dW; zo = RRW(xo) (X - xo[0:3]); src = project_point(zo) - ho + (HALF, HALF);
+ *   the pixel is valid when t is finite and > 0, zo[2] > 0 and src is finite;
+ *   bilinear sampling of the stored template T: each coordinate of src clamped to [0, B - 1], x0 = min(floor(sx),
+ *   B - 2), fx = sx - x0 (y0, fy likewise), v = (1 - fy)((1 - fx) T[y0][x0] + fx T[y0][x0+1]) + fy((1 - fx)
+ *   T[y0+1][x0] + fx T[y0+1][x0+1]); the byte is (int)(v + 0.5).
+ * Source positions outside the stored template repeat its edge pixels: a B x B template holds nothing beyond itself,
+ * which a warp that shrinks it (the camera moving away, a slanted view) would need.  When any pixel of a feature is
+ * invalid its warped template is its stored template (valid = 0).  Every operation is a correctly rounded FP64
+ * operation in the order written in the device code (csrc/sl2_model.cuh: patch_warp_setup, patch_warp_source,
+ * patch_sample; dot products and matrix rows summed from 0.0 in ascending order), so the bytes are reproducible bit
+ * for bit.
+ * Where it applies: the search of the fused step (sl2_step, sl2_step_host, sl2_step_host_async) and of
+ * sl2_make_measurements warps, for a stream with the warp on, each selected feature's template at the predicted pose
+ * x[0:7]; the search's sigma >= 10 gates and scores then apply to that template, and no other rule changes.
+ * sl2_patch_search, sl2_score_map, the SMOE and particle entry points and sl2_relocalise keep the stored templates.
+ * on = 0 (the default) is off, 1 is on: a context where no stream has it on runs exactly the path without it; one with
+ * a stream that has it on adds one kernel launch per step group holding such a stream (timed with the search in
+ * sl2_last_step_times).  Ordering like sl2_set_stream_config.  The setting belongs to the stream slot, like the match
+ * consensus and the frame source: snapshots do not carry it and a load leaves it.  The first stream turned on sizes
+ * the context's warped-template scratch (num_streams x max_features x boxsize x 16 bytes): SL2_ERR_CUDA, with the
+ * setting left off, when that allocation fails.  SL2_ERR_ARG, with the setting unchanged, for a bad stream_id, an
+ * `on` other than 0 or 1, or (get) a NULL on. */
+int sl2_set_stream_warp(sl2_ctx *ctx, int32_t stream_id, int32_t on);
+int sl2_get_stream_warp(sl2_ctx *ctx, int32_t stream_id, int32_t *on);
+/* The warped templates of features feat_index[0 .. n) of stream_id at the pose xp (7: r, q), whatever the stream's
+ * setting: what the search of a warp-on stream sees at that pose.  out: n x boxsize x boxsize u8, row-major; valid (n,
+ * may be NULL): 1 = warped, 0 = some pixel is invalid and out holds the stored template.  Joins both step
+ * groups and synchronises.  SL2_ERR_ARG, with nothing written, for: a bad stream_id; n outside [0, max_features]; a
+ * NULL feat_index, xp or out with n > 0; a feat_index outside [0, nfeat); a non-finite xp or a zero quaternion. */
+int sl2_warp_templates(sl2_ctx *ctx, int32_t stream_id, int32_t n, const int32_t *feat_index, const double *xp,
+                       uint8_t *out, uint8_t *valid);
+
 /* ---- frames (replaces the cv::Mat `frame` argument of MonoSLAM::GoOneStep, monoslam.cpp:108) */
 /* The frame ring keeps the context's width x height per stream.  A stream whose image is smaller
  * (sl2_set_stream_config) occupies the top-left width_s x height_s of its block; the rest of the block

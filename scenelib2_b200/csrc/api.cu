@@ -160,11 +160,33 @@ bool consensus_on(const sl2_ctx *c, int lo, int cnt) {
   return false;
 }
 
-// The measure stage of the streams [lo, lo + cnt) on q: the patch search over the context's own job arrays (indexed
-// by the stream number local to the launch), then the match consensus when some stream of them has it on
+// whether some stream of [lo, lo + cnt) has the planar patch warp on
+bool warp_on(const sl2_ctx *c, int lo, int cnt) {
+  for (int s = lo; s < lo + cnt; ++s)
+    if (c->warp_on[s]) return true;
+  return false;
+}
+
+// The measure stage of the streams [lo, lo + cnt) on q: when some stream of them has the warp on, every job's template
+// at the predicted pose x[0:7] (the stored one for the others) into the job-indexed scratch; the patch search over the
+// context's own job arrays (indexed by the stream number local to the launch), then the match consensus when some
+// stream of them has it on
 int measure_streams(sl2_ctx *c, int32_t slot, int lo, int cnt, Sl2Queue q) {
   const Sl2Dev &d = c->d;
+  const uint8_t *job_patches = nullptr;
+  if (warp_on(c, lo, cnt)) {
+    WarpLaunch W = {};
+    W.job_feat = d.job_feat + (size_t)lo * d.Nmax;
+    W.jobs_per_stream = d.Nmax;
+    W.stream_lo = lo;
+    W.stream_cnt = cnt;
+    W.on = c->warp_on_dev;
+    W.out = c->warp_patches.get() + (size_t)lo * d.Nmax * d.box * 16;
+    CU_TRY(c, sl2_launch_warp(d, W, q));
+    job_patches = W.out;
+  }
   SearchLaunch L = {};
+  L.job_patches = job_patches;
   L.job_feat = d.job_feat + (size_t)lo * d.Nmax;
   L.job_centre = d.job_centre + (size_t)lo * d.Nmax * 2;
   L.job_puinv = d.job_puinv + (size_t)lo * d.Nmax * 3;
@@ -312,6 +334,8 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   ALLOC(c->xv_stage, (size_t)d.slots * B * SL2_NXV);
   ALLOC(c->cons_tau2, B);
   c->cons_tau.assign(B, 0.0);
+  ALLOC(c->warp_on_dev, B);
+  c->warp_on.assign(B, 0);
 #undef ALLOC
   int rc = make_tensor_map(c);
   if (rc) return failed(rc, c->err);

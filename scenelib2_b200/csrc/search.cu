@@ -9,8 +9,8 @@
 //     tensor = [slot*stream][H][W] u8) that completes on a per-warp mbarrier; windows larger
 //     than the tile are walked tile by tile.  The TMA unit needs a 16-byte aligned box start
 //     so the box is loaded from x & ~15 and is 15 B wider.
-//   * while the TMA is in flight the warp reads the template and forms its constants (first tile
-//     only), evaluates the exact FP64 ellipse predicate for every candidate of the tile and
+//   * while the TMA is in flight the warp reads the template (the feature's stored one, or the job's warped
+//     one from SearchLaunch::job_patches: warp.cu) and forms its constants (first tile only), evaluates the exact FP64 ellipse predicate for every candidate of the tile and
 //     compacts the non-empty vertical strips (candidates of one column) into a task list with
 //     ballots, so later rounds run with full lanes.
 //   * integer phase, per lane = one strip: every image row is read once from shared memory as
@@ -118,7 +118,8 @@ __device__ __forceinline__ float approx_score(uint32_t ax, uint32_t a1, uint32_t
 // 8 at 11 x 11 (18 image rows per strip), 16 at 15 x 15 (30 rows: 1.9 instead of 2.75 row reads per candidate).
 __host__ __device__ constexpr int filter_strip(int box) { return box <= 11 ? 8 : 16; }
 
-template <int BOX, bool FILTER>
+// JOBS: the templates come from L.job_patches by job (the planar patch warp, warp.cu), else from d.patches by feature
+template <int BOX, bool FILTER, bool JOBS = false>
 __global__ void __launch_bounds__(SL2_SEARCH_WARPS * 32, FILTER ? (BOX <= 11 ? 4 : 3) : 2)
     search_kernel(const __grid_constant__ CUtensorMap tmap, const Sl2Dev d, const SearchLaunch L,
                   const DumpPtrs dump) {
@@ -185,8 +186,8 @@ __global__ void __launch_bounds__(SL2_SEARCH_WARPS * 32, FILTER ? (BOX <= 11 ? 4
   // ---- template into registers, rows zero-padded to 16 bytes in HBM --------------------------
   uint32_t T[BOX][NW];
   {
-    const uint32_t *pp =
-        reinterpret_cast<const uint32_t *>(d.patches + ((size_t)s * d.Nmax + feat) * (BOX * 16));
+    const uint32_t *pp = reinterpret_cast<const uint32_t *>(
+        JOBS ? L.job_patches + (size_t)job * (BOX * 16) : d.patches + ((size_t)s * d.Nmax + feat) * (BOX * 16));
 #pragma unroll
     for (int rr = 0; rr < BOX; ++rr)
 #pragma unroll
@@ -522,8 +523,12 @@ cudaError_t launch(const Sl2Dev &d, const CUtensorMap &tmap, const SearchLaunch 
     const int groups = (L.jobs_per_stream + SL2_SEARCH_WARPS - 1) / SL2_SEARCH_WARPS;
     const int grid = groups * L.stream_cnt;
     if (grid <= 0) return cudaSuccess;
-    return sl2_launch_kernel(search_kernel<decltype(box)::value, FILTER>, dim3(grid), dim3(SL2_SEARCH_WARPS * 32),
-                             search_smem_bytes(d), q, sl2_use_pdl(L.stream_cnt), tmap, d, L, dump);
+    constexpr int BOX = decltype(box)::value;
+    auto kern = search_kernel<BOX, FILTER>;
+    if constexpr (FILTER)  // the dump path never takes job templates
+      if (L.job_patches) kern = search_kernel<BOX, true, true>;
+    return sl2_launch_kernel(kern, dim3(grid), dim3(SL2_SEARCH_WARPS * 32), search_smem_bytes(d), q,
+                             sl2_use_pdl(L.stream_cnt), tmap, d, L, dump);
   });
 }
 
@@ -535,6 +540,8 @@ cudaError_t sl2_configure_search(const Sl2Dev &d) {
   return sl2_with_box(d.box, [&](auto box) {
     constexpr int BOX = decltype(box)::value;
     cudaError_t e = cudaFuncSetAttribute(search_kernel<BOX, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(search_kernel<BOX, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e == cudaSuccess)
       e = cudaFuncSetAttribute(search_kernel<BOX, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     return e;

@@ -222,7 +222,7 @@ inline bool sl2_box_supported(int box) {
   return sl2_with_box(box, [](auto) { return cudaSuccess; }) == cudaSuccess;
 }
 
-// launchers that files other than their own call (defined in search.cu / ekf.cu / consensus.cu / update.cu /
+// launchers that files other than their own call (defined in search.cu / ekf.cu / consensus.cu / warp.cu / update.cu /
 // records.cu / particles.cu)
 struct SearchLaunch {
   // job arrays may be the context's own (fused step) or temporaries (staged API)
@@ -236,9 +236,23 @@ struct SearchLaunch {
   uint8_t *out_found;        // by job
   double *out_best;          // by job
   int scatter_to_features;   // 1: also write d.z_uv/found/best indexed by feature
+  const uint8_t *job_patches;  // [jobs][box][16] the template of job r (warp.cu), or nullptr: d.patches[feat]
 };
 
 cudaError_t sl2_launch_search(const Sl2Dev &d, const CUtensorMap &tmap, const SearchLaunch &L, Sl2Queue q);
+// The planar patch warp (warp.cu): the template of every job of the streams [stream_lo, stream_lo + stream_cnt) at
+// the pose xp, into out[job] in the row-padded layout of Sl2Dev::patches.  A stream whose on[s] is 0 gets its stored
+// templates copied.
+struct WarpLaunch {
+  const int *job_feat;    // [stream_cnt * jobs_per_stream], -1 = no job
+  int jobs_per_stream;    // stride between streams in job_feat and out
+  int stream_lo, stream_cnt;
+  const double *xp;       // the pose (7) of a one-stream launch, or nullptr: each stream's own x[0:7]
+  const uint8_t *on;      // [B] the streams' warp settings, or nullptr: every stream warps
+  uint8_t *out;           // [jobs][box][16]
+  uint8_t *valid;         // [jobs] 1 = warped, 0 = the stored template (or no job); may be nullptr
+};
+cudaError_t sl2_launch_warp(const Sl2Dev &d, const WarpLaunch &L, Sl2Queue q);
 cudaError_t sl2_launch_predict(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *u3_dev,
                                int do_predict, int do_measure, Sl2Queue q);
 // match consensus of the streams [stream_lo, stream_lo + stream_cnt) between the search and the update; tau2_dev[s] =

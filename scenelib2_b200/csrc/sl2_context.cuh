@@ -103,6 +103,13 @@ struct sl2_ctx {
   // device array of the squared radii the consensus kernel reads
   std::vector<double> cons_tau;  // [B]
   double *cons_tau2 = nullptr;   // [B] device
+  // planar patch warp (sl2_set_stream_warp): the host mirror of every stream's setting, the device array warp_kernel
+  // reads, and the job-indexed templates [B][Nmax][box][16] the search then reads (sized when a stream first turns it
+  // on)
+  std::vector<uint8_t> warp_on;  // [B]
+  uint8_t *warp_on_dev = nullptr;  // [B] device
+  sl2::DevPtr<uint8_t> warp_patches;
+  size_t warp_patches_bytes = 0;
 };
 
 namespace sl2 {

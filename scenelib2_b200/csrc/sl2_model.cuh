@@ -1,5 +1,5 @@
 // sl2_model.cuh — the device camera and feature models of predict_kernel and particle_predict_kernel (ekf.cu),
-// consensus_kernel (consensus.cu) and reloc_kernel (reloc.cu).  Everything that decides which pixels are searched
+// consensus_kernel (consensus.cu), reloc_kernel (reloc.cu) and warp_kernel (warp.cu).  Everything that decides which pixels are searched
 // (S_i, S^-1, h_i) or which match is an inlier uses never-fused rd ops in the oracle's evaluation order.
 #pragma once
 #include "sl2_common.cuh"
@@ -132,6 +132,74 @@ __device__ __forceinline__ void unproject_point(const double *cam, const rd h[2]
   out[0] = (c0 / factor) / (-fku);
   out[1] = (c1 / factor) / (-fkv);
   out[2] = one;
+}
+
+// ---- the planar patch warp (include/sl2b200.h, sl2_set_stream_warp; warp_kernel in warp.cu) ------------------------
+// a . b, summed from 0.0 in ascending order like mat3_vec
+__device__ __forceinline__ rd dot3(const rd a[3], const rd b[3]) {
+  rd s(0.0);
+  for (int k = 0; k < 3; ++k) s = s + a[k] * b[k];
+  return s;
+}
+
+// What one feature's warp at the camera pose xp shares over its pixels: the feature y seen from xp (h, bit for bit the
+// prediction's) and from xo = xp_org (ho, the template centre), the plane through y with normal nW = xo[0:3] - y and
+// num = nW . (y - r)
+struct PatchWarp {
+  rd RRW[3][3], RRWo[3][3];  // pose_RRW(xp), pose_RRW(xo)
+  rd nW[3], num;
+  rd h[2], ho[2];
+};
+__device__ __forceinline__ void patch_warp_setup(const double *cam, const double *xp, const double *xo, const rd y[3],
+                                                 PatchWarp &w) {
+  rd d[3], z[3], uc, vc;
+  pose_RRW(xp, w.RRW);
+  zeroed_point(w.RRW, y, xp, d, z);
+  project_point(cam, z, w.h, uc, vc);
+  rd dox[3], zo[3];
+  pose_RRW(xo, w.RRWo);
+  zeroed_point(w.RRWo, y, xo, dox, zo);
+  project_point(cam, zo, w.ho, uc, vc);
+  for (int i = 0; i < 3; ++i) w.nW[i] = rd(xo[i]) - y[i];
+  w.num = dot3(w.nW, d);
+}
+
+// The source position in the stored template of the output pixel at offset (db, da) (column, row) from the centre:
+// p = h + (db, da); dW = RRW^T unproject_point(p); t = num / (nW . dW); X = r + t dW; zo = RRWo (X - xo[0:3]);
+// src = project_point(zo) - ho + (half, half).  True when the pixel is valid: t finite and > 0, zo[2] > 0, src finite.
+__device__ __forceinline__ bool patch_warp_source(const double *cam, const PatchWarp &w, const double *xp,
+                                                  const double *xo, int db, int da, int half, rd src[2]) {
+  const rd p[2] = {w.h[0] + rd((double)db), w.h[1] + rd((double)da)};
+  rd c[3], dW[3];
+  unproject_point(cam, p, c);
+  for (int i = 0; i < 3; ++i) {
+    rd s(0.0);
+    for (int k = 0; k < 3; ++k) s = s + w.RRW[k][i] * c[k];
+    dW[i] = s;
+  }
+  const rd t = w.num / dot3(w.nW, dW);
+  rd e[3], zo[3];
+  for (int i = 0; i < 3; ++i) e[i] = (rd(xp[i]) + t * dW[i]) - rd(xo[i]);
+  mat3_vec(w.RRWo, e, zo);
+  rd g[2], uc, vc;
+  project_point(cam, zo, g, uc, vc);
+  src[0] = (g[0] - w.ho[0]) + rd((double)half);
+  src[1] = (g[1] - w.ho[1]) + rd((double)half);
+  return isfinite(t.v) && t.v > 0.0 && zo[2].v > 0.0 && isfinite(src[0].v) && isfinite(src[1].v);
+}
+
+// Bilinear sample of the box x box template T (row stride ld) at the finite position src (column, row): each
+// coordinate clamped to [0, box - 1], so positions outside the template repeat its edge pixels; returns (int)(v + 0.5)
+__device__ __forceinline__ int patch_sample(const uint8_t *T, int ld, int box, const rd src[2]) {
+  const double lim = (double)(box - 1);
+  const double sx = fmin(fmax(src[0].v, 0.0), lim), sy = fmin(fmax(src[1].v, 0.0), lim);
+  const int x0 = min((int)floor(sx), box - 2), y0 = min((int)floor(sy), box - 2);
+  const rd fx = rd(sx) - rd((double)x0), fy = rd(sy) - rd((double)y0), one(1.0);
+  const uint8_t *r0 = T + y0 * ld + x0, *r1 = r0 + ld;
+  const rd top = (one - fx) * rd((double)r0[0]) + fx * rd((double)r0[1]);
+  const rd bot = (one - fx) * rd((double)r1[0]) + fx * rd((double)r1[1]);
+  const rd v = (one - fy) * top + fy * bot;
+  return (int)(v + rd(0.5)).v;
 }
 
 // Camera::Project (camera.cpp:90-114) of the camera-frame point z, and J = dh/dz

@@ -60,6 +60,7 @@ SOURCE_BPP = {SL2_SRC_GRAY8: 1, SL2_SRC_RGB24: 3, SL2_SRC_UYVY: 2}
 EXPORTS = [
     "sl2_default_config", "sl2_create", "sl2_destroy", "sl2_last_error", "sl2_sync", "sl2_version",
     "sl2_set_stream_config", "sl2_get_stream_config", "sl2_set_stream_consensus", "sl2_get_stream_consensus",
+    "sl2_set_stream_warp", "sl2_get_stream_warp", "sl2_warp_templates",
     "sl2_set_frame", "sl2_set_frames", "sl2_set_frames_dev",
     "sl2_set_stream_source", "sl2_get_stream_source", "sl2_frame_set_layout", "sl2_set_features",
     "sl2_num_features", "sl2_state_size", "sl2_set_state", "sl2_get_state", "sl2_delete_feature", "sl2_append_feature",
@@ -217,6 +218,10 @@ def load():
         L.sl2_get_stream_config.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamConfig)]
         L.sl2_set_stream_consensus.argtypes = [C.c_void_p, C.c_int32, C.c_double]
         L.sl2_get_stream_consensus.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_double)]
+        L.sl2_set_stream_warp.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
+        L.sl2_get_stream_warp.argtypes = [C.c_void_p, C.c_int32, i32p]
+        L.sl2_warp_templates.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p]
         L.sl2_set_frame.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_size_t]
         L.sl2_set_frames.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
         L.sl2_set_frames_dev.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
@@ -329,6 +334,31 @@ class Context:
         v = C.c_double()
         self._ck(self.L.sl2_get_stream_consensus(self.h, stream_id, C.byref(v)))
         return v.value
+
+    # ---- planar patch warp ----------------------------------------------------------------------
+    def set_stream_warp(self, stream_id, on):
+        """sl2_set_stream_warp: search the stream's selected features with their templates warped to the predicted
+        viewpoint (1) or with the stored templates (0, the default)."""
+        self._ck(self.L.sl2_set_stream_warp(self.h, stream_id, int(on)))
+
+    def get_stream_warp(self, stream_id):
+        v = C.c_int32()
+        self._ck(self.L.sl2_get_stream_warp(self.h, stream_id, C.byref(v)))
+        return v.value
+
+    def warp_templates(self, stream_id, feat_index, xp):
+        """sl2_warp_templates: the templates of the features feat_index warped to the camera pose xp (7: r, q), as the
+        search of a warp-on stream sees them -> (templates (n, B, B) u8, valid (n,) u8; 0 = the stored template)."""
+        feat_index = np.ascontiguousarray(feat_index, np.int32).reshape(-1)
+        xp = np.ascontiguousarray(xp, np.float64).reshape(-1)
+        if xp.size != 7:
+            raise ValueError("xp must hold 7 values (r, q)")
+        n, B = feat_index.size, self.cfg.boxsize
+        out = np.zeros((n, B, B), np.uint8)
+        valid = np.zeros(n, np.uint8)
+        self._ck(self.L.sl2_warp_templates(self.h, stream_id, n, feat_index.ctypes.data, xp.ctypes.data,
+                                           out.ctypes.data, valid.ctypes.data))
+        return out, valid
 
     # ---- frames -------------------------------------------------------------------------------
     def set_stream_source(self, stream_id, format, width=0, height=0):
