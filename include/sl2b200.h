@@ -161,6 +161,56 @@ int sl2_get_stream_warp(sl2_ctx *ctx, int32_t stream_id, int32_t *on);
 int sl2_warp_templates(sl2_ctx *ctx, int32_t stream_id, int32_t n, const int32_t *feat_index, const double *xp,
                        uint8_t *out, uint8_t *valid);
 
+/* ---- feature selection: measure the features that carry the most information (no reference counterpart) --------
+ * The reference measures the n_select visible features of largest trace(S_i) (auto_select_n_features,
+ * monoslam.cpp:187-254).  Once the map has settled, most of every feature's innovation uncertainty is the camera
+ * pose's, which they all share, so the top-trace features are largely redundant; and trace ignores that R_i grows
+ * towards the image border.  A stream with SL2_SELECT_INFORMATION picks greedily by mutual information (Davison,
+ * "Active Search for Real-Time Vision", ICCV 2005): each pick is the feature whose measurement, conditioned on the
+ * features already picked, tells most about the state, and the picks stop when the next would add min_bits or less.
+ *   Candidates: the features the trace rule would select if n_select were unlimited (visible, ranked before the first
+ *   zero trace); rho_j is candidate j's trace rank, used only to break ties.  Per candidate, from the prediction:
+ *   C_j = [[S00, S10], [S10, S11]] of the stored S_j, A_j = dh_dxp (2x7), B_j = dh_dy (2x3), R_j = Rvar_j; and
+ *   t = exp2(2 min_bits), computed once on the host when the setting is made.
+ *   Pick r = 0, 1, ... while r < n_select: over the unpicked candidates, q_j = (C00 C11 - C10 C10) / (R_j R_j)
+ *   (the conditional information of measuring j is (1/2) log2 q_j bits).  The pick i has the largest q_j among those
+ *   with C00 > 0 and q_j > t, ties going to the smallest rho; a NaN q never wins; if none qualifies the picks stop.
+ *   Pick i is written exactly as the trace rule writes a selected feature: sel_rank[i] = r, and job slot r = (i, the
+ *   centre h_i, the ellipse of the prior S_i or the search override): the search looks where the prediction says.
+ *   Then L_i = chol(C_i): l00 = sqrt(C00), l10 = C10 / l00, l11 = sqrt(C11 - l10 l10);
+ *   u = P H_i^T on rows 0..6 and every unpicked candidate's y rows: u[row][c] = ((0 + P[row][0] A_i[c][0]) + ... +
+ *   P[row][6] A_i[c][6]) + P[row][y_i] B_i[c][0] + P[row][y_i+1] B_i[c][1] + P[row][y_i+2] B_i[c][2];
+ *   for every unpicked j: c_j[a][b] = ((0 + A_j[a][0] u[0][b]) + ... + A_j[a][6] u[6][b]) + B_j[a][0] u[y_j][b] + ...
+ *   + B_j[a][2] u[y_j+2][b], then for p = 0 .. r-1, e = 0, 1: c_j[a][b] -= g_{j,p}[a][e] g_{i,p}[b][e];
+ *   g_{j,r} = c_j L_i^-T: g[a][0] = c_j[a][0] / l00, g[a][1] = (c_j[a][1] - g[a][0] l10) / l11;
+ *   C00 = C00 - g00 g00 - g01 g01, C10 = C10 - g10 g00 - g11 g01, C11 = C11 - g10 g10 - g11 g11 (left to right).
+ *   This is a block-pivoted Cholesky factorisation of the candidates' joint innovation covariance H P H^T + R whose
+ *   pivot is the largest det(C_j) / R_j^2.  nsel = the number of picks; nvisible is the trace rule's; nmeas = 0.
+ * Every operation is a correctly rounded FP64 operation (never fused) in the order written above and in the kernel
+ * (csrc/select.cu, select_kernel), so decisions are reproducible bit for bit.
+ * Where it applies: the fused step (sl2_step, sl2_step_host, sl2_step_host_async) and sl2_predict_measurements.  The
+ * search, the consensus (whose ties go to the lowest selection rank, now the information order), the warp, the
+ * update, the cull, the records and relocalisation read the job slots as with the trace rule.  A stream can end a
+ * prediction with nothing selected.
+ * mode SL2_SELECT_TRACE (the default) is the reference's rule: a context where no stream selects by information runs
+ * exactly the path without it; one where some stream does adds one kernel launch per step group holding such a
+ * stream and per sl2_predict_measurements of one (timed with the predict in sl2_last_step_times).  Ordering like
+ * sl2_set_stream_config.  The setting belongs to the stream slot, like the match consensus: snapshots do not carry it
+ * and a load leaves it.  When a stream first turns the information rule on and the factors of
+ * kmax = min(max_features, SL2_MAX_MEASURED) picks cannot stay in shared memory, the context sizes its factor scratch
+ * (num_streams x max_features x kmax x 32 bytes): SL2_ERR_CUDA, with the setting unchanged, when that allocation
+ * fails.  SL2_ERR_ARG, with the setting unchanged, for: a bad stream_id or NULL sel; an unknown mode; reserved != 0;
+ * a min_bits that is negative or not finite, or non-zero with SL2_SELECT_TRACE. */
+#define SL2_SELECT_TRACE 0       /* the reference's rule: top n_select by trace(S_i) (default) */
+#define SL2_SELECT_INFORMATION 1 /* greedy mutual information, above */
+typedef struct sl2_stream_selection {
+  int32_t mode;     /* SL2_SELECT_* */
+  int32_t reserved; /* 0 */
+  double min_bits;  /* INFORMATION: a pick must add more than min_bits bits; >= 0, finite.  TRACE: must be 0 */
+} sl2_stream_selection;
+int sl2_set_stream_selection(sl2_ctx *ctx, int32_t stream_id, const sl2_stream_selection *sel);
+int sl2_get_stream_selection(sl2_ctx *ctx, int32_t stream_id, sl2_stream_selection *sel);
+
 /* ---- frames (replaces the cv::Mat `frame` argument of MonoSLAM::GoOneStep, monoslam.cpp:108) */
 /* The frame ring keeps the context's width x height per stream.  A stream whose image is smaller
  * (sl2_set_stream_config) occupies the top-left width_s x height_s of its block; the rest of the block

@@ -336,6 +336,11 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   c->cons_tau.assign(B, 0.0);
   ALLOC(c->warp_on_dev, B);
   c->warp_on.assign(B, 0);
+  ALLOC(c->sel_mode_dev, B);
+  ALLOC(c->sel_t_dev, B);
+  c->sel.assign(B, sl2_stream_selection{});
+  c->sel_mode.assign(B, SL2_SELECT_TRACE);
+  c->sel_t.assign(B, 1.0);
 #undef ALLOC
   int rc = make_tensor_map(c);
   if (rc) return failed(rc, c->err);
@@ -493,7 +498,12 @@ static int step_group(sl2_ctx *c, int32_t slot, int lo, int cnt, Sl2Queue q, cud
   const Sl2Dev &d = c->d;
   const cudaStream_t st = q.stream;
   if (t) CU_TRY(c, cudaEventRecord(c->ev[0].get(), st));
-  CU_TRY(c, sl2_launch_predict(d, lo, cnt, nullptr, 1, 1, q));
+  const bool info = selection_on(c, lo, cnt);
+  CU_TRY(c, sl2_launch_predict(d, lo, cnt, nullptr, 1, 1, info ? c->sel_mode_dev : nullptr, q));
+  if (info) {  // part of the predict's time
+    const int rc = select_streams(c, lo, cnt, q);
+    if (rc) return rc;
+  }
   if (t) CU_TRY(c, cudaEventRecord(c->ev[1].get(), st));
   // the consensus is part of the search's time: the update times still sum to ev[2] .. ev[3]
   const int rc = measure_streams(c, slot, lo, cnt, q);

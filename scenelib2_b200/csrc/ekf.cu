@@ -179,9 +179,12 @@ __device__ int visibility_test(const double *cam, const double *xp, const rd yi[
 // ---------------------------------------------------------------------------------------------
 // kernel 1: predict (kalman.cpp:50-69) + measurement prediction / selection (monoslam.cpp:187-254)
 // ---------------------------------------------------------------------------------------------
+// sel_mode: [B] every stream's SL2_SELECT_* (sl2_set_stream_selection), or nullptr: every stream selects by trace.  An
+// SL2_SELECT_INFORMATION stream keeps the provisional rank of every candidate (visible, ranked before the first zero
+// trace) in sel_rank and leaves the truncation, the job slots and nsel to select_kernel (select.cu).
 __global__ void __launch_bounds__(128) predict_kernel(const Sl2Dev d, int stream_lo,
                                                       const double *u3, int do_predict,
-                                                      int do_measure) {
+                                                      int do_measure, const int *sel_mode) {
   pdl_prologue();
   const int s = stream_lo + blockIdx.x;
   const int tid = threadIdx.x;
@@ -305,12 +308,14 @@ __global__ void __launch_bounds__(128) predict_kernel(const Sl2Dev d, int stream
     }
   }
   __syncthreads();
-  const int nsel = min(min(sc.n_select, s_r0), s_nvis);
+  const bool info = sel_mode && sel_mode[s] == SL2_SELECT_INFORMATION;
+  // information: the candidates are every rank before the first zero score
+  const int nsel = info ? min(s_r0, s_nvis) : min(min(sc.n_select, s_r0), s_nvis);
   for (int i = tid; i < nf; i += blockDim.x) {
     int rank = d.sel_rank[fb + i];
     if (rank >= nsel) rank = -1;
     d.sel_rank[fb + i] = rank;
-    if (rank >= 0) {
+    if (rank >= 0 && !info) {
       d.job_feat[fb + rank] = i;
       d.job_centre[(fb + rank) * 2 + 0] = d.h[(fb + i) * 2 + 0];
       d.job_centre[(fb + rank) * 2 + 1] = d.h[(fb + i) * 2 + 1];
@@ -321,7 +326,7 @@ __global__ void __launch_bounds__(128) predict_kernel(const Sl2Dev d, int stream
     }
   }
   if (tid == 0) {
-    d.nsel[s] = nsel;
+    d.nsel[s] = info ? 0 : nsel;  // select_kernel writes the information count
     d.nvisible[s] = s_nvis;
     d.nmeas[s] = 0;
   }
@@ -558,12 +563,12 @@ cudaError_t sl2_launch_append(const Sl2Dev &d, int s, const double *y3_dev, cons
 }  // namespace
 
 cudaError_t sl2_launch_predict(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *u3_dev,
-                               int do_predict, int do_measure, Sl2Queue q) {
+                               int do_predict, int do_measure, const int *sel_mode_dev, Sl2Queue q) {
   if (stream_cnt <= 0) return cudaSuccess;
   // 128 threads, one feature each per pass over the map (two passes at SL2_MAX_FEATURES); the kernel needs ~255
   // registers per thread, so 128-thread CTAs are what lets two streams share an SM
   return sl2_launch_kernel(predict_kernel, dim3(stream_cnt), dim3(128), 0, q, sl2_use_pdl(stream_cnt), d,
-                           stream_lo, u3_dev, do_predict, do_measure);
+                           stream_lo, u3_dev, do_predict, do_measure, sel_mode_dev);
 }
 
 // F features, Kmax = stride between features in every per-particle array, K_dev[f] particles used
@@ -588,14 +593,19 @@ int sl2_ekf_predict(sl2_ctx *c, int32_t s, const double *u3) {
   if (bad_stream(c, s)) return fail(c, SL2_ERR_ARG, "bad stream");
   Stage u{STAGE_IN, u3 ? (size_t)24 : 0, u3};
   return staged_call(c, {&u}, [] {}, [&] {
-    CU_TRY(c, sl2_launch_predict(c->d, s, 1, u3 ? u.dev<double>() : nullptr, 1, 0, queue(c)));
+    CU_TRY(c, sl2_launch_predict(c->d, s, 1, u3 ? u.dev<double>() : nullptr, 1, 0, nullptr, queue(c)));
     return SL2_OK;
   });
 }
 
 int sl2_predict_measurements(sl2_ctx *c, int32_t s) {
   if (bad_stream(c, s)) return fail(c, SL2_ERR_ARG, "bad stream");
-  CU_TRY(c, sl2_launch_predict(c->d, s, 1, nullptr, 0, 1, queue(c)));
+  const bool info = c->sel[s].mode == SL2_SELECT_INFORMATION;
+  CU_TRY(c, sl2_launch_predict(c->d, s, 1, nullptr, 0, 1, info ? c->sel_mode_dev : nullptr, queue(c)));
+  if (info) {
+    const int rc = select_streams(c, s, 1, queue(c));
+    if (rc) return rc;
+  }
   int nv = 0;
   CU_TRY(c, cudaMemcpyAsync(&nv, c->d.nvisible + s, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   CU_TRY(c, cudaStreamSynchronize(c->stream));

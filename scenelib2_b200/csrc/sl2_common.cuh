@@ -222,8 +222,8 @@ inline bool sl2_box_supported(int box) {
   return sl2_with_box(box, [](auto) { return cudaSuccess; }) == cudaSuccess;
 }
 
-// launchers that files other than their own call (defined in search.cu / ekf.cu / consensus.cu / warp.cu / update.cu /
-// records.cu / particles.cu)
+// launchers that files other than their own call (defined in search.cu / ekf.cu / select.cu / consensus.cu / warp.cu /
+// update.cu / records.cu / particles.cu)
 struct SearchLaunch {
   // job arrays may be the context's own (fused step) or temporaries (staged API)
   const int *job_feat;       // [njobs_per_stream * B] or [n]
@@ -253,8 +253,19 @@ struct WarpLaunch {
   uint8_t *valid;         // [jobs] 1 = warped, 0 = the stored template (or no job); may be nullptr
 };
 cudaError_t sl2_launch_warp(const Sl2Dev &d, const WarpLaunch &L, Sl2Queue q);
+// sel_mode_dev: [B] the streams' SL2_SELECT_* settings, or nullptr: every stream selects by trace (ekf.cu)
 cudaError_t sl2_launch_predict(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *u3_dev,
-                               int do_predict, int do_measure, Sl2Queue q);
+                               int do_predict, int do_measure, const int *sel_mode_dev, Sl2Queue q);
+// The mutual-information selection (select.cu) of the streams [stream_lo, stream_lo + stream_cnt) whose mode[s] is
+// SL2_SELECT_INFORMATION, right after their predict_kernel: picks into sel_rank, the job slots and nsel
+struct SelectLaunch {
+  int stream_lo, stream_cnt;
+  const int *mode;  // [B] SL2_SELECT_*
+  const double *t;  // [B] exp2(2 min_bits)
+  double *g;        // [B][gstride][Nmax][4] the factors, or nullptr: shared memory
+  int gstride;      // picks per candidate in g: kmax in the scratch, else the most any stream of the launch makes
+};
+cudaError_t sl2_launch_select(const Sl2Dev &d, const SelectLaunch &L, Sl2Queue q);
 // match consensus of the streams [stream_lo, stream_lo + stream_cnt) between the search and the update; tau2_dev[s] =
 // the squared inlier radius of stream s, 0 = off (consensus.cu)
 cudaError_t sl2_launch_consensus(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *tau2_dev, Sl2Queue q);

@@ -110,6 +110,16 @@ struct sl2_ctx {
   uint8_t *warp_on_dev = nullptr;  // [B] device
   sl2::DevPtr<uint8_t> warp_patches;
   size_t warp_patches_bytes = 0;
+  // feature selection (sl2_set_stream_selection): the host mirror of every stream's setting, the device arrays
+  // predict_kernel and select_kernel read, and the factor scratch [B][kmax][Nmax][4] (sized when a stream first turns
+  // the information rule on, and only when the factors cannot stay in shared memory)
+  std::vector<sl2_stream_selection> sel;  // [B]
+  std::vector<int> sel_mode;              // [B] the sources of the device arrays' copies
+  std::vector<double> sel_t;              // [B]
+  int *sel_mode_dev = nullptr;            // [B] device: SL2_SELECT_*
+  double *sel_t_dev = nullptr;            // [B] device: exp2(2 min_bits)
+  sl2::DevPtr<double> sel_g;
+  size_t sel_g_bytes = 0;
 };
 
 namespace sl2 {
@@ -229,5 +239,9 @@ int check_stream_config(sl2_ctx *c, const sl2_stream_config *sc, const std::stri
 int install_sources(sl2_ctx *c, const std::vector<sl2_stream_source> &srcs);
 int loaded_cameras(sl2_ctx *c, int lo, const std::vector<sl2_stream_config> &cams);
 cudaError_t copy_slot_frames(sl2_ctx *c, int slot, const uint8_t *src, cudaMemcpyKind kind, Sl2Queue q);
+// select.cu: whether some stream of [lo, lo + cnt) selects by information; the selection of those streams on q, right
+// after their prediction
+bool selection_on(const sl2_ctx *c, int lo, int cnt);
+int select_streams(sl2_ctx *c, int lo, int cnt, Sl2Queue q);
 
 }  // namespace sl2

@@ -51,6 +51,13 @@ class Sl2StreamSource(C.Structure):
     _fields_ = [("format", C.c_int32), ("width", C.c_int32), ("height", C.c_int32), ("reserved", C.c_int32)]
 
 
+class Sl2StreamSelection(C.Structure):
+    """sl2_stream_selection: how a camera stream chooses the features it measures (SL2_SELECT_*)."""
+    _fields_ = [("mode", C.c_int32), ("reserved", C.c_int32), ("min_bits", C.c_double)]
+
+
+SL2_SELECT_TRACE, SL2_SELECT_INFORMATION = 0, 1
+
 SL2_SRC_GRAY_RING, SL2_SRC_GRAY8, SL2_SRC_RGB24, SL2_SRC_UYVY = 0, 1, 2, 3
 SL2_MAX_SOURCE_DIM = 4096
 SOURCE_BPP = {SL2_SRC_GRAY8: 1, SL2_SRC_RGB24: 3, SL2_SRC_UYVY: 2}
@@ -61,6 +68,7 @@ EXPORTS = [
     "sl2_default_config", "sl2_create", "sl2_destroy", "sl2_last_error", "sl2_sync", "sl2_version",
     "sl2_set_stream_config", "sl2_get_stream_config", "sl2_set_stream_consensus", "sl2_get_stream_consensus",
     "sl2_set_stream_warp", "sl2_get_stream_warp", "sl2_warp_templates",
+    "sl2_set_stream_selection", "sl2_get_stream_selection",
     "sl2_set_frame", "sl2_set_frames", "sl2_set_frames_dev",
     "sl2_set_stream_source", "sl2_get_stream_source", "sl2_frame_set_layout", "sl2_set_features",
     "sl2_num_features", "sl2_state_size", "sl2_set_state", "sl2_get_state", "sl2_delete_feature", "sl2_append_feature",
@@ -220,6 +228,8 @@ def load():
         L.sl2_get_stream_consensus.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_double)]
         L.sl2_set_stream_warp.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
         L.sl2_get_stream_warp.argtypes = [C.c_void_p, C.c_int32, i32p]
+        L.sl2_set_stream_selection.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamSelection)]
+        L.sl2_get_stream_selection.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamSelection)]
         L.sl2_warp_templates.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_void_p]
         L.sl2_set_frame.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_size_t]
@@ -334,6 +344,19 @@ class Context:
         v = C.c_double()
         self._ck(self.L.sl2_get_stream_consensus(self.h, stream_id, C.byref(v)))
         return v.value
+
+    # ---- feature selection ----------------------------------------------------------------------
+    def set_stream_selection(self, stream_id, mode, min_bits=0.0, reserved=0):
+        """sl2_set_stream_selection: choose the stream's measured features by trace (SL2_SELECT_TRACE, the default)
+        or greedily by mutual information (SL2_SELECT_INFORMATION), each pick adding more than min_bits bits."""
+        sel = Sl2StreamSelection(int(mode), int(reserved), float(min_bits))
+        self._ck(self.L.sl2_set_stream_selection(self.h, stream_id, C.byref(sel)))
+
+    def get_stream_selection(self, stream_id):
+        """-> (mode, min_bits)"""
+        sel = Sl2StreamSelection()
+        self._ck(self.L.sl2_get_stream_selection(self.h, stream_id, C.byref(sel)))
+        return sel.mode, sel.min_bits
 
     # ---- planar patch warp ----------------------------------------------------------------------
     def set_stream_warp(self, stream_id, on):
