@@ -94,7 +94,7 @@ int sl2_get_stream_config(sl2_ctx *ctx, int32_t stream_id, sl2_stream_config *sc
 /* ---- match consensus: keep wrong matches out of the EKF update (no reference counterpart) ----------------------
  * The reference trusts every match its patch search accepts.  A stream with an inlier radius tau > 0 px runs a
  * one-point RANSAC over the step's matches between the search and the update (Civera, Grasa, Davison, Montiel,
- * "1-Point RANSAC for EKF Filtering", J. Field Robotics 2010), without its rescue stage:
+ * "1-Point RANSAC for EKF Filtering", J. Field Robotics 2010); its rescue stage is sl2_set_stream_rescue, below:
  *   M = the selected features whose match succeeded, in selection-rank order; k = |M|.
  *   Every i in M is a hypothesis (exhaustive, no random sampling: a stream's result never depends on its batch
  *   position, the step groups or the launch path).  Hypothesis i is the state-only partial update from i alone:
@@ -117,6 +117,41 @@ int sl2_get_stream_config(sl2_ctx *ctx, int32_t stream_id, sl2_stream_config *sc
  * or infinite inlier_px, or (get) a NULL inlier_px. */
 int sl2_set_stream_consensus(sl2_ctx *ctx, int32_t stream_id, double inlier_px);
 int sl2_get_stream_consensus(sl2_ctx *ctx, int32_t stream_id, double *inlier_px);
+
+/* ---- consensus rescue: take back the rejected matches the updated state agrees with (no reference counterpart) ---
+ * The consensus judges every match against hypotheses built from one match each.  A feature whose own position is
+ * still uncertain (a depth ray converted by sl2_append_feature, sigma of a few cm) is predicted several pixels from
+ * its correct match by every other feature's hypothesis, so its match is rejected, its position never improves, and
+ * the cull deletes it.  A stream with the consensus on and chi2 > 0 runs the high-innovation stage of the 1-point
+ * RANSAC (Civera et al. 2010) after the update with the consensus's inliers:
+ *   1. update 1: the update with the inliers, exactly as without the rescue (normalisation and symmetrisation
+ *      included), giving x', P'.
+ *   2. for every selected feature whose match the consensus rejected (found = 2), in selection-rank order: the
+ *      prediction at x', P' (predict_kernel's code, bit for bit what a prediction of that state gives): h', dh/dxp',
+ *      dh/dy', R' and S' = H' P' H'^T + R'; nu' = z - h'; (Si00, Si01, Si11) = the S'^-1 the search forms;
+ *      w0 = Si00 nu0 + Si01 nu1, w1 = Si01 nu0 + Si11 nu1, q = nu0 w0 + nu1 w1.  The match is rescued when the
+ *      feature lies in front of the camera at x' and q <= fl(chi2); a NaN q never is.  A rescued feature's h, S, R and
+ *      Jacobians become the re-prediction, and the getters (sl2_get_features, sl2_get_feature_jacobians) show them.
+ *   3. update 2: the update with the rescued rows only, in rank order, from x', P'.  Its finish normalises the
+ *      quaternion's covariance again, so on such a step the normalisation Jacobian is applied twice.
+ *   After the step a rescued match is successful (found = 1, sl2_get_features flags bit 1): every selected feature
+ *   counts as one attempt, a rescued one as one success, and the cull sees those counters.
+ * Every operation of step 2 is a correctly rounded FP64 operation in the order written in the kernel
+ * (csrc/rescue.cu, rescue_kernel), so decisions are reproducible bit for bit.  A step in which the consensus rejected
+ * nothing, and a step in which nothing is rescued, run no second update and leave the stream exactly as without the
+ * rescue.  A step record's m and nmeas count the rows of both updates, nis = NIS_1 + NIS_2 and logdet_s =
+ * log det S_1 + log det S_2, each from its own update (in the linear case the NIS and log det of one joint update).
+ * Where it applies: the fused step (sl2_step, sl2_step_host, sl2_step_host_async) and sl2_ekf_update_measured;
+ * sl2_ekf_update with the caller's rows never rescues.  A typical chi2 is 5.991, the 95 % point of chi^2 with two
+ * degrees of freedom.  chi2 = 0 (the default) is off: a context where no stream has the consensus and the rescue on
+ * runs exactly the path without it; one with such a stream adds six kernel launches per step group holding one
+ * (timed with the update in sl2_last_step_times; sl2_last_update_times keeps timing update 1).  Ordering like
+ * sl2_set_stream_config.  The setting belongs to the stream slot, like the match consensus: snapshots do not carry it
+ * and a load leaves it.  The first stream turned on sizes the context's rescue scratch (num_streams x 20 bytes):
+ * SL2_ERR_CUDA, with the setting unchanged, when that allocation fails.  SL2_ERR_ARG, with the setting unchanged, for
+ * a bad stream_id, a negative, NaN or infinite chi2, or (get) a NULL chi2. */
+int sl2_set_stream_rescue(sl2_ctx *ctx, int32_t stream_id, double chi2);
+int sl2_get_stream_rescue(sl2_ctx *ctx, int32_t stream_id, double *chi2);
 
 /* ---- planar patch warp: match each template at the predicted viewpoint (no reference counterpart) ---------------
  * The reference searches every feature with the template stored when it was first seen, while the visibility test
@@ -424,12 +459,14 @@ int sl2_get_feature_jacobians(sl2_ctx *ctx, int32_t stream_id, double *dh_by_dxv
                               double *dh_by_dy /* n x 6 */, double *R /* n x 4 */,
                               double *nu /* n x 2 */);
 /* device-time of the kernels of the last sl2_step (ms): [0] predict+select, [1] patch search,
- * [2] EKF update, [3] cull.  Valid after sl2_enable_timing(ctx, 1). */
+ * [2] EKF update (with the consensus rescue and its second update when a stream has them on), [3] cull.  Valid after
+ * sl2_enable_timing(ctx, 1). */
 int sl2_enable_timing(sl2_ctx *ctx, int32_t on);
 int sl2_last_step_times(sl2_ctx *ctx, float *ms4);
 /* the five kernels of the EKF update of the last sl2_step (ms): [0] hp (measurement list, H P, S = H P H^T + R),
  * [1] chol (Cholesky of S), [2] solve (Y = U^-T [H P | nu]), [3] syrk (P -= Y^T Y, x += Y^T w), [4] finish
- * (normalise, symmetrise, counters).  Their sum is sl2_last_step_times()[2]. */
+ * (normalise, symmetrise, counters).  Their sum is sl2_last_step_times()[2], less the consensus rescue's kernels on a
+ * step that ran them: these times are the first update's. */
 int sl2_last_update_times(sl2_ctx *ctx, float *ms5);
 /* kernels launched by this context since creation */
 int64_t sl2_launch_count(const sl2_ctx *ctx);

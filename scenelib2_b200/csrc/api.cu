@@ -334,6 +334,8 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   ALLOC(c->xv_stage, (size_t)d.slots * B * SL2_NXV);
   ALLOC(c->cons_tau2, B);
   c->cons_tau.assign(B, 0.0);
+  ALLOC(c->resc_chi2_dev, B);
+  c->resc_chi2.assign(B, 0.0);
   ALLOC(c->warp_on_dev, B);
   c->warp_on.assign(B, 0);
   ALLOC(c->sel_mode_dev, B);
@@ -513,11 +515,19 @@ static int step_group(sl2_ctx *c, int32_t slot, int lo, int cnt, Sl2Queue q, cud
   cudaEvent_t evu[6];
   for (int i = 0; i < 6; ++i) evu[i] = c->evu[i].get();
   CU_TRY(c, sl2_launch_update(d, lo, cnt, -1, nullptr, nullptr, nullptr, nullptr, nullptr, 0, q, t ? evu : nullptr));
+  // the rescue and its second update are part of the update's time (ev[2] .. ev[3]); the update times are the first's
+  const bool rescue = rescue_on(c, lo, cnt);
+  if (rescue) {
+    const int rc2 = rescue_streams(c, lo, cnt, q);
+    if (rc2) return rc2;
+  }
   if (t) CU_TRY(c, cudaEventRecord(c->ev[3].get(), st));
   CU_TRY(c, sl2_launch_cull(d, lo, cnt, -1, q));
   if (t) CU_TRY(c, cudaEventRecord(c->ev[4].get(), st));
-  if (d.rec_depth)  // after ev[4]: the step times keep their meaning
-    CU_TRY(c, sl2_launch_records(d, lo, cnt, c->rec_steps, q));
+  if (d.rec_depth) {  // after ev[4]: the step times keep their meaning
+    const Sl2Rescue r = rescue ? rescue_args(c) : Sl2Rescue{};
+    CU_TRY(c, sl2_launch_records(d, lo, cnt, c->rec_steps, rescue ? &r : nullptr, q));
+  }
   return SL2_OK;
 }
 

@@ -119,37 +119,6 @@ __device__ void motion_model(const double *xv, const double *u3, double dt_, dou
   }
 }
 
-struct FeatPred {
-  rd h[2];
-  rd dxp[2][7];
-  rd dy[2][3];
-  rd var;
-  rd S[2][2];
-};
-
-// Pxx: shared 13x13 col-major; Pcol: global pointer to P(0, pos) (column-major, ld)
-__device__ void predict_feature(const double *cam, const double *xv, const rd yi[3],
-                                const double *Pxx, const double *Pcol, int ld, int pos,
-                                FeatPred &o) {
-  rd z[3], dz_dxp[3][7], RRW[3][3], J[2][3];
-  zeroedyi(yi, xv, z, dz_dxp, RRW);
-  project(cam, z, o.h, J);
-  for (int i = 0; i < 2; ++i) {
-    for (int j = 0; j < 7; ++j) {
-      rd s(0.0);
-      for (int k = 0; k < 3; ++k) s = s + J[i][k] * dz_dxp[k][j];
-      o.dxp[i][j] = s;
-    }
-    for (int j = 0; j < 3; ++j) {
-      rd s(0.0);
-      for (int k = 0; k < 3; ++k) s = s + J[i][k] * RRW[k][j];
-      o.dy[i][j] = s;
-    }
-  }
-  o.var = measurement_noise(cam, o.h);
-  func_Si<3>(o.dxp, o.dy, o.var, Pxx, 13, Pcol, ld, Pcol + pos, ld, o.S);
-}
-
 __device__ int visibility_test(const double *cam, const double *xp, const rd yi[3],
                                const double *xp_orig, const rd h[2]) {
   int cant = 0;

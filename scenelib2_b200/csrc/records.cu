@@ -10,6 +10,8 @@
 //                 Sl2Dev::Wp for the solve, and nothing else writes Wp: its diagonal holds the reciprocal pivots
 //                 W_ii = 1 / U_ii the solve applied.  log det S = 2 sum log U_ii = -2 sum log W_ii.
 // When m == 0 the update wrote neither G nor Wp (they hold another update's values) and the kernel reads neither.
+// A step that ran the consensus rescue's second update (rescue.cu) overwrote G and Wp with its rows; rescue_kernel kept
+// the first update's NIS and log det S, and the record holds the sums of both updates' rows and terms.
 // Entry points: sl2_enable_records (the ring) and sl2_get_records* (the most recent records, oldest first).
 #include <algorithm>
 
@@ -23,30 +25,19 @@ constexpr int REC_THREADS = 256;  // one thread per row of S: m <= 2 * SL2_MAX_M
 static_assert(2 * SL2_MAX_MEASURED <= REC_THREADS, "one thread per measurement row");
 static_assert(sizeof(sl2_step_record) == 256, "sl2_step_record is 256 bytes without padding");
 
-__global__ void __launch_bounds__(REC_THREADS) record_kernel(const Sl2Dev d, int stream_lo, long long step) {
+static_assert(REC_THREADS == 256, "update_sums reduces over 256 slots");
+
+// With the consensus rescue's scratch (resc), a stream whose step ran a second update (m2[s] > 0) records the sums of
+// both: G and Wp hold the second update's rows, the scratch the first's NIS and log det S.
+__global__ void __launch_bounds__(REC_THREADS) record_kernel(const Sl2Dev d, int stream_lo, long long step,
+                                                             const int *resc_m2, const double *resc_nis1,
+                                                             const double *resc_logdet1) {
   pdl_prologue();
   const int s = stream_lo + blockIdx.x, tid = threadIdx.x;
   __shared__ double s_nis[REC_THREADS], s_ld[REC_THREADS];
   const int m = d.upd_m[s], nf = d.nfeat[s], nc = d.ncull[s];
-  double q = 0.0, l = 0.0;
-  if (tid < m) {
-    const int n = SL2_NXV + 3 * (nf + nc);
-    const double w = d.G[((size_t)s * d.mmax + tid) * d.ldg + m + n];
-    q = mul_(w, w);
-    l = -log(d.Wp[((size_t)s * SL2_MAX_PANELS + (tid >> 4)) * 256 + (tid & 15) * 17]);
-  }
-  s_nis[tid] = q;
-  s_ld[tid] = l;
-  __syncthreads();
-  // pairwise tree over all REC_THREADS slots: the same order for every stream, every m and every launch shape
-#pragma unroll
-  for (int h = REC_THREADS / 2; h > 0; h >>= 1) {
-    if (tid < h) {
-      s_nis[tid] = add_(s_nis[tid], s_nis[tid + h]);
-      s_ld[tid] = add_(s_ld[tid], s_ld[tid + h]);
-    }
-    __syncthreads();
-  }
+  const int m2 = resc_m2 ? resc_m2[s] : 0;
+  update_sums(d, s, m2 > 0 ? m2 : m, SL2_NXV + 3 * (nf + nc), s_nis, s_ld);
   sl2_step_record *r = d.rec + (size_t)s * d.rec_depth + (size_t)(step % d.rec_depth);
   if (tid < SL2_NXV) {
     const size_t ld = d.ld;
@@ -59,18 +50,26 @@ __global__ void __launch_bounds__(REC_THREADS) record_kernel(const Sl2Dev d, int
     r->nsel = d.nsel[s];
     r->nmeas = d.nmeas[s];
     r->nculled = nc;
-    r->m = m;
-    r->nis = s_nis[0];
-    r->logdet_s = mul_(2.0, s_ld[0]);
+    if (m2 > 0) {
+      r->m = m + m2;
+      r->nis = add_(resc_nis1[s], s_nis[0]);
+      r->logdet_s = add_(resc_logdet1[s], mul_(2.0, s_ld[0]));
+    } else {
+      r->m = m;
+      r->nis = s_nis[0];
+      r->logdet_s = mul_(2.0, s_ld[0]);
+    }
   }
 }
 
 }  // namespace
 
-cudaError_t sl2_launch_records(const Sl2Dev &d, int stream_lo, int stream_cnt, int64_t step, Sl2Queue q) {
+cudaError_t sl2_launch_records(const Sl2Dev &d, int stream_lo, int stream_cnt, int64_t step, const Sl2Rescue *resc,
+                               Sl2Queue q) {
   if (stream_cnt <= 0) return cudaSuccess;
   return sl2_launch_kernel(record_kernel, dim3(stream_cnt), dim3(REC_THREADS), 0, q, sl2_use_pdl(stream_cnt), d,
-                           stream_lo, (long long)step);
+                           stream_lo, (long long)step, resc ? resc->m2 : nullptr, resc ? resc->nis1 : nullptr,
+                           resc ? resc->logdet1 : nullptr);
 }
 
 extern "C" {

@@ -126,6 +126,35 @@ static_assert(sizeof(Sl2Dev) == 336, "Sl2Dev is every kernel's by-value paramete
 #define SL2_MAX_PANELS 16  // 16-row panels of S: m <= 2 * SL2_MAX_MEASURED = 256
 static_assert(2 * SL2_MAX_MEASURED <= 16 * SL2_MAX_PANELS, "every panel of S must fit the panel tables");
 
+// found code of a match the consensus rescue took back (rescue.cu): set by rescue_kernel, turned into 1 by the second
+// update's finish kernel of the same step, so it never leaves the step
+#define SL2_FOUND_RESCUED 3
+
+// NIS = w^T w and log det S = -2 sum log W_ii of the update whose m rows G and Wp hold, for stream s whose update ran
+// on a state of n entries (records.cu says where the update leaves w and W_ii): thread tid < m takes row tid, then a
+// pairwise tree over all 256 slots, the same order for every stream, every m and every launch shape.  A block of 256
+// threads; all call; the sums are in s_nis[0] and s_ld[0] (the log det is 2 s_ld[0]) after the call.
+__device__ __forceinline__ void update_sums(const Sl2Dev &d, int s, int m, int n, double *s_nis, double *s_ld) {
+  const int tid = threadIdx.x;
+  double q = 0.0, l = 0.0;
+  if (tid < m) {
+    const double w = d.G[((size_t)s * d.mmax + tid) * d.ldg + m + n];
+    q = __dmul_rn(w, w);
+    l = -log(d.Wp[((size_t)s * SL2_MAX_PANELS + (tid >> 4)) * 256 + (tid & 15) * 17]);
+  }
+  s_nis[tid] = q;
+  s_ld[tid] = l;
+  __syncthreads();
+#pragma unroll
+  for (int h = 256 / 2; h > 0; h >>= 1) {
+    if (tid < h) {
+      s_nis[tid] = __dadd_rn(s_nis[tid], s_nis[tid + h]);
+      s_ld[tid] = __dadd_rn(s_ld[tid], s_ld[tid + h]);
+    }
+    __syncthreads();
+  }
+}
+
 // ---- correctly-rounded, never-fused FP64 helpers: the oracle is built with
 // -ffp-contract=off, so every bit-critical expression must avoid FMA contraction.
 __device__ __forceinline__ double mul_(double a, double b) { return __dmul_rn(a, b); }
@@ -274,10 +303,25 @@ cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, in
                               const int *st_feat, const double *st_Hxv, const double *st_Hy,
                               const double *st_R, const double *st_nu, int only_normalise,
                               Sl2Queue q, cudaEvent_t *ev6 = nullptr);
+// The second update of the consensus rescue: the five update kernels over the rows whose found is SL2_FOUND_RESCUED,
+// with m2 (instead of Sl2Dev::upd_m) holding each stream's row count, 0 for a stream with nothing rescued, which the
+// five kernels then leave as they found it (update.cu)
+cudaError_t sl2_launch_update_rescued(const Sl2Dev &d, int stream_lo, int stream_cnt, int *m2, Sl2Queue q);
 cudaError_t sl2_launch_cull(const Sl2Dev &d, int stream_lo, int stream_cnt, int force_index, Sl2Queue q);
+// The consensus rescue (rescue.cu): chi2[s] (0 = off) and the consensus's tau2[s] of every stream, and the per-stream
+// scratch the step records read: m2 = rows of the second update, nis1 / logdet1 = the first update's NIS and log det S
+struct Sl2Rescue {
+  const double *chi2, *tau2;  // [B]
+  int *m2;                    // [B]
+  double *nis1, *logdet1;     // [B]
+};
+// rescue_kernel then the second update of the streams [stream_lo, stream_lo + stream_cnt), after their first update
+cudaError_t sl2_launch_rescue(const Sl2Dev &d, int stream_lo, int stream_cnt, const Sl2Rescue &r, Sl2Queue q);
 // one step record per stream of [stream_lo, stream_lo + stream_cnt) into ring row step % d.rec_depth; launched after
-// the cull of the fused step (records.cu)
-cudaError_t sl2_launch_records(const Sl2Dev &d, int stream_lo, int stream_cnt, int64_t step, Sl2Queue q);
+// the cull of the fused step (records.cu).  resc: the rescue's scratch when the streams' step ran the rescue, else
+// nullptr
+cudaError_t sl2_launch_records(const Sl2Dev &d, int stream_lo, int stream_cnt, int64_t step, const Sl2Rescue *resc,
+                               Sl2Queue q);
 cudaError_t sl2_configure_search(const Sl2Dev &d);  // per context: dynamic smem opt-in
 cudaError_t sl2_configure_update(const Sl2Dev &d);
 // partially-initialised features (ekf.cu, smoe.cu, particles.cu): F features x Kmax particle slots (K_dev[f] used)

@@ -120,6 +120,12 @@ struct sl2_ctx {
   double *sel_t_dev = nullptr;            // [B] device: exp2(2 min_bits)
   sl2::DevPtr<double> sel_g;
   size_t sel_g_bytes = 0;
+  // consensus rescue (sl2_set_stream_rescue): the host mirror of every stream's chi2 (0 = off), the device array
+  // rescue_kernel reads, and the per-stream scratch [B] nis1, [B] logdet1, [B] m2 that the second update and the step
+  // records use (allocated when a stream first turns the rescue on)
+  std::vector<double> resc_chi2;  // [B]
+  double *resc_chi2_dev = nullptr;  // [B] device
+  sl2::DevPtr<uint8_t> resc_scratch;
 };
 
 namespace sl2 {
@@ -243,5 +249,10 @@ cudaError_t copy_slot_frames(sl2_ctx *c, int slot, const uint8_t *src, cudaMemcp
 // after their prediction
 bool selection_on(const sl2_ctx *c, int lo, int cnt);
 int select_streams(sl2_ctx *c, int lo, int cnt, Sl2Queue q);
+// rescue.cu: whether some stream of [lo, lo + cnt) has the consensus and the rescue on; the rescue's kernel arguments;
+// the rescue kernel and the second update of those streams on q, right after their first update
+bool rescue_on(const sl2_ctx *c, int lo, int cnt);
+Sl2Rescue rescue_args(const sl2_ctx *c);
+int rescue_streams(sl2_ctx *c, int lo, int cnt, Sl2Queue q);
 
 }  // namespace sl2

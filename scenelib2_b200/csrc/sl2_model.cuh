@@ -1,5 +1,5 @@
 // sl2_model.cuh — the device camera and feature models of predict_kernel and particle_predict_kernel (ekf.cu),
-// consensus_kernel (consensus.cu), reloc_kernel (reloc.cu) and warp_kernel (warp.cu).  Everything that decides which pixels are searched
+// consensus_kernel (consensus.cu), rescue_kernel (rescue.cu), reloc_kernel (reloc.cu) and warp_kernel (warp.cu).  Everything that decides which pixels are searched
 // (S_i, S^-1, h_i) or which match is an inlier uses never-fused rd ops in the oracle's evaluation order.
 #pragma once
 #include "sl2_common.cuh"
@@ -287,6 +287,41 @@ __device__ __forceinline__ void func_Si(const rd dxp[2][7], const rd dy[2][NY], 
       v = v + (r == c ? var : rd(0.0));
       S[r][c] = v;
     }
+}
+
+// The measurement prediction of map feature yi from the camera state xv (monoslam.cpp:289-308): h, dh/dxp, dh/dy,
+// R = var I, S; depth = the camera-frame depth of yi (not part of the reference's prediction).
+struct FeatPred {
+  rd h[2];
+  rd dxp[2][7];
+  rd dy[2][3];
+  rd var;
+  rd S[2][2];
+  rd depth;
+};
+
+// Pxx: shared 13x13 col-major; Pcol: global pointer to P(0, pos) (column-major, ld)
+__device__ void predict_feature(const double *cam, const double *xv, const rd yi[3],
+                                const double *Pxx, const double *Pcol, int ld, int pos,
+                                FeatPred &o) {
+  rd z[3], dz_dxp[3][7], RRW[3][3], J[2][3];
+  zeroedyi(yi, xv, z, dz_dxp, RRW);
+  project(cam, z, o.h, J);
+  for (int i = 0; i < 2; ++i) {
+    for (int j = 0; j < 7; ++j) {
+      rd s(0.0);
+      for (int k = 0; k < 3; ++k) s = s + J[i][k] * dz_dxp[k][j];
+      o.dxp[i][j] = s;
+    }
+    for (int j = 0; j < 3; ++j) {
+      rd s(0.0);
+      for (int k = 0; k < 3; ++k) s = s + J[i][k] * RRW[k][j];
+      o.dy[i][j] = s;
+    }
+  }
+  o.depth = z[2];
+  o.var = measurement_noise(cam, o.h);
+  func_Si<3>(o.dxp, o.dy, o.var, Pxx, 13, Pcol, ld, Pcol + pos, ld, o.S);
 }
 
 // (S^-1)00, 01, 11 of a 2x2 S: LLT, L^-1 in closed form, L^-T L^-1 (monoslam.cpp:371-374; Particle::set_S,

@@ -217,7 +217,9 @@ __device__ __forceinline__ HpSmem hp_carve(uint8_t *base, int kmax, int ld) {
 // Measurement list in selected order (successful only, monoslam.cpp:556-571) and the H rows, R, nu of every
 // measurement into shared memory; returns K (measured features) or -1 when this CTA has no row block (rows_per_block
 // rows per block, block index blockIdx.x).  Every CTA of the stream pays this prologue.  All threads must call.
-__device__ __forceinline__ int hp_tables(const Sl2Dev &d, const HpSmem &sm, int s, int rows_per_block, int staged_m,
+// row_found: the found code of the rows (1; SL2_FOUND_RESCUED for the rescue's second update, whose K adds to nmeas).
+__device__ __forceinline__ int hp_tables(const Sl2Dev &d, const HpSmem &sm, int s, int rows_per_block, int row_found,
+                                         int staged_m,
                                          const int *st_feat, const double *st_Hxv, const double *st_Hy,
                                          const double *st_R, const double *st_nu) {
   const int tid = threadIdx.x;
@@ -232,7 +234,7 @@ __device__ __forceinline__ int hp_tables(const Sl2Dev &d, const HpSmem &sm, int 
     int feat = -1;
     if (tid < d.Nmax && tid < nsel) {
       const int i = d.job_feat[fb + tid];
-      if (i >= 0 && d.found[fb + i] == 1) feat = i;
+      if (i >= 0 && d.found[fb + i] == row_found) feat = i;
     }
     // nsel <= kmax: the warps beyond the first (SL2_MAX_MEASURED + 31) / 32 select nothing
     K = block_gather(feat, sm.mfeat, sm.wcount, (SL2_MAX_MEASURED + 31) / 32);
@@ -240,7 +242,8 @@ __device__ __forceinline__ int hp_tables(const Sl2Dev &d, const HpSmem &sm, int 
   const int m = 2 * K;
   if (blockIdx.x == 0 && tid == 0) {
     d.upd_m[s] = m;
-    if (staged_m < 0) d.nmeas[s] = K;
+    if (staged_m < 0 && row_found == 1) d.nmeas[s] = K;
+    else if (staged_m < 0 && K > 0) d.nmeas[s] += K;
   }
   if (rows_per_block * (int)blockIdx.x >= m) return -1;
   for (int e = tid; e < m * HP_HRS; e += HP_THREADS) sm.Hrow[e] = 0.0;
@@ -418,7 +421,7 @@ __device__ __forceinline__ void hp_s_rows(const HpSmem &sm, const double *__rest
 // KD = dense columns of H that can be nonzero (7: fused step, 13: staged)
 template <int KD>
 __global__ void __launch_bounds__(HP_THREADS, 2) upd_hp_kernel(
-    const Sl2Dev d, int stream_lo, int staged_m, const int *st_feat, const double *st_Hxv,
+    const Sl2Dev d, int stream_lo, int row_found, int staged_m, const int *st_feat, const double *st_Hxv,
     const double *st_Hy, const double *st_R, const double *st_nu) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   pdl_prologue();
@@ -429,7 +432,7 @@ __global__ void __launch_bounds__(HP_THREADS, 2) upd_hp_kernel(
   const int n = SL2_NXV + 3 * d.nfeat[s];
   const double *__restrict__ P = d.P + (size_t)s * ld * ld;
   double *__restrict__ G = d.G + (size_t)s * d.mmax * ldg;
-  const int K = hp_tables(d, sm, s, HP_ROWS, staged_m, st_feat, st_Hxv, st_Hy, st_R, st_nu);
+  const int K = hp_tables(d, sm, s, HP_ROWS, row_found, staged_m, st_feat, st_Hxv, st_Hy, st_R, st_nu);
   if (K < 0) return;
   const int m = 2 * K;
 
@@ -461,7 +464,7 @@ __global__ void __launch_bounds__(HP_THREADS, 2) upd_hp_kernel(
 // __syncthreads per block.  The per-block steps are upd_hp's, so the results are identical.
 template <int KD>
 __global__ void __launch_bounds__(HP_THREADS, 2) upd_hp2_kernel(
-    const Sl2Dev d, int stream_lo, int staged_m, const int *st_feat, const double *st_Hxv,
+    const Sl2Dev d, int stream_lo, int row_found, int staged_m, const int *st_feat, const double *st_Hxv,
     const double *st_Hy, const double *st_R, const double *st_nu) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   pdl_prologue();
@@ -473,7 +476,7 @@ __global__ void __launch_bounds__(HP_THREADS, 2) upd_hp2_kernel(
   const int n = SL2_NXV + 3 * d.nfeat[s];
   const double *__restrict__ P = d.P + (size_t)s * ld * ld;
   double *__restrict__ G = d.G + (size_t)s * d.mmax * ldg;
-  const int K = hp_tables(d, sm, s, R2, staged_m, st_feat, st_Hxv, st_Hy, st_R, st_nu);
+  const int K = hp_tables(d, sm, s, R2, row_found, staged_m, st_feat, st_Hxv, st_Hy, st_R, st_nu);
   if (K < 0) return;
   const int m = 2 * K;
   const int j = tid;  // this thread's state column (n <= HP_THREADS: the launcher's condition)
@@ -1338,8 +1341,11 @@ __global__ void __launch_bounds__(SYRK_THREADS, 3) upd_syrk_kernel(const Sl2Dev 
 // =============================================================================================
 // kernel 4: upd_finish — normalise_state, symmetrise, counters
 // =============================================================================================
+// rescued: the consensus rescue's second update (rows found == SL2_FOUND_RESCUED): a stream with no such row returns at
+// once; the others count each rescued match as the success of the attempt the first update counted, and it becomes
+// found = 1.
 __global__ void __launch_bounds__(UPD_THREADS) upd_finish_kernel(const Sl2Dev d, int stream_lo, int staged,
-                                                                  int only_normalise) {
+                                                                  int only_normalise, int rescued) {
   pdl_prologue();
   const int s = stream_lo + blockIdx.x;
   const int tid = threadIdx.x;
@@ -1350,6 +1356,7 @@ __global__ void __launch_bounds__(UPD_THREADS) upd_finish_kernel(const Sl2Dev d,
   const double *__restrict__ x = d.x + (size_t)s * ld;
   const size_t fb = (size_t)s * d.Nmax;
   const int m = only_normalise ? 0 : d.upd_m[s];
+  if (rescued && m == 0) return;
   __shared__ int s_cull;
   // ---- normalise_state (monoslam.cpp:616-637): P <- J P J^T, J = diag(I3, dqnorm, I6, I) ---------
   if (m > 0 || only_normalise) {
@@ -1407,7 +1414,13 @@ __global__ void __launch_bounds__(UPD_THREADS) upd_finish_kernel(const Sl2Dev d,
     __syncthreads();
     for (int i = tid; i < nf; i += UPD_THREADS) {
       int att = d.attempted[fb + i], suc = d.successful[fb + i];
-      if (d.sel_rank[fb + i] >= 0) {
+      if (rescued) {
+        if (d.found[fb + i] == SL2_FOUND_RESCUED) {
+          suc += 1;
+          d.successful[fb + i] = suc;
+          d.found[fb + i] = 1;
+        }
+      } else if (d.sel_rank[fb + i] >= 0) {
         att += 1;
         if (d.found[fb + i] == 1) suc += 1;  // a match the consensus rejected (2) is an unsuccessful attempt
         d.attempted[fb + i] = att;
@@ -1472,11 +1485,13 @@ cudaError_t sl2_configure_update(const Sl2Dev &d) {
   return cudaSuccess;
 }
 
-// ev6 (optional): 6 events recorded around the 5 kernels (hp, chol, solve, syrk, finish)
-cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, int staged_m,
-                              const int *st_feat, const double *st_Hxv, const double *st_Hy,
-                              const double *st_R, const double *st_nu, int only_normalise,
-                              Sl2Queue q, cudaEvent_t *ev6) {
+namespace {
+
+// ev6 (optional): 6 events recorded around the 5 kernels (hp, chol, solve, syrk, finish); row_found: the rows' found
+// code (1, or SL2_FOUND_RESCUED for the rescue's second update)
+cudaError_t launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, int row_found, int staged_m,
+                          const int *st_feat, const double *st_Hxv, const double *st_Hy, const double *st_R,
+                          const double *st_nu, int only_normalise, Sl2Queue q, cudaEvent_t *ev6) {
   if (stream_cnt <= 0) return cudaSuccess;
   cudaError_t e;
   auto mark = [&](int i) { return ev6 ? cudaEventRecord(ev6[i], q.stream) : cudaSuccess; };
@@ -1494,8 +1509,8 @@ cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, in
     auto *k13 = piped ? upd_hp2_kernel<13> : upd_hp_kernel<13>;
     auto *k7 = piped ? upd_hp2_kernel<7> : upd_hp_kernel<7>;
     const size_t smem = hp_layout(d.kmax, d.ld, piped ? kd : 0).bytes;
-    e = sl2_launch_kernel(kd == 13 ? k13 : k7, grid, dim3(HP_THREADS), smem, q, pdl, d, stream_lo, staged_m,
-                          st_feat, st_Hxv, st_Hy, st_R, st_nu);
+    e = sl2_launch_kernel(kd == 13 ? k13 : k7, grid, dim3(HP_THREADS), smem, q, pdl, d, stream_lo, row_found,
+                          staged_m, st_feat, st_Hxv, st_Hy, st_R, st_nu);
     if (e != cudaSuccess) return e;
   }
   if ((e = mark(1)) != cudaSuccess) return e;
@@ -1528,10 +1543,29 @@ cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, in
   }
   if ((e = mark(4)) != cudaSuccess) return e;
   e = sl2_launch_kernel(upd_finish_kernel, dim3(stream_cnt), dim3(UPD_THREADS), 0, q, pdl, d, stream_lo,
-                        (int)(staged_m >= 0), only_normalise);
+                        (int)(staged_m >= 0), only_normalise, (int)(row_found == SL2_FOUND_RESCUED));
   if (e != cudaSuccess) return e;
   if ((e = mark(5)) != cudaSuccess) return e;
   return cudaGetLastError();
+}
+
+}  // namespace
+
+cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, int staged_m,
+                              const int *st_feat, const double *st_Hxv, const double *st_Hy,
+                              const double *st_R, const double *st_nu, int only_normalise,
+                              Sl2Queue q, cudaEvent_t *ev6) {
+  return launch_update(d, stream_lo, stream_cnt, 1, staged_m, st_feat, st_Hxv, st_Hy, st_R, st_nu, only_normalise, q,
+                       ev6);
+}
+
+// Sl2Dev travels by value: the second update's copy reads and writes its row counts in m2, so Sl2Dev::upd_m keeps the
+// first update's for the step record, and a stream with nothing rescued reads m = 0 in all five kernels.
+cudaError_t sl2_launch_update_rescued(const Sl2Dev &d, int stream_lo, int stream_cnt, int *m2, Sl2Queue q) {
+  Sl2Dev d2 = d;
+  d2.upd_m = m2;
+  return launch_update(d2, stream_lo, stream_cnt, SL2_FOUND_RESCUED, -1, nullptr, nullptr, nullptr, nullptr, nullptr, 0,
+                       q, nullptr);
 }
 
 extern "C" {
@@ -1564,6 +1598,10 @@ int sl2_ekf_update(sl2_ctx *c, int32_t s, int32_t m, const int32_t *feat_index, 
 int sl2_ekf_update_measured(sl2_ctx *c, int32_t s) {
   if (bad_stream(c, s)) return fail(c, SL2_ERR_ARG, "bad stream");
   CU_TRY(c, sl2_launch_update(c->d, s, 1, -1, nullptr, nullptr, nullptr, nullptr, nullptr, 0, queue(c)));
+  if (rescue_on(c, s, 1)) {  // the fused step's rescue and second update
+    const int rc = rescue_streams(c, s, 1, queue(c));
+    if (rc) return rc;
+  }
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   return SL2_OK;
 }

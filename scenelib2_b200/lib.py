@@ -67,6 +67,7 @@ SOURCE_BPP = {SL2_SRC_GRAY8: 1, SL2_SRC_RGB24: 3, SL2_SRC_UYVY: 2}
 EXPORTS = [
     "sl2_default_config", "sl2_create", "sl2_destroy", "sl2_last_error", "sl2_sync", "sl2_version",
     "sl2_set_stream_config", "sl2_get_stream_config", "sl2_set_stream_consensus", "sl2_get_stream_consensus",
+    "sl2_set_stream_rescue", "sl2_get_stream_rescue",
     "sl2_set_stream_warp", "sl2_get_stream_warp", "sl2_warp_templates",
     "sl2_set_stream_selection", "sl2_get_stream_selection",
     "sl2_set_frame", "sl2_set_frames", "sl2_set_frames_dev",
@@ -226,6 +227,8 @@ def load():
         L.sl2_get_stream_config.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamConfig)]
         L.sl2_set_stream_consensus.argtypes = [C.c_void_p, C.c_int32, C.c_double]
         L.sl2_get_stream_consensus.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_double)]
+        L.sl2_set_stream_rescue.argtypes = [C.c_void_p, C.c_int32, C.c_double]
+        L.sl2_get_stream_rescue.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_double)]
         L.sl2_set_stream_warp.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
         L.sl2_get_stream_warp.argtypes = [C.c_void_p, C.c_int32, i32p]
         L.sl2_set_stream_selection.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamSelection)]
@@ -343,6 +346,17 @@ class Context:
     def stream_consensus(self, stream_id):
         v = C.c_double()
         self._ck(self.L.sl2_get_stream_consensus(self.h, stream_id, C.byref(v)))
+        return v.value
+
+    def set_stream_rescue(self, stream_id, chi2):
+        """sl2_set_stream_rescue: after the update with the consensus's inliers, take back the rejected matches whose
+        innovation at the updated state has nu^T S^-1 nu <= chi2, and update with them (0 = off, the default; 5.991
+        is the 95 % point of chi^2 with two degrees of freedom)."""
+        self._ck(self.L.sl2_set_stream_rescue(self.h, stream_id, float(chi2)))
+
+    def stream_rescue(self, stream_id):
+        v = C.c_double()
+        self._ck(self.L.sl2_get_stream_rescue(self.h, stream_id, C.byref(v)))
         return v.value
 
     # ---- feature selection ----------------------------------------------------------------------
