@@ -246,6 +246,79 @@ typedef struct sl2_stream_selection {
 int sl2_set_stream_selection(sl2_ctx *ctx, int32_t stream_id, const sl2_stream_selection *sel);
 int sl2_get_stream_selection(sl2_ctx *ctx, int32_t stream_id, sl2_stream_selection *sel);
 
+/* ---- gyroscope: an angular-rate update between the motion prediction and the feature prediction (no reference
+ *      counterpart) ------------------------------------------------------------------------------------------------
+ * The constant-velocity model allows an angular acceleration of sigma = 6 rad/s^2: a camera that starts or stops
+ * turning faster than that has its features predicted outside their search regions.  A stream with a gyroscope takes
+ * one rate sample per step and updates its state's omega, x[10:13] (camera frame: qnew = qold * q(omega dt)), right
+ * after the motion prediction, so the feature prediction, the search ellipses and the selection already know how the
+ * camera turned; P's q-omega cross terms carry the correction into q (Pinies, Lupton, Sukkarieh, Tardos, "Inertial
+ * Aiding of Inverse Depth SLAM using a Monocular Camera", ICRA 2007).
+ * Setting, in the gyro's frame: R_gc (row-major) takes camera-frame vectors into the gyro's frame; bias b; cov C, the
+ * covariance of one sample, a sample being the mean angular rate over the stream's frame period delta_t.  The model is
+ * z = R_gc omega + b + noise(C).  When the setting is made, Rc = R_gc^T C R_gc is formed once: M[k][j] = (C[k][0]
+ * R[0][j] + C[k][1] R[1][j]) + C[k][2] R[2][j], then for i <= j Rc[i][j] = (R[0][i] M[0][j] + R[1][i] M[1][j]) +
+ * R[2][i] M[2][j], mirrored to Rc[j][i].
+ * Update of a sample z, with x and P the motion prediction (n = 13 + 3 nfeat, P(r, c) = the column-major entry):
+ *   1. dk = z[k] - b[k]; zc[i] = (R[0][i] d0 + R[1][i] d1) + R[2][i] d2.
+ *   2. S(i, j) = P(10 + i, 10 + j) + Rc[i][j] for i >= j; l00 = sqrt(S00), l10 = S10 / l00, l20 = S20 / l00,
+ *      a11 = S11 - l10 l10, l11 = sqrt(a11), l21 = (S21 - l20 l10) / l11, a22 = (S22 - l20 l20) - l21 l21,
+ *      l22 = sqrt(a22).
+ *   3. nu[i] = zc[i] - x[10 + i]; w0 = nu0 / l00, w1 = (nu1 - l10 w0) / l11, w2 = ((nu2 - l20 w0) - l21 w1) / l22;
+ *      NIS = (w0 w0 + w1 w1) + w2 w2.
+ *   If S00, a11 or a22 is not > 0, or any of S, L, nu, w and NIS is not finite, the update is skipped: x and P stay
+ *   exactly as they were (status 2).
+ *   4. for every row r < n: W[r][0] = P(r, 10) / l00, W[r][1] = (P(r, 11) - W[r][0] l10) / l11,
+ *      W[r][2] = ((P(r, 12) - W[r][0] l20) - W[r][1] l21) / l22 (W = P H^T L^-T, all from the predicted P).
+ *   5. x[r] = x[r] + ((W[r][0] w0 + W[r][1] w1) + W[r][2] w2) for r < n;
+ *      P(i, j) = P(i, j) - ((W[i][0] W[j][0] + W[i][1] W[j][1]) + W[i][2] W[j][2]) for i, j < n.  Entries outside the
+ *      n x n block stay as they are.  Multiplication is commutative in IEEE arithmetic, so P(j, i) gets the same bits
+ *      as P(i, j): P stays bit-symmetric without a mirror pass.
+ * Every operation is a correctly rounded FP64 operation (never fused) in the order written above and in the kernels
+ * (csrc/gyro.cu, gyro_prep_kernel and gyro_downdate_kernel).  Nothing is normalised: the step's visual update
+ * normalises the quaternion and symmetrises as before, and a step that measures nothing leaves the gyro-updated state
+ * un-normalised.  NIS is chi^2 with 3 degrees of freedom when R_gc, b and C are right: this is how to check them.
+ * Where it applies: the fused step (sl2_step, sl2_step_host, sl2_step_host_async) of ring slot t consumes slot t's
+ * sample of every gyro-on stream: the update runs when the sample is valid, and the step clears the sample's valid
+ * byte, so a sample is used by exactly one step; a step without a valid sample does no gyro update.  The staged form
+ * is sl2_gyro_update, between sl2_ekf_predict and sl2_predict_measurements.  The step records are unchanged: nis and
+ * logdet_s stay the visual update's, xv and pxx_diag show the state after both updates.
+ * on = 0 (the default; the getter then shows R_gc = I, b = 0, C = I) is off: a context where no stream has it on runs
+ * exactly the path without it; a step group holding a gyro-on stream splits its prediction in two launches and adds
+ * the update's two (three more launches, timed with the predict in sl2_last_step_times).  Ordering like
+ * sl2_set_stream_config.  The setting belongs to the stream slot, like the match consensus: snapshots do not carry it
+ * and a load leaves it.  A call that turns an off stream on clears that stream's samples in every slot; a call that
+ * turns a stream on or off clears its last result (status 0, NIS 0).  The first stream turned on allocates the
+ * context's gyro buffers (a sample ring of frame_slots x num_streams, the W scratch of num_streams x (13 + 3 max_features, rounded up to 8) x 3 doubles and the per-stream
+ * results): SL2_ERR_CUDA, with the setting left off, when that allocation fails.  SL2_ERR_ARG, with the setting
+ * unchanged, for: a bad stream_id or NULL g; reserved != 0 or on outside {0, 1}; a non-finite entry; an R_gc that is
+ * not a rotation (|R R^T - I| > 1e-9 in some entry, or det R <= 0); a cov that is not exactly symmetric, or whose
+ * Cholesky factor (step 2's formulas) has a pivot argument that is not > 0. */
+typedef struct sl2_stream_gyro {
+  int32_t on;       /* 0 (default) or 1 */
+  int32_t reserved; /* 0 */
+  double R_gc[9];   /* row-major rotation: camera frame -> gyro frame */
+  double bias[3];   /* rad/s, gyro frame */
+  double cov[9];    /* row-major covariance of one sample (rad/s)^2, gyro frame; symmetric positive definite */
+} sl2_stream_gyro;
+int sl2_set_stream_gyro(sl2_ctx *ctx, int32_t stream_id, const sl2_stream_gyro *g);
+int sl2_get_stream_gyro(sl2_ctx *ctx, int32_t stream_id, sl2_stream_gyro *g);
+/* The samples of streams [lo, lo + cnt) for the fused step of ring slot `slot`: rates cnt x 3 (rad/s, gyro frame),
+ * valid cnt bytes (NULL: all valid; 0 = no sample).  Ordered on the context's stream like sl2_set_stream_config;
+ * returns once the caller's buffers may be reused.  Samples of gyro-off streams are kept and never read.  SL2_ERR_ARG,
+ * with nothing written, for a bad slot or range, a NULL rates with cnt > 0, or a valid sample with a non-finite rate;
+ * SL2_ERR_STATE while no stream of the context has ever turned its gyro on. */
+int sl2_set_gyro_samples(sl2_ctx *ctx, int32_t slot, int32_t lo, int32_t cnt, const double *rates,
+                         const uint8_t *valid);
+/* The staged update of one stream with the sample rate3 (3), using the stream's setting: the same two kernels as the
+ * fused step.  SL2_ERR_ARG for a bad stream_id, a NULL or non-finite rate3; SL2_ERR_STATE when the stream's gyro is
+ * off.  Synchronises. */
+int sl2_gyro_update(sl2_ctx *ctx, int32_t stream_id, const double *rate3);
+/* The last gyro update of streams [lo, lo + cnt): status 0 (none this step), 1 (applied) or 2 (skipped: S not positive
+ * definite or not finite), and its NIS (0 unless status is 1).  Either pointer may be NULL.  Like the records, not
+ * part of a snapshot.  Joins both step groups and synchronises.  SL2_ERR_ARG for a bad range. */
+int sl2_get_gyro_results(sl2_ctx *ctx, int32_t lo, int32_t cnt, double *nis, int32_t *status);
+
 /* ---- frames (replaces the cv::Mat `frame` argument of MonoSLAM::GoOneStep, monoslam.cpp:108) */
 /* The frame ring keeps the context's width x height per stream.  A stream whose image is smaller
  * (sl2_set_stream_config) occupies the top-left width_s x height_s of its block; the rest of the block
@@ -458,7 +531,7 @@ int sl2_get_features(sl2_ctx *ctx, int32_t stream_id, double *h /* n x 2 */, dou
 int sl2_get_feature_jacobians(sl2_ctx *ctx, int32_t stream_id, double *dh_by_dxv /* n x 26 */,
                               double *dh_by_dy /* n x 6 */, double *R /* n x 4 */,
                               double *nu /* n x 2 */);
-/* device-time of the kernels of the last sl2_step (ms): [0] predict+select, [1] patch search,
+/* device-time of the kernels of the last sl2_step (ms): [0] predict+select (and the gyro update), [1] patch search,
  * [2] EKF update (with the consensus rescue and its second update when a stream has them on), [3] cull.  Valid after
  * sl2_enable_timing(ctx, 1). */
 int sl2_enable_timing(sl2_ctx *ctx, int32_t on);

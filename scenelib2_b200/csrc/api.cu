@@ -343,6 +343,9 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   c->sel.assign(B, sl2_stream_selection{});
   c->sel_mode.assign(B, SL2_SELECT_TRACE);
   c->sel_t.assign(B, 1.0);
+  sl2_stream_gyro g0 = {};  // off; a rotation and a covariance the setter accepts
+  for (int i = 0; i < 3; ++i) g0.R_gc[4 * i] = g0.cov[4 * i] = 1.0;
+  c->gyro.assign(B, g0);
 #undef ALLOC
   int rc = make_tensor_map(c);
   if (rc) return failed(rc, c->err);
@@ -501,7 +504,14 @@ static int step_group(sl2_ctx *c, int32_t slot, int lo, int cnt, Sl2Queue q, cud
   const cudaStream_t st = q.stream;
   if (t) CU_TRY(c, cudaEventRecord(c->ev[0].get(), st));
   const bool info = selection_on(c, lo, cnt);
-  CU_TRY(c, sl2_launch_predict(d, lo, cnt, nullptr, 1, 1, info ? c->sel_mode_dev : nullptr, q));
+  if (gyro_on(c, lo, cnt)) {  // the motion prediction, the gyro update, then the feature prediction
+    CU_TRY(c, sl2_launch_predict(d, lo, cnt, nullptr, 1, 0, nullptr, q));
+    const int rc = gyro_streams(c, slot, lo, cnt, q);
+    if (rc) return rc;
+    CU_TRY(c, sl2_launch_predict(d, lo, cnt, nullptr, 0, 1, info ? c->sel_mode_dev : nullptr, q));
+  } else {
+    CU_TRY(c, sl2_launch_predict(d, lo, cnt, nullptr, 1, 1, info ? c->sel_mode_dev : nullptr, q));
+  }
   if (info) {  // part of the predict's time
     const int rc = select_streams(c, lo, cnt, q);
     if (rc) return rc;

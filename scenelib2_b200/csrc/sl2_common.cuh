@@ -317,6 +317,27 @@ struct Sl2Rescue {
 };
 // rescue_kernel then the second update of the streams [stream_lo, stream_lo + stream_cnt), after their first update
 cudaError_t sl2_launch_rescue(const Sl2Dev &d, int stream_lo, int stream_cnt, const Sl2Rescue &r, Sl2Queue q);
+// The gyroscope update (gyro.cu) of the streams [stream_lo, stream_lo + stream_cnt) whose on[s] is 1, between their
+// motion prediction and their feature prediction: stream s reads its sample at index s - sample_lo of rate (3 doubles
+// each) and valid, and consumes it (valid = 0)
+struct Sl2GyroParam {  // one stream's setting as the kernels read it (sl2_set_stream_gyro)
+  double R[9];   // R_gc, row-major
+  double b[3];   // bias
+  double Rc[9];  // R_gc^T C R_gc, row-major, exactly symmetric
+};
+struct GyroLaunch {
+  int stream_lo, stream_cnt;
+  const uint8_t *on;          // [B]
+  const Sl2GyroParam *prm;    // [B]
+  const double *rate;         // [.][3]
+  uint8_t *valid;             // [.]
+  int sample_lo;
+  double *W;                  // [B][3][ld]: column c of stream s's W at W + (s * 3 + c) * ld
+  double *nis;                // [B]
+  int *status;                // [B] 0 none, 1 applied, 2 skipped
+};
+// gyro_prep_kernel then gyro_downdate_kernel
+cudaError_t sl2_launch_gyro(const Sl2Dev &d, const GyroLaunch &G, Sl2Queue q);
 // one step record per stream of [stream_lo, stream_lo + stream_cnt) into ring row step % d.rec_depth; launched after
 // the cull of the fused step (records.cu).  resc: the rescue's scratch when the streams' step ran the rescue, else
 // nullptr

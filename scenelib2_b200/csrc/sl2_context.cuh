@@ -126,6 +126,15 @@ struct sl2_ctx {
   std::vector<double> resc_chi2;  // [B]
   double *resc_chi2_dev = nullptr;  // [B] device
   sl2::DevPtr<uint8_t> resc_scratch;
+  // gyroscope (sl2_set_stream_gyro): the host mirror of every stream's setting, and the device buffers (allocated when
+  // a stream first turns it on): the on flags [B], the settings [B], the sample ring [slots][B] of rates and valid
+  // bytes, the W scratch [B][3][ld] and the results [B] nis, [B] status
+  std::vector<sl2_stream_gyro> gyro;  // [B]
+  sl2::DevPtr<uint8_t> gyro_buf;
+  uint8_t *gyro_on_dev = nullptr, *gyro_valid = nullptr;
+  Sl2GyroParam *gyro_prm = nullptr;
+  double *gyro_rate = nullptr, *gyro_W = nullptr, *gyro_nis = nullptr;
+  int *gyro_status = nullptr;
 };
 
 namespace sl2 {
@@ -254,5 +263,9 @@ int select_streams(sl2_ctx *c, int lo, int cnt, Sl2Queue q);
 bool rescue_on(const sl2_ctx *c, int lo, int cnt);
 Sl2Rescue rescue_args(const sl2_ctx *c);
 int rescue_streams(sl2_ctx *c, int lo, int cnt, Sl2Queue q);
+// gyro.cu: whether some stream of [lo, lo + cnt) has the gyroscope on; the gyro update of those streams on q with the
+// samples of ring slot `slot`, between their motion prediction and their feature prediction
+bool gyro_on(const sl2_ctx *c, int lo, int cnt);
+int gyro_streams(sl2_ctx *c, int slot, int lo, int cnt, Sl2Queue q);
 
 }  // namespace sl2

@@ -58,6 +58,13 @@ class Sl2StreamSelection(C.Structure):
 
 SL2_SELECT_TRACE, SL2_SELECT_INFORMATION = 0, 1
 
+
+class Sl2StreamGyro(C.Structure):
+    """sl2_stream_gyro: a camera stream's gyroscope: on, the camera-to-gyro rotation R_gc, the bias and the covariance
+    of one sample (row-major, gyro frame)."""
+    _fields_ = [("on", C.c_int32), ("reserved", C.c_int32), ("R_gc", C.c_double * 9), ("bias", C.c_double * 3),
+                ("cov", C.c_double * 9)]
+
 SL2_SRC_GRAY_RING, SL2_SRC_GRAY8, SL2_SRC_RGB24, SL2_SRC_UYVY = 0, 1, 2, 3
 SL2_MAX_SOURCE_DIM = 4096
 SOURCE_BPP = {SL2_SRC_GRAY8: 1, SL2_SRC_RGB24: 3, SL2_SRC_UYVY: 2}
@@ -70,6 +77,7 @@ EXPORTS = [
     "sl2_set_stream_rescue", "sl2_get_stream_rescue",
     "sl2_set_stream_warp", "sl2_get_stream_warp", "sl2_warp_templates",
     "sl2_set_stream_selection", "sl2_get_stream_selection",
+    "sl2_set_stream_gyro", "sl2_get_stream_gyro", "sl2_set_gyro_samples", "sl2_gyro_update", "sl2_get_gyro_results",
     "sl2_set_frame", "sl2_set_frames", "sl2_set_frames_dev",
     "sl2_set_stream_source", "sl2_get_stream_source", "sl2_frame_set_layout", "sl2_set_features",
     "sl2_num_features", "sl2_state_size", "sl2_set_state", "sl2_get_state", "sl2_delete_feature", "sl2_append_feature",
@@ -233,6 +241,11 @@ def load():
         L.sl2_get_stream_warp.argtypes = [C.c_void_p, C.c_int32, i32p]
         L.sl2_set_stream_selection.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamSelection)]
         L.sl2_get_stream_selection.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamSelection)]
+        L.sl2_set_stream_gyro.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamGyro)]
+        L.sl2_get_stream_gyro.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamGyro)]
+        L.sl2_set_gyro_samples.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
+        L.sl2_gyro_update.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
+        L.sl2_get_gyro_results.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
         L.sl2_warp_templates.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_void_p]
         L.sl2_set_frame.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_size_t]
@@ -396,6 +409,56 @@ class Context:
         self._ck(self.L.sl2_warp_templates(self.h, stream_id, n, feat_index.ctypes.data, xp.ctypes.data,
                                            out.ctypes.data, valid.ctypes.data))
         return out, valid
+
+    # ---- gyroscope ----------------------------------------------------------------------------
+    def set_stream_gyro(self, stream_id, on, R_gc=None, bias=None, cov=None, reserved=0):
+        """sl2_set_stream_gyro: update the stream's omega with one gyroscope sample per step, between the motion
+        prediction and the feature prediction (on = 1), or not (0, the default).  R_gc (3x3) takes camera-frame vectors
+        into the gyro's frame (default I), bias (3) is in rad/s (default 0), cov (3x3) is the covariance of one sample,
+        the mean rate over the frame period (default I)."""
+        g = Sl2StreamGyro()
+        g.on, g.reserved = int(on), int(reserved)
+        for name, v, dflt in (("R_gc", R_gc, np.eye(3)), ("bias", bias, np.zeros(3)), ("cov", cov, np.eye(3))):
+            a = np.asarray(dflt if v is None else v, np.float64).reshape(-1)
+            if a.size != len(getattr(g, name)):
+                raise ValueError("%s must hold %d values" % (name, len(getattr(g, name))))
+            getattr(g, name)[:] = [float(t) for t in a]
+        self._ck(self.L.sl2_set_stream_gyro(self.h, stream_id, C.byref(g)))
+
+    def stream_gyro(self, stream_id):
+        """-> dict(on, R_gc (3x3), bias (3), cov (3x3))"""
+        g = Sl2StreamGyro()
+        self._ck(self.L.sl2_get_stream_gyro(self.h, stream_id, C.byref(g)))
+        return dict(on=g.on, R_gc=np.array(g.R_gc).reshape(3, 3), bias=np.array(g.bias),
+                    cov=np.array(g.cov).reshape(3, 3))
+
+    def set_gyro_samples(self, slot, rates, valid=None, lo=0):
+        """sl2_set_gyro_samples: the samples (cnt x 3 rad/s, gyro frame) of streams [lo, lo + cnt) for the fused step
+        of ring slot `slot`; valid (cnt, None = all) marks the streams that have one."""
+        rates = np.ascontiguousarray(rates, np.float64).reshape(-1, 3)
+        cnt = rates.shape[0]
+        if valid is not None:
+            valid = np.ascontiguousarray(valid, np.uint8).reshape(-1)
+            if valid.size != cnt:
+                raise ValueError("valid must hold one byte per sample")
+        self._ck(self.L.sl2_set_gyro_samples(self.h, slot, lo, cnt, rates.ctypes.data,
+                                             None if valid is None else valid.ctypes.data))
+
+    def gyro_update(self, stream_id, rate3):
+        """sl2_gyro_update: the staged gyro update of one stream with one sample, between ekf_predict and
+        predict_measurements."""
+        rate3 = np.ascontiguousarray(rate3, np.float64).reshape(-1)
+        if rate3.size != 3:
+            raise ValueError("rate3 must hold 3 values")
+        self._ck(self.L.sl2_gyro_update(self.h, stream_id, rate3.ctypes.data))
+
+    def gyro_results(self, lo=0, cnt=None):
+        """sl2_get_gyro_results -> (nis (cnt,), status (cnt,): 0 none this step, 1 applied, 2 skipped)."""
+        if cnt is None:
+            cnt = self.cfg.num_streams - lo
+        nis, status = np.zeros(max(cnt, 0)), np.zeros(max(cnt, 0), np.int32)
+        self._ck(self.L.sl2_get_gyro_results(self.h, lo, cnt, nis.ctypes.data, status.ctypes.data))
+        return nis, status
 
     # ---- frames -------------------------------------------------------------------------------
     def set_stream_source(self, stream_id, format, width=0, height=0):
