@@ -196,6 +196,41 @@ int sl2_get_stream_warp(sl2_ctx *ctx, int32_t stream_id, int32_t *on);
 int sl2_warp_templates(sl2_ctx *ctx, int32_t stream_id, int32_t n, const int32_t *feat_index, const double *xp,
                        uint8_t *out, uint8_t *valid);
 
+/* ---- sub-pixel refinement: fit each match's score around the search's minimum (no reference counterpart) -------
+ * The reference's match is the integer position of the smallest correlation score (elliptical_search), so z carries a
+ * quantisation error of sigma = 1 / sqrt(12) = 0.29 px per axis.  A stream with the refinement on fits a quadratic to
+ * the search's own score at the 3 x 3 integer positions around each match and measures the fit's minimum (Shimizu,
+ * Okutomi, "Sub-Pixel Estimation Error Cancellation on Area-Based Matching", IJCV 2005, on the estimate and its bias).
+ * Which matches: every job of the stream's step whose search succeeded (found = 1 from the search, before the match
+ * consensus), with integer match (u, v).  With HALF = (boxsize - 1) / 2 and the stream's own width W x height H:
+ *   c(a, b) for a, b in {-1, 0, 1} is the search's exact score (improc.cpp:99-133, the chain of sl2_score_map) of the
+ *   window centred at (u + a, v + b) against the template the search used (the warped one when the warp is on);
+ *   c(0, 0) is the search's best score bit for bit.
+ *   z = (u, v) (not refined) when: a window leaves the image (u - 1 - HALF < 0, u + 1 + HALF > W - 1, or the same in
+ *   v); a window has sigma_g1 < 10 (the search's own gate); the fit below is not positive definite; or an offset
+ *   component is not in [-0.5, 0.5].  NaN fails every test.
+ *   The fit, every operation a correctly rounded FP64 operation with no contraction, in this order:
+ *     g_u = (c(1,0) - c(-1,0)) * 0.5;  g_v = (c(0,1) - c(0,-1)) * 0.5;
+ *     h_uu = (c(1,0) + c(-1,0)) - 2 c(0,0);  h_vv = (c(0,1) + c(0,-1)) - 2 c(0,0);
+ *     h_uv = ((c(1,1) - c(1,-1)) - (c(-1,1) - c(-1,-1))) * 0.25;  det = h_uu h_vv - h_uv h_uv;
+ *     refined only when h_uu > 0 and det > 0; du = (h_uv g_v - h_vv g_u) / det;  dv = (h_uv g_u - h_uu g_v) / det;
+ *   z = (u + du, v + dv).
+ * Where it applies: the match consensus, the EKF update (nu = z - h, both updates when the consensus rescue fires) and
+ * the rescue's gate of the fused step and of sl2_make_measurements / sl2_ekf_update_measured read the refined z;
+ * sl2_get_features returns it as z, with flags bit 3 set, and sl2_get_feature_jacobians forms nu from it.  Like the
+ * other flags, bit 3 describes the feature's last match; it is never set for an off stream.  R stays sd-based: lower
+ * the stream's sd (sl2_set_stream_config) to make the update trust the refined matches more.  sl2_patch_search,
+ * sl2_score_map, the SMOE and particle entry points and sl2_relocalise stay integer.
+ * on = 0 (the default) is off, 1 is on: a context where no stream has it on runs exactly the path without it; one with
+ * a stream that has it on adds one kernel launch per step group holding such a stream (timed with the search in
+ * sl2_last_step_times).  Ordering like sl2_set_stream_config.  The setting belongs to the stream slot, like the warp:
+ * snapshots do not carry it and a load leaves it.  A loaded stream's z is its integer match (bit 3 clear) until its
+ * next step; so is a stream's after the setting is made.  The first stream turned on sizes the context's scratch
+ * (num_streams x (17 max_features + 1) bytes): SL2_ERR_CUDA, with the setting left off, when that allocation fails.
+ * SL2_ERR_ARG, with the setting unchanged, for a bad stream_id, an `on` other than 0 or 1, or (get) a NULL on. */
+int sl2_set_stream_subpixel(sl2_ctx *ctx, int32_t stream_id, int32_t on);
+int sl2_get_stream_subpixel(sl2_ctx *ctx, int32_t stream_id, int32_t *on);
+
 /* ---- feature selection: measure the features that carry the most information (no reference counterpart) --------
  * The reference measures the n_select visible features of largest trace(S_i) (auto_select_n_features,
  * monoslam.cpp:187-254).  Once the map has settled, most of every feature's innovation uncertainty is the camera
@@ -524,7 +559,8 @@ int sl2_join(sl2_ctx *ctx);
 int sl2_get_features(sl2_ctx *ctx, int32_t stream_id, double *h /* n x 2 */, double *z /* n x 2 */,
                      double *S /* n x 4 col-major */,
                      uint8_t *flags /* bit0 selected, bit1 successful, bit2 matched and rejected by the match
-                                       consensus (sl2_set_stream_consensus) */,
+                                       consensus (sl2_set_stream_consensus), bit3 z is the sub-pixel match
+                                       (sl2_set_stream_subpixel) */,
                      int32_t *attempted, int32_t *successful, int32_t *select_rank);
 /* Feature::dh_by_dxv_ (2x13), dh_by_dy_ (2x3), R_ (2x2), nu_ (2) of the last prediction /
  * measurement, all column-major like the Eigen members (feature.h:104-112). Arrays may be NULL. */

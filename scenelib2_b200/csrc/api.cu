@@ -169,8 +169,8 @@ bool warp_on(const sl2_ctx *c, int lo, int cnt) {
 
 // The measure stage of the streams [lo, lo + cnt) on q: when some stream of them has the warp on, every job's template
 // at the predicted pose x[0:7] (the stored one for the others) into the job-indexed scratch; the patch search over the
-// context's own job arrays (indexed by the stream number local to the launch), then the match consensus when some
-// stream of them has it on
+// context's own job arrays (indexed by the stream number local to the launch), the sub-pixel refinement when some
+// stream of them has it on, then the match consensus when some stream of them has it on
 int measure_streams(sl2_ctx *c, int32_t slot, int lo, int cnt, Sl2Queue q) {
   const Sl2Dev &d = c->d;
   const uint8_t *job_patches = nullptr;
@@ -196,7 +196,12 @@ int measure_streams(sl2_ctx *c, int32_t slot, int lo, int cnt, Sl2Queue q) {
   L.slot = slot;
   L.scatter_to_features = 1;
   CU_TRY(c, sl2_launch_search(d, c->tmap, L, q));
-  if (consensus_on(c, lo, cnt)) CU_TRY(c, sl2_launch_consensus(d, lo, cnt, c->cons_tau2, q));
+  const Sl2Subpix sp = subpixel_args(c, lo, cnt);
+  if (sp.z) {
+    const int rc = subpixel_streams(c, slot, lo, cnt, job_patches, q);
+    if (rc) return rc;
+  }
+  if (consensus_on(c, lo, cnt)) CU_TRY(c, sl2_launch_consensus(d, lo, cnt, c->cons_tau2, sp, q));
   return SL2_OK;
 }
 
@@ -338,6 +343,7 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   c->resc_chi2.assign(B, 0.0);
   ALLOC(c->warp_on_dev, B);
   c->warp_on.assign(B, 0);
+  c->subpix_on.assign(B, 0);
   ALLOC(c->sel_mode_dev, B);
   ALLOC(c->sel_t_dev, B);
   c->sel.assign(B, sl2_stream_selection{});
@@ -432,6 +438,8 @@ int sl2_set_features(sl2_ctx *c, int32_t s, int32_t n, const double *y, const do
   CU_TRY(c, cudaMemsetAsync(d.sel_rank + fb, 0xff, sizeof(int) * d.Nmax, c->stream));
   CU_TRY(c, cudaMemsetAsync(d.found + fb, 0, d.Nmax, c->stream));
   CU_TRY(c, cudaMemsetAsync(d.job_feat + fb, 0xff, sizeof(int) * d.Nmax, c->stream));
+  const int rc = subpixel_forget(c, s, 1);  // a new map has no refined matches
+  if (rc) return rc;
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   return SL2_OK;
 }
@@ -524,7 +532,8 @@ static int step_group(sl2_ctx *c, int32_t slot, int lo, int cnt, Sl2Queue q, cud
   if (after_search) CU_TRY(c, cudaEventRecord(after_search, st));
   cudaEvent_t evu[6];
   for (int i = 0; i < 6; ++i) evu[i] = c->evu[i].get();
-  CU_TRY(c, sl2_launch_update(d, lo, cnt, -1, nullptr, nullptr, nullptr, nullptr, nullptr, 0, q, t ? evu : nullptr));
+  const Sl2Subpix sp = subpixel_args(c, lo, cnt);
+  CU_TRY(c, sl2_launch_update(d, lo, cnt, -1, nullptr, nullptr, nullptr, nullptr, nullptr, 0, sp, q, t ? evu : nullptr));
   // the rescue and its second update are part of the update's time (ev[2] .. ev[3]); the update times are the first's
   const bool rescue = rescue_on(c, lo, cnt);
   if (rescue) {
@@ -532,7 +541,7 @@ static int step_group(sl2_ctx *c, int32_t slot, int lo, int cnt, Sl2Queue q, cud
     if (rc2) return rc2;
   }
   if (t) CU_TRY(c, cudaEventRecord(c->ev[3].get(), st));
-  CU_TRY(c, sl2_launch_cull(d, lo, cnt, -1, q));
+  CU_TRY(c, sl2_launch_cull(d, lo, cnt, -1, sp, q));
   if (t) CU_TRY(c, cudaEventRecord(c->ev[4].get(), st));
   if (d.rec_depth) {  // after ev[4]: the step times keep their meaning
     const Sl2Rescue r = rescue ? rescue_args(c) : Sl2Rescue{};
@@ -680,6 +689,23 @@ int sl2_last_step_times(sl2_ctx *c, float *ms4) {
   return SL2_OK;
 }
 
+}  // extern "C"
+
+// The copies of stream s's sub-pixel matches and refined flags, queued on the context's stream, when it has the
+// refinement on; zr and ref stay empty otherwise
+static int read_subpixel(sl2_ctx *c, int s, std::vector<double> &zr, std::vector<uint8_t> &ref) {
+  const Sl2Subpix sp = subpixel_args(c, s, 1);
+  if (!sp.z) return SL2_OK;
+  const size_t N = c->d.Nmax, fb = (size_t)s * N;
+  zr.resize(2 * N);
+  ref.resize(N);
+  CU_TRY(c, cudaMemcpyAsync(zr.data(), sp.z + fb * 2, 16 * N, cudaMemcpyDeviceToHost, c->stream));
+  CU_TRY(c, cudaMemcpyAsync(ref.data(), sp.refined + fb, N, cudaMemcpyDeviceToHost, c->stream));
+  return SL2_OK;
+}
+
+extern "C" {
+
 int sl2_get_feature_jacobians(sl2_ctx *c, int32_t s, double *dh_by_dxv, double *dh_by_dy, double *R,
                               double *nu) {
   if (bad_stream(c, s)) return fail(c, SL2_ERR_ARG, "bad stream");
@@ -695,6 +721,10 @@ int sl2_get_feature_jacobians(sl2_ctx *c, int32_t s, double *dh_by_dxv, double *
   CU_TRY(c, cudaMemcpyAsync(rv.data(), d.Rvar + fb, 8 * rv.size(), cudaMemcpyDeviceToHost, c->stream));
   CU_TRY(c, cudaMemcpyAsync(hh.data(), d.h + fb * 2, 8 * hh.size(), cudaMemcpyDeviceToHost, c->stream));
   CU_TRY(c, cudaMemcpyAsync(zz.data(), d.z_uv + fb * 2, 4 * zz.size(), cudaMemcpyDeviceToHost, c->stream));
+  std::vector<double> zr;
+  std::vector<uint8_t> ref;
+  int rc = read_subpixel(c, s, zr, ref);
+  if (rc) return rc;
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   for (int i = 0; i < nf; ++i) {
     if (dh_by_dxv)
@@ -704,7 +734,8 @@ int sl2_get_feature_jacobians(sl2_ctx *c, int32_t s, double *dh_by_dxv, double *
       for (int col = 0; col < 3; ++col)
         for (int r = 0; r < 2; ++r) dh_by_dy[i * 6 + col * 2 + r] = dy[i * 6 + r * 3 + col];
     if (R) { R[i * 4 + 0] = rv[i]; R[i * 4 + 1] = 0.0; R[i * 4 + 2] = 0.0; R[i * 4 + 3] = rv[i]; }
-    if (nu) { nu[i * 2] = (double)zz[i * 2] - hh[i * 2]; nu[i * 2 + 1] = (double)zz[i * 2 + 1] - hh[i * 2 + 1]; }
+    if (nu)
+      for (int k = 0; k < 2; ++k) nu[i * 2 + k] = (ref.empty() || !ref[i] ? (double)zz[i * 2 + k] : zr[i * 2 + k]) - hh[i * 2 + k];
   }
   return nf;
 }
@@ -737,12 +768,19 @@ int sl2_get_features(sl2_ctx *c, int32_t s, double *h, double *z, double *S, uin
   CU_TRY(c, cudaMemcpyAsync(at.data(), d.attempted + fb, 4 * (size_t)N, cudaMemcpyDeviceToHost, c->stream));
   CU_TRY(c, cudaMemcpyAsync(su.data(), d.successful + fb, 4 * (size_t)N, cudaMemcpyDeviceToHost, c->stream));
   CU_TRY(c, cudaMemcpyAsync(fd.data(), d.found + fb, N, cudaMemcpyDeviceToHost, c->stream));
+  std::vector<double> zr;
+  std::vector<uint8_t> ref;
+  const int rc = read_subpixel(c, s, zr, ref);
+  if (rc) return rc;
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   for (int i = 0; i < nf; ++i) {
     if (h) { h[2 * i] = hh[2 * i]; h[2 * i + 1] = hh[2 * i + 1]; }
-    if (z) { z[2 * i] = (double)zz[2 * i]; z[2 * i + 1] = (double)zz[2 * i + 1]; }
+    const bool refined = !ref.empty() && ref[i];
+    if (z)
+      for (int k = 0; k < 2; ++k) z[2 * i + k] = refined ? zr[2 * i + k] : (double)zz[2 * i + k];
     if (S) for (int k = 0; k < 4; ++k) S[4 * i + k] = SS[4 * i + k];
-    if (flags) flags[i] = (uint8_t)((rk[i] >= 0 ? 1 : 0) | (fd[i] == 1 ? 2 : 0) | (fd[i] == 2 ? 4 : 0));
+    if (flags) flags[i] = (uint8_t)((rk[i] >= 0 ? 1 : 0) | (fd[i] == 1 ? 2 : 0) | (fd[i] == 2 ? 4 : 0) |
+                                    (refined ? 8 : 0));
     if (attempted) attempted[i] = at[i];
     if (successful) successful[i] = su[i];
     if (select_rank) select_rank[i] = rk[i];

@@ -6,7 +6,7 @@
 // M = the job slots r < nsel whose feature has found == 1, in rank order (match j, k = |M| <= SL2_MAX_MEASURED);
 // x, P are the predicted state and covariance.  Every operation is one correctly rounded, never-fused op (rd), in
 // this order (tests/consensus_oracle.cpp restates it op for op):
-//   per match j:  nu = (double)z - h;  (Sinv00, Sinv01, Sinv11) = sinv_from_S(S00, S10, S11);
+//   per match j:  nu = z - h (z = the sub-pixel match of a refined match, else (double) the integer match);  (Sinv00, Sinv01, Sinv11) = sinv_from_S(S00, S10, S11);
 //                 w0 = Sinv00 nu0 + Sinv01 nu1;  w1 = Sinv01 nu0 + Sinv11 nu1;
 //                 a[c] = dh_dxp[0][c] w0 + dh_dxp[1][c] w1 (c < 7);  b[c] = dh_dy[0][c] w0 + dh_dy[1][c] w1 (c < 3)
 //   hypothesis i: xp'[r] = x[r] + s,  s = ((0 + P[r,0] a_i[0]) + ... + P[r,6] a_i[6]) + P[r,yi] b_i[0] + ...
@@ -32,7 +32,8 @@ namespace {
 #define CONS_WARPS 8
 #define CONS_WORDS (SL2_MAX_MEASURED / 32)
 __global__ void __launch_bounds__(32 * CONS_WARPS) consensus_kernel(const Sl2Dev d, int stream_lo,
-                                                                  const double *__restrict__ tau2) {
+                                                                  const double *__restrict__ tau2,
+                                                                  const Sl2Subpix sp) {
   pdl_prologue();
   const int s = stream_lo + blockIdx.x;
   const double t2 = tau2[s];
@@ -74,7 +75,7 @@ __global__ void __launch_bounds__(32 * CONS_WARPS) consensus_kernel(const Sl2Dev
   for (int j = tid; j < k; j += blockDim.x) {
     const size_t g = fb + mf[j];
     const int pos = SL2_NXV + 3 * mf[j];
-    const rd zu((double)d.z_uv[g * 2]), zv((double)d.z_uv[g * 2 + 1]);
+    const rd zu(match_z(d, sp, g, 0)), zv(match_z(d, sp, g, 1));
     const rd nu0 = zu - rd(d.h[g * 2]), nu1 = zv - rd(d.h[g * 2 + 1]);
     rd si[3];
     sinv_from_S(rd(d.S[g * 4 + 0]), rd(d.S[g * 4 + 1]), rd(d.S[g * 4 + 3]), si);
@@ -139,10 +140,11 @@ __global__ void write_double_kernel(double *dst, const double v) { *dst = v; }
 
 }  // namespace
 
-cudaError_t sl2_launch_consensus(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *tau2_dev, Sl2Queue q) {
+cudaError_t sl2_launch_consensus(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *tau2_dev,
+                                 const Sl2Subpix &sp, Sl2Queue q) {
   if (stream_cnt <= 0) return cudaSuccess;
   return sl2_launch_kernel(consensus_kernel, dim3(stream_cnt), dim3(32 * CONS_WARPS), 0, q, sl2_use_pdl(stream_cnt), d,
-                           stream_lo, tau2_dev);
+                           stream_lo, tau2_dev, sp);
 }
 
 extern "C" {

@@ -377,7 +377,8 @@ __global__ void __launch_bounds__(128) particle_predict_kernel(const Sl2Dev d, i
 // kernel 3: delete_bad_features (monoslam.cpp:644-703) / delete_feature (:770-812)
 // removes the rows/columns of the culled features from x and P in place.
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) cull_kernel(const Sl2Dev d, int stream_lo, int force_index) {
+__global__ void __launch_bounds__(256) cull_kernel(const Sl2Dev d, int stream_lo, int force_index,
+                                                    const Sl2Subpix sp) {
   pdl_prologue();
   const int s = stream_lo + blockIdx.x;
   const int tid = threadIdx.x;
@@ -464,7 +465,14 @@ __global__ void __launch_bounds__(256) cull_kernel(const Sl2Dev d, int stream_lo
     for (int e = 0; e < per; ++e) d.name[(fb + k) * per + e] = d.name[(fb + i) * per + e];
       SL2_STREAM_ARRAYS(SL2_MOVE)
 #undef SL2_MOVE
+      if (sp.z) {  // and so does its sub-pixel match
+        sp.z[(fb + k) * 2 + 0] = sp.z[(fb + i) * 2 + 0];
+        sp.z[(fb + k) * 2 + 1] = sp.z[(fb + i) * 2 + 1];
+        sp.refined[fb + k] = sp.refined[fb + i];
+      }
     }
+    if (sp.z)  // the vacated slots hold no match: a feature appended there starts unrefined
+      for (int i = nk; i < nf; ++i) sp.refined[fb + i] = 0;
     // the job list of this step indexes the old feature numbering: rebuild it from the compacted ranks
     for (int r = 0; r < d.Nmax; ++r) d.job_feat[fb + r] = -1;
     int nsel_new = 0;
@@ -550,10 +558,11 @@ cudaError_t sl2_launch_particle_predict(const Sl2Dev &d, int s, int F, int Kmax,
                            lambda, h, sinv3, detS);
 }
 
-cudaError_t sl2_launch_cull(const Sl2Dev &d, int stream_lo, int stream_cnt, int force_index, Sl2Queue q) {
+cudaError_t sl2_launch_cull(const Sl2Dev &d, int stream_lo, int stream_cnt, int force_index, const Sl2Subpix &sp,
+                            Sl2Queue q) {
   if (stream_cnt <= 0) return cudaSuccess;
   return sl2_launch_kernel(cull_kernel, dim3(stream_cnt), dim3(256), 0, q, sl2_use_pdl(stream_cnt), d,
-                           stream_lo, force_index);
+                           stream_lo, force_index, sp);
 }
 
 extern "C" {
@@ -586,7 +595,7 @@ int sl2_delete_feature(sl2_ctx *c, int32_t s, int32_t index) {
   const int n = sl2_num_features(c, s);
   if (n < 0) return n;
   if (index < 0 || index >= n) return fail(c, SL2_ERR_ARG, "sl2_delete_feature: bad index");
-  CU_TRY(c, sl2_launch_cull(c->d, s, 1, index, queue(c)));
+  CU_TRY(c, sl2_launch_cull(c->d, s, 1, index, subpixel_args(c, s, 1), queue(c)));
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   return SL2_OK;
 }

@@ -10,7 +10,7 @@
 // tests/rescue_oracle.cpp restate it):
 //   predict_feature(x', P', y'_j) (sl2_model.cuh, predict_kernel's own code): h', dh/dxp', dh/dy', R' = var' I,
 //   S' = H' P' H'^T + R', depth' = camera-frame depth of y'_j;
-//   nu0 = (double)z_u - h'0, nu1 = (double)z_v - h'1;  (Si00, Si01, Si11) = sinv_from_S(S'00, S'10, S'11);
+//   nu0 = z_u - h'0, nu1 = z_v - h'1 (z: the consensus's match, sub-pixel when refined);  (Si00, Si01, Si11) = sinv_from_S(S'00, S'10, S'11);
 //   w0 = Si00 nu0 + Si01 nu1;  w1 = Si01 nu0 + Si11 nu1;  q = nu0 w0 + nu1 w1;
 //   rescued iff depth' > 0 and q <= chi2 (NaN: never): found = SL2_FOUND_RESCUED, and h, S, Rvar, dh_dxp, dh_dy take
 //   the re-prediction.
@@ -30,7 +30,8 @@ constexpr int RESC_THREADS = 256;  // update_sums reduces over 256 slots; the ga
 static_assert(SL2_MAX_MEASURED <= RESC_THREADS, "one thread per job slot");
 
 __global__ void __launch_bounds__(RESC_THREADS) rescue_kernel(const Sl2Dev d, int stream_lo, const double *chi2,
-                                                              const double *tau2, double *nis1, double *logdet1) {
+                                                              const double *tau2, double *nis1, double *logdet1,
+                                                              const Sl2Subpix sp) {
   pdl_prologue();
   const int s = stream_lo + blockIdx.x;
   const double c2 = chi2[s];
@@ -75,7 +76,7 @@ __global__ void __launch_bounds__(RESC_THREADS) rescue_kernel(const Sl2Dev d, in
     const rd yi[3] = {rd(x[pos]), rd(x[pos + 1]), rd(x[pos + 2])};
     FeatPred fp;
     predict_feature(sc.cam, xv, yi, Pxx, P + (size_t)ld * pos, ld, pos, fp);
-    const rd nu0 = rd((double)d.z_uv[g * 2]) - fp.h[0], nu1 = rd((double)d.z_uv[g * 2 + 1]) - fp.h[1];
+    const rd nu0 = rd(match_z(d, sp, g, 0)) - fp.h[0], nu1 = rd(match_z(d, sp, g, 1)) - fp.h[1];
     rd si[3];
     sinv_from_S(fp.S[0][0], fp.S[1][0], fp.S[1][1], si);
     const rd w0 = si[0] * nu0 + si[1] * nu1, w1 = si[1] * nu0 + si[2] * nu1;
@@ -99,12 +100,13 @@ __global__ void __launch_bounds__(RESC_THREADS) rescue_kernel(const Sl2Dev d, in
 
 }  // namespace
 
-cudaError_t sl2_launch_rescue(const Sl2Dev &d, int stream_lo, int stream_cnt, const Sl2Rescue &r, Sl2Queue q) {
+cudaError_t sl2_launch_rescue(const Sl2Dev &d, int stream_lo, int stream_cnt, const Sl2Rescue &r, const Sl2Subpix &sp,
+                              Sl2Queue q) {
   if (stream_cnt <= 0) return cudaSuccess;
   const cudaError_t e = sl2_launch_kernel(rescue_kernel, dim3(stream_cnt), dim3(RESC_THREADS), 0, q,
-                                          sl2_use_pdl(stream_cnt), d, stream_lo, r.chi2, r.tau2, r.nis1, r.logdet1);
+                                          sl2_use_pdl(stream_cnt), d, stream_lo, r.chi2, r.tau2, r.nis1, r.logdet1, sp);
   if (e != cudaSuccess) return e;
-  return sl2_launch_update_rescued(d, stream_lo, stream_cnt, r.m2, q);
+  return sl2_launch_update_rescued(d, stream_lo, stream_cnt, r.m2, sp, q);
 }
 
 namespace sl2 {
@@ -128,7 +130,7 @@ Sl2Rescue rescue_args(const sl2_ctx *c) {
 }
 
 int rescue_streams(sl2_ctx *c, int lo, int cnt, Sl2Queue q) {
-  CU_TRY(c, sl2_launch_rescue(c->d, lo, cnt, rescue_args(c), q));
+  CU_TRY(c, sl2_launch_rescue(c->d, lo, cnt, rescue_args(c), subpixel_args(c, lo, cnt), q));
   return SL2_OK;
 }
 

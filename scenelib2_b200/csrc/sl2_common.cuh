@@ -252,7 +252,7 @@ inline bool sl2_box_supported(int box) {
 }
 
 // launchers that files other than their own call (defined in search.cu / ekf.cu / select.cu / consensus.cu / warp.cu /
-// update.cu / records.cu / particles.cu)
+// subpixel.cu / update.cu / records.cu / particles.cu)
 struct SearchLaunch {
   // job arrays may be the context's own (fused step) or temporaries (staged API)
   const int *job_feat;       // [njobs_per_stream * B] or [n]
@@ -295,19 +295,44 @@ struct SelectLaunch {
   int gstride;      // picks per candidate in g: kmax in the scratch, else the most any stream of the launch makes
 };
 cudaError_t sl2_launch_select(const Sl2Dev &d, const SelectLaunch &L, Sl2Queue q);
+// The sub-pixel matches (subpixel.cu) the kernels that read a match take as an argument: z [B][Nmax][2] and refined
+// [B][Nmax], feature-indexed like Sl2Dev::z_uv.  z == nullptr when no stream of the launch has the refinement on; a
+// stream with it off has every refined flag 0.
+struct Sl2Subpix {
+  double *z;
+  uint8_t *refined;
+};
+// The match z of feature record f (s * Nmax + i), coordinate k, that the consensus, the update and the rescue use
+__device__ __forceinline__ double match_z(const Sl2Dev &d, const Sl2Subpix &sp, size_t f, int k) {
+  return (sp.z && sp.refined[f]) ? sp.z[f * 2 + k] : (double)d.z_uv[f * 2 + k];
+}
+// The refinement of the streams [stream_lo, stream_lo + stream_cnt) whose on[s] is 1, right after their search: every
+// job's match into out.z / out.refined
+struct SubpixelLaunch {
+  int stream_lo, stream_cnt;
+  int slot;                    // the frame ring slot the search read
+  const uint8_t *on;           // [B]
+  const uint8_t *job_patches;  // the search's SearchLaunch::job_patches: [jobs][box][16], or nullptr: d.patches[feat]
+  Sl2Subpix out;
+};
+cudaError_t sl2_launch_subpixel(const Sl2Dev &d, const SubpixelLaunch &L, Sl2Queue q);
 // match consensus of the streams [stream_lo, stream_lo + stream_cnt) between the search and the update; tau2_dev[s] =
 // the squared inlier radius of stream s, 0 = off (consensus.cu)
-cudaError_t sl2_launch_consensus(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *tau2_dev, Sl2Queue q);
+cudaError_t sl2_launch_consensus(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *tau2_dev,
+                                 const Sl2Subpix &sp, Sl2Queue q);
 // EKF update = 5 kernels (hp, chol, solve, syrk, finish); ev6 (optional) = 6 events recorded around them
 cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, int staged_m,
                               const int *st_feat, const double *st_Hxv, const double *st_Hy,
                               const double *st_R, const double *st_nu, int only_normalise,
-                              Sl2Queue q, cudaEvent_t *ev6 = nullptr);
+                              const Sl2Subpix &sp, Sl2Queue q, cudaEvent_t *ev6 = nullptr);
 // The second update of the consensus rescue: the five update kernels over the rows whose found is SL2_FOUND_RESCUED,
 // with m2 (instead of Sl2Dev::upd_m) holding each stream's row count, 0 for a stream with nothing rescued, which the
 // five kernels then leave as they found it (update.cu)
-cudaError_t sl2_launch_update_rescued(const Sl2Dev &d, int stream_lo, int stream_cnt, int *m2, Sl2Queue q);
-cudaError_t sl2_launch_cull(const Sl2Dev &d, int stream_lo, int stream_cnt, int force_index, Sl2Queue q);
+cudaError_t sl2_launch_update_rescued(const Sl2Dev &d, int stream_lo, int stream_cnt, int *m2, const Sl2Subpix &sp,
+                                      Sl2Queue q);
+// sp: the sub-pixel matches move with their features
+cudaError_t sl2_launch_cull(const Sl2Dev &d, int stream_lo, int stream_cnt, int force_index, const Sl2Subpix &sp,
+                            Sl2Queue q);
 // The consensus rescue (rescue.cu): chi2[s] (0 = off) and the consensus's tau2[s] of every stream, and the per-stream
 // scratch the step records read: m2 = rows of the second update, nis1 / logdet1 = the first update's NIS and log det S
 struct Sl2Rescue {
@@ -316,7 +341,8 @@ struct Sl2Rescue {
   double *nis1, *logdet1;     // [B]
 };
 // rescue_kernel then the second update of the streams [stream_lo, stream_lo + stream_cnt), after their first update
-cudaError_t sl2_launch_rescue(const Sl2Dev &d, int stream_lo, int stream_cnt, const Sl2Rescue &r, Sl2Queue q);
+cudaError_t sl2_launch_rescue(const Sl2Dev &d, int stream_lo, int stream_cnt, const Sl2Rescue &r, const Sl2Subpix &sp,
+                              Sl2Queue q);
 // The gyroscope update (gyro.cu) of the streams [stream_lo, stream_lo + stream_cnt) whose on[s] is 1, between their
 // motion prediction and their feature prediction: stream s reads its sample at index s - sample_lo of rate (3 doubles
 // each) and valid, and consumes it (valid = 0)

@@ -135,6 +135,10 @@ struct sl2_ctx {
   Sl2GyroParam *gyro_prm = nullptr;
   double *gyro_rate = nullptr, *gyro_W = nullptr, *gyro_nis = nullptr;
   int *gyro_status = nullptr;
+  // sub-pixel refinement (sl2_set_stream_subpixel): the host mirror of every stream's setting, and one device buffer
+  // (allocated when a stream first turns it on): z [B][Nmax][2] doubles, refined [B][Nmax] and the on flags [B]
+  std::vector<uint8_t> subpix_on;  // [B]
+  sl2::DevPtr<uint8_t> subpix_buf;
 };
 
 namespace sl2 {
@@ -267,5 +271,12 @@ int rescue_streams(sl2_ctx *c, int lo, int cnt, Sl2Queue q);
 // samples of ring slot `slot`, between their motion prediction and their feature prediction
 bool gyro_on(const sl2_ctx *c, int lo, int cnt);
 int gyro_streams(sl2_ctx *c, int slot, int lo, int cnt, Sl2Queue q);
+// subpixel.cu: the sub-pixel matches the kernels of the streams [lo, lo + cnt) read ({} when none of them has the
+// refinement on); the refinement of those streams on q, right after their search of ring slot `slot` (job_patches: the
+// search's templates); a load forgets the refinement of the streams [lo, lo + cnt): their z is the integer match until
+// their next step
+Sl2Subpix subpixel_args(const sl2_ctx *c, int lo, int cnt);
+int subpixel_streams(sl2_ctx *c, int slot, int lo, int cnt, const uint8_t *job_patches, Sl2Queue q);
+int subpixel_forget(sl2_ctx *c, int lo, int cnt);
 
 }  // namespace sl2

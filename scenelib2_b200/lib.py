@@ -76,6 +76,7 @@ EXPORTS = [
     "sl2_set_stream_config", "sl2_get_stream_config", "sl2_set_stream_consensus", "sl2_get_stream_consensus",
     "sl2_set_stream_rescue", "sl2_get_stream_rescue",
     "sl2_set_stream_warp", "sl2_get_stream_warp", "sl2_warp_templates",
+    "sl2_set_stream_subpixel", "sl2_get_stream_subpixel",
     "sl2_set_stream_selection", "sl2_get_stream_selection",
     "sl2_set_stream_gyro", "sl2_get_stream_gyro", "sl2_set_gyro_samples", "sl2_gyro_update", "sl2_get_gyro_results",
     "sl2_set_frame", "sl2_set_frames", "sl2_set_frames_dev",
@@ -239,6 +240,8 @@ def load():
         L.sl2_get_stream_rescue.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_double)]
         L.sl2_set_stream_warp.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
         L.sl2_get_stream_warp.argtypes = [C.c_void_p, C.c_int32, i32p]
+        L.sl2_set_stream_subpixel.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
+        L.sl2_get_stream_subpixel.argtypes = [C.c_void_p, C.c_int32, i32p]
         L.sl2_set_stream_selection.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamSelection)]
         L.sl2_get_stream_selection.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamSelection)]
         L.sl2_set_stream_gyro.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamGyro)]
@@ -394,6 +397,17 @@ class Context:
     def get_stream_warp(self, stream_id):
         v = C.c_int32()
         self._ck(self.L.sl2_get_stream_warp(self.h, stream_id, C.byref(v)))
+        return v.value
+
+    # ---- sub-pixel refinement ---------------------------------------------------------------------
+    def set_stream_subpixel(self, stream_id, on):
+        """sl2_set_stream_subpixel: refine the stream's matches to the minimum of a quadratic fit of the search's score
+        around them (1) or keep the integer matches (0, the default)."""
+        self._ck(self.L.sl2_set_stream_subpixel(self.h, stream_id, int(on)))
+
+    def get_stream_subpixel(self, stream_id):
+        v = C.c_int32()
+        self._ck(self.L.sl2_get_stream_subpixel(self.h, stream_id, C.byref(v)))
         return v.value
 
     def warp_templates(self, stream_id, feat_index, xp):
