@@ -163,7 +163,9 @@ int sl2_get_stream_rescue(sl2_ctx *ctx, int32_t stream_id, double *chi2);
  * y = the feature's state, xo = its xp_org,
  *   h = project_point(zeroed_point(y) from xp) (the prediction's h, bit for bit), ho = the same from xo (the centre of
  *   the stored template); the plane passes through y with world normal nW = xo[0:3] - y (not normalised);
- *   output pixel (row a, column b): p = h + (b - HALF, a - HALF); dW = RRW^T unproject_point(p);
+ *   output pixel (row a, column b): p = h + (b - HALF, a - HALF); dW = adj(RRW) unproject_point(p), RRW = the
+ *   matrix of xp (pose_RRW) and adj(RRW) = det(RRW) RRW^-1 (RRW is a rotation only when |q| = 1, and det(RRW) >= 0, so
+ *   dW points along the ray that the camera at xp sees at p);
  *   t = (nW . (y - r)) / (nW . dW); X = r + t dW; zo = RRW(xo) (X - xo[0:3]); src = project_point(zo) - ho + (HALF, HALF);
  *   the pixel is valid when t is finite and > 0, zo[2] > 0 and src is finite;
  *   bilinear sampling of the stored template T: each coordinate of src clamped to [0, B - 1], x0 = min(floor(sx),
@@ -172,7 +174,7 @@ int sl2_get_stream_rescue(sl2_ctx *ctx, int32_t stream_id, double *chi2);
  * Source positions outside the stored template repeat its edge pixels: a B x B template holds nothing beyond itself,
  * which a warp that shrinks it (the camera moving away, a slanted view) would need.  When any pixel of a feature is
  * invalid its warped template is its stored template (valid = 0).  Every operation is a correctly rounded FP64
- * operation in the order written in the device code (csrc/sl2_model.cuh: patch_warp_setup, patch_warp_source,
+ * operation in the order written in the device code (csrc/sl2_model.cuh: mat3_adj, patch_warp_setup, patch_warp_source,
  * patch_sample; dot products and matrix rows summed from 0.0 in ascending order), so the bytes are reproducible bit
  * for bit.
  * Where it applies: the search of the fused step (sl2_step, sl2_step_host, sl2_step_host_async) and of

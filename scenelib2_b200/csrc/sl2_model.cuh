@@ -142,20 +142,31 @@ __device__ __forceinline__ rd dot3(const rd a[3], const rd b[3]) {
   return s;
 }
 
+// adj(M): A[i][j] = M[j+1][i+1] M[j+2][i+2] - M[j+1][i+2] M[j+2][i+1] (indices mod 3), so that A M = det(M) I
+__device__ __forceinline__ void mat3_adj(const rd M[3][3], rd A[3][3]) {
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) {
+      const int j1 = (j + 1) % 3, j2 = (j + 2) % 3, i1 = (i + 1) % 3, i2 = (i + 2) % 3;
+      A[i][j] = M[j1][i1] * M[j2][i2] - M[j1][i2] * M[j2][i1];
+    }
+}
+
 // What one feature's warp at the camera pose xp shares over its pixels: the feature y seen from xp (h, bit for bit the
-// prediction's) and from xo = xp_org (ho, the template centre), the plane through y with normal nW = xo[0:3] - y and
+// prediction's) and from xo = xp_org (ho, the template centre), adj(RRW) (the ray's matrix: RRW is a rotation only
+// for |q| = 1, quirk Q1, so RRW^T is not its inverse), the plane through y with normal nW = xo[0:3] - y and
 // num = nW . (y - r)
 struct PatchWarp {
-  rd RRW[3][3], RRWo[3][3];  // pose_RRW(xp), pose_RRW(xo)
+  rd adj[3][3], RRWo[3][3];  // adj(pose_RRW(xp)), pose_RRW(xo)
   rd nW[3], num;
   rd h[2], ho[2];
 };
 __device__ __forceinline__ void patch_warp_setup(const double *cam, const double *xp, const double *xo, const rd y[3],
                                                  PatchWarp &w) {
-  rd d[3], z[3], uc, vc;
-  pose_RRW(xp, w.RRW);
-  zeroed_point(w.RRW, y, xp, d, z);
+  rd d[3], z[3], uc, vc, RRW[3][3];
+  pose_RRW(xp, RRW);
+  zeroed_point(RRW, y, xp, d, z);
   project_point(cam, z, w.h, uc, vc);
+  mat3_adj(RRW, w.adj);
   rd dox[3], zo[3];
   pose_RRW(xo, w.RRWo);
   zeroed_point(w.RRWo, y, xo, dox, zo);
@@ -165,18 +176,15 @@ __device__ __forceinline__ void patch_warp_setup(const double *cam, const double
 }
 
 // The source position in the stored template of the output pixel at offset (db, da) (column, row) from the centre:
-// p = h + (db, da); dW = RRW^T unproject_point(p); t = num / (nW . dW); X = r + t dW; zo = RRWo (X - xo[0:3]);
+// p = h + (db, da); dW = adj(RRW) unproject_point(p) (= det(RRW) RRW^-1 unproject_point(p), det(RRW) >= 0, and X does
+// not change with the scale of dW); t = num / (nW . dW); X = r + t dW; zo = RRWo (X - xo[0:3]);
 // src = project_point(zo) - ho + (half, half).  True when the pixel is valid: t finite and > 0, zo[2] > 0, src finite.
 __device__ __forceinline__ bool patch_warp_source(const double *cam, const PatchWarp &w, const double *xp,
                                                   const double *xo, int db, int da, int half, rd src[2]) {
   const rd p[2] = {w.h[0] + rd((double)db), w.h[1] + rd((double)da)};
   rd c[3], dW[3];
   unproject_point(cam, p, c);
-  for (int i = 0; i < 3; ++i) {
-    rd s(0.0);
-    for (int k = 0; k < 3; ++k) s = s + w.RRW[k][i] * c[k];
-    dW[i] = s;
-  }
+  mat3_vec(w.adj, c, dW);
   const rd t = w.num / dot3(w.nW, dW);
   rd e[3], zo[3];
   for (int i = 0; i < 3; ++i) e[i] = (rd(xp[i]) + t * dW[i]) - rd(xo[i]);

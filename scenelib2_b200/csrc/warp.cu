@@ -6,7 +6,8 @@
 // pixel (a, b) of the warped template at pose xp is the point of that plane the camera at xp sees at h + (b - HALF,
 // a - HALF), projected into the camera at xp_org[i] and sampled bilinearly from the stored template there
 // (patch_warp_setup, patch_warp_source, patch_sample in sl2_model.cuh: every operation one correctly rounded,
-// never-fused op in the order written; tests/warp_ref.py restates them op for op).
+// never-fused op in the order written; tests/warp_ref.py restates them op for op, tests/warp_truth.py states the
+// geometry from its definition).
 // Shape: one warp per job, WARP_WARPS jobs per CTA; the lanes take the bytes of the row-padded output (col < BOX is a
 // pixel, the rest the zero padding); the stored template is staged in shared memory.  A stream whose setting is off
 // gets its stored templates copied, so the search reads every job of the launch from one place.

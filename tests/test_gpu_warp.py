@@ -166,10 +166,13 @@ def scene(kind):
 
 # ---- 2. the measure stage against the oracle's search with the restatement's templates ----------------------------
 @pytest.mark.gpu
-def test_measure_stage_equals_the_oracle_search_of_warped_templates():
+def test_measure_stage_equals_the_oracle_search_of_templates_warped_at_non_unit_q():
+    """The search of a warp-on stream reads the restatement's templates at the predicted x[0:7], whose |q| drifts from
+    1 (x is never renormalised), so the rays go through RRW^-1 and not RRW^T."""
     sc = scene("roll")
     ctx = scene_ctx([sc])
     cam8 = sc.cam8
+    drift = 0.0
     try:
         ctx.set_stream_warp(0, 1)
         assert ctx.get_stream_warp(0) == 1
@@ -178,6 +181,7 @@ def test_measure_stage_equals_the_oracle_search_of_warped_templates():
             ctx.ekf_predict(0)
             ctx.predict_measurements(0)
             x, _ = ctx.get_state(0)
+            drift = max(drift, abs(float(np.dot(x[3:7], x[3:7])) - 1.0))
             cnt = ctx.make_measurements(0, 0)
             snap = sl2.read_snapshot(ctx.save_stream(0))
             nsel = snap["nsel"]
@@ -194,6 +198,7 @@ def test_measure_stage_equals_the_oracle_search_of_warped_templates():
             assert snap["best"][jf].tobytes() == best.tobytes(), t
             assert cnt == int(found.sum())
             ctx.ekf_update_measured(0)
+        assert drift > 0.0
     finally:
         ctx.close()
 

@@ -1,4 +1,4 @@
-"""The planar patch warp (include/sl2b200.h, sl2_set_stream_warp; csrc/sl2_model.cuh: patch_warp_setup,
+"""The planar patch warp (include/sl2b200.h, sl2_set_stream_warp; csrc/sl2_model.cuh: mat3_adj, patch_warp_setup,
 patch_warp_source, patch_sample) restated in NumPy, one IEEE double operation at a time in the kernel's order (NumPy's
 element-wise operations are correctly rounded and never fused), vectorised over the template's pixels.  The camera
 model is tests/camera_ref.py's, with unproject_point stated here."""
@@ -22,15 +22,28 @@ def _dot(a, b):
     return ((0.0 + a[0] * b[0]) + a[1] * b[1]) + a[2] * b[2]
 
 
+def adjugate(M):
+    """mat3_adj: A[i][j] = M[j+1][i+1] M[j+2][i+2] - M[j+1][i+2] M[j+2][i+1] (indices mod 3), A M = det(M) I."""
+    return [[M[(j + 1) % 3][(i + 1) % 3] * M[(j + 2) % 3][(i + 2) % 3]
+             - M[(j + 1) % 3][(i + 2) % 3] * M[(j + 2) % 3][(i + 1) % 3] for j in range(3)] for i in range(3)]
+
+
 def warp_source(cam8, B, y, xo, xp):
     """src (B, B, 2) positions in the stored template of every output pixel (row a, column b) and their validity
     (B, B) for the feature y (3) first seen from xo (7), at the camera pose xp (7); also h, the template's centre at
     xp."""
+    src, valid, h, _ = warp_points(cam8, B, y, xo, xp)
+    return src, valid, h
+
+
+def warp_points(cam8, B, y, xo, xp):
+    """warp_source, and also X (B, B, 3): the plane point each pixel's ray meets."""
     half = (B - 1) // 2
     y = [float(v) for v in y]
     xo = [float(v) for v in xo]
     xp = [float(v) for v in xp]
     R, Ro = rrw(xp), rrw(xo)
+    A = adjugate(R)
     h = project_point(cam8, camera_points(xp, y))[0]
     ho = project_point(cam8, camera_points(xo, y))[0]
     d = [y[i] - xp[i] for i in range(3)]
@@ -42,14 +55,15 @@ def warp_source(cam8, B, y, xo, xp):
     c0, c1 = unproject_point(cam8, p0, p1)
     c = [c0, c1, np.ones_like(c0)]
     with np.errstate(all="ignore"):
-        dW = [((0.0 + R[0][i] * c[0]) + R[1][i] * c[1]) + R[2][i] * c[2] for i in range(3)]
+        dW = [((0.0 + A[i][0] * c[0]) + A[i][1] * c[1]) + A[i][2] * c[2] for i in range(3)]
         t = num / _dot(nW, dW)
-        e = [(xp[i] + t * dW[i]) - xo[i] for i in range(3)]
+        X = [xp[i] + t * dW[i] for i in range(3)]
+        e = [X[i] - xo[i] for i in range(3)]
         zo = np.stack([((0.0 + Ro[i][0] * e[0]) + Ro[i][1] * e[1]) + Ro[i][2] * e[2] for i in range(3)], axis=-1)
         g = project_point(cam8, zo.reshape(-1, 3)).reshape(B, B, 2)
         src = np.stack([(g[..., 0] - ho[0]) + float(half), (g[..., 1] - ho[1]) + float(half)], axis=-1)
         valid = np.isfinite(t) & (t > 0.0) & (zo[..., 2] > 0.0) & np.isfinite(src).all(axis=-1)
-    return src, valid, h
+    return src, valid, h, np.stack(X, axis=-1)
 
 
 def sample(T, src):
