@@ -356,6 +356,66 @@ int sl2_gyro_update(sl2_ctx *ctx, int32_t stream_id, const double *rate3);
  * part of a snapshot.  Joins both step groups and synchronises.  SL2_ERR_ARG for a bad range. */
 int sl2_get_gyro_results(sl2_ctx *ctx, int32_t lo, int32_t cnt, double *nis, int32_t *status);
 
+/* ---- iterated update: relinearise the EKF update at the updated state (no reference counterpart) -------------------
+ * The plain update evaluates h and H once, at the prediction.  When an innovation is large against the curvature of h
+ * (a feature whose depth is still uncertain along its ray) that linearisation is wrong to first order: the posterior
+ * does not minimise the cost it stands for and its covariance is over-confident.  The iterated update is Gauss-Newton
+ * on J(x) = |x - x0|^2_{P0^-1} + sum |z - h(x)|^2_{R^-1} (Bell & Cathey, "The iterated Kalman filter update as a
+ * Gauss-Newton method", IEEE TAC 1993).
+ * Definitions: x0, P0 are the state and covariance after the prediction (after the gyro update when that is on); M are
+ * the step's measured rows (found == 1 after the consensus, in rank order) and z their matches (sub-pixel when
+ * refined); R is the prediction's Rvar I and stays fixed; L_0 is the prediction's linearisation, h_eff = h with
+ * Hxp = dh/dxp and Hy = dh/dy; N = max_iterations.
+ *   for i = 0 .. N-1:
+ *     pass i at L_i: S_i = H_i P0 H_i^T + R = U^T U, nu_i = z - h_eff_i (upd_hp and upd_chol, as the update forms them)
+ *       t = S_i^-1 nu_i: forward, for every 16-row panel p (rows p0 .. p0 + nb - 1) in order, w_a = sum_b W_pp[a][b]
+ *       r_b (b = 0 .. nb-1 in order, from the first product), then every later row j: r_j = r_j - U(p0 + a, j) w_a for
+ *       a = 0 .. nb-1 in order (r starts as nu); backward, for every panel from the last, t_a = sum_b W_pp[b][a] r_b
+ *       (b in order), then every earlier row j: r_j = r_j - U(j, p0 + a) t_a for a in order (r starts as w).
+ *       W_pp = U_pp^-T is the panel inverse upd_chol forms.
+ *       x_{i+1}[j] = x0[j] + sum_r (H_i P0)(r, j) t_r (r = 0 .. m-1 in order, from the first product), j < n.
+ *     delta_i = max over j < n with P0(j, j) > 0 of |x_{i+1}[j] - x_i[j]| / sqrt(P0(j, j)), x_0 = x0; NaN when an
+ *       entry of x_{i+1} is not finite.
+ *     delta_i <= tol: status 1 (converged), stop; the final update uses L_i.
+ *     relinearise every row of M at x_{i+1} with the prediction's model code (q not renormalised): h, Hxp, Hy;
+ *       dx = x0[0:7] - x_{i+1}[0:7], dy = y0 - y_{i+1}; h_eff[r] = h[r] + (((Hxp[r][0] dx0 + Hxp[r][1] dx1) + ...
+ *       + Hxp[r][6] dx6) + Hy[r][0] dy0 + ... + Hy[r][2] dy2), left to right.  Invalid when x_{i+1} has a non-finite
+ *       entry, a camera-frame depth is <= 0 or any h_eff, Hxp, Hy is not finite: status 3, stop; the final update
+ *       uses L_i.  Else L_{i+1}, iterations = i + 1.
+ *   the loop ran out: status 2; the final update uses L_N.
+ *   final update: the ordinary five-kernel update at L_final from x0, P0 (normalisation, symmetrisation, counters).
+ * Every operation above is one correctly rounded, never-fused FP64 operation in the order written (csrc/iterate.cu,
+ * iterate_kernel; tests/iterate_ref.py restates it).  max_iterations = 0 is off.  A stream whose pass 0 converges ends
+ * byte-identical to the plain update: its final update reads L_0.
+ * Where it applies: the fused step (sl2_step, sl2_step_host, sl2_step_host_async) and sl2_ekf_update_measured.
+ * sl2_ekf_update with the caller's rows never iterates, and the consensus rescue's second update stays one pass (its
+ * re-prediction is at the iterated posterior).  Unchanged: sl2_get_features and sl2_get_feature_jacobians show the
+ * step's prediction (h, H, nu = z - h at x0); step records keep their layout, and their m, nis and logdet_s describe
+ * the final update; sl2_last_update_times times the final update, sl2_last_step_times()[2] includes the passes.
+ * Cost: a step group holding a stream with the iteration on runs N_g = the largest max_iterations of its streams
+ * passes of three launches (upd_hp, upd_chol, iterate_kernel) before its update; a stream that has stopped costs an
+ * early return per launch.  A context where no stream has it on runs exactly the path without it.
+ * tol is in standard deviations of the prior: 0 always runs N relinearisations.  The setting belongs to the stream
+ * slot, like the match consensus: snapshots do not carry it and a load leaves it.  A call clears the stream's results.
+ * The first stream turned on allocates the context's iteration buffer (num_streams x max_features x 22 doubles of
+ * tables, num_streams x (13 + 3 max_features, rounded up to 8) doubles of iterate and the settings and results):
+ * SL2_ERR_CUDA, with the setting unchanged, when that fails.  SL2_ERR_ARG, with the setting unchanged, for a bad
+ * stream_id or NULL v, reserved != 0, max_iterations outside [0, SL2_MAX_ITERATIONS], or a tol that is not finite and
+ * >= 0. */
+#define SL2_MAX_ITERATIONS 8
+typedef struct sl2_stream_iterated {
+  int32_t max_iterations; /* 0 (default, off) .. SL2_MAX_ITERATIONS relinearisations */
+  int32_t reserved;       /* 0 */
+  double tol;             /* stop when the step is at most tol prior standard deviations in every entry; >= 0 */
+} sl2_stream_iterated;
+int sl2_set_stream_iterated(sl2_ctx *ctx, int32_t stream_id, const sl2_stream_iterated *v);
+int sl2_get_stream_iterated(sl2_ctx *ctx, int32_t stream_id, sl2_stream_iterated *v);
+/* The last step of streams [lo, lo + cnt): iterations (relinearisations used by the final update), status (0: off or
+ * no measured rows, 1 converged, 2 ran out, 3 invalid relinearisation) and the last delta.  Any pointer may be NULL.
+ * Not part of a snapshot.  Joins both step groups and synchronises.  SL2_ERR_ARG for a bad range. */
+int sl2_get_iterated_results(sl2_ctx *ctx, int32_t lo, int32_t cnt, int32_t *iterations, int32_t *status,
+                             double *last_delta);
+
 /* ---- frames (replaces the cv::Mat `frame` argument of MonoSLAM::GoOneStep, monoslam.cpp:108) */
 /* The frame ring keeps the context's width x height per stream.  A stream whose image is smaller
  * (sl2_set_stream_config) occupies the top-left width_s x height_s of its block; the rest of the block

@@ -352,6 +352,7 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   sl2_stream_gyro g0 = {};  // off; a rotation and a covariance the setter accepts
   for (int i = 0; i < 3; ++i) g0.R_gc[4 * i] = g0.cov[4 * i] = 1.0;
   c->gyro.assign(B, g0);
+  c->iter.assign(B, sl2_stream_iterated{});
 #undef ALLOC
   int rc = make_tensor_map(c);
   if (rc) return failed(rc, c->err);
@@ -533,7 +534,11 @@ static int step_group(sl2_ctx *c, int32_t slot, int lo, int cnt, Sl2Queue q, cud
   cudaEvent_t evu[6];
   for (int i = 0; i < 6; ++i) evu[i] = c->evu[i].get();
   const Sl2Subpix sp = subpixel_args(c, lo, cnt);
-  CU_TRY(c, sl2_launch_update(d, lo, cnt, -1, nullptr, nullptr, nullptr, nullptr, nullptr, 0, sp, q, t ? evu : nullptr));
+  // the iteration passes are part of the update's time (ev[2] .. ev[3]); the update times are the final pass's
+  const int rci = iterate_streams(c, lo, cnt, q);
+  if (rci) return rci;
+  CU_TRY(c, sl2_launch_update(d, lo, cnt, -1, nullptr, nullptr, nullptr, nullptr, nullptr, 0, sp, q, t ? evu : nullptr,
+                              iterate_args(c, lo, cnt)));
   // the rescue and its second update are part of the update's time (ev[2] .. ev[3]); the update times are the first's
   const bool rescue = rescue_on(c, lo, cnt);
   if (rescue) {

@@ -320,11 +320,33 @@ cudaError_t sl2_launch_subpixel(const Sl2Dev &d, const SubpixelLaunch &L, Sl2Que
 // the squared inlier radius of stream s, 0 = off (consensus.cu)
 cudaError_t sl2_launch_consensus(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *tau2_dev,
                                  const Sl2Subpix &sp, Sl2Queue q);
-// EKF update = 5 kernels (hp, chol, solve, syrk, finish); ev6 (optional) = 6 events recorded around them
+// The iterated EKF update (iterate.cu; include/sl2b200.h, sl2_set_stream_iterated) that upd_hp / upd_hp2 and
+// iterate_kernel take as an argument.  h == nullptr when no stream of the launch has the iteration on.  The
+// relinearised tables h_eff [B][Nmax][2], Hxp [B][Nmax][14] and Hy [B][Nmax][6] are feature-indexed like Sl2Dev::h,
+// dh_dxp and dh_dy; a stream reads them instead of those when max_it[s] > 0 and iters[s] > 0 (from pass 1 on).
+struct Sl2Iter {
+  int *max_it;        // [B] the settings' max_iterations, 0 = off
+  double *tol;        // [B]
+  double *h, *Hxp, *Hy;
+  double *x;          // [B][ld] the running iterate x_i
+  int *active;        // [B] 1 while stream s still iterates in this step
+  int *iters, *status;  // [B] the results (sl2_get_iterated_results)
+  double *delta;      // [B]
+  int pass;           // the iteration pass i >= 0, or -1: the final update
+};
+// EKF update = 5 kernels (hp, chol, solve, syrk, finish); ev6 (optional) = 6 events recorded around them.  it: the
+// iteration's tables the final update reads ({} off; pass -1)
 cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, int staged_m,
                               const int *st_feat, const double *st_Hxv, const double *st_Hy,
                               const double *st_R, const double *st_nu, int only_normalise,
-                              const Sl2Subpix &sp, Sl2Queue q, cudaEvent_t *ev6 = nullptr);
+                              const Sl2Subpix &sp, Sl2Queue q, cudaEvent_t *ev6 = nullptr, const Sl2Iter &it = {});
+// The factor half of iteration pass it.pass (update.cu): upd_hp / upd_hp2 and upd_chol over the measured rows of the
+// streams still active, at their current linearisation; an inactive stream reads m = 0
+cudaError_t sl2_launch_iterate_factor(const Sl2Dev &d, int stream_lo, int stream_cnt, const Sl2Subpix &sp,
+                                      const Sl2Iter &it, Sl2Queue q);
+// One whole iteration pass (iterate.cu): sl2_launch_iterate_factor, then iterate_kernel
+cudaError_t sl2_launch_iterate_pass(const Sl2Dev &d, int stream_lo, int stream_cnt, const Sl2Subpix &sp,
+                                    const Sl2Iter &it, Sl2Queue q);
 // The second update of the consensus rescue: the five update kernels over the rows whose found is SL2_FOUND_RESCUED,
 // with m2 (instead of Sl2Dev::upd_m) holding each stream's row count, 0 for a stream with nothing rescued, which the
 // five kernels then leave as they found it (update.cu)

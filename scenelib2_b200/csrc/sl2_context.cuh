@@ -139,6 +139,12 @@ struct sl2_ctx {
   // (allocated when a stream first turns it on): z [B][Nmax][2] doubles, refined [B][Nmax] and the on flags [B]
   std::vector<uint8_t> subpix_on;  // [B]
   sl2::DevPtr<uint8_t> subpix_buf;
+  // iterated update (sl2_set_stream_iterated): the host mirror of every stream's setting, and one device buffer
+  // (allocated when a stream first turns it on) behind iter_dev: the settings, the relinearised tables, the iterate and
+  // the per-stream results
+  std::vector<sl2_stream_iterated> iter;  // [B]
+  sl2::DevPtr<uint8_t> iter_buf;
+  Sl2Iter iter_dev = {};
 };
 
 namespace sl2 {
@@ -278,5 +284,9 @@ int gyro_streams(sl2_ctx *c, int slot, int lo, int cnt, Sl2Queue q);
 Sl2Subpix subpixel_args(const sl2_ctx *c, int lo, int cnt);
 int subpixel_streams(sl2_ctx *c, int slot, int lo, int cnt, const uint8_t *job_patches, Sl2Queue q);
 int subpixel_forget(sl2_ctx *c, int lo, int cnt);
+// iterate.cu: the iteration's tables the final update of the streams [lo, lo + cnt) reads ({} when none of them has
+// the iteration on); the iteration passes of those streams on q, right before their update
+Sl2Iter iterate_args(const sl2_ctx *c, int lo, int cnt);
+int iterate_streams(sl2_ctx *c, int lo, int cnt, Sl2Queue q);
 
 }  // namespace sl2

@@ -1,5 +1,6 @@
 // sl2_model.cuh — the device camera and feature models of predict_kernel and particle_predict_kernel (ekf.cu),
-// consensus_kernel (consensus.cu), rescue_kernel (rescue.cu), reloc_kernel (reloc.cu) and warp_kernel (warp.cu).  Everything that decides which pixels are searched
+// consensus_kernel (consensus.cu), rescue_kernel (rescue.cu), reloc_kernel (reloc.cu), warp_kernel (warp.cu) and
+// iterate_kernel (iterate.cu).  Everything that decides which pixels are searched
 // (S_i, S^-1, h_i) or which match is an inlier uses never-fused rd ops in the oracle's evaluation order.
 #pragma once
 #include "sl2_common.cuh"
@@ -308,26 +309,34 @@ struct FeatPred {
   rd depth;
 };
 
-// Pxx: shared 13x13 col-major; Pcol: global pointer to P(0, pos) (column-major, ld)
-__device__ void predict_feature(const double *cam, const double *xv, const rd yi[3],
-                                const double *Pxx, const double *Pcol, int ld, int pos,
-                                FeatPred &o) {
+// The measurement model of map feature yi seen from the camera pose xp (7: r, q): h, dh/dxp, dh/dy and the
+// camera-frame depth of yi (monoslam.cpp:289-308 without R and S).  predict_feature and iterate_kernel (iterate.cu)
+// both evaluate the model here.
+__device__ __forceinline__ void measure_feature(const double *cam, const double *xp, const rd yi[3], rd h[2],
+                                                rd dxp[2][7], rd dy[2][3], rd &depth) {
   rd z[3], dz_dxp[3][7], RRW[3][3], J[2][3];
-  zeroedyi(yi, xv, z, dz_dxp, RRW);
-  project(cam, z, o.h, J);
+  zeroedyi(yi, xp, z, dz_dxp, RRW);
+  project(cam, z, h, J);
   for (int i = 0; i < 2; ++i) {
     for (int j = 0; j < 7; ++j) {
       rd s(0.0);
       for (int k = 0; k < 3; ++k) s = s + J[i][k] * dz_dxp[k][j];
-      o.dxp[i][j] = s;
+      dxp[i][j] = s;
     }
     for (int j = 0; j < 3; ++j) {
       rd s(0.0);
       for (int k = 0; k < 3; ++k) s = s + J[i][k] * RRW[k][j];
-      o.dy[i][j] = s;
+      dy[i][j] = s;
     }
   }
-  o.depth = z[2];
+  depth = z[2];
+}
+
+// Pxx: shared 13x13 col-major; Pcol: global pointer to P(0, pos) (column-major, ld)
+__device__ void predict_feature(const double *cam, const double *xv, const rd yi[3],
+                                const double *Pxx, const double *Pcol, int ld, int pos,
+                                FeatPred &o) {
+  measure_feature(cam, xv, yi, o.h, o.dxp, o.dy, o.depth);
   o.var = measurement_noise(cam, o.h);
   func_Si<3>(o.dxp, o.dy, o.var, Pxx, 13, Pcol, ld, Pcol + pos, ld, o.S);
 }

@@ -218,13 +218,24 @@ __device__ __forceinline__ HpSmem hp_carve(uint8_t *base, int kmax, int ld) {
 // measurement into shared memory; returns K (measured features) or -1 when this CTA has no row block (rows_per_block
 // rows per block, block index blockIdx.x).  Every CTA of the stream pays this prologue.  All threads must call.
 // row_found: the found code of the rows (1; SL2_FOUND_RESCUED for the rescue's second update, whose K adds to nmeas).
-// sp: the sub-pixel matches of the fused step's rows (match_z).
+// sp: the sub-pixel matches of the fused step's rows (match_z).  it: the iterated update of the fused step's rows
+// (it.h == nullptr: off).  An iteration pass (it.pass >= 0) gathers no row of a stream that no longer iterates, so
+// that stream reads m = 0, and leaves nmeas alone; a stream that has relinearised reads h, dh/dxp and dh/dy from the
+// iteration's tables.
 __device__ __forceinline__ int hp_tables(const Sl2Dev &d, const HpSmem &sm, int s, int rows_per_block, int row_found,
                                          int staged_m,
                                          const int *st_feat, const double *st_Hxv, const double *st_Hy,
-                                         const double *st_R, const double *st_nu, const Sl2Subpix &sp) {
+                                         const double *st_R, const double *st_nu, const Sl2Subpix &sp,
+                                         const Sl2Iter &it) {
   const int tid = threadIdx.x;
   const size_t fb = (size_t)s * d.Nmax;
+  const bool iter_rows = it.h && staged_m < 0 && row_found == 1;
+  const bool iter_pass = iter_rows && it.pass >= 0;
+  const bool skip = iter_pass && !(it.pass == 0 ? it.max_it[s] > 0 : it.active[s] != 0);
+  const bool relin = iter_rows && it.pass != 0 && it.max_it[s] > 0 && it.iters[s] > 0;
+  const double *const tab_h = relin ? it.h : d.h;
+  const double *const tab_dxp = relin ? it.Hxp : d.dh_dxp;
+  const double *const tab_dy = relin ? it.Hy : d.dh_dy;
   // ---- measurement list in selected order, successful only (monoslam.cpp:556-571) --------------
   int K;
   if (staged_m >= 0) {
@@ -233,7 +244,7 @@ __device__ __forceinline__ int hp_tables(const Sl2Dev &d, const HpSmem &sm, int 
   } else {
     const int nsel = d.nsel[s];
     int feat = -1;
-    if (tid < d.Nmax && tid < nsel) {
+    if (!skip && tid < d.Nmax && tid < nsel) {
       const int i = d.job_feat[fb + tid];
       if (i >= 0 && d.found[fb + i] == row_found) feat = i;
     }
@@ -243,8 +254,11 @@ __device__ __forceinline__ int hp_tables(const Sl2Dev &d, const HpSmem &sm, int 
   const int m = 2 * K;
   if (blockIdx.x == 0 && tid == 0) {
     d.upd_m[s] = m;
-    if (staged_m < 0 && row_found == 1) d.nmeas[s] = K;
-    else if (staged_m < 0 && K > 0) d.nmeas[s] += K;
+    if (staged_m < 0 && row_found == 1) {
+      if (!iter_pass) d.nmeas[s] = K;
+    } else if (staged_m < 0 && K > 0) {
+      d.nmeas[s] += K;
+    }
   }
   if (rows_per_block * (int)blockIdx.x >= m) return -1;
   for (int e = tid; e < m * HP_HRS; e += HP_THREADS) sm.Hrow[e] = 0.0;
@@ -269,16 +283,16 @@ __device__ __forceinline__ int hp_tables(const Sl2Dev &d, const HpSmem &sm, int 
   } else {
     for (int e = tid; e < K * 14; e += HP_THREADS) {  // dh/dxv = [dh/dxp | 0] (motion_model.cpp:224-235)
       const int k = e / 14, q = e - k * 14, r = q >= 7;
-      sm.Hrow[(2 * k + r) * HP_HRS + q - 7 * r] = d.dh_dxp[(fb + sm.mfeat[k]) * 14 + q];
+      sm.Hrow[(2 * k + r) * HP_HRS + q - 7 * r] = tab_dxp[(fb + sm.mfeat[k]) * 14 + q];
     }
     for (int e = tid; e < K * 6; e += HP_THREADS) {
       const int i = e / 3, c = e - i * 3;
-      sm.Hrow[i * HP_HRS + 13 + c] = d.dh_dy[(fb + sm.mfeat[i >> 1]) * 6 + (i & 1) * 3 + c];
+      sm.Hrow[i * HP_HRS + 13 + c] = tab_dy[(fb + sm.mfeat[i >> 1]) * 6 + (i & 1) * 3 + c];
     }
     for (int e = tid; e < m; e += HP_THREADS) {
       const size_t f = fb + sm.mfeat[e >> 1];
       // nu = z - h (full_feature_model.cpp:197-200), z = (double)(u,v) (monoslam.cpp:382-383), or the sub-pixel match
-      sm.nu[e] = (rd(match_z(d, sp, f, e & 1)) - rd(d.h[f * 2 + (e & 1)])).v;
+      sm.nu[e] = (rd(match_z(d, sp, f, e & 1)) - rd(tab_h[f * 2 + (e & 1)])).v;
     }
     for (int k = tid; k < K; k += HP_THREADS) {
       const double var = d.Rvar[fb + sm.mfeat[k]];  // R_i = var * I (camera.cpp:294-299)
@@ -423,7 +437,7 @@ __device__ __forceinline__ void hp_s_rows(const HpSmem &sm, const double *__rest
 template <int KD>
 __global__ void __launch_bounds__(HP_THREADS, 2) upd_hp_kernel(
     const Sl2Dev d, int stream_lo, int row_found, int staged_m, const int *st_feat, const double *st_Hxv,
-    const double *st_Hy, const double *st_R, const double *st_nu, const Sl2Subpix sp) {
+    const double *st_Hy, const double *st_R, const double *st_nu, const Sl2Subpix sp, const Sl2Iter it) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   pdl_prologue();
   const int ld = d.ld, ldg = d.ldg;
@@ -433,7 +447,7 @@ __global__ void __launch_bounds__(HP_THREADS, 2) upd_hp_kernel(
   const int n = SL2_NXV + 3 * d.nfeat[s];
   const double *__restrict__ P = d.P + (size_t)s * ld * ld;
   double *__restrict__ G = d.G + (size_t)s * d.mmax * ldg;
-  const int K = hp_tables(d, sm, s, HP_ROWS, row_found, staged_m, st_feat, st_Hxv, st_Hy, st_R, st_nu, sp);
+  const int K = hp_tables(d, sm, s, HP_ROWS, row_found, staged_m, st_feat, st_Hxv, st_Hy, st_R, st_nu, sp, it);
   if (K < 0) return;
   const int m = 2 * K;
 
@@ -466,7 +480,7 @@ __global__ void __launch_bounds__(HP_THREADS, 2) upd_hp_kernel(
 template <int KD>
 __global__ void __launch_bounds__(HP_THREADS, 2) upd_hp2_kernel(
     const Sl2Dev d, int stream_lo, int row_found, int staged_m, const int *st_feat, const double *st_Hxv,
-    const double *st_Hy, const double *st_R, const double *st_nu, const Sl2Subpix sp) {
+    const double *st_Hy, const double *st_R, const double *st_nu, const Sl2Subpix sp, const Sl2Iter it) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   pdl_prologue();
   constexpr int R2 = HP_ROWS / 2, F2 = R2 / 2;  // rows / features per block
@@ -477,7 +491,7 @@ __global__ void __launch_bounds__(HP_THREADS, 2) upd_hp2_kernel(
   const int n = SL2_NXV + 3 * d.nfeat[s];
   const double *__restrict__ P = d.P + (size_t)s * ld * ld;
   double *__restrict__ G = d.G + (size_t)s * d.mmax * ldg;
-  const int K = hp_tables(d, sm, s, R2, row_found, staged_m, st_feat, st_Hxv, st_Hy, st_R, st_nu, sp);
+  const int K = hp_tables(d, sm, s, R2, row_found, staged_m, st_feat, st_Hxv, st_Hy, st_R, st_nu, sp, it);
   if (K < 0) return;
   const int m = 2 * K;
   const int j = tid;  // this thread's state column (n <= HP_THREADS: the launcher's condition)
@@ -1488,37 +1502,48 @@ cudaError_t sl2_configure_update(const Sl2Dev &d) {
 
 namespace {
 
+// upd_hp / upd_hp2 of the streams [stream_lo, stream_lo + stream_cnt)
+cudaError_t launch_hp(const Sl2Dev &d, int stream_lo, int stream_cnt, int row_found, int staged_m, const int *st_feat,
+                      const double *st_Hxv, const double *st_Hy, const double *st_R, const double *st_nu,
+                      const Sl2Subpix &sp, const Sl2Iter &it, Sl2Queue q) {
+  // row blocks of H P / S per stream: spread over CTAs unless the batch already fills the GPU with two streams per SM
+  // (then one CTA per stream is fastest: every CTA rebuilds the measurement list and H tables)
+  const int hp_all = (2 * upd_keven(d.kmax) + HP_ROWS - 1) / HP_ROWS;
+  const int hp_blocks = stream_cnt >= 2 * d.nsm ? 1 : hp_all;
+  const dim3 grid(hp_blocks, stream_cnt);
+  // the software-pipelined form: one CTA per stream, one state column per thread
+  const bool piped = hp_blocks == 1 && SL2_NXV + 3 * d.Nmax <= HP_THREADS;
+  const int kd = staged_m >= 0 ? 13 : 7;
+  auto *k13 = piped ? upd_hp2_kernel<13> : upd_hp_kernel<13>;
+  auto *k7 = piped ? upd_hp2_kernel<7> : upd_hp_kernel<7>;
+  const size_t smem = hp_layout(d.kmax, d.ld, piped ? kd : 0).bytes;
+  return sl2_launch_kernel(kd == 13 ? k13 : k7, grid, dim3(HP_THREADS), smem, q, sl2_use_pdl(stream_cnt), d, stream_lo,
+                           row_found, staged_m, st_feat, st_Hxv, st_Hy, st_R, st_nu, sp, it);
+}
+
+cudaError_t launch_chol(const Sl2Dev &d, int stream_lo, int stream_cnt, Sl2Queue q) {
+  return sl2_launch_kernel(upd_chol_kernel, dim3(stream_cnt), dim3(UPD_THREADS), sl2_update_smem_bytes(d), q,
+                           sl2_use_pdl(stream_cnt), d, stream_lo);
+}
+
 // ev6 (optional): 6 events recorded around the 5 kernels (hp, chol, solve, syrk, finish); row_found: the rows' found
 // code (1, or SL2_FOUND_RESCUED for the rescue's second update)
 cudaError_t launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, int row_found, int staged_m,
                           const int *st_feat, const double *st_Hxv, const double *st_Hy, const double *st_R,
-                          const double *st_nu, int only_normalise, const Sl2Subpix &sp, Sl2Queue q,
+                          const double *st_nu, int only_normalise, const Sl2Subpix &sp, const Sl2Iter &it, Sl2Queue q,
                           cudaEvent_t *ev6) {
   if (stream_cnt <= 0) return cudaSuccess;
   cudaError_t e;
   auto mark = [&](int i) { return ev6 ? cudaEventRecord(ev6[i], q.stream) : cudaSuccess; };
   if ((e = mark(0)) != cudaSuccess) return e;
-  // row blocks of H P / S per stream: spread over CTAs unless the batch already fills the GPU with two streams per SM
-  // (then one CTA per stream is fastest: every CTA rebuilds the measurement list and H tables)
-  const int hp_all = (2 * upd_keven(d.kmax) + HP_ROWS - 1) / HP_ROWS;
-  const int hp_blocks = stream_cnt >= 2 * d.nsm ? 1 : hp_all;
   const bool pdl = sl2_use_pdl(stream_cnt);
   if (!only_normalise) {
-    const dim3 grid(hp_blocks, stream_cnt);
-    // the software-pipelined form: one CTA per stream, one state column per thread
-    const bool piped = hp_blocks == 1 && SL2_NXV + 3 * d.Nmax <= HP_THREADS;
-    const int kd = staged_m >= 0 ? 13 : 7;
-    auto *k13 = piped ? upd_hp2_kernel<13> : upd_hp_kernel<13>;
-    auto *k7 = piped ? upd_hp2_kernel<7> : upd_hp_kernel<7>;
-    const size_t smem = hp_layout(d.kmax, d.ld, piped ? kd : 0).bytes;
-    e = sl2_launch_kernel(kd == 13 ? k13 : k7, grid, dim3(HP_THREADS), smem, q, pdl, d, stream_lo, row_found,
-                          staged_m, st_feat, st_Hxv, st_Hy, st_R, st_nu, sp);
+    e = launch_hp(d, stream_lo, stream_cnt, row_found, staged_m, st_feat, st_Hxv, st_Hy, st_R, st_nu, sp, it, q);
     if (e != cudaSuccess) return e;
   }
   if ((e = mark(1)) != cudaSuccess) return e;
   if (!only_normalise) {
-    e = sl2_launch_kernel(upd_chol_kernel, dim3(stream_cnt), dim3(UPD_THREADS), sl2_update_smem_bytes(d), q, pdl, d,
-                          stream_lo);
+    e = launch_chol(d, stream_lo, stream_cnt, q);
     if (e != cudaSuccess) return e;
   }
   if ((e = mark(2)) != cudaSuccess) return e;
@@ -1556,9 +1581,17 @@ cudaError_t launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, int ro
 cudaError_t sl2_launch_update(const Sl2Dev &d, int stream_lo, int stream_cnt, int staged_m,
                               const int *st_feat, const double *st_Hxv, const double *st_Hy,
                               const double *st_R, const double *st_nu, int only_normalise,
-                              const Sl2Subpix &sp, Sl2Queue q, cudaEvent_t *ev6) {
+                              const Sl2Subpix &sp, Sl2Queue q, cudaEvent_t *ev6, const Sl2Iter &it) {
   return launch_update(d, stream_lo, stream_cnt, 1, staged_m, st_feat, st_Hxv, st_Hy, st_R, st_nu, only_normalise, sp,
-                       q, ev6);
+                       it, q, ev6);
+}
+
+cudaError_t sl2_launch_iterate_factor(const Sl2Dev &d, int stream_lo, int stream_cnt, const Sl2Subpix &sp,
+                                      const Sl2Iter &it, Sl2Queue q) {
+  if (stream_cnt <= 0) return cudaSuccess;
+  cudaError_t e = launch_hp(d, stream_lo, stream_cnt, 1, -1, nullptr, nullptr, nullptr, nullptr, nullptr, sp, it, q);
+  if (e != cudaSuccess) return e;
+  return launch_chol(d, stream_lo, stream_cnt, q);
 }
 
 // Sl2Dev travels by value: the second update's copy reads and writes its row counts in m2, so Sl2Dev::upd_m keeps the
@@ -1568,7 +1601,7 @@ cudaError_t sl2_launch_update_rescued(const Sl2Dev &d, int stream_lo, int stream
   Sl2Dev d2 = d;
   d2.upd_m = m2;
   return launch_update(d2, stream_lo, stream_cnt, SL2_FOUND_RESCUED, -1, nullptr, nullptr, nullptr, nullptr, nullptr, 0,
-                       sp, q, nullptr);
+                       sp, Sl2Iter{}, q, nullptr);
 }
 
 extern "C" {
@@ -1600,8 +1633,10 @@ int sl2_ekf_update(sl2_ctx *c, int32_t s, int32_t m, const int32_t *feat_index, 
 
 int sl2_ekf_update_measured(sl2_ctx *c, int32_t s) {
   if (bad_stream(c, s)) return fail(c, SL2_ERR_ARG, "bad stream");
+  const int rc0 = iterate_streams(c, s, 1, queue(c));  // the iteration passes, when the stream has them on
+  if (rc0) return rc0;
   CU_TRY(c, sl2_launch_update(c->d, s, 1, -1, nullptr, nullptr, nullptr, nullptr, nullptr, 0, subpixel_args(c, s, 1),
-                              queue(c)));
+                              queue(c), nullptr, iterate_args(c, s, 1)));
   if (rescue_on(c, s, 1)) {  // the fused step's rescue and second update
     const int rc = rescue_streams(c, s, 1, queue(c));
     if (rc) return rc;

@@ -65,6 +65,14 @@ class Sl2StreamGyro(C.Structure):
     _fields_ = [("on", C.c_int32), ("reserved", C.c_int32), ("R_gc", C.c_double * 9), ("bias", C.c_double * 3),
                 ("cov", C.c_double * 9)]
 
+class Sl2StreamIterated(C.Structure):
+    """sl2_stream_iterated: a camera stream's iterated EKF update: relinearisations allowed (0 = off) and the step
+    tolerance in prior standard deviations."""
+    _fields_ = [("max_iterations", C.c_int32), ("reserved", C.c_int32), ("tol", C.c_double)]
+
+
+SL2_MAX_ITERATIONS = 8
+
 SL2_SRC_GRAY_RING, SL2_SRC_GRAY8, SL2_SRC_RGB24, SL2_SRC_UYVY = 0, 1, 2, 3
 SL2_MAX_SOURCE_DIM = 4096
 SOURCE_BPP = {SL2_SRC_GRAY8: 1, SL2_SRC_RGB24: 3, SL2_SRC_UYVY: 2}
@@ -79,6 +87,7 @@ EXPORTS = [
     "sl2_set_stream_subpixel", "sl2_get_stream_subpixel",
     "sl2_set_stream_selection", "sl2_get_stream_selection",
     "sl2_set_stream_gyro", "sl2_get_stream_gyro", "sl2_set_gyro_samples", "sl2_gyro_update", "sl2_get_gyro_results",
+    "sl2_set_stream_iterated", "sl2_get_stream_iterated", "sl2_get_iterated_results",
     "sl2_set_frame", "sl2_set_frames", "sl2_set_frames_dev",
     "sl2_set_stream_source", "sl2_get_stream_source", "sl2_frame_set_layout", "sl2_set_features",
     "sl2_num_features", "sl2_state_size", "sl2_set_state", "sl2_get_state", "sl2_delete_feature", "sl2_append_feature",
@@ -249,6 +258,9 @@ def load():
         L.sl2_set_gyro_samples.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
         L.sl2_gyro_update.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
         L.sl2_get_gyro_results.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
+        L.sl2_set_stream_iterated.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamIterated)]
+        L.sl2_get_stream_iterated.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamIterated)]
+        L.sl2_get_iterated_results.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
         L.sl2_warp_templates.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_void_p]
         L.sl2_set_frame.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_size_t]
@@ -473,6 +485,30 @@ class Context:
         nis, status = np.zeros(max(cnt, 0)), np.zeros(max(cnt, 0), np.int32)
         self._ck(self.L.sl2_get_gyro_results(self.h, lo, cnt, nis.ctypes.data, status.ctypes.data))
         return nis, status
+
+    # ---- iterated update -----------------------------------------------------------------------
+    def set_stream_iterated(self, stream_id, max_iterations, tol=0.0, reserved=0):
+        """sl2_set_stream_iterated: relinearise the stream's EKF update at the updated state up to max_iterations
+        times (0 = off, the default), stopping once a step moves no state entry by more than tol prior standard
+        deviations."""
+        v = Sl2StreamIterated(int(max_iterations), int(reserved), float(tol))
+        self._ck(self.L.sl2_set_stream_iterated(self.h, stream_id, C.byref(v)))
+
+    def stream_iterated(self, stream_id):
+        """-> (max_iterations, tol)"""
+        v = Sl2StreamIterated()
+        self._ck(self.L.sl2_get_stream_iterated(self.h, stream_id, C.byref(v)))
+        return v.max_iterations, v.tol
+
+    def iterated_results(self, lo=0, cnt=None):
+        """sl2_get_iterated_results -> (iterations (cnt,), status (cnt,): 0 off or nothing measured, 1 converged,
+        2 ran out, 3 invalid relinearisation, last_delta (cnt,))."""
+        if cnt is None:
+            cnt = self.cfg.num_streams - lo
+        k = max(cnt, 0)
+        it, st, dl = np.zeros(k, np.int32), np.zeros(k, np.int32), np.zeros(k)
+        self._ck(self.L.sl2_get_iterated_results(self.h, lo, cnt, it.ctypes.data, st.ctypes.data, dl.ctypes.data))
+        return it, st, dl
 
     # ---- frames -------------------------------------------------------------------------------
     def set_stream_source(self, stream_id, format, width=0, height=0):
