@@ -837,6 +837,61 @@ int sl2_relocalise(sl2_ctx *ctx, const int32_t *stream_ids, int32_t cnt, int32_t
                    int32_t *z_uv /* cnt x max_features x 2, may be NULL */,
                    uint8_t *flags /* cnt x max_features, may be NULL */);
 
+/* ---- stream recovery: detect a lost stream inside the fused step and relocalise it there (no reference counterpart)
+ * A stream that has lost its camera keeps adding failed attempts to every feature it selects, and the cull then
+ * deletes the map a relocalisation needs; a host that notices the loss from the step records must synchronise first.
+ * With recovery on, the fused step itself notices the loss, stops selecting features (so the map is kept) and tries
+ * sl2_relocalise on its own frame.  For every stream with lost_after > 0, at the end of the fused step of ring slot
+ * `slot` (after the cull and the step record, so the record keeps its meaning), with n = the step's nmeas (the count
+ * its record shows):
+ *   1. A stream that entered the step tracking: failed_steps = n < min_matches ? failed_steps + 1 : 0.  When
+ *      failed_steps >= lost_after the stream becomes lost (lost = 1, lost_steps = 0; failed_steps keeps its value) and
+ *      tries on this step.
+ *   2. A stream that entered the step lost: lost_steps = lost_steps + 1; it tries when lost_steps % retry_period == 0.
+ *   3. A try is exactly sl2_relocalise of that one stream on `slot` with the setting's reloc and Pxx: the same
+ *      full-image jobs (centre ((w - 1) / 2, (h - 1) / 2), eps = 9 / (w^2 + h^2) of the stream's own image, formed
+ *      with the same correctly rounded operations), the same hypotheses, decision and state write.  attempted = 1 and
+ *      `last` = its result.  Accepted: recoveries + 1, and the stream is tracking again with lost = failed_steps =
+ *      lost_steps = 0.  Rejected: nothing else changes and the stream stays lost.  A step without a try sets
+ *      attempted = 0 and keeps `last`.
+ *   4. A step that a stream enters lost selects no feature, under SL2_SELECT_TRACE and SL2_SELECT_INFORMATION alike,
+ *      exactly as that step would with number_of_features_to_select = 0; everything else of the step runs as usual
+ *      (motion prediction, gyro update, visibility, record).  No selection means no attempt, so the cull keeps the map.
+ * Resets: the setter, a snapshot load into the stream, sl2_set_state, sl2_set_features and an accepted sl2_relocalise
+ * of the stream return it to tracking (lost = failed_steps = lost_steps = 0); the setter also clears attempted,
+ * recoveries and last.  Turning the setting off (lost_after = 0) therefore also resumes selection.
+ * Where it applies: sl2_step, sl2_step_host and sl2_step_host_async (whose xv_out shows the state after the whole step,
+ * an accepted try included).  The staged entry points and the C++ shim never run it.  The setting and the recovery
+ * state belong to the stream slot, like the match consensus: snapshots do not carry them (the format is unchanged).
+ * Cost: a step group holding a stream with recovery on launches three more kernels per step, after the step's timing
+ * events (recover_kernel, the full-image search over the streams that try, reloc_kernel); a stream that does not try
+ * costs an early return in each.  A context where no stream has it on runs exactly the path without it.
+ * The first stream turned on allocates the context's recovery buffers (the settings and states, a job table and search
+ * results of num_streams x max_features entries): SL2_ERR_CUDA, with the setting unchanged, when that fails.
+ * SL2_ERR_ARG, with the setting unchanged, for: a bad stream_id or NULL r; reserved != 0; lost_after < 0; with
+ * lost_after > 0, min_matches < 1 or retry_period < 1, or a reloc or Pxx that sl2_relocalise refuses. */
+typedef struct sl2_stream_recovery {
+  int32_t lost_after;     /* 0 (default) = off; K >= 1: K consecutive failed steps declare the stream lost */
+  int32_t min_matches;    /* >= 1: a step fails when its nmeas is < min_matches */
+  int32_t retry_period;   /* >= 1: a lost stream tries on the step it is declared lost, then every retry_period-th */
+  int32_t reserved;       /* 0 */
+  sl2_reloc_params reloc; /* as for sl2_relocalise */
+  double Pxx[169];        /* restart covariance, 13 x 13 column-major: as for sl2_relocalise */
+} sl2_stream_recovery;
+int sl2_set_stream_recovery(sl2_ctx *ctx, int32_t stream_id, const sl2_stream_recovery *r);
+int sl2_get_stream_recovery(sl2_ctx *ctx, int32_t stream_id, sl2_stream_recovery *r);
+typedef struct sl2_recovery_result {
+  int32_t lost;          /* 1 while the stream is lost after the last step */
+  int32_t failed_steps;  /* consecutive failed steps while tracking */
+  int32_t lost_steps;    /* steps since the stream was declared lost */
+  int32_t attempted;     /* 1 when the last step tried a relocalisation */
+  int64_t recoveries;    /* accepted tries since the setting was made */
+  sl2_reloc_result last; /* the last try's result, as sl2_relocalise reports it (zero before the first) */
+} sl2_recovery_result;
+/* The recovery state of streams [lo, lo + cnt) after the last step (zero for streams never turned on).  Joins both
+ * step groups and synchronises.  SL2_ERR_ARG for a bad range or a NULL out with cnt > 0. */
+int sl2_get_recovery_results(sl2_ctx *ctx, int32_t lo, int32_t cnt, sl2_recovery_result *out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -353,6 +353,7 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   for (int i = 0; i < 3; ++i) g0.R_gc[4 * i] = g0.cov[4 * i] = 1.0;
   c->gyro.assign(B, g0);
   c->iter.assign(B, sl2_stream_iterated{});
+  c->recov.assign(B, sl2_stream_recovery{});
 #undef ALLOC
   int rc = make_tensor_map(c);
   if (rc) return failed(rc, c->err);
@@ -439,7 +440,9 @@ int sl2_set_features(sl2_ctx *c, int32_t s, int32_t n, const double *y, const do
   CU_TRY(c, cudaMemsetAsync(d.sel_rank + fb, 0xff, sizeof(int) * d.Nmax, c->stream));
   CU_TRY(c, cudaMemsetAsync(d.found + fb, 0, d.Nmax, c->stream));
   CU_TRY(c, cudaMemsetAsync(d.job_feat + fb, 0xff, sizeof(int) * d.Nmax, c->stream));
-  const int rc = subpixel_forget(c, s, 1);  // a new map has no refined matches
+  int rc = subpixel_forget(c, s, 1);  // a new map has no refined matches
+  if (rc) return rc;
+  rc = recovery_reset(c, s, 1);  // a new map: the stream is tracking
   if (rc) return rc;
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   return SL2_OK;
@@ -466,6 +469,8 @@ int sl2_set_state(sl2_ctx *c, int32_t s, const double *x, const double *P) {
   CU_TRY(c, cudaMemcpy2DAsync(d.P + (size_t)s * d.ld * d.ld, sizeof(double) * d.ld, P,
                               sizeof(double) * n, sizeof(double) * n, n, cudaMemcpyHostToDevice,
                               c->stream));
+  const int rc = recovery_reset(c, s, 1);  // a new state: the stream is tracking
+  if (rc) return rc;
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   return SL2_OK;
 }
@@ -513,13 +518,14 @@ static int step_group(sl2_ctx *c, int32_t slot, int lo, int cnt, Sl2Queue q, cud
   const cudaStream_t st = q.stream;
   if (t) CU_TRY(c, cudaEventRecord(c->ev[0].get(), st));
   const bool info = selection_on(c, lo, cnt);
+  const sl2_recovery_result *rv = recovery_args(c, lo, cnt);  // a lost stream selects nothing
   if (gyro_on(c, lo, cnt)) {  // the motion prediction, the gyro update, then the feature prediction
     CU_TRY(c, sl2_launch_predict(d, lo, cnt, nullptr, 1, 0, nullptr, q));
     const int rc = gyro_streams(c, slot, lo, cnt, q);
     if (rc) return rc;
-    CU_TRY(c, sl2_launch_predict(d, lo, cnt, nullptr, 0, 1, info ? c->sel_mode_dev : nullptr, q));
+    CU_TRY(c, sl2_launch_predict(d, lo, cnt, nullptr, 0, 1, info ? c->sel_mode_dev : nullptr, q, rv));
   } else {
-    CU_TRY(c, sl2_launch_predict(d, lo, cnt, nullptr, 1, 1, info ? c->sel_mode_dev : nullptr, q));
+    CU_TRY(c, sl2_launch_predict(d, lo, cnt, nullptr, 1, 1, info ? c->sel_mode_dev : nullptr, q, rv));
   }
   if (info) {  // part of the predict's time
     const int rc = select_streams(c, lo, cnt, q);
@@ -552,6 +558,7 @@ static int step_group(sl2_ctx *c, int32_t slot, int lo, int cnt, Sl2Queue q, cud
     const Sl2Rescue r = rescue ? rescue_args(c) : Sl2Rescue{};
     CU_TRY(c, sl2_launch_records(d, lo, cnt, c->rec_steps, rescue ? &r : nullptr, q));
   }
+  if (rv) return recover_streams(c, slot, lo, cnt, q);  // after the cull and the record: the record keeps its meaning
   return SL2_OK;
 }
 

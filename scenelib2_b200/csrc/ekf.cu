@@ -150,10 +150,13 @@ __device__ int visibility_test(const double *cam, const double *xp, const rd yi[
 // ---------------------------------------------------------------------------------------------
 // sel_mode: [B] every stream's SL2_SELECT_* (sl2_set_stream_selection), or nullptr: every stream selects by trace.  An
 // SL2_SELECT_INFORMATION stream keeps the provisional rank of every candidate (visible, ranked before the first zero
-// trace) in sel_rank and leaves the truncation, the job slots and nsel to select_kernel (select.cu).
+// trace) in sel_rank and leaves the truncation, the job slots and nsel to select_kernel (select.cu).  rv: [B] the
+// streams' recovery states (recover.cu), or nullptr: no stream of the launch has recovery on.  A stream that enters
+// the step lost selects nothing, under either rule, as with n_select = 0.
 __global__ void __launch_bounds__(128) predict_kernel(const Sl2Dev d, int stream_lo,
                                                       const double *u3, int do_predict,
-                                                      int do_measure, const int *sel_mode) {
+                                                      int do_measure, const int *sel_mode,
+                                                      const sl2_recovery_result *rv) {
   pdl_prologue();
   const int s = stream_lo + blockIdx.x;
   const int tid = threadIdx.x;
@@ -279,7 +282,7 @@ __global__ void __launch_bounds__(128) predict_kernel(const Sl2Dev d, int stream
   __syncthreads();
   const bool info = sel_mode && sel_mode[s] == SL2_SELECT_INFORMATION;
   // information: the candidates are every rank before the first zero score
-  const int nsel = info ? min(s_r0, s_nvis) : min(min(sc.n_select, s_r0), s_nvis);
+  const int nsel = (rv && rv[s].lost) ? 0 : info ? min(s_r0, s_nvis) : min(min(sc.n_select, s_r0), s_nvis);
   for (int i = tid; i < nf; i += blockDim.x) {
     int rank = d.sel_rank[fb + i];
     if (rank >= nsel) rank = -1;
@@ -540,12 +543,13 @@ cudaError_t sl2_launch_append(const Sl2Dev &d, int s, const double *y3_dev, cons
 }  // namespace
 
 cudaError_t sl2_launch_predict(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *u3_dev,
-                               int do_predict, int do_measure, const int *sel_mode_dev, Sl2Queue q) {
+                               int do_predict, int do_measure, const int *sel_mode_dev, Sl2Queue q,
+                               const sl2_recovery_result *rv_dev) {
   if (stream_cnt <= 0) return cudaSuccess;
   // 128 threads, one feature each per pass over the map (two passes at SL2_MAX_FEATURES); the kernel needs ~255
   // registers per thread, so 128-thread CTAs are what lets two streams share an SM
   return sl2_launch_kernel(predict_kernel, dim3(stream_cnt), dim3(128), 0, q, sl2_use_pdl(stream_cnt), d,
-                           stream_lo, u3_dev, do_predict, do_measure, sel_mode_dev);
+                           stream_lo, u3_dev, do_predict, do_measure, sel_mode_dev, rv_dev);
 }
 
 // F features, Kmax = stride between features in every per-particle array, K_dev[f] particles used

@@ -275,21 +275,29 @@ __device__ int reloc_support(const RelocSmem &S, const double *xp, double t2, in
   });
 }
 
-// One CTA per listed stream.  search_uv / search_found: the full-image search's results by job, job = (stream -
-// stream_lo) * Nmax + feature.  Rounds of RELOC_THREADS hypotheses: every thread solves one P3P into shared memory,
-// then warp w scores the poses of hypotheses w, w + RELOC_WARPS, ... of the round (lanes over the matches, ballot /
-// popc), keeping its best (largest support, then lowest index: it visits indices in increasing order); thread 0
-// reduces the warps' bests in the same order.  Warp 0 refines, the CTA recounts and, on acceptance, writes x and P.
+// One CTA per listed stream: ids[i], or stream_lo + i when ids is nullptr.  search_uv / search_found: the full-image
+// search's results by job, job = (stream - stream_lo) * Nmax + feature.  Stream s reads its parameters at prm and Pxx
+// advanced by s * prm_stride bytes (0: one set for every stream).  rv (the fused step's recovery, recover.cu) is nullptr
+// for sl2_relocalise; else a stream whose rv[s].attempted is 0 returns at once, the result goes to rv[s].last instead
+// of res[i], and an acceptance returns the stream to tracking.  Rounds of RELOC_THREADS hypotheses: every thread
+// solves one P3P into shared memory, then warp w scores the poses of hypotheses w, w + RELOC_WARPS, ... of the round
+// (lanes over the matches, ballot / popc), keeping its best (largest support, then lowest index: it visits indices in
+// increasing order); thread 0 reduces the warps' bests in the same order.  Warp 0 refines, the CTA recounts and, on acceptance, writes x and P.
 __global__ void __launch_bounds__(RELOC_THREADS) reloc_kernel(const Sl2Dev d, const int *__restrict__ ids,
                                                               int stream_lo, const int *__restrict__ search_uv,
                                                               const uint8_t *__restrict__ search_found,
-                                                              const sl2_reloc_params *__restrict__ prm,
-                                                              const double *__restrict__ Pxx,
+                                                              const sl2_reloc_params *__restrict__ prm0,
+                                                              const double *__restrict__ Pxx0, size_t prm_stride,
                                                               sl2_reloc_result *__restrict__ res, int *__restrict__ zuv_out,
-                                                              uint8_t *__restrict__ flags_out) {
+                                                              uint8_t *__restrict__ flags_out,
+                                                              sl2_recovery_result *__restrict__ rv) {
   extern __shared__ __align__(16) uint8_t reloc_smem[];
   RelocSmem &S = *reinterpret_cast<RelocSmem *>(reloc_smem);
-  const int i = blockIdx.x, s = ids[i];
+  const int i = blockIdx.x, s = ids ? ids[i] : stream_lo + i;
+  if (rv && !rv[s].attempted) return;  // block-uniform: a stream that does not try this step
+  const sl2_reloc_params *prm = reinterpret_cast<const sl2_reloc_params *>(reinterpret_cast<const char *>(prm0) +
+                                                                           (size_t)s * prm_stride);
+  const double *Pxx = reinterpret_cast<const double *>(reinterpret_cast<const char *>(Pxx0) + (size_t)s * prm_stride);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int ld = d.ld, nf = d.nfeat[s], n = SL2_NXV + 3 * nf;
   double *P = d.P + (size_t)s * ld * ld;
@@ -476,7 +484,11 @@ __global__ void __launch_bounds__(RELOC_THREADS) reloc_kernel(const Sl2Dev d, co
       }
     S.n_inl = cntin;
     const bool accept = have && cntin >= prm->min_inliers;
-    sl2_reloc_result &o = res[i];
+    sl2_reloc_result &o = rv ? rv[s].last : res[i];
+    if (rv && accept) {  // tracking again
+      rv[s].lost = rv[s].failed_steps = rv[s].lost_steps = 0;
+      rv[s].recoveries += 1;
+    }
     o.status = accept ? 1 : 0;
     o.matches = k;
     o.support = have ? S.win_sup : 0;
@@ -511,18 +523,24 @@ __global__ void __launch_bounds__(RELOC_THREADS) reloc_kernel(const Sl2Dev d, co
   }
 }
 
-// relocalisation of the cnt streams ids_dev[] from the full-image search's results by job (job = (stream - stream_lo) *
-// Nmax + feature): pose consensus, refinement and, on acceptance, the state write
+}  // namespace
+
+// relocalisation of the cnt streams ids_dev[] (stream_lo + i when nullptr) from the full-image search's results by job
+// (job = (stream - stream_lo) * Nmax + feature): pose consensus, refinement and, on acceptance, the state write
 cudaError_t sl2_launch_reloc(const Sl2Dev &d, int cnt, const int *ids_dev, int stream_lo, const int *search_uv,
                              const uint8_t *search_found, const sl2_reloc_params *prm_dev, const double *Pxx_dev,
-                             sl2_reloc_result *res_dev, int *zuv_dev, uint8_t *flags_dev, Sl2Queue q) {
+                             size_t prm_stride, sl2_reloc_result *res_dev, int *zuv_dev, uint8_t *flags_dev,
+                             sl2_recovery_result *rv, Sl2Queue q) {
   if (cnt <= 0) return cudaSuccess;
   const cudaError_t e =
       cudaFuncSetAttribute(reloc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RelocSmem));
   if (e != cudaSuccess) return e;
   return sl2_launch_kernel(reloc_kernel, dim3(cnt), dim3(RELOC_THREADS), sizeof(RelocSmem), q, false, d, ids_dev,
-                           stream_lo, search_uv, search_found, prm_dev, Pxx_dev, res_dev, zuv_dev, flags_dev);
+                           stream_lo, search_uv, search_found, prm_dev, Pxx_dev, prm_stride, res_dev, zuv_dev,
+                           flags_dev, rv);
 }
+
+namespace {
 
 // whether the symmetric 13 x 13 matrix A (column-major) is positive semi-definite: cyclic Jacobi eigenvalues, the
 // smallest >= -1e-12 times the largest magnitude
@@ -567,6 +585,25 @@ bool psd13(const double *A0) {
 
 }  // namespace
 
+namespace sl2 {
+
+std::string reloc_params_error(const sl2_reloc_params *p, const double *Pxx) {
+  if (!(p->inlier_px > 0.0) || !std::isfinite(p->inlier_px)) return "inlier_px must be finite and > 0";
+  if (p->min_inliers < 4 || p->reserved != 0) return "min_inliers must be >= 4 and reserved 0";
+  for (int i = 0; i < 3; ++i)
+    if (!std::isfinite(p->v[i]) || !std::isfinite(p->omega[i])) return "v and omega must be finite";
+  if (!(std::sqrt(p->omega[0] * p->omega[0] + p->omega[1] * p->omega[1] + p->omega[2] * p->omega[2]) > 0.0))
+    return "|omega| must be > 0";
+  for (int i = 0; i < 13; ++i)
+    for (int j = 0; j < 13; ++j)
+      if (!std::isfinite(Pxx[i + 13 * j]) || Pxx[i + 13 * j] != Pxx[j + 13 * i])
+        return "Pxx must be finite and symmetric";
+  if (!psd13(Pxx)) return "Pxx is not positive semi-definite";
+  return "";
+}
+
+}  // namespace sl2
+
 extern "C" {
 
 int sl2_relocalise(sl2_ctx *c, const int32_t *ids, int32_t cnt, int32_t slot, const sl2_reloc_params *p,
@@ -584,20 +621,8 @@ int sl2_relocalise(sl2_ctx *c, const int32_t *ids, int32_t cnt, int32_t slot, co
     lo = std::min(lo, s);
     hi = std::max(hi, s);
   }
-  if (!(p->inlier_px > 0.0) || !std::isfinite(p->inlier_px))
-    return fail(c, SL2_ERR_ARG, "sl2_relocalise: inlier_px must be finite and > 0");
-  if (p->min_inliers < 4 || p->reserved != 0)
-    return fail(c, SL2_ERR_ARG, "sl2_relocalise: min_inliers must be >= 4 and reserved 0");
-  for (int i = 0; i < 3; ++i)
-    if (!std::isfinite(p->v[i]) || !std::isfinite(p->omega[i]))
-      return fail(c, SL2_ERR_ARG, "sl2_relocalise: v and omega must be finite");
-  if (!(std::sqrt(p->omega[0] * p->omega[0] + p->omega[1] * p->omega[1] + p->omega[2] * p->omega[2]) > 0.0))
-    return fail(c, SL2_ERR_ARG, "sl2_relocalise: |omega| must be > 0");
-  for (int i = 0; i < 13; ++i)
-    for (int j = 0; j < 13; ++j)
-      if (!std::isfinite(Pxx[i + 13 * j]) || Pxx[i + 13 * j] != Pxx[j + 13 * i])
-        return fail(c, SL2_ERR_ARG, "sl2_relocalise: Pxx must be finite and symmetric");
-  if (!psd13(Pxx)) return fail(c, SL2_ERR_ARG, "sl2_relocalise: Pxx is not positive semi-definite");
+  const std::string why = reloc_params_error(p, Pxx);
+  if (!why.empty()) return fail(c, SL2_ERR_ARG, "sl2_relocalise: " + why);
   if (cnt == 0) return SL2_OK;
   // one search job per feature of every listed stream over the id range [lo, hi], empty jobs elsewhere
   const int R = hi - lo + 1;
@@ -638,11 +663,16 @@ int sl2_relocalise(sl2_ctx *c, const int32_t *ids, int32_t cnt, int32_t slot, co
     L.scatter_to_features = 0;
     CU_TRY(c, sl2_launch_search(d, c->tmap, L, queue(c)));
     CU_TRY(c, sl2_launch_reloc(d, cnt, is.dev<int>(), lo, su.dev<int>(), sf.d, ps.dev<sl2_reloc_params>(),
-                               px.dev<double>(), rs.dev<sl2_reloc_result>(), zo.dev<int>(), fo.d, queue(c)));
+                               px.dev<double>(), 0, rs.dev<sl2_reloc_result>(), zo.dev<int>(), fo.d, nullptr, queue(c)));
     return SL2_OK;
   });
   if (rc) return rc;
   memcpy(out, rs.h, rs.bytes);
+  for (int i = 0; i < cnt; ++i)  // an accepted stream is tracking again
+    if (out[i].status == 1) {
+      const int rr = recovery_reset(c, ids[i], 1);
+      if (rr) return rr;
+    }
   if (z_uv) memcpy(z_uv, zo.h, zo.bytes);
   if (flags) memcpy(flags, fo.h, fo.bytes);
   return SL2_OK;

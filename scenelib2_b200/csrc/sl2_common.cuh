@@ -282,9 +282,11 @@ struct WarpLaunch {
   uint8_t *valid;         // [jobs] 1 = warped, 0 = the stored template (or no job); may be nullptr
 };
 cudaError_t sl2_launch_warp(const Sl2Dev &d, const WarpLaunch &L, Sl2Queue q);
-// sel_mode_dev: [B] the streams' SL2_SELECT_* settings, or nullptr: every stream selects by trace (ekf.cu)
+// sel_mode_dev: [B] the streams' SL2_SELECT_* settings, or nullptr: every stream selects by trace; rv_dev: [B] the
+// streams' recovery states, or nullptr: no stream of the launch has recovery on (ekf.cu)
 cudaError_t sl2_launch_predict(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *u3_dev,
-                               int do_predict, int do_measure, const int *sel_mode_dev, Sl2Queue q);
+                               int do_predict, int do_measure, const int *sel_mode_dev, Sl2Queue q,
+                               const sl2_recovery_result *rv_dev = nullptr);
 // The mutual-information selection (select.cu) of the streams [stream_lo, stream_lo + stream_cnt) whose mode[s] is
 // SL2_SELECT_INFORMATION, right after their predict_kernel: picks into sel_rank, the job slots and nsel
 struct SelectLaunch {
@@ -386,6 +388,15 @@ struct GyroLaunch {
 };
 // gyro_prep_kernel then gyro_downdate_kernel
 cudaError_t sl2_launch_gyro(const Sl2Dev &d, const GyroLaunch &G, Sl2Queue q);
+// The relocalisation (reloc.cu) of the cnt streams ids_dev[] (stream_lo + i when nullptr) from the full-image search's
+// results by job (job = (stream - stream_lo) * Nmax + feature).  Stream s reads its parameters at prm_dev and Pxx_dev
+// advanced by s * prm_stride bytes.  rv: nullptr (sl2_relocalise), or the recovery states of the fused step
+// (recover.cu): only streams with rv[s].attempted run, their result goes to rv[s].last and an acceptance returns them
+// to tracking
+cudaError_t sl2_launch_reloc(const Sl2Dev &d, int cnt, const int *ids_dev, int stream_lo, const int *search_uv,
+                             const uint8_t *search_found, const sl2_reloc_params *prm_dev, const double *Pxx_dev,
+                             size_t prm_stride, sl2_reloc_result *res_dev, int *zuv_dev, uint8_t *flags_dev,
+                             sl2_recovery_result *rv, Sl2Queue q);
 // one step record per stream of [stream_lo, stream_lo + stream_cnt) into ring row step % d.rec_depth; launched after
 // the cull of the fused step (records.cu).  resc: the rescue's scratch when the streams' step ran the rescue, else
 // nullptr

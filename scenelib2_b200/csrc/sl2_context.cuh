@@ -145,6 +145,16 @@ struct sl2_ctx {
   std::vector<sl2_stream_iterated> iter;  // [B]
   sl2::DevPtr<uint8_t> iter_buf;
   Sl2Iter iter_dev = {};
+  // stream recovery (sl2_set_stream_recovery): the host mirror of every stream's setting, and one device buffer
+  // (allocated when a stream first turns it on) behind the settings [B], the states [B], the job table [B][Nmax] (feature,
+  // centre, ellipse) and the search and pose kernels' outputs [B][Nmax]
+  std::vector<sl2_stream_recovery> recov;  // [B]
+  sl2::DevPtr<uint8_t> recov_buf;
+  sl2_stream_recovery *recov_set = nullptr;
+  sl2_recovery_result *recov_state = nullptr;
+  int *recov_job_feat = nullptr, *recov_uv = nullptr, *recov_zuv = nullptr;
+  double *recov_job_centre = nullptr, *recov_job_puinv = nullptr;
+  uint8_t *recov_found = nullptr, *recov_flags = nullptr;
 };
 
 namespace sl2 {
@@ -288,5 +298,13 @@ int subpixel_forget(sl2_ctx *c, int lo, int cnt);
 // the iteration on); the iteration passes of those streams on q, right before their update
 Sl2Iter iterate_args(const sl2_ctx *c, int lo, int cnt);
 int iterate_streams(sl2_ctx *c, int lo, int cnt, Sl2Queue q);
+// reloc.cu: the checks sl2_relocalise makes of its parameters and restart covariance; an empty string when accepted
+std::string reloc_params_error(const sl2_reloc_params *p, const double *Pxx);
+// recover.cu: the recovery states predict_kernel of the streams [lo, lo + cnt) reads (nullptr when none of them has
+// recovery on); the decision, the full-image search and the pose kernel of those streams on q, at the end of their
+// step of ring slot `slot`; the return of the streams [lo, lo + cnt) to tracking (the resets of include/sl2b200.h)
+const sl2_recovery_result *recovery_args(const sl2_ctx *c, int lo, int cnt);
+int recover_streams(sl2_ctx *c, int slot, int lo, int cnt, Sl2Queue q);
+int recovery_reset(sl2_ctx *c, int lo, int cnt);
 
 }  // namespace sl2

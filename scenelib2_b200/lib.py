@@ -99,6 +99,7 @@ EXPORTS = [
     "sl2_get_features", "sl2_get_feature_jacobians", "sl2_enable_timing", "sl2_last_step_times", "sl2_last_update_times", "sl2_launch_count",
     "sl2_snapshot_layout", "sl2_snapshot_bytes", "sl2_save_streams", "sl2_load_streams", "sl2_save_streams_dev", "sl2_load_streams_dev",
     "sl2_enable_records", "sl2_get_records", "sl2_get_records_dev", "sl2_relocalise",
+    "sl2_set_stream_recovery", "sl2_get_stream_recovery", "sl2_get_recovery_results",
 ]
 
 SL2_RELOC_HYPOTHESES = 1024   # three-point hypotheses per stream and sl2_relocalise call
@@ -120,6 +121,25 @@ class Sl2RelocResult(C.Structure):
 # the same result as a NumPy structured dtype: Context.relocalise returns an array of it
 RELOC_RESULT_DTYPE = np.dtype([("status", np.int32), ("matches", np.int32), ("support", np.int32),
                                ("inliers", np.int32), ("rms_px", np.float64), ("pose", np.float64, (7,))])
+
+
+
+class Sl2StreamRecovery(C.Structure):
+    """sl2_stream_recovery: a camera stream's loss detector (lost_after = 0: off) and the relocalisation the fused
+    step then tries (the parameters and restart covariance of sl2_relocalise)."""
+    _fields_ = [("lost_after", C.c_int32), ("min_matches", C.c_int32), ("retry_period", C.c_int32),
+                ("reserved", C.c_int32), ("reloc", Sl2RelocParams), ("Pxx", C.c_double * 169)]
+
+
+class Sl2RecoveryResult(C.Structure):
+    """sl2_recovery_result: a camera stream's recovery state after the last step."""
+    _fields_ = [("lost", C.c_int32), ("failed_steps", C.c_int32), ("lost_steps", C.c_int32), ("attempted", C.c_int32),
+                ("recoveries", C.c_int64), ("last", Sl2RelocResult)]
+
+
+# the same state as a NumPy structured dtype: Context.recovery_results returns an array of it
+RECOVERY_RESULT_DTYPE = np.dtype([("lost", np.int32), ("failed_steps", np.int32), ("lost_steps", np.int32),
+                                  ("attempted", np.int32), ("recoveries", np.int64), ("last", RELOC_RESULT_DTYPE)])
 
 SL2_SNAPSHOT_MAGIC = 0x53324C53
 SL2_SNAPSHOT_VERSION = 1
@@ -297,6 +317,9 @@ def load():
         L.sl2_get_records_dev.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
         L.sl2_relocalise.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(Sl2RelocParams),
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.sl2_set_stream_recovery.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamRecovery)]
+        L.sl2_get_stream_recovery.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamRecovery)]
+        L.sl2_get_recovery_results.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
         _lib = L
     return _lib
 
@@ -888,6 +911,38 @@ class Context:
         self._ck(self.L.sl2_relocalise(self.h, ids.ctypes.data, cnt, slot, C.byref(prm), Pxx.ctypes.data,
                                        res.ctypes.data, z.ctypes.data, fl.ctypes.data))
         return res[:cnt], z[:cnt], fl[:cnt]
+
+    # ---- stream recovery ------------------------------------------------------------------------
+    def set_stream_recovery(self, stream_id, lost_after, min_matches=1, retry_period=1, inlier_px=2.0, min_inliers=6,
+                            v=(0.0, 0.0, 0.0), omega=(0.0, 0.0, 1e-3), Pxx=None, reserved=0):
+        """sl2_set_stream_recovery: after lost_after consecutive steps with fewer than min_matches successful
+        measurements (0 = off, the default), the fused step stops the stream's selection and tries sl2_relocalise on
+        its frame with these parameters: on the step that declares it lost, then every retry_period-th step."""
+        r = Sl2StreamRecovery()
+        r.lost_after, r.min_matches, r.retry_period, r.reserved = (int(lost_after), int(min_matches),
+                                                                   int(retry_period), int(reserved))
+        r.reloc.inlier_px, r.reloc.min_inliers = float(inlier_px), int(min_inliers)
+        for i in range(3):
+            r.reloc.v[i], r.reloc.omega[i] = float(v[i]), float(omega[i])
+        if Pxx is not None:
+            P = np.asarray(Pxx, np.float64).reshape(13, 13).flatten(order="F")
+            for i in range(169):
+                r.Pxx[i] = float(P[i])
+        self._ck(self.L.sl2_set_stream_recovery(self.h, stream_id, C.byref(r)))
+
+    def stream_recovery(self, stream_id):
+        """-> the stream's Sl2StreamRecovery"""
+        r = Sl2StreamRecovery()
+        self._ck(self.L.sl2_get_stream_recovery(self.h, stream_id, C.byref(r)))
+        return r
+
+    def recovery_results(self, lo=0, cnt=None):
+        """sl2_get_recovery_results -> a RECOVERY_RESULT_DTYPE array (cnt,)"""
+        if cnt is None:
+            cnt = self.cfg.num_streams - lo
+        out = np.zeros(max(cnt, 1), RECOVERY_RESULT_DTYPE)
+        self._ck(self.L.sl2_get_recovery_results(self.h, lo, cnt, out.ctypes.data))
+        return out[:max(cnt, 0)]
 
 
 def config_for_scene(sc, num_streams=1, frame_slots=1, device=0, max_features=None,
