@@ -198,6 +198,84 @@ int sl2_get_stream_warp(sl2_ctx *ctx, int32_t stream_id, int32_t *on);
 int sl2_warp_templates(sl2_ctx *ctx, int32_t stream_id, int32_t n, const int32_t *feat_index, const double *xp,
                        uint8_t *out, uint8_t *valid);
 
+/* ---- patch normals: estimate the plane of each feature's patch from the images (no reference counterpart) --------
+ * The warp above takes each patch as facing the camera that first saw it.  A stream with normals on estimates each
+ * feature's normal by aligning its stored template with the step's frame through the homography the plane induces
+ * (Molton, Davison, Reid, BMVC 2004), carries the estimate as a small Gaussian per feature, and its warp uses it.
+ * Normal of feature i (y = its state, xo = its xp_org, theta = (a, b) its estimate): nW0 = xo[0:3] - y;
+ *   R0 = row 0 of pose_RRW(xo) (camera o's x axis); q = R0 - ((R0 . nW0) / (nW0 . nW0)) nW0;
+ *   E1 = q * (sqrt(nW0 . nW0) / sqrt(q . q)); E2 = (nW0 x E1) / sqrt(nW0 . nW0);
+ *   nW(theta) = (nW0 + a E1) + b E2; theta = (0, 0) is nW0 bit for bit (it is taken as nW0, not computed).
+ * a and b are the tangents of the patch's tilt away from facing camera o.  Warp: a stream with normals on warps (in
+ * the fused step, sl2_make_measurements and sl2_warp_templates) with nW(theta_i) in place of nW0; no other rule changes.
+ * Alignment of feature i, after the step's last update (x+ = the updated, normalised state, r+ its position; h+ =
+ * project_point(zeroed_point(y) from x+); z = the match the update used, the refined one with the sub-pixel refinement
+ * on), for every job of an on stream whose found is 1 after the update (consensus inliers and rescued matches):
+ *   prior: theta- = theta_i, S- = Sigma_i + sigma_step^2 I; L = S-^-1 = [S-bb, -S-ab; -S-ab, S-aa] / (S-aa S-bb -
+ *   S-ab S-ab);
+ *   unknowns phi = (a, b, tu, tv, alpha, beta), starting at (theta-, z - h+, 1, 0);
+ *   template pixel k = (row r, column c), k = r B + c: p_o = ho + (c - HALF, r - HALF); d_o = adj(RRW(xo))
+ *   unproject_point(p_o); t = (nW(theta) . (y - xo[0:3])) / (nW(theta) . d_o); X = xo[0:3] + t d_o;
+ *   zc = RRW(x+) (X - r+); g_k = project(zc) + (tu, tv) (with dh/dz J, csrc/sl2_model.cuh: patch_warp_forward);
+ *   I(u, v) = the bilinear sample of the frame (not rounded; x0 = floor(u), fx = u - x0, same order as the warp's
+ *   sample); I_u = (I(g + (1, 0)) - I(g - (1, 0))) * 0.5, I_v likewise; e_k = (alpha I(g_k) + beta) - T_k (T = the
+ *   stored template);
+ *   Jacobian row: w = RRW(x+) d_o, Jw = J w, t_a = ((E1 . (y - xo)) - t (E1 . d_o)) / (nW . d_o) (t_b with E2);
+ *   de/da = alpha ((I_u Jw_u) + (I_v Jw_v)) t_a (b likewise), de/dtu = alpha I_u, de/dtv = alpha I_v, de/dalpha = I,
+ *   de/dbeta = 1;
+ *   sums over k: lane l of a warp takes k = l + 32 j in ascending j, then the xor-shuffle tree over offsets 16, 8, 4,
+ *   2, 1 (v + v[l ^ o]); the 21 sums of J_p J_q (p <= q), the 6 of J_p e and sum e^2;
+ *   with w2 = 1 / (sigma_i sigma_i) and dt = theta - theta-: H = (J^T J) w2 with L added to its theta block,
+ *   G = (J^T e) w2 with L dt added to its theta part, cost = (sum e^2) w2 + (dt . L dt);
+ *   valid: every pixel has t finite and > 0, zc[2] > 0 and g within [1, W - 2) x [1, H - 2) (W x H the stream's own
+ *   image, so g +- 1 px is inside it), and nW(theta) . (xo[0:3] - y) > 0 and nW(theta) . (r+ - y) > 0;
+ *   Gauss-Newton: for up to max_iterations steps: the 6 x 6 Cholesky H = L L^T (a pivot <= 0 or NaN ends the
+ *   iteration), phi' = phi - H^-1 G; phi' accepted when it is valid and its cost is below phi's, else the iteration
+ *   ends;
+ *   posterior at the last accepted phi: Sigma+ = the theta block of H^-1 (the marginal over tu, tv, alpha, beta), from
+ *   L^-1's first two columns; when at least one step was accepted and that Cholesky has positive pivots: theta_i,
+ *   Sigma_i = theta, Sigma+, count_i + 1, status 1; otherwise both are left and status is 2 (no step accepted, or the
+ *   final factor failed) or 3 (the start is not valid).  Status 0: not aligned by the stream's last alignment.
+ * Every operation is a correctly rounded, never-fused FP64 operation in the order of the device code (csrc/normals.cu,
+ * tests/normals_ref.py restates it), so the results are reproducible bit for bit whatever the batch position or the
+ * step group.  Where it applies: the fused step (sl2_step, sl2_step_host, sl2_step_host_async) after its update, the
+ * rescue's second update included, and before the cull: one more kernel launch per step group holding an on stream,
+ * timed with the update in sl2_last_step_times; sl2_align_normals is that stage alone.  A stream with normals on and the
+ * warp off still aligns, but nothing uses the estimates.
+ * Lifecycle: a feature starts unestimated (theta = 0, Sigma = sigma0^2 I, count 0, status 0) when it enters through
+ * sl2_append_feature, sl2_set_features or a snapshot load (which do not carry the estimates), and when the setter is
+ * called for its stream; estimates move with their features through the cull and sl2_delete_feature, and
+ * sl2_relocalise and the recovery keep them.
+ * max_iterations = 0 (the default) is off; 1 .. SL2_MAX_NORMAL_ITERATIONS is on.  The setting belongs to the stream
+ * slot.  The first stream turned on sizes the context's scratch (num_streams x (32 + 45 max_features) bytes):
+ * SL2_ERR_CUDA, with the setting left off, when that fails.  SL2_ERR_ARG, with the setting unchanged, for a bad stream_id,
+ * a NULL v, reserved != 0, max_iterations outside [0, SL2_MAX_NORMAL_ITERATIONS], a sigma0 or sigma_i that is not finite
+ * and > 0, or a sigma_step that is not finite and >= 0. */
+#define SL2_MAX_NORMAL_ITERATIONS 8
+typedef struct sl2_stream_normals {
+  int32_t max_iterations; /* 0 (default, off) .. SL2_MAX_NORMAL_ITERATIONS Gauss-Newton steps per alignment */
+  int32_t reserved;       /* 0 */
+  double sigma0;          /* > 0: prior sigma of each tilt component of a feature that enters the map */
+  double sigma_i;         /* > 0: grey-level noise of one pixel of the alignment */
+  double sigma_step;      /* >= 0: added (squared) to each tilt variance before every alignment */
+} sl2_stream_normals;
+int sl2_set_stream_normals(sl2_ctx *ctx, int32_t stream_id, const sl2_stream_normals *v);
+int sl2_get_stream_normals(sl2_ctx *ctx, int32_t stream_id, sl2_stream_normals *v);
+/* The estimates of features feat_index[0 .. n) of stream_id: theta (n x 2), cov (n x 3: S_aa, S_ab, S_bb), normal_w
+ * (n x 3, nW(theta) / |nW(theta)|), count (alignments accepted) and status (of the last alignment); any output may be
+ * NULL.  Set: theta and cov (exactly symmetric by construction: S_aa > 0 and S_aa S_bb - S_ab S_ab > 0, all finite),
+ * count and status 0.  Both join the step groups and synchronise.  SL2_ERR_STATE for a stream with normals off;
+ * SL2_ERR_ARG, with nothing written, for a bad stream_id, n outside [0, max_features], a NULL feat_index (or, set, a
+ * NULL theta or cov) with n > 0, an index outside [0, nfeat), a non-finite theta or a cov without positive pivots. */
+int sl2_get_patch_normals(sl2_ctx *ctx, int32_t stream_id, int32_t n, const int32_t *feat_index, double *theta,
+                          double *cov, double *normal_w, int32_t *count, uint8_t *status);
+int sl2_set_patch_normals(sl2_ctx *ctx, int32_t stream_id, int32_t n, const int32_t *feat_index, const double *theta,
+                          const double *cov);
+/* The alignment of stream_id alone on the frame of ring slot `slot`, from its current state, match list and matches:
+ * what the fused step does after its update.  Joins the step groups and synchronises.  SL2_ERR_STATE for a stream with
+ * normals off; SL2_ERR_ARG for a bad stream_id or slot. */
+int sl2_align_normals(sl2_ctx *ctx, int32_t stream_id, int32_t slot);
+
 /* ---- sub-pixel refinement: fit each match's score around the search's minimum (no reference counterpart) -------
  * The reference's match is the integer position of the smallest correlation score (elliptical_search), so z carries a
  * quantisation error of sigma = 1 / sqrt(12) = 0.29 px per axis.  A stream with the refinement on fits a quadratic to

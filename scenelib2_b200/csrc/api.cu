@@ -182,6 +182,7 @@ int measure_streams(sl2_ctx *c, int32_t slot, int lo, int cnt, Sl2Queue q) {
     W.stream_cnt = cnt;
     W.on = c->warp_on_dev;
     W.out = c->warp_patches.get() + (size_t)lo * d.Nmax * d.box * 16;
+    W.nrm = normals_args(c, lo, cnt);
     CU_TRY(c, sl2_launch_warp(d, W, q));
     job_patches = W.out;
   }
@@ -354,6 +355,7 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   c->gyro.assign(B, g0);
   c->iter.assign(B, sl2_stream_iterated{});
   c->recov.assign(B, sl2_stream_recovery{});
+  c->nrm.assign(B, sl2_stream_normals{});
 #undef ALLOC
   int rc = make_tensor_map(c);
   if (rc) return failed(rc, c->err);
@@ -443,6 +445,8 @@ int sl2_set_features(sl2_ctx *c, int32_t s, int32_t n, const double *y, const do
   int rc = subpixel_forget(c, s, 1);  // a new map has no refined matches
   if (rc) return rc;
   rc = recovery_reset(c, s, 1);  // a new map: the stream is tracking
+  if (rc) return rc;
+  rc = normals_reset(c, s, 0, d.Nmax);  // and its normals are unestimated
   if (rc) return rc;
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   return SL2_OK;
@@ -551,8 +555,11 @@ static int step_group(sl2_ctx *c, int32_t slot, int lo, int cnt, Sl2Queue q, cud
     const int rc2 = rescue_streams(c, lo, cnt, q);
     if (rc2) return rc2;
   }
+  // the normal alignment reads the updated state: after the last update, part of the update's time
+  const Sl2Normals nrm = normals_args(c, lo, cnt);
+  if (nrm.prm) CU_TRY(c, sl2_launch_normals(d, lo, cnt, slot, sp, nrm, q));
   if (t) CU_TRY(c, cudaEventRecord(c->ev[3].get(), st));
-  CU_TRY(c, sl2_launch_cull(d, lo, cnt, -1, sp, q));
+  CU_TRY(c, sl2_launch_cull(d, lo, cnt, -1, sp, q, nrm));
   if (t) CU_TRY(c, cudaEventRecord(c->ev[4].get(), st));
   if (d.rec_depth) {  // after ev[4]: the step times keep their meaning
     const Sl2Rescue r = rescue ? rescue_args(c) : Sl2Rescue{};

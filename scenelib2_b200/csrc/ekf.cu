@@ -381,7 +381,7 @@ __global__ void __launch_bounds__(128) particle_predict_kernel(const Sl2Dev d, i
 // removes the rows/columns of the culled features from x and P in place.
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) cull_kernel(const Sl2Dev d, int stream_lo, int force_index,
-                                                    const Sl2Subpix sp) {
+                                                    const Sl2Subpix sp, const Sl2Normals nrm) {
   pdl_prologue();
   const int s = stream_lo + blockIdx.x;
   const int tid = threadIdx.x;
@@ -473,6 +473,12 @@ __global__ void __launch_bounds__(256) cull_kernel(const Sl2Dev d, int stream_lo
         sp.z[(fb + k) * 2 + 1] = sp.z[(fb + i) * 2 + 1];
         sp.refined[fb + k] = sp.refined[fb + i];
       }
+      if (nrm.prm) {  // and so does its normal estimate
+        for (int e = 0; e < 2; ++e) nrm.theta[(fb + k) * 2 + e] = nrm.theta[(fb + i) * 2 + e];
+        for (int e = 0; e < 3; ++e) nrm.cov[(fb + k) * 3 + e] = nrm.cov[(fb + i) * 3 + e];
+        nrm.count[fb + k] = nrm.count[fb + i];
+        nrm.status[fb + k] = nrm.status[fb + i];
+      }
     }
     if (sp.z)  // the vacated slots hold no match: a feature appended there starts unrefined
       for (int i = nk; i < nf; ++i) sp.refined[fb + i] = 0;
@@ -563,10 +569,10 @@ cudaError_t sl2_launch_particle_predict(const Sl2Dev &d, int s, int F, int Kmax,
 }
 
 cudaError_t sl2_launch_cull(const Sl2Dev &d, int stream_lo, int stream_cnt, int force_index, const Sl2Subpix &sp,
-                            Sl2Queue q) {
+                            Sl2Queue q, const Sl2Normals &nrm) {
   if (stream_cnt <= 0) return cudaSuccess;
   return sl2_launch_kernel(cull_kernel, dim3(stream_cnt), dim3(256), 0, q, sl2_use_pdl(stream_cnt), d,
-                           stream_lo, force_index, sp);
+                           stream_lo, force_index, sp, nrm);
 }
 
 extern "C" {
@@ -599,7 +605,7 @@ int sl2_delete_feature(sl2_ctx *c, int32_t s, int32_t index) {
   const int n = sl2_num_features(c, s);
   if (n < 0) return n;
   if (index < 0 || index >= n) return fail(c, SL2_ERR_ARG, "sl2_delete_feature: bad index");
-  CU_TRY(c, sl2_launch_cull(c->d, s, 1, index, subpixel_args(c, s, 1), queue(c)));
+  CU_TRY(c, sl2_launch_cull(c->d, s, 1, index, subpixel_args(c, s, 1), queue(c), normals_args(c, s, 1)));
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   return SL2_OK;
 }
@@ -613,7 +619,9 @@ int sl2_append_feature(sl2_ctx *c, int32_t s, const double *y, const double *xp_
   const int box = c->d.box, n3 = SL2_NXV + 3 * nf + 3;
   Stage ys{STAGE_IN, 24, y}, xs{STAGE_IN, 56, xp_org}, pc{STAGE_IN, Pcol ? 8 * 3 * (size_t)n3 : 0, Pcol},
       rows{STAGE_IN, (size_t)box * 16};
-  const int rc = staged_call(
+  int rc = normals_reset(c, s, nf, 1);  // the new feature's normal is unestimated
+  if (rc) return rc;
+  rc = staged_call(
       c, {&ys, &xs, &pc, &rows}, [&] { pack_patch_rows(rows.h, patch, 1, box); },
       [&] {
         CU_TRY(c, sl2_launch_append(c->d, s, ys.dev<double>(), xs.dev<double>(), rows.d,

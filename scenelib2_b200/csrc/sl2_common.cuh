@@ -269,9 +269,20 @@ struct SearchLaunch {
 };
 
 cudaError_t sl2_launch_search(const Sl2Dev &d, const CUtensorMap &tmap, const SearchLaunch &L, Sl2Queue q);
+// The patch normals (normals.cu; include/sl2b200.h, sl2_set_stream_normals) the warp, the cull and the alignment take
+// as an argument, feature-indexed like Sl2Dev::xp_org: theta [B][Nmax][2], cov [B][Nmax][3] (S_aa, S_ab, S_bb), count
+// and status [B][Nmax].  prm == nullptr when no stream of the launch has normals on; stream s is on when
+// prm[s].max_iterations > 0.
+struct Sl2Normals {
+  const sl2_stream_normals *prm;  // [B]
+  double *theta, *cov;
+  int *count;
+  uint8_t *status;
+};
+__device__ __forceinline__ bool normals_on(const Sl2Normals &n, int s) { return n.prm && n.prm[s].max_iterations > 0; }
 // The planar patch warp (warp.cu): the template of every job of the streams [stream_lo, stream_lo + stream_cnt) at
 // the pose xp, into out[job] in the row-padded layout of Sl2Dev::patches.  A stream whose on[s] is 0 gets its stored
-// templates copied.
+// templates copied; a stream with normals on warps through its features' estimated normals.
 struct WarpLaunch {
   const int *job_feat;    // [stream_cnt * jobs_per_stream], -1 = no job
   int jobs_per_stream;    // stride between streams in job_feat and out
@@ -280,6 +291,7 @@ struct WarpLaunch {
   const uint8_t *on;      // [B] the streams' warp settings, or nullptr: every stream warps
   uint8_t *out;           // [jobs][box][16]
   uint8_t *valid;         // [jobs] 1 = warped, 0 = the stored template (or no job); may be nullptr
+  Sl2Normals nrm;         // the streams' estimated normals ({}: every stream warps with nW0)
 };
 cudaError_t sl2_launch_warp(const Sl2Dev &d, const WarpLaunch &L, Sl2Queue q);
 // sel_mode_dev: [B] the streams' SL2_SELECT_* settings, or nullptr: every stream selects by trace; rv_dev: [B] the
@@ -354,9 +366,13 @@ cudaError_t sl2_launch_iterate_pass(const Sl2Dev &d, int stream_lo, int stream_c
 // five kernels then leave as they found it (update.cu)
 cudaError_t sl2_launch_update_rescued(const Sl2Dev &d, int stream_lo, int stream_cnt, int *m2, const Sl2Subpix &sp,
                                       Sl2Queue q);
-// sp: the sub-pixel matches move with their features
+// sp, nrm: the sub-pixel matches and the normal estimates move with their features
 cudaError_t sl2_launch_cull(const Sl2Dev &d, int stream_lo, int stream_cnt, int force_index, const Sl2Subpix &sp,
-                            Sl2Queue q);
+                            Sl2Queue q, const Sl2Normals &nrm = {});
+// The normal alignment (normals.cu) of the streams [stream_lo, stream_lo + stream_cnt) with normals on, after their
+// last update, on the frame of ring slot `slot`
+cudaError_t sl2_launch_normals(const Sl2Dev &d, int stream_lo, int stream_cnt, int slot, const Sl2Subpix &sp,
+                               const Sl2Normals &nrm, Sl2Queue q);
 // The consensus rescue (rescue.cu): chi2[s] (0 = off) and the consensus's tau2[s] of every stream, and the per-stream
 // scratch the step records read: m2 = rows of the second update, nis1 / logdet1 = the first update's NIS and log det S
 struct Sl2Rescue {

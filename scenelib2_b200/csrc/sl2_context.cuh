@@ -155,6 +155,11 @@ struct sl2_ctx {
   int *recov_job_feat = nullptr, *recov_uv = nullptr, *recov_zuv = nullptr;
   double *recov_job_centre = nullptr, *recov_job_puinv = nullptr;
   uint8_t *recov_found = nullptr, *recov_flags = nullptr;
+  // patch normals (sl2_set_stream_normals): the host mirror of every stream's setting, and one device buffer
+  // (allocated when a stream first turns it on) behind the settings [B], theta, cov, count and status
+  std::vector<sl2_stream_normals> nrm;  // [B]
+  sl2::DevPtr<uint8_t> nrm_buf;
+  Sl2Normals nrm_dev = {};
 };
 
 namespace sl2 {
@@ -306,5 +311,9 @@ std::string reloc_params_error(const sl2_reloc_params *p, const double *Pxx);
 const sl2_recovery_result *recovery_args(const sl2_ctx *c, int lo, int cnt);
 int recover_streams(sl2_ctx *c, int slot, int lo, int cnt, Sl2Queue q);
 int recovery_reset(sl2_ctx *c, int lo, int cnt);
+// normals.cu: the normal estimates the kernels of the streams [lo, lo + cnt) read ({} when none of them has normals
+// on); features [f0, f0 + n) of stream s unestimated (nothing when the stream has normals off)
+Sl2Normals normals_args(const sl2_ctx *c, int lo, int cnt);
+int normals_reset(sl2_ctx *c, int s, int f0, int n);
 
 }  // namespace sl2

@@ -1,6 +1,6 @@
 // sl2_model.cuh — the device camera and feature models of predict_kernel and particle_predict_kernel (ekf.cu),
-// consensus_kernel (consensus.cu), rescue_kernel (rescue.cu), reloc_kernel (reloc.cu), warp_kernel (warp.cu) and
-// iterate_kernel (iterate.cu).  Everything that decides which pixels are searched
+// consensus_kernel (consensus.cu), rescue_kernel (rescue.cu), reloc_kernel (reloc.cu), warp_kernel (warp.cu),
+// normals_kernel (normals.cu) and iterate_kernel (iterate.cu).  Everything that decides which pixels are searched
 // (S_i, S^-1, h_i) or which match is an inlier uses never-fused rd ops in the oracle's evaluation order.
 #pragma once
 #include "sl2_common.cuh"
@@ -152,17 +152,40 @@ __device__ __forceinline__ void mat3_adj(const rd M[3][3], rd A[3][3]) {
     }
 }
 
+// The patch normal's basis (include/sl2b200.h, sl2_set_stream_normals): nW0 = xo[0:3] - y, E1 = camera o's x axis
+// (row 0 of RRWo = pose_RRW(xo)) made orthogonal to nW0 and scaled to |nW0|, E2 = nW0 x E1 / |nW0|
+struct PatchBasis {
+  rd n0[3], E1[3], E2[3];
+};
+__device__ __forceinline__ void patch_basis(const double *xo, const rd y[3], const rd RRWo[3][3], PatchBasis &b) {
+  for (int i = 0; i < 3; ++i) b.n0[i] = rd(xo[i]) - y[i];
+  const rd nn = dot3(b.n0, b.n0);
+  const rd pr = dot3(RRWo[0], b.n0) / nn;
+  rd q[3];
+  for (int i = 0; i < 3; ++i) q[i] = RRWo[0][i] - pr * b.n0[i];
+  const rd len = rsqrt_(nn), sc = len / rsqrt_(dot3(q, q));
+  for (int i = 0; i < 3; ++i) b.E1[i] = q[i] * sc;
+  b.E2[0] = (b.n0[1] * b.E1[2] - b.n0[2] * b.E1[1]) / len;
+  b.E2[1] = (b.n0[2] * b.E1[0] - b.n0[0] * b.E1[2]) / len;
+  b.E2[2] = (b.n0[0] * b.E1[1] - b.n0[1] * b.E1[0]) / len;
+}
+// nW(theta) = (nW0 + a E1) + b E2; theta = (0, 0) is nW0 itself
+__device__ __forceinline__ void patch_normal(const PatchBasis &b, rd ta, rd tb, rd nW[3]) {
+  const bool zero = ta.v == 0.0 && tb.v == 0.0;
+  for (int i = 0; i < 3; ++i) nW[i] = zero ? b.n0[i] : (b.n0[i] + ta * b.E1[i]) + tb * b.E2[i];
+}
+
 // What one feature's warp at the camera pose xp shares over its pixels: the feature y seen from xp (h, bit for bit the
 // prediction's) and from xo = xp_org (ho, the template centre), adj(RRW) (the ray's matrix: RRW is a rotation only
-// for |q| = 1, quirk Q1, so RRW^T is not its inverse), the plane through y with normal nW = xo[0:3] - y and
-// num = nW . (y - r)
+// for |q| = 1, quirk Q1, so RRW^T is not its inverse), the plane through y with normal nW = xo[0:3] - y (nW(theta)
+// when theta, the feature's estimated tilt, is given) and num = nW . (y - r)
 struct PatchWarp {
   rd adj[3][3], RRWo[3][3];  // adj(pose_RRW(xp)), pose_RRW(xo)
   rd nW[3], num;
   rd h[2], ho[2];
 };
 __device__ __forceinline__ void patch_warp_setup(const double *cam, const double *xp, const double *xo, const rd y[3],
-                                                 PatchWarp &w) {
+                                                 PatchWarp &w, const double *theta = nullptr) {
   rd d[3], z[3], uc, vc, RRW[3][3];
   pose_RRW(xp, RRW);
   zeroed_point(RRW, y, xp, d, z);
@@ -172,7 +195,13 @@ __device__ __forceinline__ void patch_warp_setup(const double *cam, const double
   pose_RRW(xo, w.RRWo);
   zeroed_point(w.RRWo, y, xo, dox, zo);
   project_point(cam, zo, w.ho, uc, vc);
-  for (int i = 0; i < 3; ++i) w.nW[i] = rd(xo[i]) - y[i];
+  if (theta && (theta[0] != 0.0 || theta[1] != 0.0)) {
+    PatchBasis b;
+    patch_basis(xo, y, w.RRWo, b);
+    patch_normal(b, rd(theta[0]), rd(theta[1]), w.nW);
+  } else {
+    for (int i = 0; i < 3; ++i) w.nW[i] = rd(xo[i]) - y[i];
+  }
   w.num = dot3(w.nW, d);
 }
 
@@ -246,6 +275,36 @@ __device__ __forceinline__ void project(const double *cam, const rd z[3], rd h[2
       for (int k = 0; k < 2; ++k) s = s + dh[i][k] * du[k][j];
       J[i][j] = s;
     }
+}
+
+// The mirror of patch_warp_source for the normal alignment (normals.cu): template pixel (db, da) (column, row offset
+// from the centre) of the camera at xo, through the plane through y with normal nW (nd = nW . (y - xo[0:3]), nE1 /
+// nE2 = E1 / E2 . (y - xo[0:3])), into the camera at x (RRW = pose_RRW(x)): p_o = ho + (db, da); d_o = adjo
+// unproject_point(p_o); den = nW . d_o; t = nd / den; zc = RRW ((xo[0:3] + t d_o) - x[0:3]); g = project(zc) (J =
+// dh/dz); Jw = J (RRW d_o); t_a = (nE1 - t (E1 . d_o)) / den, t_b likewise with E2.  True when t is finite and > 0 and
+// zc[2] > 0.
+struct PatchFwd {
+  rd g[2], Jw[2], ta, tb;
+};
+__device__ __forceinline__ bool patch_warp_forward(const double *cam, const rd adjo[3][3], const rd ho[2],
+                                                   const double *xo, const rd RRW[3][3], const double *x,
+                                                   const PatchBasis &b, const rd nW[3], rd nd, rd nE1, rd nE2, int db,
+                                                   int da, PatchFwd &o) {
+  const rd p[2] = {ho[0] + rd((double)db), ho[1] + rd((double)da)};
+  rd c[3], dO[3];
+  unproject_point(cam, p, c);
+  mat3_vec(adjo, c, dO);
+  const rd den = dot3(nW, dO);
+  const rd t = nd / den;
+  rd e[3], zc[3], w[3], J[2][3];
+  for (int i = 0; i < 3; ++i) e[i] = (rd(xo[i]) + t * dO[i]) - rd(x[i]);
+  mat3_vec(RRW, e, zc);
+  project(cam, zc, o.g, J);
+  mat3_vec(RRW, dO, w);
+  for (int i = 0; i < 2; ++i) o.Jw[i] = (J[i][0] * w[0] + J[i][1] * w[1]) + J[i][2] * w[2];
+  o.ta = (nE1 - t * dot3(b.E1, dO)) / den;
+  o.tb = (nE2 - t * dot3(b.E2, dO)) / den;
+  return isfinite(t.v) && t.v > 0.0 && zc[2].v > 0.0;
 }
 
 // Camera::MeasurementNoise, camera.cpp:282-300: R = var I

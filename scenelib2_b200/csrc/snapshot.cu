@@ -348,6 +348,8 @@ int sl2_load_streams(sl2_ctx *c, int32_t lo, int32_t cnt, const void *buf, size_
   if (rf) return rf;
   rf = recovery_reset(c, lo, cnt);  // a loaded stream is tracking
   if (rf) return rf;
+  for (int s = lo; s < lo + cnt && !rf; ++s) rf = normals_reset(c, s, 0, c->d.Nmax);  // snapshots carry no normals
+  if (rf) return rf;
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   return loaded_cameras(c, lo, cams);
 }
@@ -388,6 +390,8 @@ int sl2_load_streams_dev(sl2_ctx *c, int32_t lo, int32_t cnt, const void *buf_de
   int rf = subpixel_forget(c, lo, cnt);  // z is the integer match until the streams' next step
   if (rf) return rf;
   rf = recovery_reset(c, lo, cnt);  // a loaded stream is tracking
+  if (rf) return rf;
+  for (int s = lo; s < lo + cnt && !rf; ++s) rf = normals_reset(c, s, 0, c->d.Nmax);  // snapshots carry no normals
   if (rf) return rf;
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   return loaded_cameras(c, lo, cams);

@@ -51,7 +51,7 @@ __global__ void __launch_bounds__(32 * WARP_WARPS) warp_kernel(const Sl2Dev d, c
     const double *yp = d.x + (size_t)s * d.ld + SL2_NXV + 3 * feat;
     const rd y[3] = {rd(yp[0]), rd(yp[1]), rd(yp[2])};
     PatchWarp pw;
-    patch_warp_setup(cam, xp, xo, y, pw);
+    patch_warp_setup(cam, xp, xo, y, pw, normals_on(L.nrm, s) ? L.nrm.theta + g * 2 : nullptr);
 #pragma unroll
     for (int k = 0; k < PER; ++k) {
       const int i = lane + 32 * k, a = i >> 4, b = i & 15;
@@ -130,6 +130,7 @@ int sl2_warp_templates(sl2_ctx *c, int32_t s, int32_t n, const int32_t *feat_ind
     W.xp = xs.dev<double>();
     W.out = to.d;
     W.valid = va.d;
+    W.nrm = normals_args(c, s, 1);
     CU_TRY(c, sl2_launch_warp(c->d, W, queue(c)));
     return SL2_OK;
   });

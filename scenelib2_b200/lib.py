@@ -73,6 +73,17 @@ class Sl2StreamIterated(C.Structure):
 
 SL2_MAX_ITERATIONS = 8
 
+
+class Sl2StreamNormals(C.Structure):
+    """sl2_stream_normals: a camera stream's patch normal estimation: Gauss-Newton steps per alignment (0 = off), the
+    prior sigma of each tilt component of a new feature, the grey-level noise of one pixel and the per-alignment
+    random-walk sigma of the tilt."""
+    _fields_ = [("max_iterations", C.c_int32), ("reserved", C.c_int32), ("sigma0", C.c_double),
+                ("sigma_i", C.c_double), ("sigma_step", C.c_double)]
+
+
+SL2_MAX_NORMAL_ITERATIONS = 8
+
 SL2_SRC_GRAY_RING, SL2_SRC_GRAY8, SL2_SRC_RGB24, SL2_SRC_UYVY = 0, 1, 2, 3
 SL2_MAX_SOURCE_DIM = 4096
 SOURCE_BPP = {SL2_SRC_GRAY8: 1, SL2_SRC_RGB24: 3, SL2_SRC_UYVY: 2}
@@ -88,6 +99,8 @@ EXPORTS = [
     "sl2_set_stream_selection", "sl2_get_stream_selection",
     "sl2_set_stream_gyro", "sl2_get_stream_gyro", "sl2_set_gyro_samples", "sl2_gyro_update", "sl2_get_gyro_results",
     "sl2_set_stream_iterated", "sl2_get_stream_iterated", "sl2_get_iterated_results",
+    "sl2_set_stream_normals", "sl2_get_stream_normals", "sl2_get_patch_normals", "sl2_set_patch_normals",
+    "sl2_align_normals",
     "sl2_set_frame", "sl2_set_frames", "sl2_set_frames_dev",
     "sl2_set_stream_source", "sl2_get_stream_source", "sl2_frame_set_layout", "sl2_set_features",
     "sl2_num_features", "sl2_state_size", "sl2_set_state", "sl2_get_state", "sl2_delete_feature", "sl2_append_feature",
@@ -281,6 +294,12 @@ def load():
         L.sl2_set_stream_iterated.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamIterated)]
         L.sl2_get_stream_iterated.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamIterated)]
         L.sl2_get_iterated_results.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.sl2_set_stream_normals.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamNormals)]
+        L.sl2_get_stream_normals.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamNormals)]
+        L.sl2_get_patch_normals.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_void_p, C.c_void_p]
+        L.sl2_set_patch_normals.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.sl2_align_normals.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
         L.sl2_warp_templates.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_void_p]
         L.sl2_set_frame.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_size_t]
@@ -532,6 +551,47 @@ class Context:
         it, st, dl = np.zeros(k, np.int32), np.zeros(k, np.int32), np.zeros(k)
         self._ck(self.L.sl2_get_iterated_results(self.h, lo, cnt, it.ctypes.data, st.ctypes.data, dl.ctypes.data))
         return it, st, dl
+
+    # ---- patch normals -------------------------------------------------------------------------
+    def set_stream_normals(self, stream_id, max_iterations, sigma0=0.5, sigma_i=8.0, sigma_step=0.0, reserved=0):
+        """sl2_set_stream_normals: estimate each feature's patch normal from the images with up to max_iterations
+        Gauss-Newton steps per alignment (0 = off, the default), and warp the stream's templates through it; resets
+        the stream's estimates."""
+        v = Sl2StreamNormals(int(max_iterations), int(reserved), float(sigma0), float(sigma_i), float(sigma_step))
+        self._ck(self.L.sl2_set_stream_normals(self.h, stream_id, C.byref(v)))
+
+    def stream_normals(self, stream_id):
+        """-> dict(max_iterations, sigma0, sigma_i, sigma_step)"""
+        v = Sl2StreamNormals()
+        self._ck(self.L.sl2_get_stream_normals(self.h, stream_id, C.byref(v)))
+        return dict(max_iterations=v.max_iterations, sigma0=v.sigma0, sigma_i=v.sigma_i, sigma_step=v.sigma_step)
+
+    def patch_normals(self, stream_id, feat_index):
+        """sl2_get_patch_normals -> dict(theta (n, 2), cov (n, 3): S_aa, S_ab, S_bb, normal_w (n, 3) unit world
+        normals, count (n,) accepted alignments, status (n,): 0 not aligned, 1 accepted, 2 no step accepted,
+        3 invalid start)."""
+        feat_index = np.ascontiguousarray(feat_index, np.int32).reshape(-1)
+        n = feat_index.size
+        th, cv, nw = np.zeros((n, 2)), np.zeros((n, 3)), np.zeros((n, 3))
+        ct, st = np.zeros(n, np.int32), np.zeros(n, np.uint8)
+        self._ck(self.L.sl2_get_patch_normals(self.h, stream_id, n, feat_index.ctypes.data, th.ctypes.data,
+                                              cv.ctypes.data, nw.ctypes.data, ct.ctypes.data, st.ctypes.data))
+        return dict(theta=th, cov=cv, normal_w=nw, count=ct, status=st)
+
+    def set_patch_normals(self, stream_id, feat_index, theta, cov):
+        """sl2_set_patch_normals: the estimates theta (n, 2) and cov (n, 3: S_aa, S_ab, S_bb) of the features
+        feat_index, with count and status 0."""
+        feat_index = np.ascontiguousarray(feat_index, np.int32).reshape(-1)
+        n = feat_index.size
+        theta = np.ascontiguousarray(theta, np.float64).reshape(n, 2)
+        cov = np.ascontiguousarray(cov, np.float64).reshape(n, 3)
+        self._ck(self.L.sl2_set_patch_normals(self.h, stream_id, n, feat_index.ctypes.data, theta.ctypes.data,
+                                              cov.ctypes.data))
+
+    def align_normals(self, stream_id, slot):
+        """sl2_align_normals: the stream's normal alignment on ring slot `slot`, as the fused step runs it after its
+        update."""
+        self._ck(self.L.sl2_align_normals(self.h, stream_id, slot))
 
     # ---- frames -------------------------------------------------------------------------------
     def set_stream_source(self, stream_id, format, width=0, height=0):
