@@ -434,6 +434,81 @@ int sl2_gyro_update(sl2_ctx *ctx, int32_t stream_id, const double *rate3);
  * part of a snapshot.  Joins both step groups and synchronises.  SL2_ERR_ARG for a bad range. */
 int sl2_get_gyro_results(sl2_ctx *ctx, int32_t lo, int32_t cnt, double *nis, int32_t *status);
 
+/* ---- accelerometer: a measured linear acceleration drives the motion prediction (the reference's control input u,
+ *      motion_model.cpp:84-146, with the position term and the noise below) ---------------------------------------
+ * The constant-velocity model allows a linear acceleration of sigma = 4 m/s^2 per axis: a camera that is shoved,
+ * braked or jolted harder has its features predicted where they are not.  A stream with an accelerometer takes one
+ * specific-force sample per step and predicts with the acceleration it measures (Pinies, Lupton, Sukkarieh, Tardos,
+ * ICRA 2007).
+ * Setting: R_ac (row-major) takes camera-frame vectors into the accelerometer's frame; bias b (m/s^2) and cov C
+ * ((m/s^2)^2, the covariance of one sample), both in the accelerometer's frame; gravity g, the gravity vector in the
+ * world frame (m/s^2, the map's metres: about (0, 0, -9.81) when the world's z axis points up); sd_a >= 0 (m/s^2), the
+ * linear acceleration the sample does not explain (vibration, lever arm, timing), which replaces the model's 4 m/s^2.
+ * A sample f is the mean specific force over the frame period [t - dt, t] in the accelerometer's frame, so a device at
+ * rest reads -R_ac R(q)^T g + b.  When the setting is made, Rc = R_ac^T C R_ac is formed once, by the formula of
+ * sl2_set_stream_gyro, and s2 = sd_a sd_a.
+ * Prediction of a step with a sample, x = (r, q, v, omega) the state before the step, dt the stream's delta_t; sums
+ * written "sum" start from 0.0 and add their terms in ascending index order:
+ *   1. dk = f[k] - b[k]; fc[i] = (R_ac[0][i] d0 + R_ac[1][i] d1) + R_ac[2][i] d2.
+ *   2. R = R(q), the model's rotation of q (camera to world; Eigen's toRotationMatrix, also for |q| != 1);
+ *      a[i] = sum_k R[i][k] fc[k] + g[i].
+ *   3. D = dRq_times_a_by_dq(q, fc) (3 x 4, columns w, x, y, z; feature_model.cpp:164-185): the derivative of the
+ *      homogeneous form R(q) fc + (|q|^2 - 1) fc, which equals d(R(q) fc)/dq along directions tangent to |q| = 1;
+ *      column c is sum_k Mc[i][k] fc[k] with the reference's dR_by_dq0 / dqx / dqy / dqz matrices Mc.
+ *   4. M[i][j] = sum_m R[i][m] Rc[m][j]; for i <= j: t = sum_m M[i][m] R[j][m], plus s2 when i = j;
+ *      L[i][j] = L[j][i] = (t dt) dt.
+ *   If any of a, D and L is not finite, the step runs the reference prediction (status 2, skipped).
+ *   5. h = (0.5 dt) dt; r'[i] = (r[i] + v[i] dt) + a[i] h; q' and omega' as the reference; v'[i] = v[i] + a[i] dt.
+ *   6. F is the reference's F with F[i][3 + j] = h D[i][j] and F[7 + i][3 + j] = dt D[i][j] (i < 3, j < 4).
+ *   7. Q = Gn Pnn Gn^T with the reference's Gn and, in the kernel's order, (Gn Pnn)[i][k] =
+ *      ((0 + Gn[i][0] L[0][k]) + Gn[i][1] L[1][k]) + Gn[i][2] L[2][k] for k < 3; the angular block of Pnn stays
+ *      (6 6 dt) dt I.
+ *   8. P' = F P F^T + Q through the prediction's own passes, for the 13 x 13 block and the 13 x 3N panel.
+ * Every operation is a correctly rounded FP64 operation (never fused) in the order written above and in the kernel
+ * (csrc/ekf.cu, accel_model, motion_model and predict_kernel).  A stream that is off, a step without a valid sample
+ * and a skipped step run the reference prediction (u = 0) bit for bit.  Out of scope: the lever arm between the
+ * accelerometer and the camera, a time offset, online bias estimation and per-sample covariances.
+ * Where it applies: the fused step (sl2_step, sl2_step_host, sl2_step_host_async) of ring slot t consumes slot t's
+ * sample of every accelerometer-on stream and clears its valid byte, so a sample is used by exactly one step.  The
+ * staged form is sl2_accel_predict, in place of sl2_ekf_predict; sl2_ekf_predict(u3) stays the reference's.  With the
+ * gyroscope also on, the accelerometer's prediction is the one the gyro update follows.  No launch is added: the work
+ * is in the prediction kernel.  The step records are unchanged.
+ * on = 0 (the default; the getter then shows R_ac = I, b = 0, C = I, g = 0, sd_a = 4) is off.  Ordering like
+ * sl2_set_stream_config.  The setting belongs to the stream slot: snapshots do not carry it and a load leaves it.  A
+ * call that turns an off stream on clears that stream's samples in every slot; a call that turns a stream on or off
+ * clears its last result (status 0, a = 0).  The first stream turned on allocates the context's accelerometer buffers
+ * (a sample ring of frame_slots x num_streams and the per-stream settings and results): SL2_ERR_CUDA, with the
+ * setting left off, when that allocation fails.  SL2_ERR_ARG, with the setting unchanged, for: a bad stream_id or NULL
+ * a; reserved != 0 or on outside {0, 1}; a non-finite entry; an R_ac that is not a rotation or a cov that is not
+ * symmetric positive definite (the checks of sl2_set_stream_gyro); a negative sd_a. */
+typedef struct sl2_stream_accel {
+  int32_t on;         /* 0 (default) or 1 */
+  int32_t reserved;   /* 0 */
+  double R_ac[9];     /* row-major rotation: camera frame -> accelerometer frame */
+  double bias[3];     /* m/s^2, accelerometer frame */
+  double cov[9];      /* row-major covariance of one sample (m/s^2)^2, accelerometer frame; symmetric positive definite */
+  double gravity[3];  /* m/s^2, world frame */
+  double sd_a;        /* m/s^2, >= 0: the acceleration a sample does not explain */
+} sl2_stream_accel;
+int sl2_set_stream_accel(sl2_ctx *ctx, int32_t stream_id, const sl2_stream_accel *a);
+int sl2_get_stream_accel(sl2_ctx *ctx, int32_t stream_id, sl2_stream_accel *a);
+/* The samples of streams [lo, lo + cnt) for the fused step of ring slot `slot`: forces cnt x 3 (m/s^2, accelerometer
+ * frame), valid cnt bytes (NULL: all valid; 0 = no sample).  Ordered on the context's stream like
+ * sl2_set_stream_config; returns once the caller's buffers may be reused.  Samples of off streams are kept and never
+ * read.  SL2_ERR_ARG, with nothing written, for a bad slot or range, a NULL forces with cnt > 0, or a valid sample with
+ * a non-finite force; SL2_ERR_STATE while no stream of the context has ever turned its accelerometer on. */
+int sl2_set_accel_samples(sl2_ctx *ctx, int32_t slot, int32_t lo, int32_t cnt, const double *forces,
+                          const uint8_t *valid);
+/* The staged prediction of one stream with the sample f3 (3), in place of sl2_ekf_predict: the fused step's kernel
+ * and operations.  SL2_ERR_ARG for a bad stream_id, a NULL or non-finite f3; SL2_ERR_STATE when the stream's
+ * accelerometer is off.  Synchronises. */
+int sl2_accel_predict(sl2_ctx *ctx, int32_t stream_id, const double *f3);
+/* The last prediction of streams [lo, lo + cnt): accel (cnt x 3) the world-frame a of step 2 (0 unless status is 1;
+ * about 0 at rest when R_ac, b and g are right) and status 0 (no sample this step), 1 (applied) or 2 (skipped).
+ * Either pointer may be NULL.  Not part of a snapshot.  Joins both step groups and synchronises.  SL2_ERR_ARG for a
+ * bad range. */
+int sl2_get_accel_results(sl2_ctx *ctx, int32_t lo, int32_t cnt, double *accel, int32_t *status);
+
 /* ---- iterated update: relinearise the EKF update at the updated state (no reference counterpart) -------------------
  * The plain update evaluates h and H once, at the prediction.  When an innovation is large against the curvature of h
  * (a feature whose depth is still uncertain along its ray) that linearisation is wrong to first order: the posterior

@@ -3,7 +3,7 @@ import os
 import subprocess
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-SOURCES = ["csrc/api.cu", "csrc/search.cu", "csrc/ekf.cu", "csrc/select.cu", "csrc/consensus.cu", "csrc/rescue.cu", "csrc/gyro.cu",
+SOURCES = ["csrc/api.cu", "csrc/search.cu", "csrc/ekf.cu", "csrc/select.cu", "csrc/consensus.cu", "csrc/rescue.cu", "csrc/gyro.cu", "csrc/accel.cu",
            "csrc/warp.cu", "csrc/subpixel.cu", "csrc/iterate.cu", "csrc/normals.cu",
            "csrc/reloc.cu", "csrc/recover.cu", "csrc/update.cu", "csrc/detect.cu", "csrc/particles.cu", "csrc/smoe.cu", "csrc/snapshot.cu", "csrc/records.cu", "csrc/ingest.cu"]
 HEADERS = ["csrc/sl2_common.cuh", "csrc/sl2_context.cuh", "csrc/sl2_model.cuh", "csrc/sl2_ptx.cuh", "csrc/sl2_score.cuh",

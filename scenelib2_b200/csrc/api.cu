@@ -353,6 +353,10 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   sl2_stream_gyro g0 = {};  // off; a rotation and a covariance the setter accepts
   for (int i = 0; i < 3; ++i) g0.R_gc[4 * i] = g0.cov[4 * i] = 1.0;
   c->gyro.assign(B, g0);
+  sl2_stream_accel a0 = {};  // off; a rotation, a covariance and an sd_a the setter accepts
+  for (int i = 0; i < 3; ++i) a0.R_ac[4 * i] = a0.cov[4 * i] = 1.0;
+  a0.sd_a = 4.0;
+  c->accel.assign(B, a0);
   c->iter.assign(B, sl2_stream_iterated{});
   c->recov.assign(B, sl2_stream_recovery{});
   c->nrm.assign(B, sl2_stream_normals{});
@@ -523,13 +527,14 @@ static int step_group(sl2_ctx *c, int32_t slot, int lo, int cnt, Sl2Queue q, cud
   if (t) CU_TRY(c, cudaEventRecord(c->ev[0].get(), st));
   const bool info = selection_on(c, lo, cnt);
   const sl2_recovery_result *rv = recovery_args(c, lo, cnt);  // a lost stream selects nothing
+  const Sl2Accel acc = accel_args(c, slot, lo, cnt);  // inside the motion prediction
   if (gyro_on(c, lo, cnt)) {  // the motion prediction, the gyro update, then the feature prediction
-    CU_TRY(c, sl2_launch_predict(d, lo, cnt, nullptr, 1, 0, nullptr, q));
+    CU_TRY(c, sl2_launch_predict(d, lo, cnt, nullptr, 1, 0, nullptr, q, nullptr, acc));
     const int rc = gyro_streams(c, slot, lo, cnt, q);
     if (rc) return rc;
     CU_TRY(c, sl2_launch_predict(d, lo, cnt, nullptr, 0, 1, info ? c->sel_mode_dev : nullptr, q, rv));
   } else {
-    CU_TRY(c, sl2_launch_predict(d, lo, cnt, nullptr, 1, 1, info ? c->sel_mode_dev : nullptr, q, rv));
+    CU_TRY(c, sl2_launch_predict(d, lo, cnt, nullptr, 1, 1, info ? c->sel_mode_dev : nullptr, q, rv, acc));
   }
   if (info) {  // part of the predict's time
     const int rc = select_streams(c, lo, cnt, q);

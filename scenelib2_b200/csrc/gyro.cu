@@ -184,26 +184,40 @@ int gyro_alloc(sl2_ctx *c) {
   return SL2_OK;
 }
 
+// the setting's checks of include/sl2b200.h; an empty string when it is accepted
+std::string gyro_setting_error(const sl2_stream_gyro *g) {
+  if (g->reserved != 0 || (g->on != 0 && g->on != 1)) return "reserved must be 0 and on 0 or 1";
+  if (!finite_all(g->R_gc, 9) || !finite_all(g->bias, 3) || !finite_all(g->cov, 9)) return "non-finite value";
+  return sensor_frame_error(g->R_gc, g->cov, "R_gc");
+}
+
+Sl2GyroParam gyro_param(const sl2_stream_gyro &g) {
+  Sl2GyroParam p;
+  sensor_cov_in_camera(g.R_gc, g.cov, p.Rc);
+  for (int i = 0; i < 9; ++i) p.R[i] = g.R_gc[i];
+  for (int i = 0; i < 3; ++i) p.b[i] = g.bias[i];
+  return p;
+}
+
+}  // namespace
+
+namespace sl2 {
+
 bool finite_all(const double *v, int n) {
   for (int i = 0; i < n; ++i)
     if (!std::isfinite(v[i])) return false;
   return true;
 }
 
-// the setting's checks of include/sl2b200.h; an empty string when it is accepted
-std::string gyro_setting_error(const sl2_stream_gyro *g) {
-  if (g->reserved != 0 || (g->on != 0 && g->on != 1)) return "reserved must be 0 and on 0 or 1";
-  if (!finite_all(g->R_gc, 9) || !finite_all(g->bias, 3) || !finite_all(g->cov, 9)) return "non-finite value";
-  const double *R = g->R_gc;
+std::string sensor_frame_error(const double *R, const double *C, const std::string &rname) {
   for (int i = 0; i < 3; ++i)
     for (int j = 0; j < 3; ++j) {
       const double rr = R[3 * i] * R[3 * j] + R[3 * i + 1] * R[3 * j + 1] + R[3 * i + 2] * R[3 * j + 2];
-      if (!(std::fabs(rr - (i == j ? 1.0 : 0.0)) <= 1e-9)) return "R_gc is not a rotation";
+      if (!(std::fabs(rr - (i == j ? 1.0 : 0.0)) <= 1e-9)) return rname + " is not a rotation";
     }
   const double det = R[0] * (R[4] * R[8] - R[5] * R[7]) - R[1] * (R[3] * R[8] - R[5] * R[6]) +
                      R[2] * (R[3] * R[7] - R[4] * R[6]);
-  if (!(det > 0.0)) return "R_gc is not a rotation";
-  const double *C = g->cov;
+  if (!(det > 0.0)) return rname + " is not a rotation";
   if (C[1] != C[3] || C[2] != C[6] || C[5] != C[7]) return "cov is not symmetric";
   const double l00 = std::sqrt(C[0]), l10 = C[3] / l00, l20 = C[6] / l00;
   const double a11 = C[4] - l10 * l10, l11 = std::sqrt(a11);
@@ -214,9 +228,7 @@ std::string gyro_setting_error(const sl2_stream_gyro *g) {
 }
 
 // Rc = R^T C R: M = C R, then the upper triangle of R^T M, mirrored (include/sl2b200.h states the order)
-Sl2GyroParam gyro_param(const sl2_stream_gyro &g) {
-  Sl2GyroParam p;
-  const double *R = g.R_gc, *C = g.cov;
+void sensor_cov_in_camera(const double *R, const double *C, double Rc[9]) {
   double M[9];
   for (int k = 0; k < 3; ++k)
     for (int j = 0; j < 3; ++j) {
@@ -228,16 +240,9 @@ Sl2GyroParam gyro_param(const sl2_stream_gyro &g) {
     for (int j = i; j < 3; ++j) {
       double a = R[i] * M[j];
       a = a + R[3 + i] * M[3 + j];
-      p.Rc[3 * i + j] = p.Rc[3 * j + i] = a + R[6 + i] * M[6 + j];
+      Rc[3 * i + j] = Rc[3 * j + i] = a + R[6 + i] * M[6 + j];
     }
-  for (int i = 0; i < 9; ++i) p.R[i] = R[i];
-  for (int i = 0; i < 3; ++i) p.b[i] = g.bias[i];
-  return p;
 }
-
-}  // namespace
-
-namespace sl2 {
 
 bool gyro_on(const sl2_ctx *c, int lo, int cnt) {
   for (int s = lo; s < lo + cnt; ++s)

@@ -294,11 +294,31 @@ struct WarpLaunch {
   Sl2Normals nrm;         // the streams' estimated normals ({}: every stream warps with nW0)
 };
 cudaError_t sl2_launch_warp(const Sl2Dev &d, const WarpLaunch &L, Sl2Queue q);
+// The accelerometer (include/sl2b200.h, sl2_set_stream_accel) that predict_kernel's motion prediction takes as an
+// argument.  on == nullptr when no stream of the launch has it on.  An on stream s reads its sample at index
+// s - sample_lo of force (3 doubles each) and valid, consumes it (valid = 0) and writes its result a[s], status[s].
+struct Sl2AccelParam {  // one stream's setting as the kernel reads it (sl2_set_stream_accel)
+  double R[9];   // R_ac, row-major
+  double b[3];   // bias
+  double Rc[9];  // R_ac^T C R_ac, row-major, exactly symmetric
+  double g[3];   // gravity, world frame
+  double sd2;    // sd_a sd_a
+};
+struct Sl2Accel {
+  const uint8_t *on;           // [B]
+  const Sl2AccelParam *prm;    // [B]
+  const double *force;         // [.][3]
+  uint8_t *valid;              // [.]
+  int sample_lo;
+  double *a;                   // [B][3]
+  int *status;                 // [B] 0 none, 1 applied, 2 skipped
+};
 // sel_mode_dev: [B] the streams' SL2_SELECT_* settings, or nullptr: every stream selects by trace; rv_dev: [B] the
-// streams' recovery states, or nullptr: no stream of the launch has recovery on (ekf.cu)
+// streams' recovery states, or nullptr: no stream of the launch has recovery on; acc: the accelerometers of the
+// launch's motion prediction ({}: none) (ekf.cu)
 cudaError_t sl2_launch_predict(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *u3_dev,
                                int do_predict, int do_measure, const int *sel_mode_dev, Sl2Queue q,
-                               const sl2_recovery_result *rv_dev = nullptr);
+                               const sl2_recovery_result *rv_dev = nullptr, const Sl2Accel &acc = {});
 // The mutual-information selection (select.cu) of the streams [stream_lo, stream_lo + stream_cnt) whose mode[s] is
 // SL2_SELECT_INFORMATION, right after their predict_kernel: picks into sel_rank, the job slots and nsel
 struct SelectLaunch {

@@ -135,6 +135,15 @@ struct sl2_ctx {
   Sl2GyroParam *gyro_prm = nullptr;
   double *gyro_rate = nullptr, *gyro_W = nullptr, *gyro_nis = nullptr;
   int *gyro_status = nullptr;
+  // accelerometer (sl2_set_stream_accel): the host mirror of every stream's setting, and the device buffers (allocated
+  // when a stream first turns it on): the on flags [B], the settings [B], the sample ring [slots][B] of forces and valid
+  // bytes and the results [B][3] a, [B] status
+  std::vector<sl2_stream_accel> accel;  // [B]
+  sl2::DevPtr<uint8_t> accel_buf;
+  uint8_t *accel_on_dev = nullptr, *accel_valid = nullptr;
+  Sl2AccelParam *accel_prm = nullptr;
+  double *accel_force = nullptr, *accel_a = nullptr;
+  int *accel_status = nullptr;
   // sub-pixel refinement (sl2_set_stream_subpixel): the host mirror of every stream's setting, and one device buffer
   // (allocated when a stream first turns it on): z [B][Nmax][2] doubles, refined [B][Nmax] and the on flags [B]
   std::vector<uint8_t> subpix_on;  // [B]
@@ -292,6 +301,15 @@ int rescue_streams(sl2_ctx *c, int lo, int cnt, Sl2Queue q);
 // samples of ring slot `slot`, between their motion prediction and their feature prediction
 bool gyro_on(const sl2_ctx *c, int lo, int cnt);
 int gyro_streams(sl2_ctx *c, int slot, int lo, int cnt, Sl2Queue q);
+// gyro.cu: what the gyroscope and accelerometer settings share: every entry of v[0 .. n) finite; the checks that R
+// (row-major, named rname in the message) is a rotation and C a symmetric positive definite covariance, an empty
+// string when both hold; and Rc = R^T C R in the order include/sl2b200.h states
+bool finite_all(const double *v, int n);
+std::string sensor_frame_error(const double *R, const double *C, const std::string &rname);
+void sensor_cov_in_camera(const double *R, const double *C, double Rc[9]);
+// accel.cu: the accelerometers predict_kernel of the streams [lo, lo + cnt) reads with the samples of ring slot `slot`
+// ({} when none of them has the accelerometer on)
+Sl2Accel accel_args(const sl2_ctx *c, int slot, int lo, int cnt);
 // subpixel.cu: the sub-pixel matches the kernels of the streams [lo, lo + cnt) read ({} when none of them has the
 // refinement on); the refinement of those streams on q, right after their search of ring slot `slot` (job_patches: the
 // search's templates); a load forgets the refinement of the streams [lo, lo + cnt): their z is the integer match until

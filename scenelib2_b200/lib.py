@@ -65,6 +65,13 @@ class Sl2StreamGyro(C.Structure):
     _fields_ = [("on", C.c_int32), ("reserved", C.c_int32), ("R_gc", C.c_double * 9), ("bias", C.c_double * 3),
                 ("cov", C.c_double * 9)]
 
+class Sl2StreamAccel(C.Structure):
+    """sl2_stream_accel: a camera stream's accelerometer: on, the camera-to-accelerometer rotation R_ac, the bias and
+    the covariance of one sample (row-major, accelerometer frame, m/s^2), the world-frame gravity and sd_a."""
+    _fields_ = [("on", C.c_int32), ("reserved", C.c_int32), ("R_ac", C.c_double * 9), ("bias", C.c_double * 3),
+                ("cov", C.c_double * 9), ("gravity", C.c_double * 3), ("sd_a", C.c_double)]
+
+
 class Sl2StreamIterated(C.Structure):
     """sl2_stream_iterated: a camera stream's iterated EKF update: relinearisations allowed (0 = off) and the step
     tolerance in prior standard deviations."""
@@ -98,6 +105,8 @@ EXPORTS = [
     "sl2_set_stream_subpixel", "sl2_get_stream_subpixel",
     "sl2_set_stream_selection", "sl2_get_stream_selection",
     "sl2_set_stream_gyro", "sl2_get_stream_gyro", "sl2_set_gyro_samples", "sl2_gyro_update", "sl2_get_gyro_results",
+    "sl2_set_stream_accel", "sl2_get_stream_accel", "sl2_set_accel_samples", "sl2_accel_predict",
+    "sl2_get_accel_results",
     "sl2_set_stream_iterated", "sl2_get_stream_iterated", "sl2_get_iterated_results",
     "sl2_set_stream_normals", "sl2_get_stream_normals", "sl2_get_patch_normals", "sl2_set_patch_normals",
     "sl2_align_normals",
@@ -291,6 +300,11 @@ def load():
         L.sl2_set_gyro_samples.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
         L.sl2_gyro_update.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
         L.sl2_get_gyro_results.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
+        L.sl2_set_stream_accel.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamAccel)]
+        L.sl2_get_stream_accel.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamAccel)]
+        L.sl2_set_accel_samples.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
+        L.sl2_accel_predict.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
+        L.sl2_get_accel_results.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
         L.sl2_set_stream_iterated.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamIterated)]
         L.sl2_get_stream_iterated.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamIterated)]
         L.sl2_get_iterated_results.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -527,6 +541,59 @@ class Context:
         nis, status = np.zeros(max(cnt, 0)), np.zeros(max(cnt, 0), np.int32)
         self._ck(self.L.sl2_get_gyro_results(self.h, lo, cnt, nis.ctypes.data, status.ctypes.data))
         return nis, status
+
+    # ---- accelerometer ------------------------------------------------------------------------
+    def set_stream_accel(self, stream_id, on, R_ac=None, bias=None, cov=None, gravity=None, sd_a=4.0, reserved=0):
+        """sl2_set_stream_accel: drive the stream's motion prediction with one accelerometer sample per step (on = 1),
+        or not (0, the default).  R_ac (3x3) takes camera-frame vectors into the accelerometer's frame (default I),
+        bias (3) is in m/s^2 (default 0), cov (3x3) is the covariance of one sample, the mean specific force over the
+        frame period (default I), gravity (3) is the world-frame gravity vector in m/s^2 (default 0) and sd_a (m/s^2)
+        the acceleration a sample does not explain."""
+        a = Sl2StreamAccel()
+        a.on, a.reserved, a.sd_a = int(on), int(reserved), float(sd_a)
+        for name, v, dflt in (("R_ac", R_ac, np.eye(3)), ("bias", bias, np.zeros(3)), ("cov", cov, np.eye(3)),
+                              ("gravity", gravity, np.zeros(3))):
+            t = np.asarray(dflt if v is None else v, np.float64).reshape(-1)
+            if t.size != len(getattr(a, name)):
+                raise ValueError("%s must hold %d values" % (name, len(getattr(a, name))))
+            getattr(a, name)[:] = [float(u) for u in t]
+        self._ck(self.L.sl2_set_stream_accel(self.h, stream_id, C.byref(a)))
+
+    def stream_accel(self, stream_id):
+        """-> dict(on, R_ac (3x3), bias (3), cov (3x3), gravity (3), sd_a)"""
+        a = Sl2StreamAccel()
+        self._ck(self.L.sl2_get_stream_accel(self.h, stream_id, C.byref(a)))
+        return dict(on=a.on, R_ac=np.array(a.R_ac).reshape(3, 3), bias=np.array(a.bias),
+                    cov=np.array(a.cov).reshape(3, 3), gravity=np.array(a.gravity), sd_a=a.sd_a)
+
+    def set_accel_samples(self, slot, forces, valid=None, lo=0):
+        """sl2_set_accel_samples: the samples (cnt x 3 m/s^2, accelerometer frame) of streams [lo, lo + cnt) for the
+        fused step of ring slot `slot`; valid (cnt, None = all) marks the streams that have one."""
+        forces = np.ascontiguousarray(forces, np.float64).reshape(-1, 3)
+        cnt = forces.shape[0]
+        if valid is not None:
+            valid = np.ascontiguousarray(valid, np.uint8).reshape(-1)
+            if valid.size != cnt:
+                raise ValueError("valid must hold one byte per sample")
+        self._ck(self.L.sl2_set_accel_samples(self.h, slot, lo, cnt, forces.ctypes.data,
+                                              None if valid is None else valid.ctypes.data))
+
+    def accel_predict(self, stream_id, f3):
+        """sl2_accel_predict: the staged motion prediction of one stream with one accelerometer sample, in place of
+        ekf_predict."""
+        f3 = np.ascontiguousarray(f3, np.float64).reshape(-1)
+        if f3.size != 3:
+            raise ValueError("f3 must hold 3 values")
+        self._ck(self.L.sl2_accel_predict(self.h, stream_id, f3.ctypes.data))
+
+    def accel_results(self, lo=0, cnt=None):
+        """sl2_get_accel_results -> (a (cnt, 3) world-frame m/s^2, status (cnt,): 0 none this step, 1 applied,
+        2 skipped)."""
+        if cnt is None:
+            cnt = self.cfg.num_streams - lo
+        a, status = np.zeros((max(cnt, 0), 3)), np.zeros(max(cnt, 0), np.int32)
+        self._ck(self.L.sl2_get_accel_results(self.h, lo, cnt, a.ctypes.data, status.ctypes.data))
+        return a, status
 
     # ---- iterated update -----------------------------------------------------------------------
     def set_stream_iterated(self, stream_id, max_iterations, tol=0.0, reserved=0):
