@@ -198,6 +198,72 @@ int sl2_get_stream_warp(sl2_ctx *ctx, int32_t stream_id, int32_t *on);
 int sl2_warp_templates(sl2_ctx *ctx, int32_t stream_id, int32_t n, const int32_t *feat_index, const double *xp,
                        uint8_t *out, uint8_t *valid);
 
+/* ---- exposure blur: match each template through the motion blur the predicted motion makes (no reference
+ * counterpart) ---------------------------------------------------------------------------------------------------
+ * A camera that moves while its shutter is open smears every feature along the image motion: at 3 rad/s and a 1/60 s
+ * exposure a 320 x 240 camera's features become ~10 px streaks, and a sharp template no longer matches them.  A stream
+ * with the blur on searches each selected feature with its template averaged over the poses the predicted motion
+ * (v, omega of the predicted state) passes through while the shutter is open (Jin, Favaro, Cipolla, "Visual Tracking
+ * in the Presence of Motion Blur", CVPR 2005; Klein, Murray, "Improving the Agility of Keyframe-Based SLAM", ECCV 2008).
+ * Blurred template of job feature i at the predicted state x (13: r, q, v, omega), with cam, HALF, y, xo, the plane's
+ * nW (nW(theta) with normals on) and the bilinear sampling of the warp above, and h0 = the warp's h at x[0:7] (the
+ * prediction's h, bit for bit):
+ *   pose at time s: x[0:7] itself for s = 0 (not composed); otherwise r_s = r + v s, q_s = q (x) qw with qw =
+ *   QuaternionFromAngularVelocity(omega s) (the motion model's: av = omega s, angle = sqrt(av . av), qw = (cos(angle /
+ *   2), (sin(angle / 2) / angle) av), the identity for angle = 0; (x) the Hamilton product in the motion model's
+ *   order), every component formed as in the motion model's prediction over dt = s;
+ *   reference camera: with the warp on, the camera at xo with centre ho (the warp's); with it off, the pose x[0:7]
+ *   with centre h0 (the blur alone, relative to the unwarped view);
+ *   source of output pixel d = (b - HALF, a - HALF) at time s: the ray the pose at s sees at p = h0 + d
+ *   (unproject_point(p), one for all times) cut with the plane and projected into the reference camera, src(s) =
+ *   project_point(zo) - centre + (HALF, HALF), valid by the warp's rule; with the warp off and s = 0, src(0) = (b, a)
+ *   with no round trip;
+ *   times s- = offset - exposure * 0.5, s_c = offset, s+ = offset + exposure * 0.5;
+ *   samples: L = sqrt(dx dx + dy dy) with (dx, dy) = src(s+) - src(s-) at d = (0, 0); K = min(32, max(1, ceil(L)));
+ *   K = 1: v = the bilinear value (not rounded) at src(s_c);
+ *   K > 1: D1 = src(s+) - src(s-), D2 = (src(s+) - 2 src(s_c)) + src(s-) per coordinate; for k = 0 .. K - 1,
+ *   u = ((k + 0.5) / K) - 0.5, src_k = (src(s_c) + u D1) + ((2 u) u) D2 (the quadratic through the three, samples
+ *   at most one template pixel apart up to a 32 px streak); v = (sum over ascending k from 0.0 of the bilinear value
+ *   at src_k) / K;
+ *   the byte is (int)(v + 0.5).
+ * Every operation is a correctly rounded, never-fused FP64 operation in this order (csrc/sl2_model.cuh:
+ * quat_from_angular_velocity, patch_ray_source, patch_bilinear; csrc/warp.cu: blur_job), except that sin and cos are
+ * the device's, as in the motion model.  The needed sources are the centre's src(s-) and src(s+) and every pixel's
+ * src(s_c) (K = 1) or its three (K > 1); when one of them is invalid or L is not finite, the job gets its unblurred
+ * template: the warp's when the warp is on and valid, else the stored one.  Positions outside the stored template
+ * repeat its edge pixels, as in the warp.  exposure = 0 and offset = 0 give K = 1 at s = 0: the warp's bytes, or the
+ * stored template with the warp off.
+ * Where it applies: the search of the fused step (sl2_step, sl2_step_host, sl2_step_host_async) and of
+ * sl2_make_measurements, and the sub-pixel refinement, for a stream with the blur on, at the predicted state; the
+ * search's sigma >= 10 gates and scores then apply to the blurred template (which fails them more often than a sharp
+ * one), and no other rule changes.  The normal alignment still compares the stored, sharp template with the blurred
+ * frame.  sl2_patch_search, sl2_score_map, the SMOE and particle entry points, sl2_relocalise and the recovery's
+ * full-image search keep the stored templates.
+ * on = 0 (the default) is off, 1 is on: a context where no stream has it on runs exactly the path without it; a step
+ * group holding an on stream and no warp-on stream adds one kernel launch (the warp's, timed with the search in
+ * sl2_last_step_times), and one that already warps adds none.  Ordering like sl2_set_stream_config.  The setting
+ * belongs to the stream slot, like the warp: snapshots do not carry it and a load leaves it.  The first stream turned
+ * on (warp or blur) sizes the warp's job-template scratch: SL2_ERR_CUDA, with the setting left off, when that
+ * allocation fails.  SL2_ERR_ARG, with the setting unchanged, for a bad stream_id, a NULL b, reserved != 0, an `on`
+ * other than 0 or 1, an exposure that is not finite and >= 0, or an offset that is not finite. */
+typedef struct sl2_stream_blur {
+  int32_t on;       /* 0 (default) or 1 */
+  int32_t reserved; /* 0 */
+  double exposure;  /* s, finite, >= 0: the shutter's open time */
+  double offset;    /* s, finite: the exposure's middle relative to the frame's time (the predicted state's time);
+                       -exposure / 2 for a camera that stamps the end of the exposure */
+} sl2_stream_blur;
+int sl2_set_stream_blur(sl2_ctx *ctx, int32_t stream_id, const sl2_stream_blur *b);
+int sl2_get_stream_blur(sl2_ctx *ctx, int32_t stream_id, sl2_stream_blur *b);
+/* The templates features feat_index[0 .. n) of stream_id get in the fused search at the state xv (13: r, q, v,
+ * omega), with the stream's own blur, warp and normals settings.  out: n x boxsize x boxsize u8, row-major; valid (n,
+ * may be NULL): 0 = the stored template, 1 = warped without blur, 2 = blurred; samples (n, may be NULL): K of a
+ * blurred template, 0 otherwise.  Joins both step groups and synchronises.  SL2_ERR_ARG, with nothing written, for: a
+ * bad stream_id; n outside [0, max_features]; a NULL feat_index, xv or out with n > 0; a feat_index outside [0, nfeat);
+ * a non-finite xv or a zero quaternion. */
+int sl2_blur_templates(sl2_ctx *ctx, int32_t stream_id, int32_t n, const int32_t *feat_index, const double *xv,
+                       uint8_t *out, uint8_t *valid, int32_t *samples);
+
 /* ---- patch normals: estimate the plane of each feature's patch from the images (no reference counterpart) --------
  * The warp above takes each patch as facing the camera that first saw it.  A stream with normals on estimates each
  * feature's normal by aligning its stored template with the step's frame through the homography the plane induces

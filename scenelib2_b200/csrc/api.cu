@@ -167,14 +167,23 @@ bool warp_on(const sl2_ctx *c, int lo, int cnt) {
   return false;
 }
 
-// The measure stage of the streams [lo, lo + cnt) on q: when some stream of them has the warp on, every job's template
-// at the predicted pose x[0:7] (the stored one for the others) into the job-indexed scratch; the patch search over the
-// context's own job arrays (indexed by the stream number local to the launch), the sub-pixel refinement when some
-// stream of them has it on, then the match consensus when some stream of them has it on
+// whether some stream of [lo, lo + cnt) has the exposure blur on
+bool blur_on(const sl2_ctx *c, int lo, int cnt) {
+  for (int s = lo; s < lo + cnt; ++s)
+    if (c->blur[s].on) return true;
+  return false;
+}
+
+// The measure stage of the streams [lo, lo + cnt) on q: when some stream of them has the warp or the blur on, every
+// job's template at the predicted state (warped, blurred, or the stored one, by each stream's settings) into the
+// job-indexed scratch; the patch search over the context's own job arrays (indexed by the stream number local to the
+// launch), the sub-pixel refinement when some stream of them has it on, then the match consensus when some stream of
+// them has it on
 int measure_streams(sl2_ctx *c, int32_t slot, int lo, int cnt, Sl2Queue q) {
   const Sl2Dev &d = c->d;
   const uint8_t *job_patches = nullptr;
-  if (warp_on(c, lo, cnt)) {
+  const bool blur = blur_on(c, lo, cnt);
+  if (blur || warp_on(c, lo, cnt)) {
     WarpLaunch W = {};
     W.job_feat = d.job_feat + (size_t)lo * d.Nmax;
     W.jobs_per_stream = d.Nmax;
@@ -183,6 +192,7 @@ int measure_streams(sl2_ctx *c, int32_t slot, int lo, int cnt, Sl2Queue q) {
     W.on = c->warp_on_dev;
     W.out = c->warp_patches.get() + (size_t)lo * d.Nmax * d.box * 16;
     W.nrm = normals_args(c, lo, cnt);
+    W.blur = blur ? c->blur_dev : nullptr;
     CU_TRY(c, sl2_launch_warp(d, W, q));
     job_patches = W.out;
   }
@@ -344,6 +354,8 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   c->resc_chi2.assign(B, 0.0);
   ALLOC(c->warp_on_dev, B);
   c->warp_on.assign(B, 0);
+  ALLOC(c->blur_dev, B);
+  c->blur.assign(B, sl2_stream_blur{});
   c->subpix_on.assign(B, 0);
   ALLOC(c->sel_mode_dev, B);
   ALLOC(c->sel_t_dev, B);

@@ -282,16 +282,20 @@ struct Sl2Normals {
 __device__ __forceinline__ bool normals_on(const Sl2Normals &n, int s) { return n.prm && n.prm[s].max_iterations > 0; }
 // The planar patch warp (warp.cu): the template of every job of the streams [stream_lo, stream_lo + stream_cnt) at
 // the pose xp, into out[job] in the row-padded layout of Sl2Dev::patches.  A stream whose on[s] is 0 gets its stored
-// templates copied; a stream with normals on warps through its features' estimated normals.
+// templates copied; a stream with normals on warps through its features' estimated normals.  With blur set (the
+// exposure blur, include/sl2b200.h sl2_set_stream_blur), a stream whose blur[s].on is 1 gets its templates blurred
+// over the exposure at the state xp (13 numbers: r, q, v, omega).
 struct WarpLaunch {
   const int *job_feat;    // [stream_cnt * jobs_per_stream], -1 = no job
   int jobs_per_stream;    // stride between streams in job_feat and out
   int stream_lo, stream_cnt;
-  const double *xp;       // the pose (7) of a one-stream launch, or nullptr: each stream's own x[0:7]
+  const double *xp;       // the state (7, or 13 with blur) of a one-stream launch, or nullptr: each stream's own x
   const uint8_t *on;      // [B] the streams' warp settings, or nullptr: every stream warps
   uint8_t *out;           // [jobs][box][16]
-  uint8_t *valid;         // [jobs] 1 = warped, 0 = the stored template (or no job); may be nullptr
+  uint8_t *valid;         // [jobs] 2 = blurred, 1 = warped, 0 = the stored template (or no job); may be nullptr
   Sl2Normals nrm;         // the streams' estimated normals ({}: every stream warps with nW0)
+  const sl2_stream_blur *blur;  // [B] the streams' blur settings, or nullptr: no stream of the launch blurs
+  int *samples;           // [jobs] K of a blurred template, 0 otherwise; may be nullptr
 };
 cudaError_t sl2_launch_warp(const Sl2Dev &d, const WarpLaunch &L, Sl2Queue q);
 // The accelerometer (include/sl2b200.h, sl2_set_stream_accel) that predict_kernel's motion prediction takes as an

@@ -110,6 +110,10 @@ struct sl2_ctx {
   uint8_t *warp_on_dev = nullptr;  // [B] device
   sl2::DevPtr<uint8_t> warp_patches;
   size_t warp_patches_bytes = 0;
+  // exposure blur (sl2_set_stream_blur): the host mirror of every stream's setting and the device array warp_kernel
+  // reads; it writes the warp's job-indexed templates
+  std::vector<sl2_stream_blur> blur;  // [B]
+  sl2_stream_blur *blur_dev = nullptr;  // [B] device
   // feature selection (sl2_set_stream_selection): the host mirror of every stream's setting, the device arrays
   // predict_kernel and select_kernel read, and the factor scratch [B][kmax][Nmax][4] (sized when a stream first turns
   // the information rule on, and only when the factors cannot stay in shared memory)

@@ -20,6 +20,24 @@ __device__ Quat quat_mul(const Quat &a, const Quat &b) {
   return q;
 }
 
+// QuaternionFromAngularVelocity (math_util.cpp:61-80) of the rotation vector av (omega t): the identity for |av| = 0.
+// The motion model (ekf.cu) and the exposure blur (warp.cu) both turn q by it.
+__device__ __forceinline__ Quat quat_from_angular_velocity(const rd av[3]) {
+  const rd angle = rsqrt_(av[0] * av[0] + av[1] * av[1] + av[2] * av[2]);
+  Quat q;
+  if (angle.v > 0.0) {
+    const rd sn(sin((angle / rd(2.0)).v)), cs(cos((angle / rd(2.0)).v));
+    const rd s = sn / angle;
+    q.x = s * av[0];
+    q.y = s * av[1];
+    q.z = s * av[2];
+    q.w = cs;
+  } else {
+    q.w = rd(1.0);
+  }
+  return q;
+}
+
 // Eigen::Quaterniond::inverse(): conjugate / squaredNorm, the zero quaternion when the norm is 0
 __device__ __forceinline__ Quat quat_inverse(const Quat &q) {
   const rd n2 = q.w * q.w + q.x * q.x + q.y * q.y + q.z * q.z;
@@ -182,14 +200,32 @@ __device__ __forceinline__ void patch_normal(const PatchBasis &b, rd ta, rd tb, 
   for (int i = 0; i < 3; ++i) nW[i] = zero ? b.n0[i] : (b.n0[i] + ta * b.E1[i]) + tb * b.E2[i];
 }
 
+// A camera pose that views a feature's plane (through y, normal nW): adj(RRW) of the pose (the ray's matrix: RRW is a
+// rotation only for |q| = 1, quirk Q1, so RRW^T is not its inverse), its position r and num = nW . (y - r)
+struct PatchPose {
+  rd adj[3][3], r[3], num;
+};
+// The camera a source position is taken in: its RRW, its position r and the centre c of the template cut there
+struct PatchRef {
+  rd RRW[3][3], r[3], c[2];
+};
+// num and r of the pose xp, whose RRW = pose_RRW(xp) and d = y - xp[0:3] (zeroed_point) are given
+__device__ __forceinline__ void patch_pose_terms(const double *xp, const rd RRW[3][3], const rd d[3], const rd nW[3],
+                                                 PatchPose &p) {
+  mat3_adj(RRW, p.adj);
+  for (int i = 0; i < 3; ++i) p.r[i] = rd(xp[i]);
+  p.num = dot3(nW, d);
+}
+
 // What one feature's warp at the camera pose xp shares over its pixels: the feature y seen from xp (h, bit for bit the
-// prediction's) and from xo = xp_org (ho, the template centre), adj(RRW) (the ray's matrix: RRW is a rotation only
-// for |q| = 1, quirk Q1, so RRW^T is not its inverse), the plane through y with normal nW = xo[0:3] - y (nW(theta)
-// when theta, the feature's estimated tilt, is given) and num = nW . (y - r)
+// prediction's), the pose xp itself (at), the camera at xo = xp_org with the template centre ho = y seen from xo
+// (ref), and the plane through y with normal nW = xo[0:3] - y (nW(theta) when theta, the feature's estimated tilt, is
+// given)
 struct PatchWarp {
-  rd adj[3][3], RRWo[3][3];  // adj(pose_RRW(xp)), pose_RRW(xo)
-  rd nW[3], num;
-  rd h[2], ho[2];
+  PatchPose at;
+  PatchRef ref;
+  rd nW[3];
+  rd h[2];
 };
 __device__ __forceinline__ void patch_warp_setup(const double *cam, const double *xp, const double *xo, const rd y[3],
                                                  PatchWarp &w, const double *theta = nullptr) {
@@ -197,45 +233,53 @@ __device__ __forceinline__ void patch_warp_setup(const double *cam, const double
   pose_RRW(xp, RRW);
   zeroed_point(RRW, y, xp, d, z);
   project_point(cam, z, w.h, uc, vc);
-  mat3_adj(RRW, w.adj);
   rd dox[3], zo[3];
-  pose_RRW(xo, w.RRWo);
-  zeroed_point(w.RRWo, y, xo, dox, zo);
-  project_point(cam, zo, w.ho, uc, vc);
+  pose_RRW(xo, w.ref.RRW);
+  zeroed_point(w.ref.RRW, y, xo, dox, zo);
+  project_point(cam, zo, w.ref.c, uc, vc);
+  for (int i = 0; i < 3; ++i) w.ref.r[i] = rd(xo[i]);
   if (theta && (theta[0] != 0.0 || theta[1] != 0.0)) {
     PatchBasis b;
-    patch_basis(xo, y, w.RRWo, b);
+    patch_basis(xo, y, w.ref.RRW, b);
     patch_normal(b, rd(theta[0]), rd(theta[1]), w.nW);
   } else {
     for (int i = 0; i < 3; ++i) w.nW[i] = rd(xo[i]) - y[i];
   }
-  w.num = dot3(w.nW, d);
+  patch_pose_terms(xp, RRW, d, w.nW, w.at);
 }
 
-// The source position in the stored template of the output pixel at offset (db, da) (column, row) from the centre:
-// p = h + (db, da); dW = adj(RRW) unproject_point(p) (= det(RRW) RRW^-1 unproject_point(p), det(RRW) >= 0, and X does
-// not change with the scale of dW); t = num / (nW . dW); X = r + t dW; zo = RRWo (X - xo[0:3]);
-// src = project_point(zo) - ho + (half, half).  True when the pixel is valid: t finite and > 0, zo[2] > 0, src finite.
-__device__ __forceinline__ bool patch_warp_source(const double *cam, const PatchWarp &w, const double *xp,
-                                                  const double *xo, int db, int da, int half, rd src[2]) {
-  const rd p[2] = {w.h[0] + rd((double)db), w.h[1] + rd((double)da)};
-  rd c[3], dW[3];
-  unproject_point(cam, p, c);
-  mat3_vec(w.adj, c, dW);
-  const rd t = w.num / dot3(w.nW, dW);
+// The source position, in the template cut around ref.c in the camera ref, of the ray c (unproject_point of an image
+// point) seen from the pose v: dW = adj(RRW) c (= det(RRW) RRW^-1 c, det(RRW) >= 0, and X does not change with the
+// scale of dW); t = num / (nW . dW); X = r + t dW; zo = ref.RRW (X - ref.r); src = project_point(zo) - ref.c +
+// (half, half).  True when the source is valid: t finite and > 0, zo[2] > 0, src finite.
+__device__ __forceinline__ bool patch_ray_source(const double *cam, const PatchPose &v, const PatchRef &ref,
+                                                 const rd nW[3], const rd c[3], int half, rd src[2]) {
+  rd dW[3];
+  mat3_vec(v.adj, c, dW);
+  const rd t = v.num / dot3(nW, dW);
   rd e[3], zo[3];
-  for (int i = 0; i < 3; ++i) e[i] = (rd(xp[i]) + t * dW[i]) - rd(xo[i]);
-  mat3_vec(w.RRWo, e, zo);
+  for (int i = 0; i < 3; ++i) e[i] = (v.r[i] + t * dW[i]) - ref.r[i];
+  mat3_vec(ref.RRW, e, zo);
   rd g[2], uc, vc;
   project_point(cam, zo, g, uc, vc);
-  src[0] = (g[0] - w.ho[0]) + rd((double)half);
-  src[1] = (g[1] - w.ho[1]) + rd((double)half);
+  src[0] = (g[0] - ref.c[0]) + rd((double)half);
+  src[1] = (g[1] - ref.c[1]) + rd((double)half);
   return isfinite(t.v) && t.v > 0.0 && zo[2].v > 0.0 && isfinite(src[0].v) && isfinite(src[1].v);
 }
 
-// Bilinear sample of the box x box template T (row stride ld) at the finite position src (column, row): each
-// coordinate clamped to [0, box - 1], so positions outside the template repeat its edge pixels; returns (int)(v + 0.5)
-__device__ __forceinline__ int patch_sample(const uint8_t *T, int ld, int box, const rd src[2]) {
+// The warp's source position in the stored template of the output pixel at offset (db, da) (column, row) from the
+// centre: patch_ray_source of unproject_point(h + (db, da)) from the pose xp into the camera at xo
+__device__ __forceinline__ bool patch_warp_source(const double *cam, const PatchWarp &w, int db, int da, int half,
+                                                  rd src[2]) {
+  const rd p[2] = {w.h[0] + rd((double)db), w.h[1] + rd((double)da)};
+  rd c[3];
+  unproject_point(cam, p, c);
+  return patch_ray_source(cam, w.at, w.ref, w.nW, c, half, src);
+}
+
+// Bilinear value (not rounded) of the box x box template T (row stride ld) at the finite position src (column, row):
+// each coordinate clamped to [0, box - 1], so positions outside the template repeat its edge pixels
+__device__ __forceinline__ rd patch_bilinear(const uint8_t *T, int ld, int box, const rd src[2]) {
   const double lim = (double)(box - 1);
   const double sx = fmin(fmax(src[0].v, 0.0), lim), sy = fmin(fmax(src[1].v, 0.0), lim);
   const int x0 = min((int)floor(sx), box - 2), y0 = min((int)floor(sy), box - 2);
@@ -243,8 +287,11 @@ __device__ __forceinline__ int patch_sample(const uint8_t *T, int ld, int box, c
   const uint8_t *r0 = T + y0 * ld + x0, *r1 = r0 + ld;
   const rd top = (one - fx) * rd((double)r0[0]) + fx * rd((double)r0[1]);
   const rd bot = (one - fx) * rd((double)r1[0]) + fx * rd((double)r1[1]);
-  const rd v = (one - fy) * top + fy * bot;
-  return (int)(v + rd(0.5)).v;
+  return (one - fy) * top + fy * bot;
+}
+// patch_bilinear rounded to the byte (int)(v + 0.5)
+__device__ __forceinline__ int patch_sample(const uint8_t *T, int ld, int box, const rd src[2]) {
+  return (int)(patch_bilinear(T, ld, box, src) + rd(0.5)).v;
 }
 
 // Camera::Project (camera.cpp:90-114) of the camera-frame point z, and J = dh/dz

@@ -72,6 +72,12 @@ class Sl2StreamAccel(C.Structure):
                 ("cov", C.c_double * 9), ("gravity", C.c_double * 3), ("sd_a", C.c_double)]
 
 
+class Sl2StreamBlur(C.Structure):
+    """sl2_stream_blur: a camera stream's exposure blur: on, the exposure (s) and the exposure's middle relative to
+    the frame's time (s)."""
+    _fields_ = [("on", C.c_int32), ("reserved", C.c_int32), ("exposure", C.c_double), ("offset", C.c_double)]
+
+
 class Sl2StreamIterated(C.Structure):
     """sl2_stream_iterated: a camera stream's iterated EKF update: relinearisations allowed (0 = off) and the step
     tolerance in prior standard deviations."""
@@ -102,6 +108,7 @@ EXPORTS = [
     "sl2_set_stream_config", "sl2_get_stream_config", "sl2_set_stream_consensus", "sl2_get_stream_consensus",
     "sl2_set_stream_rescue", "sl2_get_stream_rescue",
     "sl2_set_stream_warp", "sl2_get_stream_warp", "sl2_warp_templates",
+    "sl2_set_stream_blur", "sl2_get_stream_blur", "sl2_blur_templates",
     "sl2_set_stream_subpixel", "sl2_get_stream_subpixel",
     "sl2_set_stream_selection", "sl2_get_stream_selection",
     "sl2_set_stream_gyro", "sl2_get_stream_gyro", "sl2_set_gyro_samples", "sl2_gyro_update", "sl2_get_gyro_results",
@@ -291,6 +298,10 @@ def load():
         L.sl2_get_stream_rescue.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_double)]
         L.sl2_set_stream_warp.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
         L.sl2_get_stream_warp.argtypes = [C.c_void_p, C.c_int32, i32p]
+        L.sl2_set_stream_blur.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamBlur)]
+        L.sl2_get_stream_blur.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamBlur)]
+        L.sl2_blur_templates.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p]
         L.sl2_set_stream_subpixel.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
         L.sl2_get_stream_subpixel.argtypes = [C.c_void_p, C.c_int32, i32p]
         L.sl2_set_stream_selection.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Sl2StreamSelection)]
@@ -491,6 +502,38 @@ class Context:
         self._ck(self.L.sl2_warp_templates(self.h, stream_id, n, feat_index.ctypes.data, xp.ctypes.data,
                                            out.ctypes.data, valid.ctypes.data))
         return out, valid
+
+    # ---- exposure blur ------------------------------------------------------------------------
+    def set_stream_blur(self, stream_id, on, exposure=0.0, offset=0.0, reserved=0):
+        """sl2_set_stream_blur: search the stream's selected features with their templates blurred along the predicted
+        motion over the exposure (seconds; offset = the exposure's middle relative to the frame's time) (on = 1), or
+        not (0, the default)."""
+        b = Sl2StreamBlur()
+        b.on, b.reserved, b.exposure, b.offset = int(on), int(reserved), float(exposure), float(offset)
+        self._ck(self.L.sl2_set_stream_blur(self.h, stream_id, C.byref(b)))
+
+    def stream_blur(self, stream_id):
+        """-> dict(on, exposure, offset)"""
+        b = Sl2StreamBlur()
+        self._ck(self.L.sl2_get_stream_blur(self.h, stream_id, C.byref(b)))
+        return dict(on=b.on, exposure=b.exposure, offset=b.offset)
+
+    def blur_templates(self, stream_id, feat_index, xv):
+        """sl2_blur_templates: the templates the fused search of the stream uses for the features feat_index at the
+        state xv (13: r, q, v, omega), with the stream's blur, warp and normals settings -> (templates (n, B, B) u8,
+        valid (n,) u8: 0 stored, 1 warped, 2 blurred, samples (n,) i32: K of a blurred template, else 0)."""
+        feat_index = np.ascontiguousarray(feat_index, np.int32).reshape(-1)
+        xv = np.ascontiguousarray(xv, np.float64).reshape(-1)
+        if xv.size < 13:
+            raise ValueError("xv must hold 13 values (r, q, v, omega)")
+        xv = np.ascontiguousarray(xv[:13])
+        n, B = feat_index.size, self.cfg.boxsize
+        out = np.zeros((n, B, B), np.uint8)
+        valid = np.zeros(n, np.uint8)
+        samples = np.zeros(n, np.int32)
+        self._ck(self.L.sl2_blur_templates(self.h, stream_id, n, feat_index.ctypes.data, xv.ctypes.data,
+                                           out.ctypes.data, valid.ctypes.data, samples.ctypes.data))
+        return out, valid, samples
 
     # ---- gyroscope ----------------------------------------------------------------------------
     def set_stream_gyro(self, stream_id, on, R_gc=None, bias=None, cov=None, reserved=0):
