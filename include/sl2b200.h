@@ -91,6 +91,21 @@ const char *sl2_version(void);
 int sl2_set_stream_config(sl2_ctx *ctx, int32_t stream_id, const sl2_stream_config *sc);
 int sl2_get_stream_config(sl2_ctx *ctx, int32_t stream_id, sl2_stream_config *sc);
 
+/* ---- per-stream options ----------------------------------------------------------------------------------------
+ * The sections from the match consensus to the iterated update, and the stream recovery, each give a camera stream an
+ * opt-in setting: a setter, and a getter that returns the setting as the setter accepted it.  Every setter keeps this
+ * contract; each section states only what is its own.
+ *   Ordering like sl2_set_stream_config: work queued before the call uses the old setting, and the next call that runs
+ *   the feature (including the next fused step) uses the new one.  A setter launches no kernel.
+ *   The setting belongs to the stream slot, like the frame source: snapshots do not carry it and a load leaves it.
+ *   Every stream starts with the feature off, and a context where no stream has it on runs exactly the path without
+ *   it.
+ *   When the feature has a device buffer ("Buffer:" in its section, payload sizes), the first stream turned on sizes
+ *   it, each part at a 256-byte boundary, which may add padding: SL2_ERR_CUDA, with the setting left off, when that
+ *   allocation fails.  Results read as zeros until a stream first turns the feature on.
+ *   SL2_ERR_ARG, with the setting unchanged, for a bad stream_id, a NULL setting (get: a NULL output), and the values
+ *   the section lists. */
+
 /* ---- match consensus: keep wrong matches out of the EKF update (no reference counterpart) ----------------------
  * The reference trusts every match its patch search accepts.  A stream with an inlier radius tau > 0 px runs a
  * one-point RANSAC over the step's matches between the search and the update (Civera, Grasa, Davison, Montiel,
@@ -111,10 +126,7 @@ int sl2_get_stream_config(sl2_ctx *ctx, int32_t stream_id, sl2_stream_config *sc
  *   A step record's nmeas, m, nis and logdet_s describe the rows that entered the update.
  * Every operation is a correctly rounded FP64 operation in the order written in the kernel (csrc/consensus.cu,
  * consensus_kernel), so decisions are reproducible bit for bit.
- * inlier_px = 0 (the default) is off: a context where no stream has it on runs exactly the path without it.
- * Ordering like sl2_set_stream_config.  The setting belongs to the stream slot, like the frame source: snapshots do
- * not carry it and a load leaves it.  SL2_ERR_ARG, with the setting unchanged, for a bad stream_id, a negative, NaN
- * or infinite inlier_px, or (get) a NULL inlier_px. */
+ * inlier_px = 0 (the default) is off.  SL2_ERR_ARG for a negative, NaN or infinite inlier_px. */
 int sl2_set_stream_consensus(sl2_ctx *ctx, int32_t stream_id, double inlier_px);
 int sl2_get_stream_consensus(sl2_ctx *ctx, int32_t stream_id, double *inlier_px);
 
@@ -145,11 +157,8 @@ int sl2_get_stream_consensus(sl2_ctx *ctx, int32_t stream_id, double *inlier_px)
  * sl2_ekf_update with the caller's rows never rescues.  A typical chi2 is 5.991, the 95 % point of chi^2 with two
  * degrees of freedom.  chi2 = 0 (the default) is off: a context where no stream has the consensus and the rescue on
  * runs exactly the path without it; one with such a stream adds six kernel launches per step group holding one
- * (timed with the update in sl2_last_step_times; sl2_last_update_times keeps timing update 1).  Ordering like
- * sl2_set_stream_config.  The setting belongs to the stream slot, like the match consensus: snapshots do not carry it
- * and a load leaves it.  The first stream turned on sizes the context's rescue scratch (num_streams x 20 bytes):
- * SL2_ERR_CUDA, with the setting unchanged, when that allocation fails.  SL2_ERR_ARG, with the setting unchanged, for
- * a bad stream_id, a negative, NaN or infinite chi2, or (get) a NULL chi2. */
+ * (timed with the update in sl2_last_step_times; sl2_last_update_times keeps timing update 1).  Buffer: the rescue
+ * scratch, num_streams x 20 bytes.  SL2_ERR_ARG for a negative, NaN or infinite chi2. */
 int sl2_set_stream_rescue(sl2_ctx *ctx, int32_t stream_id, double chi2);
 int sl2_get_stream_rescue(sl2_ctx *ctx, int32_t stream_id, double *chi2);
 
@@ -181,13 +190,9 @@ int sl2_get_stream_rescue(sl2_ctx *ctx, int32_t stream_id, double *chi2);
  * sl2_make_measurements warps, for a stream with the warp on, each selected feature's template at the predicted pose
  * x[0:7]; the search's sigma >= 10 gates and scores then apply to that template, and no other rule changes.
  * sl2_patch_search, sl2_score_map, the SMOE and particle entry points and sl2_relocalise keep the stored templates.
- * on = 0 (the default) is off, 1 is on: a context where no stream has it on runs exactly the path without it; one with
- * a stream that has it on adds one kernel launch per step group holding such a stream (timed with the search in
- * sl2_last_step_times).  Ordering like sl2_set_stream_config.  The setting belongs to the stream slot, like the match
- * consensus and the frame source: snapshots do not carry it and a load leaves it.  The first stream turned on sizes
- * the context's warped-template scratch (num_streams x max_features x boxsize x 16 bytes): SL2_ERR_CUDA, with the
- * setting left off, when that allocation fails.  SL2_ERR_ARG, with the setting unchanged, for a bad stream_id, an
- * `on` other than 0 or 1, or (get) a NULL on. */
+ * on = 0 (the default) is off, 1 is on: a step group holding a stream that has it on adds one kernel launch (timed
+ * with the search in sl2_last_step_times).  Buffer: the warped-template scratch, num_streams x max_features x boxsize
+ * x 16 bytes.  SL2_ERR_ARG for an `on` other than 0 or 1. */
 int sl2_set_stream_warp(sl2_ctx *ctx, int32_t stream_id, int32_t on);
 int sl2_get_stream_warp(sl2_ctx *ctx, int32_t stream_id, int32_t *on);
 /* The warped templates of features feat_index[0 .. n) of stream_id at the pose xp (7: r, q), whatever the stream's
@@ -239,13 +244,11 @@ int sl2_warp_templates(sl2_ctx *ctx, int32_t stream_id, int32_t n, const int32_t
  * one), and no other rule changes.  The normal alignment still compares the stored, sharp template with the blurred
  * frame.  sl2_patch_search, sl2_score_map, the SMOE and particle entry points, sl2_relocalise and the recovery's
  * full-image search keep the stored templates.
- * on = 0 (the default) is off, 1 is on: a context where no stream has it on runs exactly the path without it; a step
- * group holding an on stream and no warp-on stream adds one kernel launch (the warp's, timed with the search in
- * sl2_last_step_times), and one that already warps adds none.  Ordering like sl2_set_stream_config.  The setting
- * belongs to the stream slot, like the warp: snapshots do not carry it and a load leaves it.  The first stream turned
- * on (warp or blur) sizes the warp's job-template scratch: SL2_ERR_CUDA, with the setting left off, when that
- * allocation fails.  SL2_ERR_ARG, with the setting unchanged, for a bad stream_id, a NULL b, reserved != 0, an `on`
- * other than 0 or 1, an exposure that is not finite and >= 0, or an offset that is not finite. */
+ * on = 0 (the default) is off, 1 is on: a step group holding an on stream and no warp-on stream adds one kernel launch
+ * (the warp's, timed with the search in sl2_last_step_times), and one that already warps adds none.  Buffer: the
+ * warp's job-template scratch, shared with the warp (sized by the first stream turned on for either).  SL2_ERR_ARG for
+ * reserved != 0, an `on` other than 0 or 1, an exposure that is not finite and >= 0, or an offset that is not
+ * finite. */
 typedef struct sl2_stream_blur {
   int32_t on;       /* 0 (default) or 1 */
   int32_t reserved; /* 0 */
@@ -312,11 +315,10 @@ int sl2_blur_templates(sl2_ctx *ctx, int32_t stream_id, int32_t n, const int32_t
  * sl2_append_feature, sl2_set_features or a snapshot load (which do not carry the estimates), and when the setter is
  * called for its stream; estimates move with their features through the cull and sl2_delete_feature, and
  * sl2_relocalise and the recovery keep them.
- * max_iterations = 0 (the default) is off; 1 .. SL2_MAX_NORMAL_ITERATIONS is on.  The setting belongs to the stream
- * slot.  The first stream turned on sizes the context's scratch (num_streams x (32 + 45 max_features) bytes):
- * SL2_ERR_CUDA, with the setting left off, when that fails.  SL2_ERR_ARG, with the setting unchanged, for a bad stream_id,
- * a NULL v, reserved != 0, max_iterations outside [0, SL2_MAX_NORMAL_ITERATIONS], a sigma0 or sigma_i that is not finite
- * and > 0, or a sigma_step that is not finite and >= 0. */
+ * max_iterations = 0 (the default) is off; 1 .. SL2_MAX_NORMAL_ITERATIONS is on.  The setter synchronises.  Buffer:
+ * num_streams x (32 + 45 max_features) bytes.  SL2_ERR_ARG for reserved != 0, max_iterations outside
+ * [0, SL2_MAX_NORMAL_ITERATIONS], a sigma0 or sigma_i that is not finite and > 0, or a sigma_step that is not finite
+ * and >= 0. */
 #define SL2_MAX_NORMAL_ITERATIONS 8
 typedef struct sl2_stream_normals {
   int32_t max_iterations; /* 0 (default, off) .. SL2_MAX_NORMAL_ITERATIONS Gauss-Newton steps per alignment */
@@ -367,13 +369,10 @@ int sl2_align_normals(sl2_ctx *ctx, int32_t stream_id, int32_t slot);
  * other flags, bit 3 describes the feature's last match; it is never set for an off stream.  R stays sd-based: lower
  * the stream's sd (sl2_set_stream_config) to make the update trust the refined matches more.  sl2_patch_search,
  * sl2_score_map, the SMOE and particle entry points and sl2_relocalise stay integer.
- * on = 0 (the default) is off, 1 is on: a context where no stream has it on runs exactly the path without it; one with
- * a stream that has it on adds one kernel launch per step group holding such a stream (timed with the search in
- * sl2_last_step_times).  Ordering like sl2_set_stream_config.  The setting belongs to the stream slot, like the warp:
- * snapshots do not carry it and a load leaves it.  A loaded stream's z is its integer match (bit 3 clear) until its
- * next step; so is a stream's after the setting is made.  The first stream turned on sizes the context's scratch
- * (num_streams x (17 max_features + 1) bytes): SL2_ERR_CUDA, with the setting left off, when that allocation fails.
- * SL2_ERR_ARG, with the setting unchanged, for a bad stream_id, an `on` other than 0 or 1, or (get) a NULL on. */
+ * on = 0 (the default) is off, 1 is on: a step group holding a stream that has it on adds one kernel launch (timed
+ * with the search in sl2_last_step_times).  A loaded stream's z is its integer match (bit 3 clear) until its next
+ * step; so is a stream's after the setting is made.  Buffer: num_streams x (17 max_features + 1) bytes.  SL2_ERR_ARG
+ * for an `on` other than 0 or 1. */
 int sl2_set_stream_subpixel(sl2_ctx *ctx, int32_t stream_id, int32_t on);
 int sl2_get_stream_subpixel(sl2_ctx *ctx, int32_t stream_id, int32_t *on);
 
@@ -408,15 +407,11 @@ int sl2_get_stream_subpixel(sl2_ctx *ctx, int32_t stream_id, int32_t *on);
  * search, the consensus (whose ties go to the lowest selection rank, now the information order), the warp, the
  * update, the cull, the records and relocalisation read the job slots as with the trace rule.  A stream can end a
  * prediction with nothing selected.
- * mode SL2_SELECT_TRACE (the default) is the reference's rule: a context where no stream selects by information runs
- * exactly the path without it; one where some stream does adds one kernel launch per step group holding such a
- * stream and per sl2_predict_measurements of one (timed with the predict in sl2_last_step_times).  Ordering like
- * sl2_set_stream_config.  The setting belongs to the stream slot, like the match consensus: snapshots do not carry it
- * and a load leaves it.  When a stream first turns the information rule on and the factors of
- * kmax = min(max_features, SL2_MAX_MEASURED) picks cannot stay in shared memory, the context sizes its factor scratch
- * (num_streams x max_features x kmax x 32 bytes): SL2_ERR_CUDA, with the setting unchanged, when that allocation
- * fails.  SL2_ERR_ARG, with the setting unchanged, for: a bad stream_id or NULL sel; an unknown mode; reserved != 0;
- * a min_bits that is negative or not finite, or non-zero with SL2_SELECT_TRACE. */
+ * mode SL2_SELECT_TRACE (the default) is the reference's rule and counts as off; a step group holding a stream that
+ * selects by information adds one kernel launch, and so does sl2_predict_measurements of one (timed with the predict
+ * in sl2_last_step_times).  Buffer: only when the factors of kmax = min(max_features, SL2_MAX_MEASURED) picks cannot
+ * stay in shared memory, the factor scratch, num_streams x max_features x kmax x 32 bytes.  SL2_ERR_ARG for an unknown
+ * mode; reserved != 0; a min_bits that is negative or not finite, or non-zero with SL2_SELECT_TRACE. */
 #define SL2_SELECT_TRACE 0       /* the reference's rule: top n_select by trace(S_i) (default) */
 #define SL2_SELECT_INFORMATION 1 /* greedy mutual information, above */
 typedef struct sl2_stream_selection {
@@ -464,17 +459,14 @@ int sl2_get_stream_selection(sl2_ctx *ctx, int32_t stream_id, sl2_stream_selecti
  * byte, so a sample is used by exactly one step; a step without a valid sample does no gyro update.  The staged form
  * is sl2_gyro_update, between sl2_ekf_predict and sl2_predict_measurements.  The step records are unchanged: nis and
  * logdet_s stay the visual update's, xv and pxx_diag show the state after both updates.
- * on = 0 (the default; the getter then shows R_gc = I, b = 0, C = I) is off: a context where no stream has it on runs
- * exactly the path without it; a step group holding a gyro-on stream splits its prediction in two launches and adds
- * the update's two (three more launches, timed with the predict in sl2_last_step_times).  Ordering like
- * sl2_set_stream_config.  The setting belongs to the stream slot, like the match consensus: snapshots do not carry it
- * and a load leaves it.  A call that turns an off stream on clears that stream's samples in every slot; a call that
- * turns a stream on or off clears its last result (status 0, NIS 0).  The first stream turned on allocates the
- * context's gyro buffers (a sample ring of frame_slots x num_streams, the W scratch of num_streams x (13 + 3 max_features, rounded up to 8) x 3 doubles and the per-stream
- * results): SL2_ERR_CUDA, with the setting left off, when that allocation fails.  SL2_ERR_ARG, with the setting
- * unchanged, for: a bad stream_id or NULL g; reserved != 0 or on outside {0, 1}; a non-finite entry; an R_gc that is
- * not a rotation (|R R^T - I| > 1e-9 in some entry, or det R <= 0); a cov that is not exactly symmetric, or whose
- * Cholesky factor (step 2's formulas) has a pivot argument that is not > 0. */
+ * on = 0 (the default; the getter then shows R_gc = I, b = 0, C = I) is off; a step group holding a gyro-on stream
+ * splits its prediction in two launches and adds the update's two (three more launches, timed with the predict in
+ * sl2_last_step_times).  A call that turns an off stream on clears that stream's samples in every slot; a call that
+ * turns a stream on or off clears its last result (status 0, NIS 0).  Buffer: a sample ring of frame_slots x
+ * num_streams, the W scratch of num_streams x (13 + 3 max_features, rounded up to 8) x 3 doubles and the per-stream
+ * settings and results.  SL2_ERR_ARG for: reserved != 0 or on outside {0, 1}; a non-finite entry; an R_gc that is not
+ * a rotation (|R R^T - I| > 1e-9 in some entry, or det R <= 0); a cov that is not exactly symmetric, or whose Cholesky
+ * factor (step 2's formulas) has a pivot argument that is not > 0. */
 typedef struct sl2_stream_gyro {
   int32_t on;       /* 0 (default) or 1 */
   int32_t reserved; /* 0 */
@@ -539,14 +531,11 @@ int sl2_get_gyro_results(sl2_ctx *ctx, int32_t lo, int32_t cnt, double *nis, int
  * staged form is sl2_accel_predict, in place of sl2_ekf_predict; sl2_ekf_predict(u3) stays the reference's.  With the
  * gyroscope also on, the accelerometer's prediction is the one the gyro update follows.  No launch is added: the work
  * is in the prediction kernel.  The step records are unchanged.
- * on = 0 (the default; the getter then shows R_ac = I, b = 0, C = I, g = 0, sd_a = 4) is off.  Ordering like
- * sl2_set_stream_config.  The setting belongs to the stream slot: snapshots do not carry it and a load leaves it.  A
- * call that turns an off stream on clears that stream's samples in every slot; a call that turns a stream on or off
- * clears its last result (status 0, a = 0).  The first stream turned on allocates the context's accelerometer buffers
- * (a sample ring of frame_slots x num_streams and the per-stream settings and results): SL2_ERR_CUDA, with the
- * setting left off, when that allocation fails.  SL2_ERR_ARG, with the setting unchanged, for: a bad stream_id or NULL
- * a; reserved != 0 or on outside {0, 1}; a non-finite entry; an R_ac that is not a rotation or a cov that is not
- * symmetric positive definite (the checks of sl2_set_stream_gyro); a negative sd_a. */
+ * on = 0 (the default; the getter then shows R_ac = I, b = 0, C = I, g = 0, sd_a = 4) is off.  A call that turns an
+ * off stream on clears that stream's samples in every slot; a call that turns a stream on or off clears its last
+ * result (status 0, a = 0).  Buffer: a sample ring of frame_slots x num_streams and the per-stream settings and
+ * results.  SL2_ERR_ARG for: reserved != 0 or on outside {0, 1}; a non-finite entry; an R_ac that is not a rotation or
+ * a cov that is not symmetric positive definite (the checks of sl2_set_stream_gyro); a negative sd_a. */
 typedef struct sl2_stream_accel {
   int32_t on;         /* 0 (default) or 1 */
   int32_t reserved;   /* 0 */
@@ -613,14 +602,11 @@ int sl2_get_accel_results(sl2_ctx *ctx, int32_t lo, int32_t cnt, double *accel, 
  * the final update; sl2_last_update_times times the final update, sl2_last_step_times()[2] includes the passes.
  * Cost: a step group holding a stream with the iteration on runs N_g = the largest max_iterations of its streams
  * passes of three launches (upd_hp, upd_chol, iterate_kernel) before its update; a stream that has stopped costs an
- * early return per launch.  A context where no stream has it on runs exactly the path without it.
- * tol is in standard deviations of the prior: 0 always runs N relinearisations.  The setting belongs to the stream
- * slot, like the match consensus: snapshots do not carry it and a load leaves it.  A call clears the stream's results.
- * The first stream turned on allocates the context's iteration buffer (num_streams x max_features x 22 doubles of
- * tables, num_streams x (13 + 3 max_features, rounded up to 8) doubles of iterate and the settings and results):
- * SL2_ERR_CUDA, with the setting unchanged, when that fails.  SL2_ERR_ARG, with the setting unchanged, for a bad
- * stream_id or NULL v, reserved != 0, max_iterations outside [0, SL2_MAX_ITERATIONS], or a tol that is not finite and
- * >= 0. */
+ * early return per launch.
+ * tol is in standard deviations of the prior: 0 always runs N relinearisations.  A call clears the stream's results.
+ * Buffer: num_streams x max_features x 22 doubles of tables, num_streams x (13 + 3 max_features, rounded up to 8)
+ * doubles of iterate and the settings and results.  SL2_ERR_ARG for reserved != 0, max_iterations outside
+ * [0, SL2_MAX_ITERATIONS], or a tol that is not finite and >= 0. */
 #define SL2_MAX_ITERATIONS 8
 typedef struct sl2_stream_iterated {
   int32_t max_iterations; /* 0 (default, off) .. SL2_MAX_ITERATIONS relinearisations */
@@ -1080,15 +1066,15 @@ int sl2_relocalise(sl2_ctx *ctx, const int32_t *stream_ids, int32_t cnt, int32_t
  * of the stream return it to tracking (lost = failed_steps = lost_steps = 0); the setter also clears attempted,
  * recoveries and last.  Turning the setting off (lost_after = 0) therefore also resumes selection.
  * Where it applies: sl2_step, sl2_step_host and sl2_step_host_async (whose xv_out shows the state after the whole step,
- * an accepted try included).  The staged entry points and the C++ shim never run it.  The setting and the recovery
- * state belong to the stream slot, like the match consensus: snapshots do not carry them (the format is unchanged).
+ * an accepted try included).  The staged entry points and the C++ shim never run it.  The recovery state belongs to the
+ * stream slot like the setting (one of the per-stream options, above): snapshots do not carry it (the format is
+ * unchanged).
  * Cost: a step group holding a stream with recovery on launches three more kernels per step, after the step's timing
  * events (recover_kernel, the full-image search over the streams that try, reloc_kernel); a stream that does not try
- * costs an early return in each.  A context where no stream has it on runs exactly the path without it.
- * The first stream turned on allocates the context's recovery buffers (the settings and states, a job table and search
- * results of num_streams x max_features entries): SL2_ERR_CUDA, with the setting unchanged, when that fails.
- * SL2_ERR_ARG, with the setting unchanged, for: a bad stream_id or NULL r; reserved != 0; lost_after < 0; with
- * lost_after > 0, min_matches < 1 or retry_period < 1, or a reloc or Pxx that sl2_relocalise refuses. */
+ * costs an early return in each.
+ * Buffer: the settings and states, a job table and search results of num_streams x max_features entries.  SL2_ERR_ARG
+ * for: reserved != 0; lost_after < 0; with lost_after > 0, min_matches < 1 or retry_period < 1, or a reloc or Pxx that
+ * sl2_relocalise refuses. */
 typedef struct sl2_stream_recovery {
   int32_t lost_after;     /* 0 (default) = off; K >= 1: K consecutive failed steps declare the stream lost */
   int32_t min_matches;    /* >= 1: a step fails when its nmeas is < min_matches */

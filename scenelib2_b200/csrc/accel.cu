@@ -11,36 +11,6 @@ using namespace sl2;
 
 namespace {
 
-// the offsets of the accelerometer buffers in one allocation, each 256-byte aligned; returns the total
-size_t accel_layout(const Sl2Dev &d, size_t off[6]) {
-  const size_t B = d.B, slots = d.slots;
-  const size_t bytes[6] = {B, B * sizeof(Sl2AccelParam), slots * B * 3 * sizeof(double), slots * B,
-                           B * 3 * sizeof(double), B * sizeof(int)};
-  size_t o = 0;
-  for (int i = 0; i < 6; ++i) {
-    off[i] = o;
-    o += (bytes[i] + 255) & ~(size_t)255;
-  }
-  return o;
-}
-
-int accel_alloc(sl2_ctx *c) {
-  size_t off[6];
-  const size_t bytes = accel_layout(c->d, off);
-  DevPtr<uint8_t> h;
-  CU_TRY(c, cuda_malloc(h, bytes));
-  CU_TRY(c, cudaMemsetAsync(h.get(), 0, bytes, c->stream));
-  uint8_t *b = h.get();
-  c->accel_on_dev = b + off[0];
-  c->accel_prm = reinterpret_cast<Sl2AccelParam *>(b + off[1]);
-  c->accel_force = reinterpret_cast<double *>(b + off[2]);
-  c->accel_valid = b + off[3];
-  c->accel_a = reinterpret_cast<double *>(b + off[4]);
-  c->accel_status = reinterpret_cast<int *>(b + off[5]);
-  c->accel_buf = std::move(h);
-  return SL2_OK;
-}
-
 // the setting's checks of include/sl2b200.h; an empty string when it is accepted
 std::string accel_setting_error(const sl2_stream_accel *a) {
   if (a->reserved != 0 || (a->on != 0 && a->on != 1)) return "reserved must be 0 and on 0 or 1";
@@ -75,15 +45,12 @@ Sl2Accel accel_table(const sl2_ctx *c) {
 namespace sl2 {
 
 Sl2Accel accel_args(const sl2_ctx *c, int slot, int lo, int cnt) {
-  for (int s = lo; s < lo + cnt; ++s)
-    if (c->accel[s].on) {
-      Sl2Accel A = accel_table(c);
-      A.force = c->accel_force + (size_t)slot * c->d.B * 3;
-      A.valid = c->accel_valid + (size_t)slot * c->d.B;
-      A.sample_lo = 0;
-      return A;
-    }
-  return {};
+  if (!any_stream(c, lo, cnt, [](const StreamOptions &o) { return o.accel.on != 0; })) return {};
+  Sl2Accel A = accel_table(c);
+  A.force = c->accel_force + (size_t)slot * c->d.B * 3;
+  A.valid = c->accel_valid + (size_t)slot * c->d.B;
+  A.sample_lo = 0;
+  return A;
 }
 
 }  // namespace sl2
@@ -94,29 +61,35 @@ int sl2_set_stream_accel(sl2_ctx *c, int32_t s, const sl2_stream_accel *a) {
   if (bad_stream(c, s) || !a) return fail(c, SL2_ERR_ARG, "sl2_set_stream_accel: bad argument");
   const std::string why = accel_setting_error(a);
   if (!why.empty()) return fail(c, SL2_ERR_ARG, "sl2_set_stream_accel: " + why);
+  const Sl2Dev &d = c->d;
   if (a->on && !c->accel_buf) {
-    const int rc = accel_alloc(c);
+    const size_t B = d.B, slots = d.slots;
+    const int rc = alloc_sections(c, c->accel_buf,
+                                  {{&c->accel_on_dev, B}, {&c->accel_prm, B * sizeof(Sl2AccelParam)},
+                                   {&c->accel_force, slots * B * 3 * sizeof(double)}, {&c->accel_valid, slots * B},
+                                   {&c->accel_a, B * 3 * sizeof(double)}, {&c->accel_status, B * sizeof(int)}});
     if (rc) return rc;
   }
+  const sl2_stream_accel &old = c->opt[s].accel;
   if (c->accel_buf) {  // pageable copies have read their sources when they return; ordered on the stream, no launch
     const Sl2AccelParam p = accel_param(*a);
     const uint8_t on = (uint8_t)a->on;
     CU_TRY(c, cudaMemcpyAsync(c->accel_prm + s, &p, sizeof p, cudaMemcpyHostToDevice, c->stream));
-    if (a->on && !c->accel[s].on)  // turned on: no stale sample
-      CU_TRY(c, cudaMemset2DAsync(c->accel_valid + s, c->d.B, 0, 1, c->d.slots, c->stream));
-    if (a->on != c->accel[s].on) {  // turned on or off: no stale result
+    if (a->on && !old.on)  // turned on: no stale sample
+      CU_TRY(c, cudaMemset2DAsync(c->accel_valid + s, d.B, 0, 1, d.slots, c->stream));
+    if (a->on != old.on) {  // turned on or off: no stale result
       CU_TRY(c, cudaMemsetAsync(c->accel_a + 3 * (size_t)s, 0, 3 * sizeof(double), c->stream));
       CU_TRY(c, cudaMemsetAsync(c->accel_status + s, 0, sizeof(int), c->stream));
     }
     CU_TRY(c, cudaMemcpyAsync(c->accel_on_dev + s, &on, 1, cudaMemcpyHostToDevice, c->stream));
   }
-  c->accel[s] = *a;
+  c->opt[s].accel = *a;
   return SL2_OK;
 }
 
 int sl2_get_stream_accel(sl2_ctx *c, int32_t s, sl2_stream_accel *a) {
   if (bad_stream(c, s) || !a) return fail(c, SL2_ERR_ARG, "sl2_get_stream_accel: bad argument");
-  *a = c->accel[s];
+  *a = c->opt[s].accel;
   return SL2_OK;
 }
 
@@ -141,7 +114,7 @@ int sl2_set_accel_samples(sl2_ctx *c, int32_t slot, int32_t lo, int32_t cnt, con
 
 int sl2_accel_predict(sl2_ctx *c, int32_t s, const double *f3) {
   if (bad_stream(c, s) || !f3 || !finite_all(f3, 3)) return fail(c, SL2_ERR_ARG, "sl2_accel_predict: bad argument");
-  if (!c->accel[s].on) return fail(c, SL2_ERR_STATE, "sl2_accel_predict: the stream's accelerometer is off");
+  if (!c->opt[s].accel.on) return fail(c, SL2_ERR_STATE, "sl2_accel_predict: the stream's accelerometer is off");
   Stage f{STAGE_IN, 24, f3}, v{STAGE_IN, 1};
   return staged_call(c, {&f, &v}, [&] { v.h[0] = 1; }, [&] {
     Sl2Accel A = accel_table(c);
@@ -155,18 +128,8 @@ int sl2_accel_predict(sl2_ctx *c, int32_t s, const double *f3) {
 
 int sl2_get_accel_results(sl2_ctx *c, int32_t lo, int32_t cnt, double *accel, int32_t *status) {
   if (bad_range(c, lo, cnt)) return fail(c, SL2_ERR_ARG, "sl2_get_accel_results: bad range");
-  if (!c->accel_buf) {  // never on: no sample has been applied
-    if (accel) std::fill(accel, accel + 3 * (size_t)cnt, 0.0);
-    if (status) std::fill(status, status + cnt, 0);
-    return SL2_OK;
-  }
-  if (accel && cnt)
-    CU_TRY(c, cudaMemcpyAsync(accel, c->accel_a + 3 * (size_t)lo, sizeof(double) * 3 * cnt, cudaMemcpyDeviceToHost,
-                              c->stream));
-  if (status && cnt)
-    CU_TRY(c, cudaMemcpyAsync(status, c->accel_status + lo, sizeof(int) * cnt, cudaMemcpyDeviceToHost, c->stream));
-  CU_TRY(c, cudaStreamSynchronize(c->stream));
-  return SL2_OK;
+  return read_results(c, c->accel_buf != nullptr, lo, cnt,
+                      {{accel, c->accel_a, 3 * sizeof(double)}, {status, c->accel_status, sizeof(int)}});
 }
 
 }  // extern "C"

@@ -61,6 +61,50 @@ bool bad_range(sl2_ctx *c, int lo, int cnt) {
   return !c || lo < 0 || cnt < 0 || lo > c->cfg.num_streams - cnt;
 }
 
+StreamOptions stream_option_defaults() {
+  StreamOptions o = {};  // every feature off, SL2_SELECT_TRACE
+  for (int i = 0; i < 3; ++i) {  // a rotation and a covariance the gyro and accel setters accept
+    o.gyro.R_gc[4 * i] = o.gyro.cov[4 * i] = 1.0;
+    o.accel.R_ac[4 * i] = o.accel.cov[4 * i] = 1.0;
+  }
+  o.accel.sd_a = 4.0;  // the motion model's
+  return o;
+}
+
+int alloc_sections(sl2_ctx *c, DevPtr<uint8_t> &buf, std::initializer_list<Section> secs) {
+  size_t bytes = 0;
+  for (const Section &x : secs) bytes += (x.bytes + 255) & ~(size_t)255;
+  DevPtr<uint8_t> h;
+  CU_TRY(c, cuda_malloc(h, bytes));
+  CU_TRY(c, cudaMemsetAsync(h.get(), 0, bytes, c->stream));
+  uint8_t *at = h.get();
+  for (const Section &x : secs) {
+    x.place(x.ptr, at);
+    at += (x.bytes + 255) & ~(size_t)255;
+  }
+  buf = std::move(h);
+  return SL2_OK;
+}
+
+int read_results(sl2_ctx *c, bool allocated, int lo, int cnt, std::initializer_list<ResultCopy> outs) {
+  for (const ResultCopy &r : outs) {
+    if (!r.dst) continue;
+    if (!allocated) memset(r.dst, 0, r.per_stream * cnt);
+    else if (cnt)
+      CU_TRY(c, cudaMemcpyAsync(r.dst, static_cast<const uint8_t *>(r.src) + r.per_stream * lo, r.per_stream * cnt,
+                                cudaMemcpyDeviceToHost, c->stream));
+  }
+  if (allocated) CU_TRY(c, cudaStreamSynchronize(c->stream));
+  return SL2_OK;
+}
+
+int streams_restarted(sl2_ctx *c, int lo, int cnt) {
+  int rc = subpixel_forget(c, lo, cnt);
+  if (!rc) rc = recovery_reset(c, lo, cnt);
+  for (int s = lo; s < lo + cnt && !rc; ++s) rc = normals_reset(c, s, 0, c->d.Nmax);
+  return rc;
+}
+
 int stage_reserve(sl2_ctx *c, size_t bytes) {
   return grow_scratch(c, (bytes + 4095) & ~(size_t)4095, c->stg_bytes, c->stg_dev, &c->stg_host);
 }
@@ -153,27 +197,6 @@ int make_tensor_map(sl2_ctx *c) {
 // the row travels as a kernel parameter, so the write is ordered on the stream like any other launch
 __global__ void write_cam_row_kernel(Sl2StreamCam *dst, const Sl2StreamCam row) { *dst = row; }
 
-// whether some stream of [lo, lo + cnt) has the match consensus on
-bool consensus_on(const sl2_ctx *c, int lo, int cnt) {
-  for (int s = lo; s < lo + cnt; ++s)
-    if (c->cons_tau[s] > 0.0) return true;
-  return false;
-}
-
-// whether some stream of [lo, lo + cnt) has the planar patch warp on
-bool warp_on(const sl2_ctx *c, int lo, int cnt) {
-  for (int s = lo; s < lo + cnt; ++s)
-    if (c->warp_on[s]) return true;
-  return false;
-}
-
-// whether some stream of [lo, lo + cnt) has the exposure blur on
-bool blur_on(const sl2_ctx *c, int lo, int cnt) {
-  for (int s = lo; s < lo + cnt; ++s)
-    if (c->blur[s].on) return true;
-  return false;
-}
-
 // The measure stage of the streams [lo, lo + cnt) on q: when some stream of them has the warp or the blur on, every
 // job's template at the predicted state (warped, blurred, or the stored one, by each stream's settings) into the
 // job-indexed scratch; the patch search over the context's own job arrays (indexed by the stream number local to the
@@ -182,8 +205,8 @@ bool blur_on(const sl2_ctx *c, int lo, int cnt) {
 int measure_streams(sl2_ctx *c, int32_t slot, int lo, int cnt, Sl2Queue q) {
   const Sl2Dev &d = c->d;
   const uint8_t *job_patches = nullptr;
-  const bool blur = blur_on(c, lo, cnt);
-  if (blur || warp_on(c, lo, cnt)) {
+  const bool blur = any_stream(c, lo, cnt, [](const StreamOptions &o) { return o.blur.on != 0; });
+  if (blur || any_stream(c, lo, cnt, [](const StreamOptions &o) { return o.warp != 0; })) {
     WarpLaunch W = {};
     W.job_feat = d.job_feat + (size_t)lo * d.Nmax;
     W.jobs_per_stream = d.Nmax;
@@ -212,7 +235,8 @@ int measure_streams(sl2_ctx *c, int32_t slot, int lo, int cnt, Sl2Queue q) {
     const int rc = subpixel_streams(c, slot, lo, cnt, job_patches, q);
     if (rc) return rc;
   }
-  if (consensus_on(c, lo, cnt)) CU_TRY(c, sl2_launch_consensus(d, lo, cnt, c->cons_tau2, sp, q));
+  if (any_stream(c, lo, cnt, [](const StreamOptions &o) { return o.inlier_px > 0.0; }))
+    CU_TRY(c, sl2_launch_consensus(d, lo, cnt, c->cons_tau2, sp, q));
   return SL2_OK;
 }
 
@@ -348,30 +372,15 @@ int sl2_create(const sl2_config *cfg, sl2_ctx **out) {
   ALLOC(d.upd_m, B);
   ALLOC(d.Wp, B * SL2_MAX_PANELS * 256);
   ALLOC(c->xv_stage, (size_t)d.slots * B * SL2_NXV);
+  c->opt.assign(B, stream_option_defaults());
   ALLOC(c->cons_tau2, B);
-  c->cons_tau.assign(B, 0.0);
   ALLOC(c->resc_chi2_dev, B);
-  c->resc_chi2.assign(B, 0.0);
   ALLOC(c->warp_on_dev, B);
-  c->warp_on.assign(B, 0);
   ALLOC(c->blur_dev, B);
-  c->blur.assign(B, sl2_stream_blur{});
-  c->subpix_on.assign(B, 0);
   ALLOC(c->sel_mode_dev, B);
   ALLOC(c->sel_t_dev, B);
-  c->sel.assign(B, sl2_stream_selection{});
   c->sel_mode.assign(B, SL2_SELECT_TRACE);
   c->sel_t.assign(B, 1.0);
-  sl2_stream_gyro g0 = {};  // off; a rotation and a covariance the setter accepts
-  for (int i = 0; i < 3; ++i) g0.R_gc[4 * i] = g0.cov[4 * i] = 1.0;
-  c->gyro.assign(B, g0);
-  sl2_stream_accel a0 = {};  // off; a rotation, a covariance and an sd_a the setter accepts
-  for (int i = 0; i < 3; ++i) a0.R_ac[4 * i] = a0.cov[4 * i] = 1.0;
-  a0.sd_a = 4.0;
-  c->accel.assign(B, a0);
-  c->iter.assign(B, sl2_stream_iterated{});
-  c->recov.assign(B, sl2_stream_recovery{});
-  c->nrm.assign(B, sl2_stream_normals{});
 #undef ALLOC
   int rc = make_tensor_map(c);
   if (rc) return failed(rc, c->err);
@@ -458,11 +467,7 @@ int sl2_set_features(sl2_ctx *c, int32_t s, int32_t n, const double *y, const do
   CU_TRY(c, cudaMemsetAsync(d.sel_rank + fb, 0xff, sizeof(int) * d.Nmax, c->stream));
   CU_TRY(c, cudaMemsetAsync(d.found + fb, 0, d.Nmax, c->stream));
   CU_TRY(c, cudaMemsetAsync(d.job_feat + fb, 0xff, sizeof(int) * d.Nmax, c->stream));
-  int rc = subpixel_forget(c, s, 1);  // a new map has no refined matches
-  if (rc) return rc;
-  rc = recovery_reset(c, s, 1);  // a new map: the stream is tracking
-  if (rc) return rc;
-  rc = normals_reset(c, s, 0, d.Nmax);  // and its normals are unestimated
+  const int rc = streams_restarted(c, s, 1);
   if (rc) return rc;
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   return SL2_OK;
@@ -537,10 +542,11 @@ static int step_group(sl2_ctx *c, int32_t slot, int lo, int cnt, Sl2Queue q, cud
   const Sl2Dev &d = c->d;
   const cudaStream_t st = q.stream;
   if (t) CU_TRY(c, cudaEventRecord(c->ev[0].get(), st));
-  const bool info = selection_on(c, lo, cnt);
+  const bool info = any_stream(c, lo, cnt, [](const StreamOptions &o) { return o.sel.mode == SL2_SELECT_INFORMATION; });
   const sl2_recovery_result *rv = recovery_args(c, lo, cnt);  // a lost stream selects nothing
   const Sl2Accel acc = accel_args(c, slot, lo, cnt);  // inside the motion prediction
-  if (gyro_on(c, lo, cnt)) {  // the motion prediction, the gyro update, then the feature prediction
+  // the motion prediction, the gyro update, then the feature prediction
+  if (any_stream(c, lo, cnt, [](const StreamOptions &o) { return o.gyro.on != 0; })) {
     CU_TRY(c, sl2_launch_predict(d, lo, cnt, nullptr, 1, 0, nullptr, q, nullptr, acc));
     const int rc = gyro_streams(c, slot, lo, cnt, q);
     if (rc) return rc;
@@ -567,7 +573,7 @@ static int step_group(sl2_ctx *c, int32_t slot, int lo, int cnt, Sl2Queue q, cud
   CU_TRY(c, sl2_launch_update(d, lo, cnt, -1, nullptr, nullptr, nullptr, nullptr, nullptr, 0, sp, q, t ? evu : nullptr,
                               iterate_args(c, lo, cnt)));
   // the rescue and its second update are part of the update's time (ev[2] .. ev[3]); the update times are the first's
-  const bool rescue = rescue_on(c, lo, cnt);
+  const bool rescue = any_stream(c, lo, cnt, [](const StreamOptions &o) { return o.chi2 > 0.0 && o.inlier_px > 0.0; });
   if (rescue) {
     const int rc2 = rescue_streams(c, lo, cnt, q);
     if (rc2) return rc2;

@@ -136,8 +136,6 @@ __global__ void __launch_bounds__(32 * CONS_WARPS) consensus_kernel(const Sl2Dev
     if (!((mask[win][j >> 5] >> (j & 31)) & 1u)) d.found[fb + mf[j]] = 2;
 }
 
-__global__ void write_double_kernel(double *dst, const double v) { *dst = v; }
-
 }  // namespace
 
 cudaError_t sl2_launch_consensus(const Sl2Dev &d, int stream_lo, int stream_cnt, const double *tau2_dev,
@@ -154,14 +152,15 @@ int sl2_set_stream_consensus(sl2_ctx *c, int32_t s, double inlier_px) {
   if (!std::isfinite(inlier_px) || inlier_px < 0.0)
     return fail(c, SL2_ERR_ARG, "sl2_set_stream_consensus: the inlier radius must be finite and >= 0");
   const double tau = inlier_px == 0.0 ? 0.0 : inlier_px;  // -0 is off like +0
-  CU_TRY(c, sl2_launch_kernel(write_double_kernel, dim3(1), dim3(1), 0, queue(c), false, c->cons_tau2 + s, tau * tau));
-  c->cons_tau[s] = tau;
+  const double tau2 = tau * tau;  // a pageable copy has read tau2 when it returns; ordered on the stream, no launch
+  CU_TRY(c, cudaMemcpyAsync(c->cons_tau2 + s, &tau2, sizeof tau2, cudaMemcpyHostToDevice, c->stream));
+  c->opt[s].inlier_px = tau;
   return SL2_OK;
 }
 
 int sl2_get_stream_consensus(sl2_ctx *c, int32_t s, double *inlier_px) {
   if (bad_stream(c, s) || !inlier_px) return fail(c, SL2_ERR_ARG, "sl2_get_stream_consensus: bad argument");
-  *inlier_px = c->cons_tau[s];
+  *inlier_px = c->opt[s].inlier_px;
   return SL2_OK;
 }
 

@@ -659,7 +659,7 @@ int sl2_ekf_predict(sl2_ctx *c, int32_t s, const double *u3) {
 
 int sl2_predict_measurements(sl2_ctx *c, int32_t s) {
   if (bad_stream(c, s)) return fail(c, SL2_ERR_ARG, "bad stream");
-  const bool info = c->sel[s].mode == SL2_SELECT_INFORMATION;
+  const bool info = c->opt[s].sel.mode == SL2_SELECT_INFORMATION;
   CU_TRY(c, sl2_launch_predict(c->d, s, 1, nullptr, 0, 1, info ? c->sel_mode_dev : nullptr, queue(c)));
   if (info) {
     const int rc = select_streams(c, s, 1, queue(c));

@@ -153,37 +153,6 @@ GyroLaunch gyro_args(const sl2_ctx *c, int lo, int cnt) {
   return G;
 }
 
-// the offsets of the gyro buffers in one allocation, each 256-byte aligned; returns the total
-size_t gyro_layout(const Sl2Dev &d, size_t off[7]) {
-  const size_t B = d.B, slots = d.slots;
-  const size_t bytes[7] = {B, B * sizeof(Sl2GyroParam), slots * B * 3 * sizeof(double), slots * B,
-                           B * 3 * (size_t)d.ld * sizeof(double), B * sizeof(double), B * sizeof(int)};
-  size_t o = 0;
-  for (int i = 0; i < 7; ++i) {
-    off[i] = o;
-    o += (bytes[i] + 255) & ~(size_t)255;
-  }
-  return o;
-}
-
-int gyro_alloc(sl2_ctx *c) {
-  size_t off[7];
-  const size_t bytes = gyro_layout(c->d, off);
-  DevPtr<uint8_t> h;
-  CU_TRY(c, cuda_malloc(h, bytes));
-  CU_TRY(c, cudaMemsetAsync(h.get(), 0, bytes, c->stream));
-  uint8_t *b = h.get();
-  c->gyro_on_dev = b + off[0];
-  c->gyro_prm = reinterpret_cast<Sl2GyroParam *>(b + off[1]);
-  c->gyro_rate = reinterpret_cast<double *>(b + off[2]);
-  c->gyro_valid = b + off[3];
-  c->gyro_W = reinterpret_cast<double *>(b + off[4]);
-  c->gyro_nis = reinterpret_cast<double *>(b + off[5]);
-  c->gyro_status = reinterpret_cast<int *>(b + off[6]);
-  c->gyro_buf = std::move(h);
-  return SL2_OK;
-}
-
 // the setting's checks of include/sl2b200.h; an empty string when it is accepted
 std::string gyro_setting_error(const sl2_stream_gyro *g) {
   if (g->reserved != 0 || (g->on != 0 && g->on != 1)) return "reserved must be 0 and on 0 or 1";
@@ -244,12 +213,6 @@ void sensor_cov_in_camera(const double *R, const double *C, double Rc[9]) {
     }
 }
 
-bool gyro_on(const sl2_ctx *c, int lo, int cnt) {
-  for (int s = lo; s < lo + cnt; ++s)
-    if (c->gyro[s].on) return true;
-  return false;
-}
-
 int gyro_streams(sl2_ctx *c, int slot, int lo, int cnt, Sl2Queue q) {
   GyroLaunch G = gyro_args(c, lo, cnt);
   G.rate = c->gyro_rate + (size_t)slot * c->d.B * 3;
@@ -267,29 +230,36 @@ int sl2_set_stream_gyro(sl2_ctx *c, int32_t s, const sl2_stream_gyro *g) {
   if (bad_stream(c, s) || !g) return fail(c, SL2_ERR_ARG, "sl2_set_stream_gyro: bad argument");
   const std::string why = gyro_setting_error(g);
   if (!why.empty()) return fail(c, SL2_ERR_ARG, "sl2_set_stream_gyro: " + why);
+  const Sl2Dev &d = c->d;
   if (g->on && !c->gyro_buf) {
-    const int rc = gyro_alloc(c);
+    const size_t B = d.B, slots = d.slots;
+    const int rc = alloc_sections(c, c->gyro_buf,
+                                  {{&c->gyro_on_dev, B}, {&c->gyro_prm, B * sizeof(Sl2GyroParam)},
+                                   {&c->gyro_rate, slots * B * 3 * sizeof(double)}, {&c->gyro_valid, slots * B},
+                                   {&c->gyro_W, B * 3 * (size_t)d.ld * sizeof(double)},
+                                   {&c->gyro_nis, B * sizeof(double)}, {&c->gyro_status, B * sizeof(int)}});
     if (rc) return rc;
   }
+  const sl2_stream_gyro &old = c->opt[s].gyro;
   if (c->gyro_buf) {  // pageable copies have read their sources when they return; ordered on the stream, no launch
     const Sl2GyroParam p = gyro_param(*g);
     const uint8_t on = (uint8_t)g->on;
     CU_TRY(c, cudaMemcpyAsync(c->gyro_prm + s, &p, sizeof p, cudaMemcpyHostToDevice, c->stream));
-    if (g->on && !c->gyro[s].on)  // turned on: no stale sample
-      CU_TRY(c, cudaMemset2DAsync(c->gyro_valid + s, c->d.B, 0, 1, c->d.slots, c->stream));
-    if (g->on != c->gyro[s].on) {  // turned on or off: no stale result
+    if (g->on && !old.on)  // turned on: no stale sample
+      CU_TRY(c, cudaMemset2DAsync(c->gyro_valid + s, d.B, 0, 1, d.slots, c->stream));
+    if (g->on != old.on) {  // turned on or off: no stale result
       CU_TRY(c, cudaMemsetAsync(c->gyro_nis + s, 0, sizeof(double), c->stream));
       CU_TRY(c, cudaMemsetAsync(c->gyro_status + s, 0, sizeof(int), c->stream));
     }
     CU_TRY(c, cudaMemcpyAsync(c->gyro_on_dev + s, &on, 1, cudaMemcpyHostToDevice, c->stream));
   }
-  c->gyro[s] = *g;
+  c->opt[s].gyro = *g;
   return SL2_OK;
 }
 
 int sl2_get_stream_gyro(sl2_ctx *c, int32_t s, sl2_stream_gyro *g) {
   if (bad_stream(c, s) || !g) return fail(c, SL2_ERR_ARG, "sl2_get_stream_gyro: bad argument");
-  *g = c->gyro[s];
+  *g = c->opt[s].gyro;
   return SL2_OK;
 }
 
@@ -315,7 +285,7 @@ int sl2_set_gyro_samples(sl2_ctx *c, int32_t slot, int32_t lo, int32_t cnt, cons
 int sl2_gyro_update(sl2_ctx *c, int32_t s, const double *rate3) {
   if (bad_stream(c, s) || !rate3 || !finite_all(rate3, 3))
     return fail(c, SL2_ERR_ARG, "sl2_gyro_update: bad argument");
-  if (!c->gyro[s].on) return fail(c, SL2_ERR_STATE, "sl2_gyro_update: the stream's gyroscope is off");
+  if (!c->opt[s].gyro.on) return fail(c, SL2_ERR_STATE, "sl2_gyro_update: the stream's gyroscope is off");
   Stage r{STAGE_IN, 24, rate3}, v{STAGE_IN, 1};
   return staged_call(c, {&r, &v}, [&] { v.h[0] = 1; }, [&] {
     GyroLaunch G = gyro_args(c, s, 1);
@@ -329,17 +299,8 @@ int sl2_gyro_update(sl2_ctx *c, int32_t s, const double *rate3) {
 
 int sl2_get_gyro_results(sl2_ctx *c, int32_t lo, int32_t cnt, double *nis, int32_t *status) {
   if (bad_range(c, lo, cnt)) return fail(c, SL2_ERR_ARG, "sl2_get_gyro_results: bad range");
-  if (!c->gyro_buf) {  // never on: no update has run
-    if (nis) std::fill(nis, nis + cnt, 0.0);
-    if (status) std::fill(status, status + cnt, 0);
-    return SL2_OK;
-  }
-  if (nis && cnt)
-    CU_TRY(c, cudaMemcpyAsync(nis, c->gyro_nis + lo, sizeof(double) * cnt, cudaMemcpyDeviceToHost, c->stream));
-  if (status && cnt)
-    CU_TRY(c, cudaMemcpyAsync(status, c->gyro_status + lo, sizeof(int) * cnt, cudaMemcpyDeviceToHost, c->stream));
-  CU_TRY(c, cudaStreamSynchronize(c->stream));
-  return SL2_OK;
+  return read_results(c, c->gyro_buf != nullptr, lo, cnt,
+                      {{nis, c->gyro_nis, sizeof(double)}, {status, c->gyro_status, sizeof(int)}});
 }
 
 }  // extern "C"

@@ -190,49 +190,10 @@ __global__ void __launch_bounds__(IT_THREADS) iterate_kernel(const Sl2Dev d, int
   }
 }
 
-// the offsets of the iteration buffers in one allocation, each 256-byte aligned; returns the total
-size_t iter_layout(const Sl2Dev &d, size_t off[10]) {
-  const size_t B = d.B, F = (size_t)d.B * d.Nmax;
-  const size_t bytes[10] = {B * sizeof(int),      B * sizeof(double),     F * 2 * sizeof(double),
-                            F * 14 * sizeof(double), F * 6 * sizeof(double), B * (size_t)d.ld * sizeof(double),
-                            B * sizeof(int),      B * sizeof(int),        B * sizeof(int),
-                            B * sizeof(double)};
-  size_t o = 0;
-  for (int i = 0; i < 10; ++i) {
-    off[i] = o;
-    o += (bytes[i] + 255) & ~(size_t)255;
-  }
-  return o;
-}
-
-int iter_alloc(sl2_ctx *c) {
-  size_t off[10];
-  const size_t bytes = iter_layout(c->d, off);
-  DevPtr<uint8_t> h;
-  CU_TRY(c, cuda_malloc(h, bytes));
-  CU_TRY(c, cudaMemsetAsync(h.get(), 0, bytes, c->stream));
-  uint8_t *b = h.get();
-  Sl2Iter t = {};
-  t.max_it = reinterpret_cast<int *>(b + off[0]);
-  t.tol = reinterpret_cast<double *>(b + off[1]);
-  t.h = reinterpret_cast<double *>(b + off[2]);
-  t.Hxp = reinterpret_cast<double *>(b + off[3]);
-  t.Hy = reinterpret_cast<double *>(b + off[4]);
-  t.x = reinterpret_cast<double *>(b + off[5]);
-  t.active = reinterpret_cast<int *>(b + off[6]);
-  t.iters = reinterpret_cast<int *>(b + off[7]);
-  t.status = reinterpret_cast<int *>(b + off[8]);
-  t.delta = reinterpret_cast<double *>(b + off[9]);
-  t.pass = -1;
-  c->iter_dev = t;
-  c->iter_buf = std::move(h);
-  return SL2_OK;
-}
-
 // the most iteration passes any stream of [lo, lo + cnt) runs
 int iter_passes(const sl2_ctx *c, int lo, int cnt) {
   int N = 0;
-  for (int s = lo; s < lo + cnt; ++s) N = std::max(N, (int)c->iter[s].max_iterations);
+  for (int s = lo; s < lo + cnt; ++s) N = std::max(N, (int)c->opt[s].iter.max_iterations);
   return N;
 }
 
@@ -279,8 +240,16 @@ int sl2_set_stream_iterated(sl2_ctx *c, int32_t s, const sl2_stream_iterated *v)
   sl2_stream_iterated w = *v;
   if (w.tol == 0.0) w.tol = 0.0;  // -0 like +0
   if (w.max_iterations > 0 && !c->iter_buf) {
-    const int rc = iter_alloc(c);
+    const size_t B = c->d.B, F = (size_t)c->d.B * c->d.Nmax;
+    Sl2Iter &t = c->iter_dev;  // pass -1: the final update
+    const int rc = alloc_sections(c, c->iter_buf,
+                                  {{&t.max_it, B * sizeof(int)}, {&t.tol, B * sizeof(double)},
+                                   {&t.h, F * 2 * sizeof(double)}, {&t.Hxp, F * 14 * sizeof(double)},
+                                   {&t.Hy, F * 6 * sizeof(double)}, {&t.x, B * (size_t)c->d.ld * sizeof(double)},
+                                   {&t.active, B * sizeof(int)}, {&t.iters, B * sizeof(int)},
+                                   {&t.status, B * sizeof(int)}, {&t.delta, B * sizeof(double)}});
     if (rc) return rc;
+    t.pass = -1;
   }
   if (c->iter_buf) {  // pageable copies have read their sources when they return; ordered on the stream, no launch
     const int nmax = w.max_iterations;
@@ -291,35 +260,23 @@ int sl2_set_stream_iterated(sl2_ctx *c, int32_t s, const sl2_stream_iterated *v)
     CU_TRY(c, cudaMemsetAsync(c->iter_dev.status + s, 0, sizeof(int), c->stream));
     CU_TRY(c, cudaMemsetAsync(c->iter_dev.delta + s, 0, sizeof(double), c->stream));
   }
-  c->iter[s] = w;
+  c->opt[s].iter = w;
   return SL2_OK;
 }
 
 int sl2_get_stream_iterated(sl2_ctx *c, int32_t s, sl2_stream_iterated *v) {
   if (bad_stream(c, s) || !v) return fail(c, SL2_ERR_ARG, "sl2_get_stream_iterated: bad argument");
-  *v = c->iter[s];
+  *v = c->opt[s].iter;
   return SL2_OK;
 }
 
 int sl2_get_iterated_results(sl2_ctx *c, int32_t lo, int32_t cnt, int32_t *iterations, int32_t *status,
                              double *last_delta) {
   if (bad_range(c, lo, cnt)) return fail(c, SL2_ERR_ARG, "sl2_get_iterated_results: bad range");
-  if (!c->iter_buf) {  // never on: no iteration has run
-    if (iterations) std::fill(iterations, iterations + cnt, 0);
-    if (status) std::fill(status, status + cnt, 0);
-    if (last_delta) std::fill(last_delta, last_delta + cnt, 0.0);
-    return SL2_OK;
-  }
-  if (iterations && cnt)
-    CU_TRY(c, cudaMemcpyAsync(iterations, c->iter_dev.iters + lo, sizeof(int) * cnt, cudaMemcpyDeviceToHost,
-                              c->stream));
-  if (status && cnt)
-    CU_TRY(c, cudaMemcpyAsync(status, c->iter_dev.status + lo, sizeof(int) * cnt, cudaMemcpyDeviceToHost, c->stream));
-  if (last_delta && cnt)
-    CU_TRY(c, cudaMemcpyAsync(last_delta, c->iter_dev.delta + lo, sizeof(double) * cnt, cudaMemcpyDeviceToHost,
-                              c->stream));
-  CU_TRY(c, cudaStreamSynchronize(c->stream));
-  return SL2_OK;
+  const Sl2Iter &t = c->iter_dev;
+  return read_results(c, c->iter_buf != nullptr, lo, cnt,
+                      {{iterations, t.iters, sizeof(int)}, {status, t.status, sizeof(int)},
+                       {last_delta, t.delta, sizeof(double)}});
 }
 
 }  // extern "C"

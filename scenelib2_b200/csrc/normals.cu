@@ -292,21 +292,6 @@ __global__ void normals_io_kernel(const Sl2Dev d, const Sl2Normals N, int s, int
   status[j] = N.status[f];
 }
 
-// the context's buffer: the settings [B], theta [B][Nmax][2], cov [B][Nmax][3], count [B][Nmax], status [B][Nmax]
-size_t normals_bytes(const Sl2Dev &d) {
-  return (size_t)d.B * (sizeof(sl2_stream_normals) + (size_t)d.Nmax * (5 * sizeof(double) + sizeof(int) + 1));
-}
-Sl2Normals normals_all(uint8_t *base, const Sl2Dev &d) {
-  const size_t BN = (size_t)d.B * d.Nmax;
-  Sl2Normals n;
-  n.prm = reinterpret_cast<sl2_stream_normals *>(base);
-  n.theta = reinterpret_cast<double *>(base + d.B * sizeof(sl2_stream_normals));
-  n.cov = n.theta + BN * 2;
-  n.count = reinterpret_cast<int *>(n.cov + BN * 3);
-  n.status = reinterpret_cast<uint8_t *>(n.count + BN);
-  return n;
-}
-
 bool normals_params_ok(const sl2_stream_normals *v) {
   return v && v->reserved == 0 && v->max_iterations >= 0 && v->max_iterations <= SL2_MAX_NORMAL_ITERATIONS &&
          std::isfinite(v->sigma0) && v->sigma0 > 0.0 && std::isfinite(v->sigma_i) && v->sigma_i > 0.0 &&
@@ -329,17 +314,16 @@ cudaError_t sl2_launch_normals(const Sl2Dev &d, int stream_lo, int stream_cnt, i
 namespace sl2 {
 
 Sl2Normals normals_args(const sl2_ctx *c, int lo, int cnt) {
-  if (!c->nrm_buf) return {};
-  for (int s = lo; s < lo + cnt; ++s)
-    if (c->nrm[s].max_iterations > 0) return c->nrm_dev;
-  return {};
+  const auto on = [](const StreamOptions &o) { return o.nrm.max_iterations > 0; };
+  return c->nrm_buf && any_stream(c, lo, cnt, on) ? c->nrm_dev : Sl2Normals{};
 }
 
 int normals_reset(sl2_ctx *c, int s, int f0, int n) {
-  if (!c->nrm_buf || c->nrm[s].max_iterations == 0 || n <= 0) return SL2_OK;
+  const sl2_stream_normals &v = c->opt[s].nrm;
+  if (!c->nrm_buf || v.max_iterations == 0 || n <= 0) return SL2_OK;
   const Sl2Normals &N = c->nrm_dev;
   const size_t f = (size_t)s * c->d.Nmax + f0;
-  const double v0 = c->nrm[s].sigma0 * c->nrm[s].sigma0;
+  const double v0 = v.sigma0 * v.sigma0;
   std::vector<double> cov((size_t)n * 3);  // pageable: the copy has read it when cudaMemcpyAsync returns
   for (int j = 0; j < n; ++j) {
     cov[j * 3] = v0;
@@ -360,16 +344,16 @@ extern "C" {
 int sl2_set_stream_normals(sl2_ctx *c, int32_t s, const sl2_stream_normals *v) {
   if (bad_stream(c, s) || !normals_params_ok(v)) return fail(c, SL2_ERR_ARG, "sl2_set_stream_normals: bad argument");
   if (v->max_iterations > 0 && !c->nrm_buf) {
-    DevPtr<uint8_t> h;
-    const size_t bytes = normals_bytes(c->d);
-    CU_TRY(c, cuda_malloc(h, bytes));
-    CU_TRY(c, cudaMemsetAsync(h.get(), 0, bytes, c->stream));
-    c->nrm_dev = normals_all(h.get(), c->d);
-    c->nrm_buf = std::move(h);
+    const size_t B = c->d.B, BN = (size_t)c->d.B * c->d.Nmax;
+    Sl2Normals &N = c->nrm_dev;
+    const int rc = alloc_sections(c, c->nrm_buf,
+                                  {{&N.prm, B * sizeof(sl2_stream_normals)}, {&N.theta, BN * 2 * sizeof(double)},
+                                   {&N.cov, BN * 3 * sizeof(double)}, {&N.count, BN * sizeof(int)}, {&N.status, BN}});
+    if (rc) return rc;
   }
-  c->nrm[s] = *v;
+  c->opt[s].nrm = *v;
   if (c->nrm_buf) {
-    CU_TRY(c, cudaMemcpyAsync(const_cast<sl2_stream_normals *>(c->nrm_dev.prm) + s, &c->nrm[s],
+    CU_TRY(c, cudaMemcpyAsync(const_cast<sl2_stream_normals *>(c->nrm_dev.prm) + s, &c->opt[s].nrm,
                               sizeof(sl2_stream_normals), cudaMemcpyHostToDevice, c->stream));
     const int rc = normals_reset(c, s, 0, c->d.Nmax);
     if (rc) return rc;
@@ -380,7 +364,7 @@ int sl2_set_stream_normals(sl2_ctx *c, int32_t s, const sl2_stream_normals *v) {
 
 int sl2_get_stream_normals(sl2_ctx *c, int32_t s, sl2_stream_normals *v) {
   if (bad_stream(c, s) || !v) return fail(c, SL2_ERR_ARG, "sl2_get_stream_normals: bad argument");
-  *v = c->nrm[s];
+  *v = c->opt[s].nrm;
   return SL2_OK;
 }
 
@@ -388,7 +372,8 @@ int sl2_get_patch_normals(sl2_ctx *c, int32_t s, int32_t n, const int32_t *feat_
                           double *normal_w, int32_t *count, uint8_t *status) {
   if (bad_stream(c, s) || n < 0 || n > c->cfg.max_features || (n > 0 && !feat_index))
     return fail(c, SL2_ERR_ARG, "sl2_get_patch_normals: bad argument");
-  if (c->nrm[s].max_iterations == 0) return fail(c, SL2_ERR_STATE, "sl2_get_patch_normals: the stream has normals off");
+  if (c->opt[s].nrm.max_iterations == 0)
+    return fail(c, SL2_ERR_STATE, "sl2_get_patch_normals: the stream has normals off");
   int rc = check_feature_indices(c, s, feat_index, n, "sl2_get_patch_normals: feature index out of range");
   if (rc || n == 0) return rc;
   const size_t N = n;
@@ -413,7 +398,8 @@ int sl2_set_patch_normals(sl2_ctx *c, int32_t s, int32_t n, const int32_t *feat_
                           const double *cov) {
   if (bad_stream(c, s) || n < 0 || n > c->cfg.max_features || (n > 0 && (!feat_index || !theta || !cov)))
     return fail(c, SL2_ERR_ARG, "sl2_set_patch_normals: bad argument");
-  if (c->nrm[s].max_iterations == 0) return fail(c, SL2_ERR_STATE, "sl2_set_patch_normals: the stream has normals off");
+  if (c->opt[s].nrm.max_iterations == 0)
+    return fail(c, SL2_ERR_STATE, "sl2_set_patch_normals: the stream has normals off");
   for (int j = 0; j < n; ++j) {
     const double a = cov[j * 3], b = cov[j * 3 + 1], e = cov[j * 3 + 2];
     if (!std::isfinite(theta[j * 2]) || !std::isfinite(theta[j * 2 + 1]) || !std::isfinite(a) || !std::isfinite(b) ||
@@ -434,7 +420,7 @@ int sl2_set_patch_normals(sl2_ctx *c, int32_t s, int32_t n, const int32_t *feat_
 
 int sl2_align_normals(sl2_ctx *c, int32_t s, int32_t slot) {
   if (bad_stream(c, s) || bad_slot(c, slot)) return fail(c, SL2_ERR_ARG, "sl2_align_normals: bad stream/slot");
-  if (c->nrm[s].max_iterations == 0) return fail(c, SL2_ERR_STATE, "sl2_align_normals: the stream has normals off");
+  if (c->opt[s].nrm.max_iterations == 0) return fail(c, SL2_ERR_STATE, "sl2_align_normals: the stream has normals off");
   CU_TRY(c, sl2_launch_normals(c->d, s, 1, slot, subpixel_args(c, s, 1), normals_args(c, s, 1), queue(c)));
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   return SL2_OK;

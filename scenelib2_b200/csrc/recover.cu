@@ -78,40 +78,6 @@ __global__ void __launch_bounds__(RECOVER_THREADS) recover_kernel(const Sl2Dev d
   }
 }
 
-// the offsets of the recovery buffers in one allocation, each 256-byte aligned; returns the total
-size_t recovery_layout(const Sl2Dev &d, size_t off[9]) {
-  const size_t B = d.B, BN = (size_t)d.B * d.Nmax;
-  const size_t bytes[9] = {B * sizeof(sl2_stream_recovery), B * sizeof(sl2_recovery_result), BN * sizeof(int),
-                           BN * 2 * sizeof(double), BN * 3 * sizeof(double), BN * 2 * sizeof(int), BN,
-                           BN * 2 * sizeof(int), BN};
-  size_t o = 0;
-  for (int i = 0; i < 9; ++i) {
-    off[i] = o;
-    o += (bytes[i] + 255) & ~(size_t)255;
-  }
-  return o;
-}
-
-int recovery_alloc(sl2_ctx *c) {
-  size_t off[9];
-  const size_t bytes = recovery_layout(c->d, off);
-  DevPtr<uint8_t> h;
-  CU_TRY(c, cuda_malloc(h, bytes));
-  CU_TRY(c, cudaMemsetAsync(h.get(), 0, bytes, c->stream));
-  uint8_t *b = h.get();
-  c->recov_set = reinterpret_cast<sl2_stream_recovery *>(b + off[0]);
-  c->recov_state = reinterpret_cast<sl2_recovery_result *>(b + off[1]);
-  c->recov_job_feat = reinterpret_cast<int *>(b + off[2]);
-  c->recov_job_centre = reinterpret_cast<double *>(b + off[3]);
-  c->recov_job_puinv = reinterpret_cast<double *>(b + off[4]);
-  c->recov_uv = reinterpret_cast<int *>(b + off[5]);
-  c->recov_found = b + off[6];
-  c->recov_zuv = reinterpret_cast<int *>(b + off[7]);
-  c->recov_flags = b + off[8];
-  c->recov_buf = std::move(h);
-  return SL2_OK;
-}
-
 // the setting's checks of include/sl2b200.h; an empty string when it is accepted
 std::string recovery_setting_error(const sl2_stream_recovery *r) {
   if (r->reserved != 0) return "reserved must be 0";
@@ -126,9 +92,8 @@ std::string recovery_setting_error(const sl2_stream_recovery *r) {
 namespace sl2 {
 
 const sl2_recovery_result *recovery_args(const sl2_ctx *c, int lo, int cnt) {
-  for (int s = lo; s < lo + cnt; ++s)
-    if (c->recov[s].lost_after > 0) return c->recov_state;
-  return nullptr;
+  return any_stream(c, lo, cnt, [](const StreamOptions &o) { return o.recov.lost_after > 0; }) ? c->recov_state
+                                                                                                 : nullptr;
 }
 
 int recover_streams(sl2_ctx *c, int slot, int lo, int cnt, Sl2Queue q) {
@@ -177,34 +142,32 @@ int sl2_set_stream_recovery(sl2_ctx *c, int32_t s, const sl2_stream_recovery *r)
   const std::string why = recovery_setting_error(r);
   if (!why.empty()) return fail(c, SL2_ERR_ARG, "sl2_set_stream_recovery: " + why);
   if (r->lost_after > 0 && !c->recov_buf) {
-    const int rc = recovery_alloc(c);
+    const size_t B = c->d.B, BN = (size_t)c->d.B * c->d.Nmax;
+    const int rc = alloc_sections(
+        c, c->recov_buf,
+        {{&c->recov_set, B * sizeof(sl2_stream_recovery)}, {&c->recov_state, B * sizeof(sl2_recovery_result)},
+         {&c->recov_job_feat, BN * sizeof(int)}, {&c->recov_job_centre, BN * 2 * sizeof(double)},
+         {&c->recov_job_puinv, BN * 3 * sizeof(double)}, {&c->recov_uv, BN * 2 * sizeof(int)}, {&c->recov_found, BN},
+         {&c->recov_zuv, BN * 2 * sizeof(int)}, {&c->recov_flags, BN}});
     if (rc) return rc;
   }
   if (c->recov_buf) {  // pageable copies have read their sources when they return; ordered on the stream, no launch
     CU_TRY(c, cudaMemcpyAsync(c->recov_set + s, r, sizeof *r, cudaMemcpyHostToDevice, c->stream));
     CU_TRY(c, cudaMemsetAsync(c->recov_state + s, 0, sizeof(sl2_recovery_result), c->stream));  // tracking, no result
   }
-  c->recov[s] = *r;
+  c->opt[s].recov = *r;
   return SL2_OK;
 }
 
 int sl2_get_stream_recovery(sl2_ctx *c, int32_t s, sl2_stream_recovery *r) {
   if (bad_stream(c, s) || !r) return fail(c, SL2_ERR_ARG, "sl2_get_stream_recovery: bad argument");
-  *r = c->recov[s];
+  *r = c->opt[s].recov;
   return SL2_OK;
 }
 
 int sl2_get_recovery_results(sl2_ctx *c, int32_t lo, int32_t cnt, sl2_recovery_result *out) {
   if (bad_range(c, lo, cnt) || (cnt > 0 && !out)) return fail(c, SL2_ERR_ARG, "sl2_get_recovery_results: bad argument");
-  if (cnt == 0) return SL2_OK;
-  if (!c->recov_buf) {  // never on
-    memset(out, 0, sizeof(sl2_recovery_result) * cnt);
-    return SL2_OK;
-  }
-  CU_TRY(c, cudaMemcpyAsync(out, c->recov_state + lo, sizeof(sl2_recovery_result) * cnt, cudaMemcpyDeviceToHost,
-                            c->stream));
-  CU_TRY(c, cudaStreamSynchronize(c->stream));
-  return SL2_OK;
+  return read_results(c, c->recov_buf != nullptr, lo, cnt, {{out, c->recov_state, sizeof(sl2_recovery_result)}});
 }
 
 }  // extern "C"

@@ -111,21 +111,10 @@ cudaError_t sl2_launch_rescue(const Sl2Dev &d, int stream_lo, int stream_cnt, co
 
 namespace sl2 {
 
-bool rescue_on(const sl2_ctx *c, int lo, int cnt) {
-  for (int s = lo; s < lo + cnt; ++s)
-    if (c->resc_chi2[s] > 0.0 && c->cons_tau[s] > 0.0) return true;
-  return false;
-}
-
 Sl2Rescue rescue_args(const sl2_ctx *c) {
-  const size_t B = c->d.B;
-  uint8_t *base = c->resc_scratch.get();
-  Sl2Rescue r;
+  Sl2Rescue r = c->resc_dev;
   r.chi2 = c->resc_chi2_dev;
   r.tau2 = c->cons_tau2;
-  r.nis1 = reinterpret_cast<double *>(base);
-  r.logdet1 = r.nis1 + B;
-  r.m2 = reinterpret_cast<int *>(r.logdet1 + B);
   return r;
 }
 
@@ -143,22 +132,22 @@ int sl2_set_stream_rescue(sl2_ctx *c, int32_t s, double chi2) {
   if (!std::isfinite(chi2) || chi2 < 0.0)
     return fail(c, SL2_ERR_ARG, "sl2_set_stream_rescue: chi2 must be finite and >= 0");
   const double v = chi2 == 0.0 ? 0.0 : chi2;  // -0 is off like +0
-  if (v > 0.0 && !c->resc_scratch) {  // [B] nis1, [B] logdet1, [B] m2
-    const size_t bytes = (size_t)c->d.B * (2 * sizeof(double) + sizeof(int));
-    DevPtr<uint8_t> h;
-    CU_TRY(c, cuda_malloc(h, bytes));
-    CU_TRY(c, cudaMemsetAsync(h.get(), 0, bytes, c->stream));
-    c->resc_scratch = std::move(h);
+  if (v > 0.0 && !c->resc_buf) {
+    const size_t B = c->d.B;
+    Sl2Rescue &r = c->resc_dev;
+    const int rc = alloc_sections(
+        c, c->resc_buf, {{&r.nis1, B * sizeof(double)}, {&r.logdet1, B * sizeof(double)}, {&r.m2, B * sizeof(int)}});
+    if (rc) return rc;
   }
   // a pageable copy has read v when it returns; ordered on the stream like a launch, and no launch of its own
   CU_TRY(c, cudaMemcpyAsync(c->resc_chi2_dev + s, &v, sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  c->resc_chi2[s] = v;
+  c->opt[s].chi2 = v;
   return SL2_OK;
 }
 
 int sl2_get_stream_rescue(sl2_ctx *c, int32_t s, double *chi2) {
   if (bad_stream(c, s) || !chi2) return fail(c, SL2_ERR_ARG, "sl2_get_stream_rescue: bad argument");
-  *chi2 = c->resc_chi2[s];
+  *chi2 = c->opt[s].chi2;
   return SL2_OK;
 }
 

@@ -224,17 +224,11 @@ cudaError_t sl2_launch_select(const Sl2Dev &d, const SelectLaunch &L, Sl2Queue q
 
 namespace sl2 {
 
-bool selection_on(const sl2_ctx *c, int lo, int cnt) {
-  for (int s = lo; s < lo + cnt; ++s)
-    if (c->sel[s].mode == SL2_SELECT_INFORMATION) return true;
-  return false;
-}
-
 int select_streams(sl2_ctx *c, int lo, int cnt, Sl2Queue q) {
   const Sl2Dev &d = c->d;
   int npick = 1;  // the most picks a stream of the launch can make
   for (int s = lo; s < lo + cnt; ++s)
-    if (c->sel[s].mode == SL2_SELECT_INFORMATION)
+    if (c->opt[s].sel.mode == SL2_SELECT_INFORMATION)
       npick = std::max(npick, std::min(d.kmax, (int)c->cams[s].number_of_features_to_select));
   SelectLaunch L = {};
   L.stream_lo = lo;
@@ -279,13 +273,13 @@ int sl2_set_stream_selection(sl2_ctx *c, int32_t s, const sl2_stream_selection *
   sl2_stream_selection v = {};
   v.mode = mode;
   v.min_bits = bits == 0.0 ? 0.0 : bits;  // -0 like +0
-  c->sel[s] = v;
+  c->opt[s].sel = v;
   return SL2_OK;
 }
 
 int sl2_get_stream_selection(sl2_ctx *c, int32_t s, sl2_stream_selection *sel) {
   if (bad_stream(c, s) || !sel) return fail(c, SL2_ERR_ARG, "sl2_get_stream_selection: bad argument");
-  *sel = c->sel[s];
+  *sel = c->opt[s].sel;
   return SL2_OK;
 }
 

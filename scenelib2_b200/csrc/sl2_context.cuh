@@ -53,6 +53,23 @@ cudaError_t cuda_stream_create(Stream &h);
 // cmp_b), its camera states have been copied to the host (out)
 struct SlotEvents { Event h2d, cmp, cmp_b, out; };
 
+// One camera stream's opt-in settings as their setters accepted them (include/sl2b200.h, the per-stream options); the
+// getters read them back and the fused step decides from them which stages a step group runs.  Every stream starts
+// with stream_option_defaults().
+struct StreamOptions {
+  double inlier_px;                // sl2_set_stream_consensus, 0 = off
+  double chi2;                     // sl2_set_stream_rescue, 0 = off
+  uint8_t warp, subpixel;          // sl2_set_stream_warp, sl2_set_stream_subpixel
+  sl2_stream_blur blur;
+  sl2_stream_selection sel;
+  sl2_stream_gyro gyro;
+  sl2_stream_accel accel;
+  sl2_stream_iterated iter;
+  sl2_stream_recovery recov;
+  sl2_stream_normals nrm;
+};
+StreamOptions stream_option_defaults();
+
 }  // namespace sl2
 
 struct sl2_ctx {
@@ -99,78 +116,58 @@ struct sl2_ctx {
   sl2::DevPtr<uint8_t> src_stage;    // [slots][src_slot_bytes] + 16 bytes of slack for the kernel's aligned loads
   size_t src_stage_bytes = 0, src_slot_bytes = 0;
   sl2::Event ev_src;                 // recorded on `stream` behind the last table write
-  // match consensus (sl2_set_stream_consensus): the host mirror of every stream's inlier radius (0 = off) and the
-  // device array of the squared radii the consensus kernel reads
-  std::vector<double> cons_tau;  // [B]
-  double *cons_tau2 = nullptr;   // [B] device
-  // planar patch warp (sl2_set_stream_warp): the host mirror of every stream's setting, the device array warp_kernel
-  // reads, and the job-indexed templates [B][Nmax][box][16] the search then reads (sized when a stream first turns it
-  // on)
-  std::vector<uint8_t> warp_on;  // [B]
-  uint8_t *warp_on_dev = nullptr;  // [B] device
+  // the per-stream options: every stream's settings, then what the features' kernels read.  The [B] device arrays are
+  // allocated with the context; each DevPtr<uint8_t> buffer is allocated by alloc_sections when a stream first turns
+  // its feature on, and the pointers after it point into it.
+  std::vector<sl2::StreamOptions> opt;  // [B]
+  double *cons_tau2 = nullptr;          // [B] consensus: squared inlier radii
+  uint8_t *warp_on_dev = nullptr;       // [B]
+  sl2_stream_blur *blur_dev = nullptr;  // [B]
+  // the job-indexed templates [B][Nmax][box][16] the warp and the blur write and the search reads
   sl2::DevPtr<uint8_t> warp_patches;
   size_t warp_patches_bytes = 0;
-  // exposure blur (sl2_set_stream_blur): the host mirror of every stream's setting and the device array warp_kernel
-  // reads; it writes the warp's job-indexed templates
-  std::vector<sl2_stream_blur> blur;  // [B]
-  sl2_stream_blur *blur_dev = nullptr;  // [B] device
-  // feature selection (sl2_set_stream_selection): the host mirror of every stream's setting, the device arrays
-  // predict_kernel and select_kernel read, and the factor scratch [B][kmax][Nmax][4] (sized when a stream first turns
-  // the information rule on, and only when the factors cannot stay in shared memory)
-  std::vector<sl2_stream_selection> sel;  // [B]
-  std::vector<int> sel_mode;              // [B] the sources of the device arrays' copies
+  // selection: the sources of the device arrays' copies, the device arrays predict_kernel and select_kernel read, and
+  // the factor scratch [B][kmax][Nmax][4] (only when the factors cannot stay in shared memory)
+  std::vector<int> sel_mode;              // [B]
   std::vector<double> sel_t;              // [B]
-  int *sel_mode_dev = nullptr;            // [B] device: SL2_SELECT_*
-  double *sel_t_dev = nullptr;            // [B] device: exp2(2 min_bits)
+  int *sel_mode_dev = nullptr;            // [B] SL2_SELECT_*
+  double *sel_t_dev = nullptr;            // [B] exp2(2 min_bits)
   sl2::DevPtr<double> sel_g;
   size_t sel_g_bytes = 0;
-  // consensus rescue (sl2_set_stream_rescue): the host mirror of every stream's chi2 (0 = off), the device array
-  // rescue_kernel reads, and the per-stream scratch [B] nis1, [B] logdet1, [B] m2 that the second update and the step
-  // records use (allocated when a stream first turns the rescue on)
-  std::vector<double> resc_chi2;  // [B]
-  double *resc_chi2_dev = nullptr;  // [B] device
-  sl2::DevPtr<uint8_t> resc_scratch;
-  // gyroscope (sl2_set_stream_gyro): the host mirror of every stream's setting, and the device buffers (allocated when
-  // a stream first turns it on): the on flags [B], the settings [B], the sample ring [slots][B] of rates and valid
-  // bytes, the W scratch [B][3][ld] and the results [B] nis, [B] status
-  std::vector<sl2_stream_gyro> gyro;  // [B]
+  // rescue: chi2, and the scratch nis1, logdet1, m2 [B] that the second update and the step records use
+  double *resc_chi2_dev = nullptr;  // [B]
+  sl2::DevPtr<uint8_t> resc_buf;
+  Sl2Rescue resc_dev = {};
+  // gyroscope: the on flags and settings [B], the sample ring [slots][B] of rates and valid bytes, the W scratch
+  // [B][3][ld] and the results nis, status [B]
   sl2::DevPtr<uint8_t> gyro_buf;
   uint8_t *gyro_on_dev = nullptr, *gyro_valid = nullptr;
   Sl2GyroParam *gyro_prm = nullptr;
   double *gyro_rate = nullptr, *gyro_W = nullptr, *gyro_nis = nullptr;
   int *gyro_status = nullptr;
-  // accelerometer (sl2_set_stream_accel): the host mirror of every stream's setting, and the device buffers (allocated
-  // when a stream first turns it on): the on flags [B], the settings [B], the sample ring [slots][B] of forces and valid
-  // bytes and the results [B][3] a, [B] status
-  std::vector<sl2_stream_accel> accel;  // [B]
+  // accelerometer: the on flags and settings [B], the sample ring [slots][B] of forces and valid bytes and the results
+  // a [B][3], status [B]
   sl2::DevPtr<uint8_t> accel_buf;
   uint8_t *accel_on_dev = nullptr, *accel_valid = nullptr;
   Sl2AccelParam *accel_prm = nullptr;
   double *accel_force = nullptr, *accel_a = nullptr;
   int *accel_status = nullptr;
-  // sub-pixel refinement (sl2_set_stream_subpixel): the host mirror of every stream's setting, and one device buffer
-  // (allocated when a stream first turns it on): z [B][Nmax][2] doubles, refined [B][Nmax] and the on flags [B]
-  std::vector<uint8_t> subpix_on;  // [B]
+  // sub-pixel refinement: z [B][Nmax][2], refined [B][Nmax] and the on flags [B]
   sl2::DevPtr<uint8_t> subpix_buf;
-  // iterated update (sl2_set_stream_iterated): the host mirror of every stream's setting, and one device buffer
-  // (allocated when a stream first turns it on) behind iter_dev: the settings, the relinearised tables, the iterate and
-  // the per-stream results
-  std::vector<sl2_stream_iterated> iter;  // [B]
+  Sl2Subpix subpix_dev = {};
+  uint8_t *subpix_on_dev = nullptr;
+  // iterated update: the settings, the relinearised tables, the iterate and the per-stream results
   sl2::DevPtr<uint8_t> iter_buf;
   Sl2Iter iter_dev = {};
-  // stream recovery (sl2_set_stream_recovery): the host mirror of every stream's setting, and one device buffer
-  // (allocated when a stream first turns it on) behind the settings [B], the states [B], the job table [B][Nmax] (feature,
-  // centre, ellipse) and the search and pose kernels' outputs [B][Nmax]
-  std::vector<sl2_stream_recovery> recov;  // [B]
+  // recovery: the settings [B], the states [B], the job table [B][Nmax] (feature, centre, ellipse) and the search and
+  // pose kernels' outputs [B][Nmax]
   sl2::DevPtr<uint8_t> recov_buf;
   sl2_stream_recovery *recov_set = nullptr;
   sl2_recovery_result *recov_state = nullptr;
   int *recov_job_feat = nullptr, *recov_uv = nullptr, *recov_zuv = nullptr;
   double *recov_job_centre = nullptr, *recov_job_puinv = nullptr;
   uint8_t *recov_found = nullptr, *recov_flags = nullptr;
-  // patch normals (sl2_set_stream_normals): the host mirror of every stream's setting, and one device buffer
-  // (allocated when a stream first turns it on) behind the settings [B], theta, cov, count and status
-  std::vector<sl2_stream_normals> nrm;  // [B]
+  // normals: the settings [B], theta, cov, count and status [B][Nmax]
   sl2::DevPtr<uint8_t> nrm_buf;
   Sl2Normals nrm_dev = {};
 };
@@ -201,6 +198,37 @@ inline void enter(sl2_ctx *c, bool join = true) {
 bool bad_stream(sl2_ctx *c, int s);         // enters; true for a null context or a stream outside it
 bool bad_slot(sl2_ctx *c, int s);           // a frame slot outside the ring
 bool bad_range(sl2_ctx *c, int lo, int cnt);  // enters; true for a null context or streams [lo, lo + cnt) outside it
+
+// whether pred(c->opt[s]) holds for some stream s of [lo, lo + cnt)
+template <typename Pred> bool any_stream(const sl2_ctx *c, int lo, int cnt, Pred pred) {
+  for (int s = lo; s < lo + cnt; ++s)
+    if (pred(c->opt[s])) return true;
+  return false;
+}
+
+// One section of a feature's device buffer: alloc_sections points *ptr at its `bytes`
+struct Section {
+  template <typename T>
+  Section(T **p, size_t n)
+      : ptr(p), bytes(n), place([](void *q, uint8_t *at) { *static_cast<T **>(q) = reinterpret_cast<T *>(at); }) {}
+  void *ptr;
+  size_t bytes;
+  void (*place)(void *ptr, uint8_t *at);
+};
+// A feature's buffer, allocated when a stream first turns the feature on: the sections in order, each at a 256-byte
+// boundary, in one allocation zero-filled on the context's stream.  `buf` and the section pointers are set only once
+// the allocation and the fill have both succeeded, so a failure (SL2_ERR_CUDA) leaves the feature unallocated.
+int alloc_sections(sl2_ctx *c, DevPtr<uint8_t> &buf, std::initializer_list<Section> secs);
+
+// One output of a results getter: `per_stream` bytes of stream s at src + s * per_stream on the device
+struct ResultCopy {
+  void *dst;
+  const void *src;
+  size_t per_stream;
+};
+// The results of streams [lo, lo + cnt) into every non-null dst: zeros when the feature's buffer was never allocated
+// (no stream has run it), else one copy each and one synchronise
+int read_results(sl2_ctx *c, bool allocated, int lo, int cnt, std::initializer_list<ResultCopy> outs);
 
 // Grows a scratch buffer, whose contents never outlive a call, to `bytes`: the old one is released once the context's
 // stream is done with it (and before the new allocation, so the peak stays one buffer), then the device buffer and its
@@ -292,18 +320,17 @@ int check_stream_config(sl2_ctx *c, const sl2_stream_config *sc, const std::stri
 int install_sources(sl2_ctx *c, const std::vector<sl2_stream_source> &srcs);
 int loaded_cameras(sl2_ctx *c, int lo, const std::vector<sl2_stream_config> &cams);
 cudaError_t copy_slot_frames(sl2_ctx *c, int slot, const uint8_t *src, cudaMemcpyKind kind, Sl2Queue q);
-// select.cu: whether some stream of [lo, lo + cnt) selects by information; the selection of those streams on q, right
-// after their prediction
-bool selection_on(const sl2_ctx *c, int lo, int cnt);
+// streams [lo, lo + cnt) start over with a new map (sl2_set_features, the snapshot loads): no refined matches,
+// tracking, and every normal unestimated
+int streams_restarted(sl2_ctx *c, int lo, int cnt);
+// select.cu: the selection of the streams [lo, lo + cnt) on q, right after their prediction
 int select_streams(sl2_ctx *c, int lo, int cnt, Sl2Queue q);
-// rescue.cu: whether some stream of [lo, lo + cnt) has the consensus and the rescue on; the rescue's kernel arguments;
-// the rescue kernel and the second update of those streams on q, right after their first update
-bool rescue_on(const sl2_ctx *c, int lo, int cnt);
+// rescue.cu: the rescue's kernel arguments; the rescue kernel and the second update of the streams [lo, lo + cnt) on
+// q, right after their first update
 Sl2Rescue rescue_args(const sl2_ctx *c);
 int rescue_streams(sl2_ctx *c, int lo, int cnt, Sl2Queue q);
-// gyro.cu: whether some stream of [lo, lo + cnt) has the gyroscope on; the gyro update of those streams on q with the
-// samples of ring slot `slot`, between their motion prediction and their feature prediction
-bool gyro_on(const sl2_ctx *c, int lo, int cnt);
+// gyro.cu: the gyro update of the streams [lo, lo + cnt) on q with the samples of ring slot `slot`, between their
+// motion prediction and their feature prediction
 int gyro_streams(sl2_ctx *c, int slot, int lo, int cnt, Sl2Queue q);
 // gyro.cu: what the gyroscope and accelerometer settings share: every entry of v[0 .. n) finite; the checks that R
 // (row-major, named rname in the message) is a rotation and C a symmetric positive definite covariance, an empty

@@ -344,11 +344,7 @@ int sl2_load_streams(sl2_ctx *c, int32_t lo, int32_t cnt, const void *buf, size_
     CU_TRY(c, sl2_launch_unpack(c->d, k, reinterpret_cast<const Sl2SnapLoad *>(c->stg_dev.get()),
                                 c->stg_dev.get() + pb, sb, queue(c)));
   }
-  int rf = subpixel_forget(c, lo, cnt);  // z is the integer match until the streams' next step
-  if (rf) return rf;
-  rf = recovery_reset(c, lo, cnt);  // a loaded stream is tracking
-  if (rf) return rf;
-  for (int s = lo; s < lo + cnt && !rf; ++s) rf = normals_reset(c, s, 0, c->d.Nmax);  // snapshots carry no normals
+  const int rf = streams_restarted(c, lo, cnt);
   if (rf) return rf;
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   return loaded_cameras(c, lo, cams);
@@ -387,11 +383,7 @@ int sl2_load_streams_dev(sl2_ctx *c, int32_t lo, int32_t cnt, const void *buf_de
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   if (bad) return fail(c, SL2_ERR_ARG, "sl2_load_streams_dev: sel_rank or job_feat out of range");
   CU_TRY(c, sl2_launch_unpack(c->d, cnt, q_dev, in, stride, queue(c)));
-  int rf = subpixel_forget(c, lo, cnt);  // z is the integer match until the streams' next step
-  if (rf) return rf;
-  rf = recovery_reset(c, lo, cnt);  // a loaded stream is tracking
-  if (rf) return rf;
-  for (int s = lo; s < lo + cnt && !rf; ++s) rf = normals_reset(c, s, 0, c->d.Nmax);  // snapshots carry no normals
+  const int rf = streams_restarted(c, lo, cnt);
   if (rf) return rf;
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   return loaded_cameras(c, lo, cams);

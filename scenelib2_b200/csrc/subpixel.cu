@@ -98,16 +98,6 @@ __global__ void __launch_bounds__(32 * SUBPIX_WARPS) subpixel_kernel(const Sl2De
   }
 }
 
-// the context's buffer: z [B][Nmax][2] doubles, refined [B][Nmax], on [B]
-size_t subpix_bytes(const Sl2Dev &d) { return (size_t)d.B * d.Nmax * (2 * sizeof(double) + 1) + d.B; }
-uint8_t *subpix_on_dev(const sl2_ctx *c) {
-  return c->subpix_buf.get() + (size_t)c->d.B * c->d.Nmax * (2 * sizeof(double) + 1);
-}
-Sl2Subpix subpix_all(const sl2_ctx *c) {
-  uint8_t *base = c->subpix_buf.get();
-  return {reinterpret_cast<double *>(base), base + (size_t)c->d.B * c->d.Nmax * 2 * sizeof(double)};
-}
-
 }  // namespace
 
 cudaError_t sl2_launch_subpixel(const Sl2Dev &d, const SubpixelLaunch &L, Sl2Queue q) {
@@ -122,10 +112,8 @@ cudaError_t sl2_launch_subpixel(const Sl2Dev &d, const SubpixelLaunch &L, Sl2Que
 namespace sl2 {
 
 Sl2Subpix subpixel_args(const sl2_ctx *c, int lo, int cnt) {
-  if (!c->subpix_buf) return {};
-  for (int s = lo; s < lo + cnt; ++s)
-    if (c->subpix_on[s]) return subpix_all(c);
-  return {};
+  if (!c->subpix_buf || !any_stream(c, lo, cnt, [](const StreamOptions &o) { return o.subpixel != 0; })) return {};
+  return c->subpix_dev;
 }
 
 int subpixel_streams(sl2_ctx *c, int slot, int lo, int cnt, const uint8_t *job_patches, Sl2Queue q) {
@@ -133,16 +121,16 @@ int subpixel_streams(sl2_ctx *c, int slot, int lo, int cnt, const uint8_t *job_p
   L.stream_lo = lo;
   L.stream_cnt = cnt;
   L.slot = slot;
-  L.on = subpix_on_dev(c);
+  L.on = c->subpix_on_dev;
   L.job_patches = job_patches;
-  L.out = subpix_all(c);
+  L.out = c->subpix_dev;
   CU_TRY(c, sl2_launch_subpixel(c->d, L, q));
   return SL2_OK;
 }
 
 int subpixel_forget(sl2_ctx *c, int lo, int cnt) {
   if (c->subpix_buf && cnt > 0)
-    CU_TRY(c, cudaMemsetAsync(subpix_all(c).refined + (size_t)lo * c->d.Nmax, 0, (size_t)cnt * c->d.Nmax, c->stream));
+    CU_TRY(c, cudaMemsetAsync(c->subpix_dev.refined + (size_t)lo * c->d.Nmax, 0, (size_t)cnt * c->d.Nmax, c->stream));
   return SL2_OK;
 }
 
@@ -153,25 +141,25 @@ extern "C" {
 int sl2_set_stream_subpixel(sl2_ctx *c, int32_t s, int32_t on) {
   if (bad_stream(c, s) || (on != 0 && on != 1)) return fail(c, SL2_ERR_ARG, "sl2_set_stream_subpixel: bad argument");
   if (on && !c->subpix_buf) {
-    DevPtr<uint8_t> h;
-    const size_t bytes = subpix_bytes(c->d);
-    CU_TRY(c, cuda_malloc(h, bytes));
-    CU_TRY(c, cudaMemsetAsync(h.get(), 0, bytes, c->stream));
-    c->subpix_buf = std::move(h);
+    const size_t BN = (size_t)c->d.B * c->d.Nmax;
+    Sl2Subpix &sp = c->subpix_dev;
+    const int rc = alloc_sections(
+        c, c->subpix_buf, {{&sp.z, BN * 2 * sizeof(double)}, {&sp.refined, BN}, {&c->subpix_on_dev, (size_t)c->d.B}});
+    if (rc) return rc;
   }
   if (c->subpix_buf) {
-    CU_TRY(c, cudaMemsetAsync(subpix_on_dev(c) + s, on, 1, c->stream));
+    CU_TRY(c, cudaMemsetAsync(c->subpix_on_dev + s, on, 1, c->stream));
     // the refined flags describe steps the stream ran with the refinement on, and an off stream has none
     const int rc = subpixel_forget(c, s, 1);
     if (rc) return rc;
   }
-  c->subpix_on[s] = (uint8_t)on;
+  c->opt[s].subpixel = (uint8_t)on;
   return SL2_OK;
 }
 
 int sl2_get_stream_subpixel(sl2_ctx *c, int32_t s, int32_t *on) {
   if (bad_stream(c, s) || !on) return fail(c, SL2_ERR_ARG, "sl2_get_stream_subpixel: bad argument");
-  *on = c->subpix_on[s];
+  *on = c->opt[s].subpixel;
   return SL2_OK;
 }
 

@@ -1637,7 +1637,8 @@ int sl2_ekf_update_measured(sl2_ctx *c, int32_t s) {
   if (rc0) return rc0;
   CU_TRY(c, sl2_launch_update(c->d, s, 1, -1, nullptr, nullptr, nullptr, nullptr, nullptr, 0, subpixel_args(c, s, 1),
                               queue(c), nullptr, iterate_args(c, s, 1)));
-  if (rescue_on(c, s, 1)) {  // the fused step's rescue and second update
+  // the fused step's rescue and second update
+  if (any_stream(c, s, 1, [](const StreamOptions &o) { return o.chi2 > 0.0 && o.inlier_px > 0.0; })) {
     const int rc = rescue_streams(c, s, 1, queue(c));
     if (rc) return rc;
   }

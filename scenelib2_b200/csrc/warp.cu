@@ -250,13 +250,13 @@ int sl2_set_stream_warp(sl2_ctx *c, int32_t s, int32_t on) {
     if (rc) return rc;
   }
   CU_TRY(c, cudaMemsetAsync(c->warp_on_dev + s, on, 1, c->stream));
-  c->warp_on[s] = (uint8_t)on;
+  c->opt[s].warp = (uint8_t)on;
   return SL2_OK;
 }
 
 int sl2_get_stream_warp(sl2_ctx *c, int32_t s, int32_t *on) {
   if (bad_stream(c, s) || !on) return fail(c, SL2_ERR_ARG, "sl2_get_stream_warp: bad argument");
-  *on = c->warp_on[s];
+  *on = c->opt[s].warp;
   return SL2_OK;
 }
 
@@ -306,13 +306,13 @@ int sl2_set_stream_blur(sl2_ctx *c, int32_t s, const sl2_stream_blur *b) {
   }
   const sl2_stream_blur v = *b;  // pageable copies have read their sources when they return; ordered on the stream
   CU_TRY(c, cudaMemcpyAsync(c->blur_dev + s, &v, sizeof v, cudaMemcpyHostToDevice, c->stream));
-  c->blur[s] = v;
+  c->opt[s].blur = v;
   return SL2_OK;
 }
 
 int sl2_get_stream_blur(sl2_ctx *c, int32_t s, sl2_stream_blur *b) {
   if (bad_stream(c, s) || !b) return fail(c, SL2_ERR_ARG, "sl2_get_stream_blur: bad argument");
-  *b = c->blur[s];
+  *b = c->opt[s].blur;
   return SL2_OK;
 }
 

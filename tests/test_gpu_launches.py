@@ -178,6 +178,29 @@ def test_zero_size_and_refused_calls_launch_nothing():
 
 
 @pytest.mark.gpu
+def test_option_setters_launch_nothing():
+    """Every per-stream option setter writes its device copies with ordered copies, no kernel: the first turn-on (which
+    sizes the feature's buffer), a turn-off and a repeat each add 0 launches.  sl2_set_stream_config launches one."""
+    ctx, _ = _scene_ctx()
+    setters = {"consensus": (lambda on: ctx.set_stream_consensus(1, 2.0 * on)),
+               "rescue": (lambda on: ctx.set_stream_rescue(1, 5.991 * on)),
+               "warp": (lambda on: ctx.set_stream_warp(1, on)),
+               "blur": (lambda on: ctx.set_stream_blur(1, on, exposure=0.01)),
+               "subpixel": (lambda on: ctx.set_stream_subpixel(1, on)),
+               "selection": (lambda on: ctx.set_stream_selection(1, on, min_bits=0.5 * on)),
+               "gyro": (lambda on: ctx.set_stream_gyro(1, on)),
+               "accel": (lambda on: ctx.set_stream_accel(1, on)),
+               "iterated": (lambda on: ctx.set_stream_iterated(1, 2 * on)),
+               "recovery": (lambda on: ctx.set_stream_recovery(1, 3 * on, Pxx=1e-6 * np.eye(13))),
+               "normals": (lambda on: ctx.set_stream_normals(1, 2 * on))}
+    for name, set_on in setters.items():
+        for on in (1, 0, 1, 1, 0):
+            assert _launches(ctx, lambda: set_on(on))[1] == 0, (name, on)
+    assert _launches(ctx, lambda: ctx.set_stream_config(1))[1] == 1
+    ctx.close()
+
+
+@pytest.mark.gpu
 def test_snapshots():
     """The device save is one launch and the device load two (check, unpack); a device blob the check kernel refuses
     costs that one launch.  The host forms launch once per staging group of streams."""
